@@ -1,4 +1,4 @@
-"""bench.py — denoising-steps/sec of the DAWN denoising UNet on B200 (BASELINE.json metric).
+"""bench.py — denoising-steps/sec of the DAWN denoising UNet on H100 (BASELINE.json metric).
 
   python bench.py --gpus N --steps K --warmup W            # our CUDA path
   python bench.py --impl reference --gpus N --steps K ...  # the reference's CPU algorithm (oracle port) on host cores
@@ -9,7 +9,7 @@ N > 1 (torchrun, one rank per GPU): ONE clip of 200*N frames is sharded by conti
 GPU (weak scaling), exactly: +-40-frame halo exchange before each of the 10 temporal attentions (ncclSend/Recv) and a
 16-double all-reduce per GroupNorm (40 per step) inside the library; `value` counts 200-frame-clip equivalents
 (frames denoised per second / 200).  `--replicas` runs one independent 200-frame clip per GPU instead.
-Prints ONE JSON line on rank 0.
+Prints ONE JSON line on rank 0.  --dump-outputs DIR writes the eps of the last timed step (rank 0) as DIR/eps.npy (float32).
 """
 import argparse
 import json
@@ -34,16 +34,11 @@ CPU_SAMPLE_FRAMES = 16
 
 
 def peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        with open(p) as f:
-            d = json.load(f)
-        return dict(hbm=d["hbm_gbs"], tensor=d.get("bf16_tflops_sustained", d["bf16_tflops"]), src="measured (MEASURED_PEAKS.json, bf16 sustained)")
-    return dict(hbm=6650.0, tensor=1400.0, src="fallback (B200_PROFILING.md)")
+    return dict(hbm=3350.0, tensor=989.0, src="NVIDIA H100 SXM data sheet (700 W): HBM3 3.35 TB/s, dense fp16/bf16 989 TFLOP/s")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
     def __init__(self, gpu_index):
@@ -250,6 +245,7 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--replicas", action="store_true", help="N > 1: independent clips per GPU instead of one frame-sharded clip")
     ap.add_argument("--no-clip", action="store_true", help="skip the whole-clip pipeline (configs[4]) measurement")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the eps of the last timed step as DIR/eps.npy (float32)")
     ap.add_argument("--cpu-baseline-worker", action="store_true", help=argparse.SUPPRESS)
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
@@ -264,7 +260,7 @@ def main():
                               f"replicas x{args.gpus} (one 200-frame clip per GPU, no collective)" if args.replicas else
                               f"exact frame sharding x{args.gpus}: one {F_CLIP * args.gpus}-frame clip, {F_CLIP} frames/GPU; per step 10 halo "
                               "exchanges (ncclSend/Recv of 40 boundary frames) + 40 GroupNorm all-reduces (16 fp64) over NVLink"),
-              "l2": "per-step working set ~7 GB >> 126 MB L2 (inputs larger than L2, no explicit flush)"}
+              "l2": "per-step working set ~7 GB >> 50 MB L2 (inputs larger than L2, no explicit flush)"}
 
     if args.cpu_baseline_worker:
         cb, _ = cpu_baseline_run(sd_cpu, 3, 1)
@@ -359,6 +355,10 @@ def main():
                 "allreduce_impl": "one kernel over NVLink peer memory (cudaIpc mailboxes)" if os.environ.get("DAWN_P2P", "1") != "0" else "ncclAllReduce",
                 "halo_impl": "pack copy + grouped ncclSend/ncclRecv with the two neighbours"}
     log(f"device-resident: {ms_per_step:.2f} ms/step")
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "eps.npy"), out_d.cpu().numpy().astype(np.float32))     # (3, 200, 64, 64): 9.8 MB
 
     # ---------------- end to end through the C-ABI with HOST buffers (H2D inputs + D2H eps every step)
     xt_h, fea_h, cond_h = x_t.pin_memory(), fea.pin_memory(), cond.pin_memory()
@@ -421,20 +421,12 @@ def main():
                      "alg_tflops": (v["flops"] / (v["ms"] * 1e-3) / 1e12) if v["ms"] > 0 and v["flops"] > 0 else None,
                      "alg_gbs": (v["bytes"] / (v["ms"] * 1e-3) / 1e9) if v["ms"] > 0 and v["bytes"] > 0 else None}
                  for k, v in prof.items() if v["count"] > 0}
-    traffic = {}
-    import glob
-    tfiles = sorted(glob.glob(os.path.join(ROOT, "profiles", "r*_traffic.json")))
-    tpath = tfiles[-1] if tfiles else ""             # newest committed ncu --set full capture (same kernels as this HEAD: profiles/README.md)
-    if tpath and os.path.exists(tpath):              # dram bytes per launch of exactly these launches
-        with open(tpath) as f:
-            traffic = json.load(f)
-
     def tensor_view(cat, kernel, note):
         v = prof[cat]
         n = max(v["count"], 1)
         tf = v["flops"] / (v["ms"] * 1e-3) / 1e12 if v["ms"] > 0 else 0.0
         return {"kernel": kernel, "bound": "tensor", "achieved": tf, "peak": pk["tensor"], "unit": "TFLOP/s", "frac": tf / pk["tensor"],
-                "traffic": traffic.get(cat, {}).get("dram_bytes_per_launch"), "peak_source": pk["src"],
+                "peak_source": pk["src"],
                 "alg_flops_per_launch": v["flops"] / n, "alg_bytes_per_launch": v["bytes"] / n, "avg_launch_ms": v["ms"] / n,
                 "launches_per_step": v["count"] // args.steps, "share_of_step": v["ms"] / total_kernel_ms if total_kernel_ms else 0,
                 "note": note}
@@ -443,17 +435,17 @@ def main():
                   "fp32-level parity, so the attainable fraction of the bf16 peak is 1/3")
     # the kernel with the largest share of the step: fused per-pixel temporal attention at level 0 (4096 px x 200 f x 64 ch)
     roofline = tensor_view("temporal_fused_l0",
-                           "temporal_tc_kernel @ level 0 (LayerNorm + QKV projection + rotary + banded softmax attention + out-projection "
-                           "+ residual per pixel sequence; tcgen05 kind::f16 FP16x3, TMEM accumulators, P from TMEM)",
+                           "temporal_fused_kernel @ level 0 (LayerNorm + QKV projection + rotary + banded softmax attention + out-projection "
+                           "+ residual per pixel sequence; mma.sync m16n8k16 FP16x3)",
                            split_note + "; flops = QKV 80.5 + attention 61 + out-proj 26.8 GFLOP per launch")
-    # second view: the tcgen05 halo-tile 3x3 conv (64 -> 64 channels, 819 200 px), the largest tcgen05 kernel
-    roofline_conv3 = tensor_view("conv3x3_l0", "tc_conv3_kernel<64> @ level 0 (halo-tile tcgen05 3x3 conv 64->64 ch, FP16x3 kind::f16, TMEM accumulators)",
+    # second view: the halo-tile 3x3 conv (64 -> 64 channels, 819 200 px), the largest wgmma kernel
+    roofline_conv3 = tensor_view("conv3x3_l0", "tc_conv3_kernel<64> @ level 0 (halo-tile wgmma 3x3 conv 64->64 ch, FP16x3 m64n64k16, register accumulators)",
                                  split_note)
     # third view: an HBM-bound kernel of the path — SiLU(GroupNorm(y)) + residual (reads y and the residual, writes the block output)
     gna = prof["gn_apply"]
     gna_gbs = gna["bytes"] / (gna["ms"] * 1e-3) / 1e9 if gna["ms"] > 0 else 0.0
     roofline_hbm = {"kernel": "gn_apply_kernel (SiLU(GroupNorm(y)) + residual, all levels)", "bound": "hbm", "achieved": gna_gbs, "peak": pk["hbm"],
-                    "unit": "GB/s", "frac": gna_gbs / pk["hbm"], "traffic": traffic.get("gn_apply_l0", {}).get("dram_bytes_per_launch"),
+                    "unit": "GB/s", "frac": gna_gbs / pk["hbm"],
                     "launches_per_step": gna["count"] // args.steps, "share_of_step": gna["ms"] / total_kernel_ms if total_kernel_ms else 0}
     # whole-step roofline for context (BASELINE.md: F_alg 3834.6 GFLOP, B_alg 22.9 GB per step at this config)
     step_roof = {"F_alg_gflop": 3834.6, "B_alg_gb": 22.9,

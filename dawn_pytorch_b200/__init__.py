@@ -1,4 +1,4 @@
-"""B200-native (sm_100a) implementation of DAWN's per-step denoising UNet behind the reference's
+"""H100-native (sm_90a) implementation of DAWN's per-step denoising UNet behind the reference's
 Python module interface (DynamicNfUnet3D / DynamicNfGaussianDiffusion)."""
 from .unet import DynamicNfUnet3D, Unet3D  # noqa: F401
 from .diffusion import DynamicNfGaussianDiffusion, GaussianDiffusion  # noqa: F401

@@ -29,7 +29,7 @@ def _load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             f"{LIB_PATH} is missing: build it with `python dawn_pytorch_b200/build.py` "
-            "(nvcc, sm_100a). There is no CPU or PyTorch fallback for the DAWN denoising UNet.")
+            "(nvcc, sm_90a). There is no CPU or PyTorch fallback for the DAWN denoising UNet.")
     lib = ctypes.CDLL(LIB_PATH)
     vp, i64p, fp, cp = ctypes.c_void_p, ctypes.POINTER(ctypes.c_int64), ctypes.c_void_p, ctypes.c_char_p
     lib.dawn_unet_create.argtypes = [ctypes.POINTER(DawnUnetCfg), ctypes.POINTER(vp)]
@@ -54,8 +54,6 @@ def _load():
     lib.dawn_unet_workspace_bytes.restype = ctypes.c_int64
     lib.dawn_selftest_tc_gemm.argtypes = [ctypes.c_int] * 7 + [ctypes.POINTER(ctypes.c_float)] * 2
     lib.dawn_selftest_attention.argtypes = [ctypes.c_int] * 3 + [ctypes.POINTER(ctypes.c_float)] * 2
-    lib.dawn_temporal_tc_plan.argtypes = [ctypes.c_int] * 4 + [ctypes.POINTER(ctypes.c_int)]
-    lib.dawn_selftest_temporal_tc.argtypes = [ctypes.c_int] * 5 + [ctypes.POINTER(ctypes.c_float)] * 2 + [ctypes.POINTER(ctypes.c_uint64), ctypes.POINTER(ctypes.c_float)]
     lib.dawn_nccl_unique_id.argtypes = [ctypes.c_char_p]
     lib.dawn_unet_init_shard.argtypes = [vp, ctypes.c_char_p, ctypes.c_int, ctypes.c_int, ctypes.c_int]
     lib.dawn_unet_shard_ipc_export.argtypes = [vp, ctypes.c_char_p]
@@ -92,7 +90,7 @@ EXPORTS = ["dawn_unet_create", "dawn_unet_destroy", "dawn_unet_set_param", "dawn
            "dawn_unet_set_num_frames", "dawn_nccl_unique_id", "dawn_unet_init_shard", "dawn_unet_shard_ipc_export", "dawn_unet_shard_ipc_import", "dawn_unet_set_clip_invariants", "dawn_unet_forward",
            "dawn_unet_forward_x3", "dawn_unet_forward_host", "dawn_unet_set_tap", "dawn_unet_tap_shape",
            "dawn_unet_profile_enable", "dawn_unet_profile_read", "dawn_unet_last_launch_count", "dawn_unet_workspace_bytes", "dawn_ddim_step", "dawn_unet_ddim_step", "dawn_unet_sampler_capture", "dawn_unet_sampler_launch",
-           "dawn_selftest_tc_gemm", "dawn_selftest_attention", "dawn_selftest_temporal_tc", "dawn_temporal_tc_plan", "dawn_last_error", "dawn_build_info"]
+           "dawn_selftest_tc_gemm", "dawn_selftest_attention", "dawn_last_error", "dawn_build_info"]
 
 
 LFG_EXPORTS = ["dawn_lfg_create", "dawn_lfg_destroy", "dawn_lfg_set_param", "dawn_lfg_commit_params", "dawn_lfg_set_geometry",

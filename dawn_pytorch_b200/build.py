@@ -1,4 +1,4 @@
-"""Build libdawn_unet.so (sm_100a only) in-tree with nvcc.  `python dawn_pytorch_b200/build.py [--force]`."""
+"""Build libdawn_unet.so (sm_90a only) in-tree with nvcc.  `python dawn_pytorch_b200/build.py [--force]`."""
 import hashlib
 import os
 import subprocess
@@ -10,7 +10,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libdawn_unet.so")
 OBJ = os.path.join(HERE, "build")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC", "-Xptxas", "-v", "--expt-relaxed-constexpr"]
 
 

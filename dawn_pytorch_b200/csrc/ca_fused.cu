@@ -6,7 +6,7 @@
 //
 // Every frame has exactly two keys per cross-attention (its conditioning token and the learned null token), so the attention output
 // is an affine function of one gate per head; unet.cu folds to_out / LayerNorm into per-frame tables (T, G) and the block only needs
-// Wt = rstd * [1, gate_0..7] per cross-attention.  The unfused path ran a tcgen05 GEMM with N = 192 (three 64-column tiles, each
+// Wt = rstd * [1, gate_0..7] per cross-attention.  The unfused path ran a wgmma GEMM with N = 192 (three 64-column tiles, each
 // re-gathering and re-splitting the A rows; gates through HBM) plus ca_rstd_kernel.  Here a warp owns 16 pixels: q comes out of
 // mma.sync (3-term FP16 split, fp32 accumulate) 64 columns at a time, the accumulator layout gives each quad one head per n-tile, and
 // the gates never leave the SM.
@@ -271,7 +271,7 @@ int launch_ci(CaFusedArgs a, cudaStream_t st) {
 // a1 = SiLU(FiLM(GroupNorm(y))) + Wt (M x 32) * T_f (32 x co)      (first half of a conditioned ResnetBlock, U:366-380, 454-463)
 // A streaming kernel: Wt rows arrive straight in A-fragment order from global memory, the frame's table T_f sits in shared memory as
 // fp16 hi|lo, the K = 32 product is 6 mma.sync per 8 channels, and the epilogue reads y / writes a1 in 32-byte quad segments.
-// (x0, x1) -> packed fp16 hi pair / lo pair with the round-to-nearest 11-bit split of the tcgen05 producers (tc_common.cuh split_f16x2)
+// (x0, x1) -> packed fp16 hi pair / lo pair with the round-to-nearest 11-bit split of the wgmma GEMM producers (tc_common.cuh split_f16x2)
 __device__ __forceinline__ void split_rn(float x0, float x1, uint32_t& hi, uint32_t& lo) {
   const float h0 = __uint_as_float((__float_as_uint(x0) + 0x1000u) & 0xFFFFE000u);
   const float h1 = __uint_as_float((__float_as_uint(x1) + 0x1000u) & 0xFFFFE000u);

@@ -23,7 +23,7 @@ struct GnHcondArgs {
   const float* T; int ldbT;       // [F][32][ldbT] per-frame tables
   const float* Y; int ldy;        // conv1 output
   float* Out; int ldo;            // a1 (fp32), or
-  unsigned short *Out16h, *Out16l; // a1 as two dense fp16 planes [F*P][co] (hi | lo of the tcgen05 split): the consuming 3x3 conv then
+  unsigned short *Out16h, *Out16l; // a1 as two dense fp16 planes [F*P][co] (hi | lo of the wgmma-kernel split): the consuming 3x3 conv then
                                   // fetches its halo tiles by TMA with no conversion pass; same bytes as the fp32 row
   int F, P, co;
   const double* gn_stats; double gn_count; int cpg;     // clip-wide GroupNorm sums (sum, sumsq per group)

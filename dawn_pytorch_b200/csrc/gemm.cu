@@ -1,7 +1,7 @@
 // Universal implicit GEMM, warp-level mma.sync m16n8k8 with 3xTF32 split precision
 // (hi*hi + hi*lo + lo*hi, fp32 accumulate): SURVEY Appendix D shows single-pass TF32/BF16 break the
 // rtol 1e-3 / atol 1e-4 parity bar, the 3-term split sits at the fp32 re-association floor.
-// This is the robust baseline contraction path; the tcgen05 path (tc_gemm.cu) takes over the
+// This is the robust baseline contraction path; the wgmma path (tc_gemm.cu) takes over the
 // large regular contractions.
 #include "common.cuh"
 #include "gemm.cuh"
@@ -130,7 +130,7 @@ __global__ void __launch_bounds__(THREADS, 2) gemm_kernel(const GemmParams p) {
         split_tf32(a[8 * A_LD + 4], ahi[mt][3], alo[mt][3]);
       }
       // The tensor core accumulates with round-toward-zero; chained over K that bias grows ~K*2^-24
-      // (measured on B200: 1.4e-4 at K=14112).  So each k-step's 3-term product lands in a zeroed
+      // (1.4e-4 at K=14112).  So each k-step's 3-term product lands in a zeroed
       // fragment and is added to the running sum with an ordinary round-to-nearest FADD.
 #pragma unroll
       for (int nt = 0; nt < 4; ++nt) {

@@ -20,7 +20,7 @@ enum Epi : int {
 struct GemmParams {
   // A operand (gathered)
   const float* A; int lda; int Cin;
-  // optional pre-split copy of A (fp16 hi and lo planes, dense rows of Cin halfs): the tcgen05 producers then only copy
+  // optional pre-split copy of A (fp16 hi and lo planes, dense rows of Cin halfs): the wgmma-kernel producers then only copy
   const unsigned short* A16h = nullptr; const unsigned short* A16l = nullptr;
   int want_split = 0;      // host side: ask Ctx::gemm to build the pre-split copy
   int up2 = 0;             // halo conv3 kernel only: 64-column block j of the output is parity class j of a 2x upsampled grid
@@ -37,16 +37,16 @@ struct GemmParams {
   int perm_f_lo, perm_f_hi;  // perm_out only: rows whose frame f lies outside [f_lo, f_hi) are dropped, the rest go to frame f - f_lo
   // B operand [K][ldb] (ldb multiple of 64, zero padded)
   const float* B; int ldb; long long b_batch_stride;
-  const float* Bimg;       // optional tcgen05 image of B (tc_pack_weights), or null
-  float tc_scale;          // accumulator rescale of the tcgen05 path: 1 / (activation scale * weight image scale)
+  const float* Bimg;       // optional wgmma image of B (tc_pack_weights), or null
+  float tc_scale;          // accumulator rescale of the wgmma path: 1 / (activation scale * weight image scale)
   // output
   float* Out; int ldo; int OH, OW, out_stride, oy0, ox0;
   const float* bias;
   const float* Res; int ldr;
   double* stats; int cpg;  // GroupNorm accumulators [groups][2], channels per group
   // LayerNorm fold
-  const float* rowstats;   // [M][2] (mu, rstd); null on the tcgen05 path when ln_inline is set
-  int ln_inline;           // tcgen05 1x1 GEMMs: the producers accumulate each row's sum / sum of squares while they stream it
+  const float* rowstats;   // [M][2] (mu, rstd); null on the wgmma path when ln_inline is set
+  int ln_inline;           // wgmma 1x1 GEMMs: the producers accumulate each row's sum / sum of squares while they stream it
   const float* wsum;       // [N]  sum_k B[k][n]
   const float* rot;        // [F][16][2] (cos, sin)
   int P;                   // positions per frame (row -> frame index)
@@ -60,11 +60,11 @@ struct GemmParams {
   const float* film;       // [2N] scale | shift, or null
   double gn_count;         // elements per group
   const int* skip_flag; int skip_if;   // mma.sync kernel only: return at once when *skip_flag == skip_if (device-side path selection)
-  int drain;                   // tcgen05 kernels: K panels (tc_gemm) / taps (tc_conv3) accumulated inside TMEM before the fp32 drain; 0 = default
+  int drain;                   // wgmma kernels: K panels (tc_gemm) / taps (tc_conv3) accumulated in registers before the fp32 drain; 0 = default
                                // (4 panels = K 256 / 9 taps = K 576).  The tensor core adds with round-toward-zero: un-normalised conv stacks
                                // (LFG decoder) drain every panel / tap to keep the bias below the fp32 tolerance.
-  int exp_shift;               // experiment (tcgen05 path, BN = 64): A operand stored/addressed this many rows into the swizzle atom
-  unsigned long long* trace;   // optional [16] cycle counters written by CTA 0 of the tcgen05 kernel (debug)
+  int exp_shift;               // experiment (wgmma path, BN = 64): A operand stored/addressed this many rows into the swizzle atom
+  unsigned long long* trace;   // optional [16] cycle counters written by CTA 0 of the wgmma kernel (debug)
 };
 
 // pixel index (f * P + p) of row m in sequence-blocked order

@@ -395,7 +395,7 @@ int launch_ca_rstd(const float* gates, const float* G, int M, int P, float* Wt, 
 }
 
 // =========================================================================== fp16 hi | lo copy of an activation
-// x (M rows, C channels, row stride ld) -> dense hi[M][C], lo[M][C]: the same 11-bit split the tcgen05 producers apply on the fly
+// x (M rows, C channels, row stride ld) -> dense hi[M][C], lo[M][C]: the same 11-bit split the wgmma GEMM producers apply on the fly
 __global__ void split_rows_kernel(const float* __restrict__ x, int ld, int C, long long M, uint2* __restrict__ hi,
                                   uint2* __restrict__ lo) {
   const int c4n = C >> 2;

@@ -1,7 +1,7 @@
 // Host-side orchestration + C-ABI of the LFG flow decoder (include/dawn_lfg.h; reference LFG/modules/generator.py:132-171).
 // One handle = one GPU.  The source-image encoder runs once per clip (dawn_lfg_set_source); dawn_lfg_decode turns a batch of
 // frames' (flow, occlusion) maps into images: warp + blend (apply_optical) -> 6 pre-activation ResBlocks -> 2 up blocks with
-// warped skips -> 7x7 conv + sigmoid -> blend with the warped source image.  Convolutions run on the tcgen05 kernels of the
+// warped skips -> 7x7 conv + sigmoid -> blend with the warped source image.  Convolutions run on the wgmma kernels of the
 // UNet (tc_conv3.cu / tc_gemm.cu, FP16x3 split precision, fp32 accumulation); eval-mode BatchNorms are folded into the conv
 // that precedes them (conv -> BN) or applied as a per-channel affine in the elementwise pass (BN -> ReLU -> conv).
 #include <algorithm>
@@ -37,7 +37,7 @@ struct HostParam {
   std::vector<float> data;
   std::vector<int64_t> shape;
 };
-struct ConvPack {            // [tap * ci_pad + c][ldb] fp32 (+ tcgen05 image), bias [ldb]
+struct ConvPack {            // [tap * ci_pad + c][ldb] fp32 (+ wgmma weight image), bias [ldb]
   float* w = nullptr; float* img = nullptr; float img_scale = 1.f; float* b = nullptr;
   int K = 0, N = 0, ldb = 0, ci_pad = 0;
 };
@@ -215,9 +215,8 @@ void base_params(GemmParams& p, const float* A, int lda, int Cin, int frames, in
   p.P = Hh * Ww;
   p.q_post_scale = 1.f;
   // 14 convolutions without a normalisation in between: the tensor core's round-toward-zero accumulation is a systematic bias that
-  // compounds through the stack, so the TMEM accumulators are drained into RN fp32 registers every 3 taps / K panels (K = 192) instead
-  // of every 9 / 4.  Measured on B200 (internal taps against the oracle, unscaled tolerance): default 0.98-1.31 x tol, every tap
-  // 0.10-0.17 x tol at +20 % decode time; every third tap keeps ~3x headroom at a third of that cost.
+  // compounds through the stack, so the register accumulators are drained into the RN fp32 tile every 3 taps / K panels (K = 192) instead
+  // of every 9 / 4.
   p.drain = 3;
 }
 void set_weights(GemmParams& p, const ConvPack& w) {

@@ -1,5 +1,5 @@
-// Shared device helpers of the tcgen05 kernels (tc_gemm.cu, tc_conv3.cu): mbarrier / bulk-copy / tcgen05 PTX wrappers,
-// UMMA shared-memory descriptors, the fp16 hi/lo split and the coalesced row store.
+// Shared device helpers of the wgmma kernels (tc_gemm.cu, tc_conv3.cu): mbarrier / bulk-copy / wgmma PTX wrappers,
+// shared-memory matrix descriptors, the fp16 hi/lo split and the coalesced row store.
 #pragma once
 #include <cuda_fp16.h>
 #include "common.cuh"
@@ -44,77 +44,63 @@ __device__ __forceinline__ void bulk_copy_g2s(void* smem_dst, const void* gsrc, 
                : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// Elected-lane forms for an issuer WARP that runs its control flow warp-uniformly (all 32 lanes wait on the barriers and compute the
-// operands; one lane -- always the same one, so the commits track its MMAs -- executes the instruction).  With provably uniform operands
-// the descriptors stay in uniform registers and an MMA costs one UTCHMMA; issued from inside an `if (lane == 0)` region every operand
-// goes through a per-lane R2UR loop (~75 cycles of issue per MMA, more than the tensor pipe needs for a 128 x 64 x 16 MMA).
-__device__ __forceinline__ bool elect_one() {
-  uint32_t r;
+
+// ---------------------------------------------------------------- wgmma (sm_90a warpgroup MMA, accumulators in registers)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from touching accumulator registers across an in-flight wgmma
+__device__ __forceinline__ void wgmma_fence_acc(float (&d)[32]) {
+#pragma unroll
+  for (int i = 0; i < 32; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// D(64 x 64, f32) (+)= A(64 x 16, f16, K-major) * B(64 x 16, f16, K-major)^T; scale_d = 0 overwrites D
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
   asm volatile(
       "{\n\t"
-      ".reg .pred q;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, q;\n\t"
-      "}" : "=r"(r));
-  return r != 0;
-}
-__device__ __forceinline__ void tc_mma_f16_elected(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p, q;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tc_commit_elected(uint64_t* bar) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred q;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t"
-      "}" ::"r"(smem_u32(bar))
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+      ".reg .pred p;\n\t"
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n\t"
-      "tcgen05.wait::ld.sync.aligned;"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t"
+      "}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+        "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
+        "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(scale_d)
       : "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
 }
 
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n\t"
-      "tcgen05.wait::ld.sync.aligned;"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+// K-major, 128-byte-swizzled operand: rows of 128 B, 8-row groups `sbo` bytes apart (1024 B for a dense panel), layout SWIZZLE_128B.
+// The swizzle follows absolute shared-memory address bits, so an operand may start at any 128-byte row of a 1024-byte-aligned image.
+__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t sbo = 1024) {
+  return (uint64_t)((saddr >> 4) & 0x3FFF) | (1ull << 16) | ((uint64_t)((sbo >> 4) & 0x3FFF) << 32) | (1ull << 62);
 }
 
-// K-major, 128-byte-swizzled operand panel: rows of 128 B, 8-row atoms of 1024 B (SBO), descriptor version 1 (sm_100)
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
-  return (uint64_t)((saddr >> 4) & 0x3FFF) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
+// A consumer warpgroup's 64 x 64 accumulator fragment (rows r0 + [0, 64) of a [128][kStageLd] fp32 tile): the first drain of a tile
+// stores, later drains add (round-to-nearest fp32 adds outside the tensor core, see tc_gemm.cu)
+constexpr int kStageLd = 68;                  // floats per staged row (64 + 4 pad: conflict-free float4 row reads)
+__device__ __forceinline__ void stage_fragment(float* stage, int r0, const float (&d)[32], bool first, int wtid) {
+  const int w = wtid >> 5, l = wtid & 31;
+  float* p0 = stage + (size_t)(r0 + w * 16 + (l >> 2)) * kStageLd + 2 * (l & 3);
+  float* p1 = p0 + 8 * kStageLd;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    float2* a = reinterpret_cast<float2*>(p0 + 8 * j);
+    float2* b = reinterpret_cast<float2*>(p1 + 8 * j);
+    if (first) {
+      *a = make_float2(d[4 * j], d[4 * j + 1]);
+      *b = make_float2(d[4 * j + 2], d[4 * j + 3]);
+    } else {
+      const float2 x = *a, y = *b;
+      *a = make_float2(x.x + d[4 * j], x.y + d[4 * j + 1]);
+      *b = make_float2(y.x + d[4 * j + 2], y.y + d[4 * j + 3]);
+    }
+  }
 }
-// descriptor for an operand whose first row sits `shift` rows (of 128 B) into a 1024-byte swizzle atom
+
 // byte offset of 16-byte chunk c (0..7) of row r inside a swizzled panel
 __device__ __forceinline__ uint32_t swz(int r, int c) { return (uint32_t)((r >> 3) * 1024 + (r & 7) * 128 + ((c ^ (r & 7)) << 4)); }
 

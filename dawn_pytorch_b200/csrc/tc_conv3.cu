@@ -1,14 +1,14 @@
-// tcgen05 3x3 convolution with a shared-memory HALO tile (sm_100a) — the Block.proj of the reference (U:229, 234).
+// wgmma 3x3 convolution with a shared-memory HALO tile (sm_90a) — the Block.proj of the reference (U:229, 234).
 //
 // tc_gemm.cu treats a 3x3 conv as 9 independent K panels per 64 channels: the same activations are gathered, split to
 // fp16 hi/lo and stored 9 times.  Here a CTA stages the (16+2) x (8+2) pixel halo of its 16x8-pixel output tile ONCE per
-// 64-channel chunk (6.3x less gather/convert/store work) and the 9 taps are 9 shifted operand windows over that tile:
-// measured on B200, with descriptor base_offset = 0 the UMMA 128-byte swizzle follows ABSOLUTE shared-memory address bits,
-// so a K-major operand may start at any 128-byte row and use any row-multiple stride between its 8-row groups:
+// 64-channel chunk (6.3x less gather/convert/store work) and the 9 taps are 9 shifted operand windows over that tile.
+// With descriptor base_offset = 0 the 128-byte swizzle follows ABSOLUTE shared-memory address bits, so a K-major operand
+// may start at any 128-byte row and use any row-multiple stride between its 8-row groups:
 //     window(dy,dx): start = halo + ((dy+1)*10 + (dx+1))*128 B,  stride between 8-pixel rows (SBO) = 10*128 B.
-// Everything else follows tc_gemm.cu: FP16x3 split precision, TMEM double-buffered accumulators drained into RN fp32
-// registers (once per 64-channel chunk = 108 MMAs), persistent warp-specialised CTA (8 producer warps, 4/8 epilogue warps,
-// MMA issuer, weight loader), row-per-thread epilogue with bias + GroupNorm partial statistics.
+// Everything else follows tc_gemm.cu: FP16x3 split precision, register accumulators drained into an RN fp32 tile in shared
+// memory (once per 64-channel chunk), persistent warp-specialised CTA (8 producer warps, 1/2 consumer warpgroups, weight
+// loader), row-per-thread epilogue with bias + GroupNorm partial statistics.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cstdlib>
@@ -32,23 +32,19 @@ constexpr int HROWS = HH * HW;                 // 180 halo pixels = 180 rows of 
 constexpr int A_HALO = 23 * 1024;              // 180 * 128 = 23040 B, padded to 23 KB (keeps 1024-byte alignment)
 constexpr int NPROD = 256;
 
+// B stages: what fits in 227 KB next to the halo stages and the consumers' 128 x 64 fp32 staging tiles (34 KB each)
 template <int BN>
 struct CCfg {
   static constexpr int NWG = BN / 64;
   static constexpr int B_PANEL = BN * 128;                     // one (tap, chunk) weight panel, hi or lo
   static constexpr int A_STAGES = 2;
-  static constexpr int B_STAGES = (BN == 64) ? 4 : 3;
+  static constexpr int B_STAGES = (BN == 64) ? 4 : 2;
   static constexpr int A_BYTES = A_STAGES * 2 * A_HALO;        // hi + lo
   static constexpr int B_BYTES = B_STAGES * 2 * B_PANEL;
-  static constexpr int EPI_STAGE = NWG * 4 * 32 * 20 * 4;
-  static constexpr int SMEM_DYN = A_BYTES + B_BYTES + EPI_STAGE + 1024;
-  static constexpr int NTHREADS = NPROD + 128 * NWG + 64;
-  static constexpr int MMA_WARP = (NPROD + 128 * NWG) / 32;
-  static constexpr int LOAD_WARP = MMA_WARP + 1;
-  // BN == 64: one N=128 MMA multiplies A_hi with [B_hi | B_lo] (two 64-column accumulators, summed by the epilogue):
-  // 2 instead of 3 instructions per k-step, and the N=64 instruction was issue-bound at about the cost of an N=128 one.
-  static constexpr int ACC_COLS = (BN == 64) ? 128 : BN;
-  static constexpr int TMEM_COLS = 2 * ACC_COLS;
+  static constexpr int ACC_STAGE = NWG * 128 * kStageLd * 4;
+  static constexpr int SMEM_DYN = A_BYTES + B_BYTES + ACC_STAGE + 1024;
+  static constexpr int NTHREADS = NPROD + 128 * NWG + 32;      // producers | consumers | loader warp
+  static constexpr int LOAD_WARP = (NPROD + 128 * NWG) / 32;
 };
 
 // A-operand source: TMA = false: fp32 activations, gathered / split / swizzled by the 8 producer warps.  TMA = true: the activation exists as
@@ -62,35 +58,26 @@ __global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const G
                                                                           const __grid_constant__ CUtensorMap tm_lo) {
   using C = CCfg<BN>;
   constexpr int B_PANEL = C::B_PANEL, A_STAGES = C::A_STAGES, B_STAGES = C::B_STAGES, NWG = C::NWG;
-  constexpr int MMA_WARP = C::MMA_WARP, LOAD_WARP = C::LOAD_WARP, TMEM_COLS = C::TMEM_COLS, ACC_COLS = C::ACC_COLS;
+  constexpr int LOAD_WARP = C::LOAD_WARP;
   extern __shared__ uint8_t smem_raw[];
-  __shared__ uint64_t a_full[A_STAGES], a_free[A_STAGES], b_full[B_STAGES], b_free[B_STAGES], acc_full[2], acc_free[2];
-  __shared__ uint32_t s_tmem_base;
+  __shared__ uint64_t a_full[A_STAGES], a_free[A_STAGES], b_full[B_STAGES], b_free[B_STAGES];
   __shared__ float s_stat[NWG][16];
   __shared__ __align__(16) float s_bias[NWG][64];       // bias of this epilogue warpgroup's 64 columns (single n-tile: constant for the whole launch)
 
   const int tid = threadIdx.x, lane = tid & 31;
-  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);          // warp-uniform by construction (the MMA warp relies on it)
+  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);          // warp-uniform by construction
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   uint8_t* smemA = smem;
   uint8_t* smemB = smem + C::A_BYTES;
   uint8_t* smemE = smemB + C::B_BYTES;
 
   if (tid == 0) {
-    for (int s = 0; s < A_STAGES; ++s) { mbar_init(&a_full[s], TMA ? 1 : NPROD); mbar_init(&a_free[s], 1); }
-    for (int s = 0; s < B_STAGES; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_free[s], 1); }
-    mbar_init(&acc_full[0], 1); mbar_init(&acc_full[1], 1);
-    mbar_init(&acc_free[0], 128 * NWG); mbar_init(&acc_free[1], 128 * NWG);
+    // a_free / b_free: one arrive per consumer warp once its MMAs on the slot have completed
+    for (int s = 0; s < A_STAGES; ++s) { mbar_init(&a_full[s], TMA ? 1 : NPROD); mbar_init(&a_free[s], 4 * NWG); }
+    for (int s = 0; s < B_STAGES; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_free[s], 4 * NWG); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == MMA_WARP) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem_base)), "r"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = s_tmem_base;
 
   const int H = p.IH, W = p.IW;
   const int F = p.M / (H * W);
@@ -193,90 +180,18 @@ __global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const G
           }
       }
     }
-  } else if (warp == MMA_WARP) {
-    // =============================================================== MMA issuer: the whole warp, warp-uniform control flow, one elected
-    // lane per MMA / commit (tc_common.cuh: elect_one)
-    {
-      const uint32_t tmem_base_u = __shfl_sync(0xffffffffu, tmem_base, 0);      // read from shared memory: make it a provably uniform value
-      const uint32_t idesc = (1u << 4) | (0u << 7) | (0u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-      const uint32_t idesc2 = (1u << 4) | (0u << 7) | (0u << 10) | ((uint32_t)((2 * BN) >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-      constexpr uint64_t SBO_HALO = (uint64_t)(HW * 128 / 16);   // 10 pixel rows of 128 B between 8-row groups
-      uint32_t ait = 0, bit = 0, cg = 0;
-      const int dt = (p.drain == 1 || p.drain == 3) ? p.drain : 9;   // taps accumulated in TMEM before a drain
-      const bool tr = TR && (p.trace != nullptr) && blockIdx.x == 0;
-      long long t_acc = 0, t_a = 0, t_b = 0, t_issue = 0, t0 = 0;
-      const long long t_begin = clock64();
-      uint32_t ntiles_done = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++ntiles_done) {
-        for (int cc = 0; cc < NCH; ++cc, ++ait) {
-          const int sa = ait % A_STAGES;
-          if (tr) t0 = clock64();
-          mbar_wait(&a_full[sa], (ait / A_STAGES) & 1);
-          if (tr) { const long long t1 = clock64(); t_a += t1 - t0; t0 = t1; }
-          fence_proxy_async();
-          tc_fence_after();
-          const uint32_t a_hi = smem_u32(smemA + sa * 2 * A_HALO), a_lo = a_hi + A_HALO;
-          uint32_t buf = 0, d = 0;
-          int in_group = 0;
-          for (int tap = 0; tap < 9; ++tap, ++bit) {
-            if (in_group == 0) {
-              buf = cg & 1;
-              if (tr) t0 = clock64();
-              mbar_wait(&acc_free[buf], ((cg >> 1) & 1) ^ 1);
-              if (tr) { const long long t1 = clock64(); t_acc += t1 - t0; t0 = t1; }
-              tc_fence_after();
-              d = tmem_base_u + buf * ACC_COLS;
-            }
-            const int sb = bit % B_STAGES;
-            if (tr) t0 = clock64();
-            mbar_wait(&b_full[sb], (bit / B_STAGES) & 1);
-            if (tr) { const long long t1 = clock64(); t_b += t1 - t0; t0 = t1; }
-            tc_fence_after();
-            const int ky = tap / 3, kx = tap - ky * 3;          // window start: halo pixel (ky, kx)
-            const uint32_t woff = (uint32_t)((ky * HW + kx) * 128);
-            // K-major SW128 descriptors: start address, LBO = 1 (unused), SBO, version 1, layout SWIZZLE_128B, base_offset 0
-            const uint64_t ahi = (uint64_t)(((a_hi + woff) >> 4) & 0x3FFF) | (1ull << 16) | (SBO_HALO << 32) | (1ull << 46) | (2ull << 61);
-            const uint64_t alo = (uint64_t)(((a_lo + woff) >> 4) & 0x3FFF) | (1ull << 16) | (SBO_HALO << 32) | (1ull << 46) | (2ull << 61);
-            const uint32_t sbaddr = smem_u32(smemB + sb * 2 * B_PANEL);
-            const uint64_t bhi = make_desc(sbaddr), blo = make_desc(sbaddr + B_PANEL);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const uint64_t o = (uint64_t)(j * 2);
-              if (BN == 64) {
-                // the lo panel follows the hi panel in the stage: rows 64..127 of one N=128 operand
-                tc_mma_f16_elected(d, ahi + o, bhi + o, idesc2, (in_group == 0 && j == 0) ? 0u : 1u);
-                tc_mma_f16_elected(d, alo + o, bhi + o, idesc, 1u);
-              } else {
-                tc_mma_f16_elected(d, alo + o, bhi + o, idesc, (in_group == 0 && j == 0) ? 0u : 1u);
-                tc_mma_f16_elected(d, ahi + o, blo + o, idesc, 1u);
-                tc_mma_f16_elected(d, ahi + o, bhi + o, idesc, 1u);
-              }
-            }
-            tc_commit_elected(&b_free[sb]);
-            if (++in_group == dt) { tc_commit_elected(&acc_full[buf]); ++cg; in_group = 0; }
-            if (tr) t_issue += clock64() - t0;
-          }
-          tc_commit_elected(&a_free[sa]);
-        }
-      }
-      if (tr && lane == 0) {
-        p.trace[0] = (unsigned long long)(clock64() - t_begin); p.trace[1] = ntiles_done;
-        p.trace[2] = (unsigned long long)t_acc; p.trace[3] = (unsigned long long)t_a;
-        p.trace[4] = (unsigned long long)t_b; p.trace[5] = (unsigned long long)t_issue;
-      }
-    }
   } else {
-    // =============================================================== accumulate + epilogue
+    // =============================================================== consumers: MMA (two m64n64 per k-step: output rows 0-63 and
+    // 64-127 of this warpgroup's 64 columns) + row-per-thread epilogue read back from the staged fp32 tile
     const int wg = (warp - 8) >> 2, ew = (warp - 8) & 3;
     const int row_in_tile = ew * 32 + lane;
-    const uint32_t lane_addr = (uint32_t)(ew * 32) << 16;
     const int etid = (tid - NPROD) & 127;
     float* s_st = s_stat[wg];
     const int bar_id = 2 + wg;
-    float* wbuf = reinterpret_cast<float*>(smemE) + ((wg * 4 + ew) * 32 * 20);
-    uint32_t cg = 0;
-    // GroupNorm partial sums (U:230).  Reducing them per tile (16 warp reductions, shared and global atomics, two barriers) cost 7.2k of the
-    // 12.2k cycles a 64 -> 64 tile takes (cycle trace, profiles/r2_f_conv3_trace.md).  With a single n-tile every epilogue thread owns the same
+    float* stage = reinterpret_cast<float*>(smemE) + wg * 128 * kStageLd;
+    float* wbuf = stage + ew * 32 * kStageLd;                 // this warp's own staged rows, free once they are read back
+    // GroupNorm partial sums (U:230).  Reducing them per tile (16 warp reductions, shared and global atomics, two barriers) costs more
+    // than half of a 64 -> 64 tile.  With a single n-tile every epilogue thread owns the same
     // 64 columns for the whole persistent loop, so it keeps fp32 running sums per 8-column block and the warps reduce them (in fp64) only
     // every 8 tiles and at the end: at most 64 values per fp32 partial sum.
     const bool defer_stats = (p.stats != nullptr) && tiles_n == 1;
@@ -284,7 +199,7 @@ __global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const G
     int pending = 0;
 #pragma unroll
     for (int i = 0; i < 8; ++i) { gs[i] = 0.f; gss[i] = 0.f; }
-    // with one n-tile the 64 bias values never change: fetch them once instead of 16 L2 round trips per tile (1.0-1.7k cycles per tile in the trace)
+    // with one n-tile the 64 bias values never change: fetch them once instead of 16 L2 round trips per tile
     const bool bias_smem = (p.bias != nullptr) && tiles_n == 1;
     if (bias_smem) {
       if (etid < 64) s_bias[wg][etid] = __ldg(p.bias + wg * 64 + etid);
@@ -307,37 +222,73 @@ __global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const G
       pending = 0;
     };
     const bool tre = TR && (p.trace != nullptr) && blockIdx.x == 0 && etid == 0 && wg == 0;
-    long long te_wait = 0, te_drain = 0, te_final = 0, te0 = 0, te_bias = 0, te_store = 0, te1 = 0;
+    long long te_final = 0, te0 = 0, te_bias = 0, te_store = 0, te1 = 0;
+    constexpr uint32_t SBO_HALO = HW * 128;                    // 10 pixel rows of 128 B between 8-row groups
+    constexpr uint32_t H2 = 8 * HW * 128;                      // output rows 64-127 start 8 halo rows further down
+    const int dt = (p.drain == 1 || p.drain == 3) ? p.drain : 9;   // taps accumulated in registers before a drain
+    uint32_t ait = 0, bit = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       int f, y0, x0, nt;
       decode(tile, f, y0, x0, nt);
       const int n0 = nt * BN + wg * 64;
-      float acc[64];
+      float d0[32], d1[32];
+      bool first_drain = true;
+      for (int cc = 0; cc < NCH; ++cc, ++ait) {
+        const int sa = ait % A_STAGES;
+        mbar_wait(&a_full[sa], (ait / A_STAGES) & 1);
+        fence_proxy_async();
+        const uint32_t a_hi = smem_u32(smemA + sa * 2 * A_HALO), a_lo = a_hi + A_HALO;
+        int in_group = 0, pend = -1;                           // B stage whose MMAs are still in flight
+        for (int tap = 0; tap < 9; ++tap, ++bit) {
+          const int sb = bit % B_STAGES;
+          mbar_wait(&b_full[sb], (bit / B_STAGES) & 1);
+          const int ky = tap / 3, kx = tap - ky * 3;          // window start: halo pixel (ky, kx)
+          const uint32_t woff = (uint32_t)((ky * HW + kx) * 128);
+          const uint64_t ahi = make_desc(a_hi + woff, SBO_HALO), alo = make_desc(a_lo + woff, SBO_HALO);
+          const uint64_t ahi2 = make_desc(a_hi + woff + H2, SBO_HALO), alo2 = make_desc(a_lo + woff + H2, SBO_HALO);
+          const uint32_t sbaddr = smem_u32(smemB + sb * 2 * B_PANEL) + wg * 64 * 128;
+          const uint64_t bhi = make_desc(sbaddr), blo = make_desc(sbaddr + B_PANEL);
+          wgmma_fence();
 #pragma unroll
-      for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-      const int ndrain = NCH * ((p.drain == 1 || p.drain == 3) ? 9 / p.drain : 1);
-      for (int cc = 0; cc < ndrain; ++cc, ++cg) {
-        const uint32_t buf = cg & 1;
-        if (tre) te0 = clock64();
-        mbar_wait(&acc_full[buf], (cg >> 1) & 1);
-        if (tre) { const long long t1 = clock64(); te_wait += t1 - te0; te0 = t1; }
-        tc_fence_after();
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          float v[16];
-          tmem_ld16(tmem_base + lane_addr + buf * ACC_COLS + wg * 64 + q * 16, v);
-#pragma unroll
-          for (int i = 0; i < 16; ++i) acc[q * 16 + i] += v[i];
-          if (BN == 64) {                                         // hi*lo partial products live in the second 64 columns
-            tmem_ld16(tmem_base + lane_addr + buf * ACC_COLS + 64 + q * 16, v);
-#pragma unroll
-            for (int i = 0; i < 16; ++i) acc[q * 16 + i] += v[i];
+          for (int j = 0; j < 4; ++j) {
+            const uint64_t o = (uint64_t)(j * 2);
+            const uint32_t acc = (in_group == 0 && j == 0) ? 0u : 1u;
+            wgmma_m64n64k16(d0, alo + o, bhi + o, acc);
+            wgmma_m64n64k16(d1, alo2 + o, bhi + o, acc);
+            wgmma_m64n64k16(d0, ahi + o, blo + o, 1u);
+            wgmma_m64n64k16(d1, ahi2 + o, blo + o, 1u);
+            wgmma_m64n64k16(d0, ahi + o, bhi + o, 1u);
+            wgmma_m64n64k16(d1, ahi2 + o, bhi + o, 1u);
+          }
+          wgmma_commit();
+          if (++in_group == dt) {
+            wgmma_wait<0>();
+            wgmma_fence_acc(d0); wgmma_fence_acc(d1);
+            if (lane == 0) { if (pend >= 0) mbar_arrive(&b_free[pend]); mbar_arrive(&b_free[sb]); }
+            pend = -1;
+            stage_fragment(stage, 0, d0, first_drain, etid);
+            stage_fragment(stage, 64, d1, first_drain, etid);
+            first_drain = false;
+            in_group = 0;
+          } else {
+            wgmma_wait<1>();
+            if (lane == 0 && pend >= 0) mbar_arrive(&b_free[pend]);
+            pend = sb;
           }
         }
-        tc_fence_before();
-        mbar_arrive(&acc_free[buf]);
-        if (tre) te_drain += clock64() - te0;
+        if (lane == 0) mbar_arrive(&a_free[sa]);               // 9 % dt == 0: every MMA of the chunk has completed
       }
+      asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
+      float acc[64];
+      {
+        const float4* src = reinterpret_cast<const float4*>(stage + row_in_tile * kStageLd);
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+          const float4 v = src[i];
+          acc[4 * i] = v.x; acc[4 * i + 1] = v.y; acc[4 * i + 2] = v.z; acc[4 * i + 3] = v.w;
+        }
+      }
+      __syncwarp();
       if (tre) te0 = clock64();
 #pragma unroll
       for (int i = 0; i < 64; ++i) acc[i] *= p.tc_scale;
@@ -405,19 +356,12 @@ __global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const G
         }
       }
       if (tre) te_final += clock64() - te0;
+      asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");     // the staged tile is rewritten by the next tile's first drain
     }
     if (defer_stats && pending > 0) flush_stats();
     if (tre) {
-      p.trace[9] = (unsigned long long)te_wait; p.trace[12] = (unsigned long long)te_drain; p.trace[10] = (unsigned long long)te_final;
-      p.trace[13] = (unsigned long long)te_bias; p.trace[14] = (unsigned long long)te_store;
+      p.trace[10] = (unsigned long long)te_final; p.trace[13] = (unsigned long long)te_bias; p.trace[14] = (unsigned long long)te_store;
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (warp == MMA_WARP) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS));
   }
 }
 

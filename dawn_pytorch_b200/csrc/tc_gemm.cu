@@ -1,20 +1,18 @@
-// tcgen05 implicit GEMM for the DAWN UNet contractions (sm_100a): Out = epilogue(A (gathered, fp32) x B (weights)).
+// wgmma implicit GEMM for the DAWN UNet contractions (sm_90a): Out = epilogue(A (gathered, fp32) x B (weights)).
 //
 //   * 128-row position tile x 64/128-column output tile, K streamed in 64-element panels (= one 128-byte swizzle row of fp16).
 //   * fp32-level parity needs the 3-term split  hi*hi + hi*lo + lo*hi  (SURVEY App. D).  The pieces are FP16
-//     (kind::f16, K = 16 per instruction): an fp16 piece carries the same 11-bit significand as a TF32 piece, so
-//     hi+lo keeps ~22 bits like 3xTF32, but every tcgen05.mma does twice the work and reads half the bytes
-//     (measured: ~70 cycles of issue cost per tcgen05.mma regardless of N made the K=8 TF32 form issue-bound).
+//     (K = 16 per instruction): an fp16 piece carries the same 11-bit significand as a TF32 piece, so hi+lo keeps
+//     ~22 bits like 3xTF32, but every MMA does twice the work of a K = 8 TF32 one and reads half the bytes.
 //     fp16's narrow exponent is handled with an exact power-of-two pre-scale of each weight matrix (undone in the
 //     epilogue); activations stay unscaled (|x| < 65504; tiny lo pieces go subnormal, abs error <= 2^-25).  A is split on the fly by the producer warps, B is pre-split and pre-swizzled on the
 //     host into ready-to-copy shared-memory images (1-D bulk copies, no tensor maps).
-//   * The tensor core adds into its accumulator with round-toward-zero; chained over a long K that is a biased
-//     error (measured 1.4e-4 at K=14112).  So TMEM holds TWO accumulator buffers; every CHUNK panels the issuer
-//     flips buffers (first MMA overwrites) and the epilogue warps drain the finished buffer into fp32 registers
-//     with ordinary round-to-nearest adds while the next chunk is already being multiplied.
+//   * The tensor core adds into its accumulator with truncation; chained over a long K that is a biased error
+//     (1.4e-4 at K=14112).  So the register accumulator only spans CHUNK panels (first MMA overwrites) and is then
+//     added into an fp32 tile in shared memory with ordinary round-to-nearest adds.
 //   * persistent CTAs, warp roles: 0-7 A producers (gather + split + swizzled st.shared, global loads prefetched
-//     two panels ahead in registers), 8-11 accumulate/epilogue (each thread owns one output row), 12 MMA issuer
-//     (one elected thread), 13 weight loader (one elected thread).
+//     two panels ahead in registers), then BN/64 consumer warpgroups (wgmma on 128 rows x 64 columns each, then the
+//     epilogue with one output row per thread, read back from the staged tile), last a weight loader (one thread).
 #include <cuda_fp16.h>
 #include "common.cuh"
 #include "gemm.cuh"
@@ -26,24 +24,23 @@ namespace {
 
 constexpr int BM = 128;
 constexpr int BKP = 64;                 // K elements per panel row (64 fp16 = 128 bytes)
-constexpr int CHUNK = 4;                // panels accumulated inside TMEM before a drain (K = 128)
+constexpr int CHUNK = 4;                // panels accumulated in the register accumulator before a drain (K = 256)
 constexpr int A_PANEL_MIN = BM * 128;    // 16 KB
 constexpr int NPROD = 256;              // producer threads (warps 0-7)
 
-// BN = 64: one epilogue warpgroup, 4 stages of 48 KB.  BN = 128: two epilogue warpgroups (64 columns each), 3 stages of 64 KB.
+// BN = 64: one consumer warpgroup, 3 stages of 48 KB.  BN = 128: two consumer warpgroups (64 columns each), 2 stages of 64 KB.
+// Each consumer warpgroup also owns a 128 x 64 fp32 staging tile (34 KB); the stage counts are what fits next to it in 227 KB.
 template <int BN>
 struct Cfg {
-  static constexpr int NWG = BN / 64;                        // epilogue warpgroups
+  static constexpr int NWG = BN / 64;                        // consumer warpgroups
   static constexpr int A_PANEL = A_PANEL_MIN;
   static constexpr int B_PANEL = BN * 128;
   static constexpr int STAGE_BYTES = 2 * A_PANEL + 2 * B_PANEL;
-  static constexpr int STAGES = (BN == 64) ? 4 : 3;
-  static constexpr int NTHREADS = NPROD + 128 * NWG + 64;    // producers | epilogue | MMA warp | loader warp
-  static constexpr int MMA_WARP = (NPROD + 128 * NWG) / 32;
-  static constexpr int LOAD_WARP = MMA_WARP + 1;
-  static constexpr int TMEM_COLS = 2 * BN;                   // two accumulator buffers
-  static constexpr int EPI_STAGE = NWG * 4 * 32 * 20 * 4;     // per epilogue warp: 32 rows x (16 + 4 pad) floats
-  static constexpr int SMEM_DYN = STAGES * STAGE_BYTES + EPI_STAGE + 1024;
+  static constexpr int STAGES = (BN == 64) ? 3 : 2;
+  static constexpr int NTHREADS = NPROD + 128 * NWG + 32;    // producers | consumers | loader warp
+  static constexpr int LOAD_WARP = (NPROD + 128 * NWG) / 32;
+  static constexpr int ACC_STAGE = NWG * BM * tc::kStageLd * 4;
+  static constexpr int SMEM_DYN = STAGES * STAGE_BYTES + ACC_STAGE + 1024;
 };
 
 using namespace tc;
@@ -54,34 +51,25 @@ template <int EPI, int BN>
 __global__ void __launch_bounds__(Cfg<BN>::NTHREADS, 1) tc_gemm_kernel(const GemmParams p, const float* __restrict__ Bimg, int KC,
                                                                        int tiles_m, int tiles_n) {
   using C = Cfg<BN>;
-  constexpr int STAGES = C::STAGES, STAGE_BYTES = C::STAGE_BYTES, B_PANEL = C::B_PANEL, TMEM_COLS = C::TMEM_COLS, A_PANEL = C::A_PANEL;
-  constexpr int MMA_WARP = C::MMA_WARP, LOAD_WARP = C::LOAD_WARP, NWG = C::NWG;
+  constexpr int STAGES = C::STAGES, STAGE_BYTES = C::STAGE_BYTES, B_PANEL = C::B_PANEL, A_PANEL = C::A_PANEL;
+  constexpr int LOAD_WARP = C::LOAD_WARP, NWG = C::NWG;
   extern __shared__ uint8_t smem_raw[];
-  __shared__ uint64_t a_full[STAGES], b_full[STAGES], slot_free[STAGES], acc_full[2], acc_free[2];
-  __shared__ uint32_t s_tmem_base;
+  __shared__ uint64_t a_full[STAGES], b_full[STAGES], slot_free[STAGES];
   __shared__ RowInfo s_rows[3][BM];
   __shared__ float2 s_ln[8][BM];              // (mu, rstd) per tile row, ring over this CTA's tiles (producers run ahead of the epilogue)
   __shared__ float s_stat[NWG][16];
   __shared__ __align__(16) float s_biasv[1024];  // the whole bias vector, fetched once per CTA (the per-tile __ldg round trip was 1-3k cycles of an epilogue-bound tile)
 
   const int tid = threadIdx.x, lane = tid & 31;
-  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);          // warp-uniform by construction (the MMA warp relies on it)
+  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);          // warp-uniform by construction
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
 
   if (tid == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&a_full[s], NPROD); mbar_init(&b_full[s], 1); mbar_init(&slot_free[s], 1); }
-    mbar_init(&acc_full[0], 1); mbar_init(&acc_full[1], 1);
-    mbar_init(&acc_free[0], 128 * NWG); mbar_init(&acc_free[1], 128 * NWG);
+    // slot_free: one arrive per consumer warp once its MMAs on the slot have completed
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&a_full[s], NPROD); mbar_init(&b_full[s], 1); mbar_init(&slot_free[s], 4 * NWG); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == MMA_WARP) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem_base)), "r"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = s_tmem_base;
 
   const int total_tiles = tiles_m * tiles_n;
   const int Ps = p.OHs * p.OWs;
@@ -192,9 +180,9 @@ __global__ void __launch_bounds__(Cfg<BN>::NTHREADS, 1) tc_gemm_kernel(const Gem
         }
       }
       // no proxy fence here: fence.proxy.async compiles to MEMBAR.ALL.CTA + FENCE.VIEW.ASYNC and would make every
-      // producer thread drain its outstanding prefetch loads once per panel (measured ~1000 cycles).  The st.shared
-      // above and this arrive retire in order through the same shared-memory pipe; the issuer thread runs the proxy
-      // fence after acquiring a_full (it has no loads in flight), before the async-proxy reads of tcgen05.mma.
+      // producer thread drain its outstanding prefetch loads once per panel.  The st.shared above and this arrive
+      // retire in order through the same shared-memory pipe; the consumers run the proxy fence after acquiring a_full
+      // (they have no loads in flight), before the async-proxy reads of wgmma.
       mbar_arrive_relaxed(&a_full[s]);
       if (tr) p.trace[7] += (unsigned long long)(clock64() - t0);
       ++it;
@@ -283,104 +271,82 @@ __global__ void __launch_bounds__(Cfg<BN>::NTHREADS, 1) tc_gemm_kernel(const Gem
       }
       if (p.trace != nullptr && blockIdx.x == 0) p.trace[8] = (unsigned long long)tl_wait;
     }
-  } else if (warp == MMA_WARP) {
-    // =============================================================== MMA issuer: the whole warp, warp-uniform control flow, one elected
-    // lane per MMA / commit (tc_common.cuh: elect_one)
-    {
-      const uint32_t tmem_base_u = __shfl_sync(0xffffffffu, tmem_base, 0);      // read from shared memory: make it a provably uniform value
-      const uint32_t idesc = (1u << 4) | (0u << 7) | (0u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);   // D f32, A/B f16, K-major
-      const int CH = (p.drain > 0 && p.drain < CHUNK) ? p.drain : CHUNK;
-      uint32_t it = 0, cg = 0;
-      const bool tr = (p.trace != nullptr) && blockIdx.x == 0;
-      long long t_acc = 0, t_a = 0, t_b = 0, t_issue = 0, t0 = 0, t_begin = clock64();
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        for (int kc = 0; kc < KC; ++kc, ++it) {
-          const int s = it % STAGES;
-          const uint32_t round = it / STAGES;
-          const bool chunk_first = (kc % CH) == 0;
-          const bool chunk_last = ((kc % CH) == CH - 1) || (kc == KC - 1);
-          const uint32_t buf = cg & 1;
-          if (tr) t0 = clock64();
-          if (chunk_first) {
-            mbar_wait(&acc_free[buf], ((cg >> 1) & 1) ^ 1);
-            tc_fence_after();
-          }
-          if (tr) { const long long t1 = clock64(); t_acc += t1 - t0; t0 = t1; }
-          mbar_wait(&a_full[s], round & 1);
-          if (tr) { const long long t1 = clock64(); t_a += t1 - t0; t0 = t1; }
-          mbar_wait(&b_full[s], round & 1);
-          if (tr) { const long long t1 = clock64(); t_b += t1 - t0; t0 = t1; }
-          fence_proxy_async();          // generic-proxy operand writes of the producers -> async proxy (see store_item)
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + s * STAGE_BYTES);
-          const uint64_t ahi = make_desc(sa), alo = make_desc(sa + A_PANEL);
-          const uint64_t bhi = make_desc(sa + 2 * A_PANEL), blo = make_desc(sa + 2 * A_PANEL + B_PANEL);
-          const uint32_t d = tmem_base_u + buf * BN;
-#pragma unroll
-          for (int j = 0; j < BKP / 16; ++j) {
-            const uint64_t o = (uint64_t)(j * 2);               // +32 bytes per k-step, in 16-byte units
-            tc_mma_f16_elected(d, alo + o, bhi + o, idesc, (chunk_first && j == 0) ? 0u : 1u);
-            tc_mma_f16_elected(d, ahi + o, blo + o, idesc, 1u);
-            tc_mma_f16_elected(d, ahi + o, bhi + o, idesc, 1u);
-          }
-          tc_commit_elected(&slot_free[s]);
-          if (chunk_last) { tc_commit_elected(&acc_full[buf]); ++cg; }
-          if (tr) t_issue += clock64() - t0;
-        }
-      }
-      if (tr && lane == 0) {
-        p.trace[0] = (unsigned long long)(clock64() - t_begin); p.trace[1] = it;
-        p.trace[2] = (unsigned long long)t_acc; p.trace[3] = (unsigned long long)t_a;
-        p.trace[4] = (unsigned long long)t_b; p.trace[5] = (unsigned long long)t_issue;
-      }
-    }
   } else {
-    // =============================================================== accumulate + epilogue (warps 8 .. 8+4*NWG-1)
-    // warpgroup wg owns output columns [64 wg, 64 wg + 64) of the tile; inside it warp ew = warp % 4 reads TMEM lanes 32 ew ..
+    // =============================================================== consumers (warps 8 .. 8+4*NWG-1): MMA + epilogue
+    // warpgroup wg owns output columns [64 wg, 64 wg + 64) of the tile (two m64n64 MMAs per k-step: rows 0-63 and 64-127);
+    // in the epilogue thread etid owns tile row etid (row-per-thread layout, read back from the staged fp32 tile)
     const int wg = (warp - 8) >> 2;
     const int ew = (warp - 8) & 3;
     const int row_in_tile = ew * 32 + lane;
-    const uint32_t lane_addr = (uint32_t)(ew * 32) << 16;
     const int etid = (tid - NPROD) & 127;
     float* s_st = s_stat[wg];
     const int bar_id = 2 + wg;
     constexpr int EN = 64;                                 // columns per epilogue thread
-    float* wbuf = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES) + ((wg * 4 + ew) * 32 * 20);
-    uint32_t cg = 0;
+    float* stage = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES) + wg * BM * kStageLd;
+    float* wbuf = stage + ew * 32 * kStageLd;              // this warp's own staged rows, free once they are read back
     int Te = -1;
     const bool bias_s = (p.bias != nullptr) && p.N <= 1024;
     if (bias_s) {
       for (int i = (tid - NPROD); i < p.N; i += 128 * NWG) s_biasv[i] = __ldg(p.bias + i);
       asm volatile("bar.sync 4, %0;" ::"n"(128 * NWG) : "memory");
     }
-    long long te_wait = 0, te_final = 0, te_drain = 0, te_store = 0, te_pre = 0;
+    const int CH = (p.drain > 0 && p.drain < CHUNK) ? p.drain : CHUNK;
+    uint32_t it = 0;
+    long long te_final = 0, te_store = 0, te_pre = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       ++Te;
       const int m0 = (tile / tiles_n) * BM, n0 = (tile % tiles_n) * BN + wg * EN;
-      float acc[EN];
+      float d0[32], d1[32];
+      int pend = -1;                                       // stage whose MMAs are still in flight (released one panel later)
+      for (int kc = 0; kc < KC; ++kc, ++it) {
+        const int s = it % STAGES;
+        const uint32_t round = it / STAGES;
+        const bool chunk_first = (kc % CH) == 0;
+        const bool chunk_last = ((kc % CH) == CH - 1) || (kc == KC - 1);
+        mbar_wait(&a_full[s], round & 1);
+        mbar_wait(&b_full[s], round & 1);
+        fence_proxy_async();          // generic-proxy operand writes of the producers -> async proxy (see store_item)
+        const uint32_t sa = smem_u32(smem + s * STAGE_BYTES);
+        const uint64_t ahi = make_desc(sa), alo = make_desc(sa + A_PANEL);
+        const uint64_t bhi = make_desc(sa + 2 * A_PANEL + wg * 64 * 128), blo = make_desc(sa + 2 * A_PANEL + B_PANEL + wg * 64 * 128);
+        constexpr uint64_t H2 = 64 * 128 / 16;                // rows 64-127 of the A panel
+        wgmma_fence();
 #pragma unroll
-      for (int i = 0; i < EN; ++i) acc[i] = 0.f;
-      const int CH = (p.drain > 0 && p.drain < CHUNK) ? p.drain : CHUNK;
-      const int nchunks = (KC + CH - 1) / CH;
-      for (int c = 0; c < nchunks; ++c, ++cg) {
-        const uint32_t buf = cg & 1;
-        const bool tr = (p.trace != nullptr) && blockIdx.x == 0 && etid == 0;
-        long long t0 = 0;
-        if (tr) t0 = clock64();
-        mbar_wait(&acc_full[buf], (cg >> 1) & 1);
-        if (tr) { const long long t1 = clock64(); te_wait += t1 - t0; t0 = t1; }
-        tc_fence_after();
-#pragma unroll
-        for (int q = 0; q < EN / 16; ++q) {
-          float v[16];
-          tmem_ld16(tmem_base + lane_addr + buf * BN + wg * EN + q * 16, v);
-#pragma unroll
-          for (int i = 0; i < 16; ++i) acc[q * 16 + i] += v[i];
+        for (int j = 0; j < BKP / 16; ++j) {
+          const uint64_t o = (uint64_t)(j * 2);               // +32 bytes per k-step, in 16-byte units
+          const uint32_t acc = (chunk_first && j == 0) ? 0u : 1u;
+          wgmma_m64n64k16(d0, alo + o, bhi + o, acc);
+          wgmma_m64n64k16(d1, alo + H2 + o, bhi + o, acc);
+          wgmma_m64n64k16(d0, ahi + o, blo + o, 1u);
+          wgmma_m64n64k16(d1, ahi + H2 + o, blo + o, 1u);
+          wgmma_m64n64k16(d0, ahi + o, bhi + o, 1u);
+          wgmma_m64n64k16(d1, ahi + H2 + o, bhi + o, 1u);
         }
-        tc_fence_before();
-        mbar_arrive(&acc_free[buf]);
-        if (tr) te_drain += clock64() - t0;
+        wgmma_commit();
+        if (chunk_last) {
+          wgmma_wait<0>();
+          wgmma_fence_acc(d0); wgmma_fence_acc(d1);
+          if (lane == 0) { if (pend >= 0) mbar_arrive(&slot_free[pend]); mbar_arrive(&slot_free[s]); }
+          pend = -1;
+          stage_fragment(stage, 0, d0, kc < CH, etid);
+          stage_fragment(stage, 64, d1, kc < CH, etid);
+        } else {
+          wgmma_wait<1>();
+          if (lane == 0 && pend >= 0) mbar_arrive(&slot_free[pend]);
+          pend = s;
+        }
       }
+      asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
+      float acc[EN];
+      {
+        const float4* src = reinterpret_cast<const float4*>(stage + row_in_tile * kStageLd);
+#pragma unroll
+        for (int i = 0; i < EN / 4; ++i) {
+          const float4 v = src[i];
+          acc[4 * i] = v.x; acc[4 * i + 1] = v.y; acc[4 * i + 2] = v.z; acc[4 * i + 3] = v.w;
+        }
+      }
+      __syncwarp();
 
       // ---------------------------------------------------------- final epilogue: this thread owns row m
       const bool tr_e = (p.trace != nullptr) && blockIdx.x == 0 && etid == 0;
@@ -534,18 +500,11 @@ __global__ void __launch_bounds__(Cfg<BN>::NTHREADS, 1) tc_gemm_kernel(const Gem
         }
       }
       if (tr_e) te_final += clock64() - te0;
+      asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");     // the staged tile is rewritten by the next tile's first drain
     }
     if (p.trace != nullptr && blockIdx.x == 0 && etid == 0 && wg == 0) {
-      p.trace[9] = (unsigned long long)te_wait; p.trace[10] = (unsigned long long)te_final; p.trace[12] = (unsigned long long)te_drain;
-      p.trace[14] = (unsigned long long)te_store; p.trace[13] = (unsigned long long)te_pre;
+      p.trace[10] = (unsigned long long)te_final; p.trace[14] = (unsigned long long)te_store; p.trace[13] = (unsigned long long)te_pre;
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (warp == MMA_WARP) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS));
   }
 }
 

@@ -1,4 +1,4 @@
-// tcgen05 (5th-gen tensor core, TMEM accumulators) implicit GEMM — see tc_gemm.cu
+// wgmma (Hopper warpgroup MMA) implicit GEMM — see tc_gemm.cu
 #pragma once
 #include <cuda_runtime.h>
 #include <vector>

@@ -16,7 +16,6 @@
 #include "kernels.cuh"
 #include "tc_gemm.cuh"
 #include "temporal_fused.cuh"
-#include "temporal_tc.cuh"
 #include "sla_fused.cuh"
 #include "ca_fused.cuh"
 #include "sampler.cuh"
@@ -119,8 +118,6 @@ struct AttnW {     // temporal attention / mid spatial attention (U:648-725)
   int C = 0; float Wqkv_scale = 1.f; float *Wqkv = nullptr, *wsum = nullptr, *Wqkv_img = nullptr; ConvW out;
   // fused per-pixel kernel (temporal_fused.cu), 64-channel levels only
   uint16_t *fq = nullptr, *fo = nullptr; float f_inv_wscale = 1.f, f_inv_oscale = 1.f;
-  // tcgen05 kernel (temporal_tc.cu): swizzled shared-memory images per head
-  uint8_t *tq = nullptr, *to = nullptr; float t_inv_wscale = 1.f, t_inv_oscale = 1.f;
 };
 struct SlaW {      // spatial linear attention (U:602-627)
   int C = 0; float Wqkv_scale = 1.f; float *Wqkv = nullptr, *wsum = nullptr, *Wqkv_img = nullptr, *WoutT = nullptr, *bout = nullptr;
@@ -189,15 +186,14 @@ struct dawn_unet {
   int cond_dim = 0, tdim = 0;
   std::unordered_map<std::string, HostParam> raw;
   bool committed = false;
-  bool use_tc = true;                          // tcgen05 contraction path (DAWN_TC=0 falls back to mma.sync)
-  bool use_conv3 = true;                       // halo-tile tcgen05 3x3 conv (DAWN_TC_CONV3=0 falls back to the per-tap GEMM)
+  bool use_tc = true;                          // wgmma contraction path (DAWN_TC=0 falls back to mma.sync)
+  bool use_conv3 = true;                       // halo-tile wgmma 3x3 conv (DAWN_TC_CONV3=0 falls back to the per-tap GEMM)
   bool use_presplit = true;                    // fp16 hi|lo pre-split of A for multi-n-tile 3x3 convs (DAWN_PRESPLIT=0: off)
   bool use_fused_ca = true;                    // fused cross-attention gate kernel for ci <= 128 (DAWN_FUSED_CA=0: unfused)
   bool use_fused_sla = true;                   // fused SLA context on 64-channel levels (DAWN_FUSED_SLA=0: unfused)
   int conv3_tma = 1;                           // halo conv fed by TMA from fp16 hi|lo planes: 1 (default) = second conv of a ResBlock, whose input the
                                                // GroupNorm/cross-attention kernel writes pre-split; 2 = every halo conv through a split pass
                                                // (measurement only); 0 = off (DAWN_CONV3_TMA)
-  bool use_ta_tc = true;                       // tcgen05 temporal attention on 64-channel levels (DAWN_TA_TC=0: mma.sync kernel)
   bool use_fused_ta = true;                    // fused per-pixel temporal attention on 64-channel levels (DAWN_FUSED_TA=0: unfused)
   bool use_attn_tc = true;                     // tensor-core attention core (DAWN_ATTN_TC=0 falls back to SIMT)
 
@@ -210,7 +206,6 @@ struct dawn_unet {
   int cin_pad = 0;
   float *time_freqs = nullptr, *tW1 = nullptr, *tb1 = nullptr, *tW2 = nullptr, *tb2 = nullptr;
   float *rel_bias = nullptr, *rot_freqs = nullptr;
-  float* ttc_table = nullptr;                  // [8][kTtcTable] bias * log2(e) inside the band, -1e30 outside (temporal_tc.cu)
   std::vector<ResBlockW> rb;                   // all resnet blocks
   std::map<std::string, int> rb_index;
   AttnW init_ta, mid_sa, mid_ta;
@@ -291,7 +286,7 @@ void free_all(std::vector<void*>& v) {
 }
 inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
 
-// tcgen05 image of a [K][ldb] weight matrix (only for shapes the tcgen05 kernel accepts)
+// wgmma weight image of a [K][ldb] weight matrix (only for shapes the wgmma kernel accepts)
 int upload_tc_image(dawn_unet* h, const std::vector<float>& m, int K, int N, int ldb, float** img, float* scale) {
   *img = nullptr; *scale = 1.f;
   if (!h->use_tc || N % 64 != 0 || K % 64 != 0) return 0;
@@ -458,13 +453,6 @@ int pack_attn(dawn_unet* h, const std::string& norm_name, const std::string& fn,
     memcpy(tq.data(), Wq.data(), Wq.size() * 2); memcpy(to.data(), Wo.data(), Wo.size() * 2);
     DAWN_TRY(dev_upload(h, tq, &dq)); DAWN_TRY(dev_upload(h, to, &dout));
     a->fq = reinterpret_cast<uint16_t*>(dq); a->fo = reinterpret_cast<uint16_t*>(dout);
-    std::vector<uint8_t> Tq, To;
-    temporal_tc_pack(wq.data(), o->data.data(), Tq, To, &a->t_inv_wscale, &a->t_inv_oscale);
-    std::vector<float> uq(Tq.size() / 4), uo(To.size() / 4);
-    memcpy(uq.data(), Tq.data(), Tq.size()); memcpy(uo.data(), To.data(), To.size());
-    float *dtq = nullptr, *dto = nullptr;
-    DAWN_TRY(dev_upload(h, uq, &dtq)); DAWN_TRY(dev_upload(h, uo, &dto));
-    a->tq = reinterpret_cast<uint8_t*>(dtq); a->to = reinterpret_cast<uint8_t*>(dto);
   }
   return 0;
 }
@@ -668,7 +656,7 @@ int Ctx::gemm(const GemmParams& p, int epi, int cat) {
 
 int tap(Ctx& c, const std::string& name, const Act& a);
 
-// LayerNorm-folded 1x1 GEMM: on the tcgen05 path the producers compute the row statistics themselves (no separate
+// LayerNorm-folded 1x1 GEMM: on the wgmma path the producers compute the row statistics themselves (no separate
 // rowstats launch, no second read of the input); otherwise run rowstats_kernel into the global buffer.
 int ln_gemm(Ctx& c, GemmParams& p, int epi, int cat, const float* x, int ldx, int C, int rows) {
   dawn_unet* h = c.h;
@@ -742,7 +730,7 @@ int resblock(Ctx& c, const ResBlockW& r, const Act& x, const Act& out) {
   }
   DAWN_TRY(conv_same(c, x, r.c1, 3, y, r.st1));
   DAWN_TRY(gn_allreduce(c, r.st1));
-  // a1 is consumed by the second conv only: when that conv runs on the halo-tile tcgen05 kernel, a1 is written as two fp16 planes
+  // a1 is consumed by the second conv only: when that conv runs on the halo-tile wgmma kernel, a1 is written as two fp16 planes
   // (hi | lo, the same bytes as the fp32 row) and the conv fetches its tiles by TMA
   const unsigned short *a1h = nullptr, *a1l = nullptr;
   if (r.cond && h->use_fused_ca && gn_hcond_supported(r.co, P) && h->conv3_tma >= 1 && h->use_tc && h->use_conv3 && r.c2.img != nullptr) {
@@ -830,33 +818,7 @@ int temporal_attn(Ctx& c, const AttnW& w, const Act& x, const Act& dst, const st
     DAWN_NCCL_OK(g_nccl.GroupEnd());
     xe = Act{h->XE, x.C, x.C, x.H, x.W};
   }
-  // tcgen05 kernel: one work unit per pixel while the sequence fits one 240-frame window (a 200-frame shard plus one halo); longer sequences
-  // are cut into segments that each pay the full two-tile cost.  Since the issuer warps run warp-uniformly (r2-h) two segments of a
-  // 280-frame sequence (a 200-frame shard with both halos) take 3.5 ms at level 0, against ~4.3 ms for the mma.sync kernel that keeps the
-  // whole sequence on chip: the tcgen05 kernel is used whenever it supports the shape (DAWN_TA_TC=0 selects the older kernels).
-  const bool ttc_ok = h->use_ta_tc && w.tq && h->ttc_table && temporal_tc_supported(x.C, Fe, h->cfg.win_width, hl, hl + F);
   const bool fused_ok = h->use_fused_ta && w.fq && temporal_fused_supported(x.C, Fe, h->cfg.win_width, hl, hl + F);
-  if (ttc_ok) {
-    // long sequences are cut into segments whose windows overlap: an in-place layer would let one segment read rows another already
-    // replaced, so the input is copied aside first (sharded runs already read from the halo-extended copy)
-    if (Fe > kTtcWindowMax && xe.p == dst.p) {
-      h->launches++;
-      DAWN_CUDA_OK(cudaMemcpy2DAsync(h->XE, (size_t)x.C * sizeof(float), x.p, (size_t)x.ld * sizeof(float), (size_t)x.C * sizeof(float),
-                                     (size_t)F * P, cudaMemcpyDeviceToDevice, c.st));
-      xe = Act{h->XE, x.C, x.C, x.H, x.W};
-    }
-    TemporalTcArgs a{};
-    a.x = xe.p; a.ldx = xe.ld; a.res = x.p; a.ldr = x.ld; a.out = dst.p; a.ldo = dst.ld;
-    a.F = Fe; a.P = P; a.q_lo = hl; a.q_hi = hl + F;
-    a.Wqkv = w.tq; a.Wout = w.to; a.rot = h->ROT; a.table = h->ttc_table; a.band = h->cfg.win_width;
-    a.inv_wscale = w.t_inv_wscale; a.inv_oscale = w.t_inv_oscale;
-    double pairs = 0;
-    for (int i = hl; i < hl + F; ++i) pairs += std::min(Fe - 1, i + a.band) - std::max(0, i - a.band) + 1;
-    ProfScope ps(c, x.H == h->lH[0] ? PC_TEMPORAL_L0 : PC_ATTN_CORE, 2.0 * Me * x.C * 768 + 4.0 * 32 * 8 * P * pairs + 2.0 * F * P * 256 * x.C,
-                 4.0 * (Me + 2.0 * F * P) * x.C);
-    DAWN_TRY(launch_temporal_tc(a, c.st));
-    return tap(c, name, dst);
-  }
   if (fused_ok) {
     TemporalFusedArgs a{};
     a.x = xe.p; a.ldx = xe.ld; a.res = x.p; a.ldr = x.ld; a.out = dst.p; a.ldo = dst.ld;
@@ -1167,7 +1129,7 @@ int forward_core(dawn_unet* h, const int64_t* t_dev, float* out, cudaStream_t st
 extern "C" {
 
 const char* dawn_last_error(void) { return g_last_error.c_str(); }
-const char* dawn_build_info(void) { return "dawn_unet sm_100a; contractions: tcgen05 kind::f16 FP16x3 (TMEM accumulators) + mma.sync m16n8k16 FP16x3 fused attention kernels; fallback mma.sync 3xTF32"; }
+const char* dawn_build_info(void) { return "dawn_unet sm_90a; contractions: wgmma m64n64k16 FP16x3 (register accumulators, RN fp32 drains) + mma.sync m16n8k16 FP16x3 fused attention kernels; fallback mma.sync 3xTF32"; }
 
 // The kernel launchers cache per-function attributes (dynamic shared-memory opt-in, SM count) in process-wide statics: the
 // library is built for ONE GPU PER PROCESS (torchrun / one rank per GPU).  A second device in the same process would launch
@@ -1199,7 +1161,6 @@ int dawn_unet_create(const dawn_unet_cfg* cfg, dawn_unet** out) {
   { const char* e = getenv("DAWN_TC"); h->use_tc = !(e && e[0] == '0'); }
   { const char* e = getenv("DAWN_ATTN_TC"); h->use_attn_tc = !(e && e[0] == '0'); }
   { const char* e = getenv("DAWN_FUSED_TA"); h->use_fused_ta = !(e && e[0] == '0'); }
-  { const char* e = getenv("DAWN_TA_TC"); h->use_ta_tc = !(e && e[0] == '0'); }
   { const char* e = getenv("DAWN_CONV3_TMA"); h->conv3_tma = (e && e[0] >= '0' && e[0] <= '2') ? e[0] - '0' : 1; }
   { const char* e = getenv("DAWN_FUSED_SLA"); h->use_fused_sla = !(e && e[0] == '0'); }
   { const char* e = getenv("DAWN_FUSED_CA"); h->use_fused_ca = !(e && e[0] == '0'); }
@@ -1267,14 +1228,6 @@ int dawn_unet_commit_params(dawn_unet* h) {
   }
   DAWN_TRY(upload_raw(h, "aux.time_freqs", {dim / 2}, &h->time_freqs));
   DAWN_TRY(upload_raw(h, "aux.rel_bias", {8, 2 * cfg.win_width + 1}, &h->rel_bias));
-  h->ttc_table = nullptr;
-  if (cfg.win_width >= 1 && cfg.win_width <= kTtcBandMax) {
-    const HostParam* rb;
-    DAWN_TRY(need(h, "aux.rel_bias", {8, 2 * cfg.win_width + 1}, &rb));
-    std::vector<float> tab;
-    temporal_tc_table(rb->data.data(), cfg.win_width, tab);
-    DAWN_TRY(dev_upload(h, tab, &h->ttc_table));
-  }
   DAWN_TRY(upload_raw(h, "time_mlp.1.weight", {h->tdim, dim}, &h->tW1));
   DAWN_TRY(upload_raw(h, "time_mlp.1.bias", {h->tdim}, &h->tb1));
   DAWN_TRY(upload_raw(h, "time_mlp.3.weight", {h->tdim, h->tdim}, &h->tW2));
@@ -1491,7 +1444,7 @@ int dawn_unet_forward(dawn_unet* h, const float* x, const int64_t* t, const floa
     p.Out = h->XR + dim; p.ldo = 2 * dim;
     p.skip_flag = vary; p.skip_if = 0;
     ProfScope ps(c, PC_CONV_OTHER, 2.0 * p.M * (double)p.N * p.K, 4.0 * p.M * ((double)p.Cin + p.N));
-    DAWN_TRY(launch_gemm(p, EPI_PLAIN, st));      // Cin = 288 is not a tcgen05 shape: always the mma.sync kernel (it has the skip flag)
+    DAWN_TRY(launch_gemm(p, EPI_PLAIN, st));      // Cin = 288 is not a wgmma-kernel shape: always the mma.sync kernel (it has the skip flag)
   }
   if (vary) {
     DAWN_TRY(init_map(h, x + (size_t)3 * h->F * H0 * W0, (long long)h->F * H0 * W0, st, vary, 1));
@@ -1778,7 +1731,7 @@ int dawn_selftest_attention(int nseq, int L, int temporal, float* max_abs_diff, 
   return rc;
 }
 
-// random k x k conv through both contraction kernels; reports max |tcgen05 - mma.sync| over outputs and GN statistics
+// random k x k conv through both contraction kernels; reports max |wgmma - mma.sync| over outputs and GN statistics
 int dawn_selftest_tc_gemm(int F, int H, int W, int Cin, int N, int ksize, int with_stats, float* max_abs_diff, float* max_abs_ref) {
   DAWN_CHECK(max_abs_diff && max_abs_ref, "null argument");
   const int M = F * H * W, K = ksize * ksize * Cin, ldb = round_up(N, 64);

@@ -211,7 +211,7 @@ class GaussianDiffusion(nn.Module):
         return img
 
     def forward(self, *a, **k):
-        raise NotImplementedError("training (p_losses) is out of scope of the B200 denoiser")
+        raise NotImplementedError("training (p_losses) is out of scope of this denoiser")
 
 
 class DynamicNfGaussianDiffusion(GaussianDiffusion):

@@ -31,7 +31,7 @@ class Face_loc_Encoder(nn.Module):
     @torch.no_grad()
     def forward(self, x):
         if x.device.type != "cuda":
-            raise DawnError("Face_loc_Encoder runs on CUDA (sm_100a) only; there is no CPU path")
+            raise DawnError("Face_loc_Encoder runs on CUDA (sm_90a) only; there is no CPU path")
         b, ci, H, W = x.shape
         x = x.contiguous().float()
         st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
@@ -63,7 +63,7 @@ class FlowDiffusion(nn.Module):
             # calls .train() on unet/diffusion (FD:171-175) and UVG calls model.eval() right after.  Accept it, stay in eval mode;
             # the training entry points (forward / p_losses) raise.
             import warnings
-            warnings.warn("FlowDiffusion(is_train=True): the B200 wrapper is inference-only and stays in eval mode")
+            warnings.warn("FlowDiffusion(is_train=True): this wrapper is inference-only and stays in eval mode")
         self.use_residual_flow = use_residual_flow
         if generator_params is None:
             if config_pth is not None:
@@ -154,4 +154,4 @@ class FlowDiffusion(nn.Module):
         return out
 
     def forward(self, *a, **k):
-        raise NotImplementedError("FlowDiffusion.forward is the training step (FD:203-323): out of scope of the B200 inference path")
+        raise NotImplementedError("FlowDiffusion.forward is the training step (FD:203-323): out of scope of this inference path")

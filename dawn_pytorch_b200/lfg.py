@@ -6,7 +6,7 @@ Same constructor keywords and the same state_dict keys/shapes for everything the
 `generator.load_state_dict(checkpoint['generator'])` (FlowDiffusion.__init__, FD:120) works: the checkpoint's
 `pixelwise_flow_predictor.*` entries — used by `forward` during LFG training only — are dropped on load.
 The reference decodes frame by frame with batch 1 in a Python loop (FD:375-383); here the source encoder runs once per
-clip and all frames are decoded as one batch by hand-written sm_100a CUDA kernels behind include/dawn_lfg.h.
+clip and all frames are decoded as one batch by hand-written sm_90a CUDA kernels behind include/dawn_lfg.h.
 The sub-modules only HOLD parameters; there is no PyTorch fallback.
 """
 import ctypes
@@ -84,7 +84,7 @@ class Generator(nn.Module):
 
     def train(self, mode=True):
         if mode:
-            raise NotImplementedError("the B200 LFG decoder is inference-only (eval-mode BatchNorm, FD:121)")
+            raise NotImplementedError("this LFG decoder is inference-only (eval-mode BatchNorm, FD:121)")
         return super().train(False)
 
     def __del__(self):
@@ -102,7 +102,7 @@ class Generator(nn.Module):
 
     def _ensure(self, device, frames, H, W, fh, fw):
         if device.type != "cuda":
-            raise _lib.DawnError("the LFG decoder runs on CUDA (sm_100a) only; there is no CPU path")
+            raise _lib.DawnError("the LFG decoder runs on CUDA (sm_90a) only; there is no CPU path")
         idx = device.index if device.index is not None else torch.cuda.current_device()
         if self._handle is not None and self._device_index != idx:
             lib.dawn_lfg_destroy(self._handle)

@@ -5,7 +5,7 @@ Same constructor keywords, `forward`, `forward_with_cond_scale`, `update_num_fra
 `has_cond`, and a state_dict whose 900 keys/shapes equal the reference's (SURVEY Appendix B), so
 `diffusion.load_state_dict(checkpoint['diffusion'])` (unified_video_generator.py:527-528) works unchanged.
 The sub-modules below only HOLD parameters (names, shapes, default initialisers); all arithmetic runs in
-hand-written sm_100a CUDA kernels behind the C-ABI in include/dawn_unet.h.  There is no PyTorch fallback.
+hand-written sm_90a CUDA kernels behind the C-ABI in include/dawn_unet.h.  There is no PyTorch fallback.
 """
 import ctypes
 import os
@@ -246,7 +246,7 @@ class Unet3D(nn.Module):
 
     def _ensure(self, device, F, h, w):
         if device.type != "cuda":
-            raise _lib.DawnError("the DAWN denoising UNet runs on CUDA (sm_100a) only; there is no CPU path")
+            raise _lib.DawnError("the DAWN denoising UNet runs on CUDA (sm_90a) only; there is no CPU path")
         idx = device.index if device.index is not None else torch.cuda.current_device()
         if self._handle is not None and self._device_index != idx:
             lib.dawn_unet_destroy(self._handle)

@@ -1,4 +1,4 @@
-/* dawn_lfg.h — C-ABI of the B200-native LFG flow decoder (SURVEY.md §8f N1): the stage of DAWN that turns the sampled latent
+/* dawn_lfg.h — C-ABI of the H100-native LFG flow decoder (SURVEY.md §8f N1): the stage of DAWN that turns the sampled latent
  * flow / occlusion maps into video frames.
  *
  * Reference seam: `Generator.compute_fea` and `Generator.forward_with_flow` (LFG/modules/generator.py:132-171), called by

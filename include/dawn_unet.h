@@ -1,4 +1,4 @@
-/* dawn_unet.h — C-ABI of the B200-native DAWN denoising UNet (one "denoising step").
+/* dawn_unet.h — C-ABI of the H100-native DAWN denoising UNet (one "denoising step").
  *
  * The reference has no FFI layer: its seam is the Python nn.Module `DynamicNfUnet3D`
  * (DM_3/modules/video_flow_diffusion_multiGPU_v0_crema_plus_faceemb_ca_multi_test.py:728-965) held by
@@ -137,24 +137,13 @@ int dawn_unet_sampler_capture(dawn_unet* h, float* x, float* eps, const float* n
                               const float* coef, int nsteps, float q, void* scratch);
 int dawn_unet_sampler_launch(dawn_unet* h, void* stream);
 
-/* self-test of the tcgen05 contraction kernel against the mma.sync kernel on a random k x k convolution
+/* self-test of the wgmma contraction kernel against the mma.sync kernel on a random k x k convolution
  * (F frames of H x W, Cin -> N channels); reports max |difference| (outputs and, if requested, GroupNorm sums). */
 int dawn_selftest_tc_gemm(int F, int H, int W, int Cin, int N, int ksize, int with_stats, float* max_abs_diff, float* max_abs_ref);
 
 /* self-test of the tensor-core attention core against the SIMT fp32 kernel on random q/k/v:
  * temporal != 0: nseq pixel sequences of L frames, band 40 with bias; else nseq frames of L tokens, full attention */
 int dawn_selftest_attention(int nseq, int L, int temporal, float* max_abs_diff, float* max_abs_ref);
-
-/* work decomposition of the tcgen05 temporal-attention kernel (host only): out receives 14 ints per segment
- * {w0, wn, qa, qb, tile0{r0, r1, q0, q1, kb}, tile1{r0, r1, q0, q1, kb}} (room for 16 segments); returns the segment count, 0 = unsupported. */
-int dawn_temporal_tc_plan(int F, int band, int q_lo, int q_hi, int* out);
-
-/* self-test of the tcgen05 temporal-attention kernel (64-channel levels) on random data: err[0] projection accumulator (relative),
- * err[1] scores, err[2] attention output, err[3] layer output of pixel 0 (all absolute, against a double-precision host computation),
- * err[4] all pixels against the mma.sync kernel (-1 where it does not support the shape), err[5] NaN count.
- * trace48 / ms (optional, both or neither): cycle counters of CTA 0 and the duration of a second, un-instrumented-output run. */
-int dawn_selftest_temporal_tc(int F, int P, int band, int q_lo, int q_hi, float* err, float* max_abs_ref, unsigned long long* trace48,
-                              float* ms);
 
 const char* dawn_last_error(void);
 const char* dawn_build_info(void);

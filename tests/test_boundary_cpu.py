@@ -21,7 +21,7 @@ def test_library_exports_every_declared_symbol():
     for sym in declared:
         assert hasattr(_lib.lib, sym), f"{sym} declared in include/dawn_unet.h but not exported"
     assert declared == set(_lib.EXPORTS)
-    assert b"sm_100a" in _lib.lib.dawn_build_info()
+    assert b"sm_90a" in _lib.lib.dawn_build_info()
 
 
 def test_state_dict_schema_equals_reference(schema):

@@ -12,7 +12,7 @@ from oracle import lfg_oracle as L
 from oracle import weights as W
 from tests import gpu_common as G
 
-pytestmark = pytest.mark.gpu            # validated on B200: grid 4.2e-6, frames 0.154 x tol (profiles/r1_o_e2e.md)
+pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 TAG, PROBE_N = 'e2e', 4096

@@ -10,7 +10,7 @@ import torch
 from oracle import lfg_oracle as L
 from oracle import weights as W
 
-pytestmark = pytest.mark.gpu            # validated on B200 (profiles/r1_n_lfg_diag.log)
+pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLD = os.path.join(ROOT, "tests", "golden")

@@ -2,6 +2,6 @@
 D=gpurun_out/${1:-prof2}; mkdir -p $D
 timeout 400 ncu --metrics gpu__time_duration.sum,dram__bytes_read.sum,dram__bytes_write.sum --clock-control none --csv --log-file $D/launches.csv python tools/profile_step.py 2 > $D/launches.out 2>&1
 tail -1 $D/launches.out
-timeout 500 ncu --set full --clock-control none --import-source on -k 'regex:temporal_tc_kernel|tc_conv3_kernel|gn_apply_kernel|gn_hcond_kernel' -s 20 -c 12 -f -o $D/full python tools/profile_step.py 1 > $D/full.out 2>&1
+timeout 500 ncu --set full --clock-control none --import-source on -k 'regex:temporal_fused_kernel|tc_conv3_kernel|gn_apply_kernel|gn_hcond_kernel' -s 20 -c 12 -f -o $D/full python tools/profile_step.py 1 > $D/full.out 2>&1
 ncu -i $D/full.ncu-rep --page raw --csv > $D/full_raw.csv 2>/dev/null; rm -f $D/full.ncu-rep
 gzip -f $D/launches.csv; tail -2 $D/full.out; du -sh $D

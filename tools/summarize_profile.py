@@ -52,7 +52,7 @@ def main(src, tag, title):
     tot_ns = sum(a[1] for a in agg.values()); tot_b = sum(a[2] for a in agg.values())
     rd = sum(l["rd"] for l in step); wr = sum(l["wr"] for l in step)
     with open(tag + "_launch_summary.md", "w") as f:
-        f.write(f"# {title} — ncu launch list of one denoising step (B200, 200 f x 64x64, {len(step)} launches)\n\n")
+        f.write(f"# {title} — ncu launch list of one denoising step (H100, 200 f x 64x64, {len(step)} launches)\n\n")
         f.write("Command: `ncu --metrics gpu__time_duration.sum,dram__bytes_read.sum,dram__bytes_write.sum --clock-control none --csv python "
                 "tools/profile_step.py 2` (`tools/gpu_call_final2.sh`; the last full step of the script; per-launch times are cold-cache / "
                 "serialised: compare SHARES).  Summarised by `tools/summarize_profile.py`.\n\n")
@@ -74,7 +74,7 @@ def main(src, tag, title):
                 "ncu_ms": sum(l["ns"] for l in xs) / len(xs) / 1e6}
     traffic = {"source": f"ncu --metrics dram__bytes_read.sum,dram__bytes_write.sum --clock-control none, {title} "
                          f"({os.path.basename(tag)}_launch_summary.md): bytes per launch at the bench shape (200 f x 64x64), level-0 launches of one step",
-               "temporal_fused_l0": per_launch(lambda n: "temporal_tc_kernel" in n),
+               "temporal_fused_l0": per_launch(lambda n: "temporal_fused_kernel" in n),
                "conv3x3_l0": per_launch(lambda n: "tc_conv3_kernel<64" in n, pick_max=False),      # every 64-output-channel (= level-0) 3x3 conv of the step
                "gn_apply_l0": per_launch(lambda n: "gn_apply_kernel" in n),
                "whole_step": {"dram_bytes": tot_b, "ncu_ms": tot_ns / 1e6, "launches": len(step)}}
@@ -88,7 +88,7 @@ def main(src, tag, title):
         cr = [i for i, h in enumerate(hdr) if h.endswith("dram__bytes_read.sum")][0]
         cw = [i for i, h in enumerate(hdr) if h.endswith("dram__bytes_write.sum")][0]
         cd = [i for i, h in enumerate(hdr) if h.endswith("gpu__time_duration.sum")][0]
-        for cat, pat in (("temporal_fused_l0", "temporal_tc_kernel"), ("conv3x3_l0", "tc_conv3_kernel<64"), ("gn_apply_l0", "gn_apply_kernel")):
+        for cat, pat in (("temporal_fused_l0", "temporal_fused_kernel"), ("conv3x3_l0", "tc_conv3_kernel<64"), ("gn_apply_l0", "gn_apply_kernel")):
             xs = [r for r in data if pat in r[4]]
             if xs:
                 traffic[cat] = {"dram_bytes_per_launch": sum(float(r[cr]) * byt[units[cr]] + float(r[cw]) * byt[units[cw]] for r in xs) / len(xs),
@@ -114,7 +114,7 @@ def main(src, tag, title):
                 ("stall wait", "smsp__average_warps_issue_stalled_wait_per_issue_active.ratio"),
                 ("stall short_scoreboard", "smsp__average_warps_issue_stalled_short_scoreboard_per_issue_active.ratio")]
         with open(tag + "_ncu_full_summary.md", "w") as f:
-            f.write(f"# {title} — `ncu --set full --clock-control none --import-source on`, {len(data)} launches (B200, 200 f x 64x64; `tools/gpu_call_ncufull.sh`)\n\n")
+            f.write(f"# {title} — `ncu --set full --clock-control none --import-source on`, {len(data)} launches (H100, 200 f x 64x64; `tools/gpu_call_ncufull.sh`)\n\n")
             f.write("| metric | " + " | ".join(f"launch {i}" for i in range(len(data))) + " |\n|---|" + "---:|" * len(data) + "\n")
             f.write("| kernel | " + " | ".join(short(r[4])[:44] for r in data) + " |\n")
             for label, key in want:

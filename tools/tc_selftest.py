@@ -1,4 +1,4 @@
-"""GPU: tcgen05 GEMM vs mma.sync GEMM on random convs; each case in its own time-boxed subprocess."""
+"""GPU: wgmma GEMM vs mma.sync GEMM on random convs; each case in its own time-boxed subprocess."""
 import ctypes
 import subprocess
 import sys
