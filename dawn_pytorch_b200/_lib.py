@@ -21,6 +21,29 @@ class DawnLfgCfg(ctypes.Structure):
                 ("num_down_blocks", ctypes.c_int), ("num_bottleneck_blocks", ctypes.c_int), ("skips", ctypes.c_int)]
 
 
+PATH_MMA_SYNC, PATH_TC_GEMM, PATH_TC_GEMM_PRESPLIT, PATH_TC_CONV3, PATH_TC_CONV3_TMA = range(5)
+EPI_PLAIN, EPI_QKV_TEMPORAL, EPI_QKV_SLA, EPI_QKV_MID, EPI_CA_GATE, EPI_GN_APPLY = range(6)
+
+
+class DawnContractionCase(ctypes.Structure):
+    """include/dawn_unet.h: dawn_contraction_case (pointers are device addresses)"""
+    _i, _p = ctypes.c_int, ctypes.c_void_p
+    _fields_ = [("path", _i), ("epi", _i),
+                ("F", _i), ("IH", _i), ("IW", _i), ("Cin", _i), ("lda", _i),
+                ("ntaps", _i), ("dy", _i * 52), ("dx", _i * 52), ("in_stride", _i),
+                ("OHs", _i), ("OWs", _i), ("OH", _i), ("OW", _i), ("out_stride", _i), ("oy0", _i), ("ox0", _i),
+                ("up2", _i),
+                ("perm_pb", _i), ("perm_F", _i), ("perm_in", _i), ("perm_out", _i), ("perm_f_lo", _i), ("perm_f_hi", _i),
+                ("P", _i),
+                ("N", _i), ("ldb", _i), ("ldo", _i), ("ldr", _i), ("drain", _i), ("ln_inline", _i),
+                ("rows_per_batch", _i), ("b_batch_stride", ctypes.c_longlong), ("cpg", _i),
+                ("q_post_scale", ctypes.c_float),
+                ("A", _p), ("B", _p), ("bias", _p), ("Res", _p), ("Out", _p),
+                ("stats", _p), ("rowstats", _p), ("wsum", _p), ("rot", _p),
+                ("kq", _p), ("nkq", _p), ("gates", _p),
+                ("Y", _p), ("ldy", _i), ("gn_stats", _p), ("gn_w", _p), ("gn_b", _p), ("film", _p), ("gn_count", ctypes.c_double)]
+
+
 class DawnError(RuntimeError):
     pass
 
@@ -54,6 +77,7 @@ def _load():
     lib.dawn_unet_workspace_bytes.restype = ctypes.c_int64
     lib.dawn_selftest_tc_gemm.argtypes = [ctypes.c_int] * 7 + [ctypes.POINTER(ctypes.c_float)] * 2
     lib.dawn_selftest_attention.argtypes = [ctypes.c_int] * 3 + [ctypes.POINTER(ctypes.c_float)] * 2
+    lib.dawn_test_contraction.argtypes = [ctypes.POINTER(DawnContractionCase), vp]
     lib.dawn_nccl_unique_id.argtypes = [ctypes.c_char_p]
     lib.dawn_unet_init_shard.argtypes = [vp, ctypes.c_char_p, ctypes.c_int, ctypes.c_int, ctypes.c_int]
     lib.dawn_unet_shard_ipc_export.argtypes = [vp, ctypes.c_char_p]
@@ -90,7 +114,7 @@ EXPORTS = ["dawn_unet_create", "dawn_unet_destroy", "dawn_unet_set_param", "dawn
            "dawn_unet_set_num_frames", "dawn_nccl_unique_id", "dawn_unet_init_shard", "dawn_unet_shard_ipc_export", "dawn_unet_shard_ipc_import", "dawn_unet_set_clip_invariants", "dawn_unet_forward",
            "dawn_unet_forward_x3", "dawn_unet_forward_host", "dawn_unet_set_tap", "dawn_unet_tap_shape",
            "dawn_unet_profile_enable", "dawn_unet_profile_read", "dawn_unet_last_launch_count", "dawn_unet_workspace_bytes", "dawn_ddim_step", "dawn_unet_ddim_step", "dawn_unet_sampler_capture", "dawn_unet_sampler_launch",
-           "dawn_selftest_tc_gemm", "dawn_selftest_attention", "dawn_last_error", "dawn_build_info"]
+           "dawn_test_contraction", "dawn_selftest_tc_gemm", "dawn_selftest_attention", "dawn_last_error", "dawn_build_info"]
 
 
 LFG_EXPORTS = ["dawn_lfg_create", "dawn_lfg_destroy", "dawn_lfg_set_param", "dawn_lfg_commit_params", "dawn_lfg_set_geometry",

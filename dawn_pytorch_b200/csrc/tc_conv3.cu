@@ -433,6 +433,8 @@ int launch_c3(const GemmParams& p, const float* Bimg, cudaStream_t st) {
 bool tc_conv3_supported(const GemmParams& p, int epi) {
   if (epi != EPI_PLAIN || p.Res != nullptr || p.perm_in || p.perm_out) return false;
   if (p.ntaps != 9 || p.in_stride != 1 || p.out_stride != 1 || p.oy0 != 0 || p.ox0 != 0) return false;
+  for (int t = 0; t < 9; ++t)                                  // the kernel's windows are the taps of a same-padded 3x3, in row-major order
+    if (p.dy[t] != t / 3 - 1 || p.dx[t] != t % 3 - 1) return false;
   if (p.IH != p.OH || p.IW != p.OW || p.OHs != p.OH || p.OWs != p.OW) return false;
   if (p.IH % TH != 0 || p.IW % TW != 0) return false;
   if (p.Cin % 64 != 0 || p.N % 64 != 0 || p.K != 9 * p.Cin) return false;

@@ -85,6 +85,7 @@ __global__ void __launch_bounds__(Cfg<BN>::NTHREADS, 1) tc_gemm_kernel(const Gem
     const int n_items = my_tiles * KC;
     int last_table = -1;
     float ln_s[4] = {0.f, 0.f, 0.f, 0.f}, ln_ss[4] = {0.f, 0.f, 0.f, 0.f};   // LayerNorm partial sums of this thread's 4 rows
+    float ln_pv[4] = {0.f, 0.f, 0.f, 0.f};                                    // per-row shift (the row's first element)
     uint32_t it = 0;
     long long tp_wait = 0, tp_work = 0, tp_load = 0;       // trace accumulators (registers; written once at the end)
 
@@ -145,6 +146,13 @@ __global__ void __launch_bounds__(Cfg<BN>::NTHREADS, 1) tc_gemm_kernel(const Gem
       if (tr) { const long long t1 = clock64(); p.trace[6] += (unsigned long long)(t1 - t0); t0 = t1; }
       uint8_t* a_hi = smem + s * STAGE_BYTES;
       uint8_t* a_lo = a_hi + A_PANEL;
+      const int Ts = (int)(it / (uint32_t)KC), kcs = (int)(it - (uint32_t)Ts * KC);
+      if (p.ln_inline && kcs == 0) {
+        // shift each row by its first element before summing: one-pass E[x^2] - mu^2 in fp32 cancels catastrophically when
+        // |mu| >> sigma (a row at mu = 100 sigma lost ~1e-3 of its rstd); the lane holding chunk 0 of the row broadcasts it
+#pragma unroll
+        for (int q = 0; q < 4; ++q) ln_pv[q] = __shfl_sync(0xffffffffu, v[2 * q].x, lane & ~7);
+      }
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
         uint32_t h[4], l[4];
@@ -156,13 +164,14 @@ __global__ void __launch_bounds__(Cfg<BN>::NTHREADS, 1) tc_gemm_kernel(const Gem
         *reinterpret_cast<uint4*>(a_hi + off) = make_uint4(h[0], h[1], h[2], h[3]);
         *reinterpret_cast<uint4*>(a_lo + off) = make_uint4(l[0], l[1], l[2], l[3]);
         if (p.ln_inline) {
-          const float4 a = v[2 * q], b = v[2 * q + 1];
+          const float pv = ln_pv[q];
+          const float4 a = make_float4(v[2 * q].x - pv, v[2 * q].y - pv, v[2 * q].z - pv, v[2 * q].w - pv);
+          const float4 b = make_float4(v[2 * q + 1].x - pv, v[2 * q + 1].y - pv, v[2 * q + 1].z - pv, v[2 * q + 1].w - pv);
           ln_s[q] += ((a.x + a.y) + (a.z + a.w)) + ((b.x + b.y) + (b.z + b.w));
           ln_ss[q] += ((a.x * a.x + a.y * a.y) + (a.z * a.z + a.w * a.w)) + ((b.x * b.x + b.y * b.y) + (b.z * b.z + b.w * b.w));
         }
       }
       if (p.ln_inline) {
-        const int Ts = (int)(it / (uint32_t)KC), kcs = (int)(it - (uint32_t)Ts * KC);
         if (kcs == KC - 1) {                                   // the row is complete: reduce over the 8 lanes that share it
 #pragma unroll
           for (int q = 0; q < 4; ++q) {
@@ -171,9 +180,9 @@ __global__ void __launch_bounds__(Cfg<BN>::NTHREADS, 1) tc_gemm_kernel(const Gem
             for (int o = 1; o < 8; o <<= 1) { sx += __shfl_xor_sync(0xffffffffu, sx, o); sxx += __shfl_xor_sync(0xffffffffu, sxx, o); }
             if (c16 == 0) {
               const float inv = 1.0f / (float)p.K;
-              const float mu = sx * inv;
-              const float var = fmaxf(sxx * inv - mu * mu, 0.f);
-              s_ln[Ts & 7][r0 + 32 * q] = make_float2(mu, 1.0f / sqrtf(var + 1e-5f));
+              const float dm = sx * inv;                       // mean of the shifted row
+              const float var = fmaxf(sxx * inv - dm * dm, 0.f);
+              s_ln[Ts & 7][r0 + 32 * q] = make_float2(ln_pv[q] + dm, 1.0f / sqrtf(var + 1e-5f));
             }
             ln_s[q] = 0.f; ln_ss[q] = 0.f;
           }

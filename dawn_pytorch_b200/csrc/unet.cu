@@ -1791,11 +1791,19 @@ int dawn_selftest_tc_gemm(int F, int H, int W, int Cin, int N, int ksize, int wi
     cudaMemcpy(o1.data(), dO1, o1.size() * 4, cudaMemcpyDeviceToHost);
     cudaMemcpy(o2.data(), dO2, o2.size() * 4, cudaMemcpyDeviceToHost);
     float md = 0.f, mr = 0.f;
-    for (size_t i = 0; i < o1.size(); ++i) { md = std::max(md, std::fabs(o1[i] - o2[i])); mr = std::max(mr, std::fabs(o1[i])); }
+    // a NaN difference must win the max (std::max keeps its first argument when the comparison is false)
+    for (size_t i = 0; i < o1.size(); ++i) {
+      const float d = std::fabs(o1[i] - o2[i]);
+      md = (d > md || d != d) ? d : md;
+      mr = std::max(mr, std::fabs(o1[i]));
+    }
     if (with_stats) {
       double st[32];
       cudaMemcpy(st, dS, sizeof(st), cudaMemcpyDeviceToHost);
-      for (int i = 0; i < 16; ++i) md = std::max(md, (float)(std::fabs(st[i] - st[16 + i]) / std::max(1.0, std::fabs(st[i]))));
+      for (int i = 0; i < 16; ++i) {
+        const float d = (float)(std::fabs(st[i] - st[16 + i]) / std::max(1.0, std::fabs(st[i])));
+        md = (d > md || d != d) ? d : md;
+      }
     }
     *max_abs_diff = md; *max_abs_ref = mr;
   }

@@ -141,6 +141,45 @@ int dawn_unet_sampler_launch(dawn_unet* h, void* stream);
  * (F frames of H x W, Cin -> N channels); reports max |difference| (outputs and, if requested, GroupNorm sums). */
 int dawn_selftest_tc_gemm(int F, int H, int W, int Cin, int N, int ksize, int with_stats, float* max_abs_diff, float* max_abs_ref);
 
+/* One contraction through exactly one kernel path, for per-kernel tests against a high-precision reference.
+ * Out[m, n] = epilogue( sum_{tap, c} A[pixel(m, tap), c] * B[tap*Cin + c, n] ) with the product's GemmParams semantics
+ * (dawn_pytorch_b200/csrc/gemm.cuh): rows m = (f, i, j) over an F x OHs x OWs output sub-grid (M = F*OHs*OWs), input pixel
+ * (i*in_stride + dy[t], j*in_stride + dx[t]) of an F x IH x IW image with row stride lda, output pixel
+ * (f*OH + i*out_stride + oy0) * OW + j*out_stride + ox0 with row stride ldo.  B is fp32 [K][ldb], K = ntaps*Cin.
+ * The wgmma paths build their weight image and accumulator scale from B the way the network's weight upload does.
+ * Returns -1 and launches nothing when the chosen path does not accept the geometry (it never falls back to
+ * another kernel), -2 on a CUDA error; synchronises the stream before it returns. */
+enum {
+  DAWN_PATH_MMA_SYNC = 0,          /* mma.sync 3xTF32 implicit GEMM (every epilogue, per-frame B) */
+  DAWN_PATH_TC_GEMM = 1,           /* wgmma implicit GEMM, fp32 gather producers */
+  DAWN_PATH_TC_GEMM_PRESPLIT = 2,  /* wgmma implicit GEMM, A pre-split into fp16 hi | lo planes, cp.async producers */
+  DAWN_PATH_TC_CONV3 = 3,          /* wgmma 3x3 halo-tile conv, fp32 gather producers */
+  DAWN_PATH_TC_CONV3_TMA = 4       /* wgmma 3x3 halo-tile conv, A pre-split, halo tiles fetched by TMA */
+};
+typedef struct {
+  int path, epi;                   /* DAWN_PATH_*; epilogue: 0 plain, 1 qkv+rotary, 2 qkv+SLA softmax, 3 qkv, 4 cross-attn gate, 5 GN apply */
+  int F, IH, IW, Cin, lda;
+  int ntaps; int dy[52]; int dx[52]; int in_stride;
+  int OHs, OWs, OH, OW, out_stride, oy0, ox0;
+  int up2;                         /* halo conv: 64-column block j of the output is parity class j of the 2x grid */
+  int perm_pb, perm_F, perm_in, perm_out, perm_f_lo, perm_f_hi;
+  int P;                           /* rows per frame (rotary / gate frame index, sequence-blocked order) */
+  int N, ldb, ldo, ldr, drain, ln_inline;
+  int rows_per_batch;              /* 0 = M */
+  long long b_batch_stride;        /* floats between per-batch B matrices (mma.sync only) */
+  int cpg;                         /* GroupNorm channels per group */
+  float q_post_scale;
+  /* device pointers owned by the caller */
+  const float* A; const float* B; const float* bias; const float* Res; float* Out;
+  double* stats;                   /* [16] GroupNorm partial sums, accumulated into */
+  const float* rowstats;           /* [rows][2] (mu, rstd) */
+  const float* wsum;               /* [N] column sums of B */
+  const float* rot;                /* [frames][16][2] */
+  const float* kq; const float* nkq; float* gates;
+  const float* Y; int ldy; const double* gn_stats; const float* gn_w; const float* gn_b; const float* film; double gn_count;
+} dawn_contraction_case;
+int dawn_test_contraction(const dawn_contraction_case* c, void* stream);
+
 /* self-test of the tensor-core attention core against the SIMT fp32 kernel on random q/k/v:
  * temporal != 0: nseq pixel sequences of L frames, band 40 with bias; else nseq frames of L tokens, full attention */
 int dawn_selftest_attention(int nseq, int L, int temporal, float* max_abs_diff, float* max_abs_ref);
