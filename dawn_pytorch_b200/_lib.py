@@ -75,7 +75,6 @@ def _load():
     lib.dawn_unet_last_launch_count.restype = ctypes.c_int64
     lib.dawn_unet_workspace_bytes.argtypes = [vp]
     lib.dawn_unet_workspace_bytes.restype = ctypes.c_int64
-    lib.dawn_selftest_tc_gemm.argtypes = [ctypes.c_int] * 7 + [ctypes.POINTER(ctypes.c_float)] * 2
     lib.dawn_selftest_attention.argtypes = [ctypes.c_int] * 3 + [ctypes.POINTER(ctypes.c_float)] * 2
     lib.dawn_test_contraction.argtypes = [ctypes.POINTER(DawnContractionCase), vp]
     lib.dawn_nccl_unique_id.argtypes = [ctypes.c_char_p]
@@ -114,7 +113,7 @@ EXPORTS = ["dawn_unet_create", "dawn_unet_destroy", "dawn_unet_set_param", "dawn
            "dawn_unet_set_num_frames", "dawn_nccl_unique_id", "dawn_unet_init_shard", "dawn_unet_shard_ipc_export", "dawn_unet_shard_ipc_import", "dawn_unet_set_clip_invariants", "dawn_unet_forward",
            "dawn_unet_forward_x3", "dawn_unet_forward_host", "dawn_unet_set_tap", "dawn_unet_tap_shape",
            "dawn_unet_profile_enable", "dawn_unet_profile_read", "dawn_unet_last_launch_count", "dawn_unet_workspace_bytes", "dawn_ddim_step", "dawn_unet_ddim_step", "dawn_unet_sampler_capture", "dawn_unet_sampler_launch",
-           "dawn_test_contraction", "dawn_selftest_tc_gemm", "dawn_selftest_attention", "dawn_last_error", "dawn_build_info"]
+           "dawn_test_contraction", "dawn_selftest_attention", "dawn_last_error", "dawn_build_info"]
 
 
 LFG_EXPORTS = ["dawn_lfg_create", "dawn_lfg_destroy", "dawn_lfg_set_param", "dawn_lfg_commit_params", "dawn_lfg_set_geometry",

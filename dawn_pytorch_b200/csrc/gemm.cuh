@@ -63,8 +63,6 @@ struct GemmParams {
   int drain;                   // wgmma kernels: K panels (tc_gemm) / taps (tc_conv3) accumulated in registers before the fp32 drain; 0 = default
                                // (4 panels = K 256 / 9 taps = K 576).  The tensor core adds with round-toward-zero: un-normalised conv stacks
                                // (LFG decoder) drain every panel / tap to keep the bias below the fp32 tolerance.
-  int exp_shift;               // experiment (wgmma path, BN = 64): A operand stored/addressed this many rows into the swizzle atom
-  unsigned long long* trace;   // optional [16] cycle counters written by CTA 0 of the wgmma kernel (debug)
 };
 
 // pixel index (f * P + p) of row m in sequence-blocked order

@@ -105,48 +105,9 @@ int launch_gn_apply(const float* Y, int ldy, int C, int M, const double* stats, 
 }
 
 // =========================================================================== small dense layers (per frame GEMV)
-// one warp per output; grid (ceil(Nout/8), F).  act: 1 = SiLU on the input
-template <int ACT>
-__device__ __forceinline__ void frame_linear_body(const float* __restrict__ x, int ldx, int off, int K,
-                                                  const float* __restrict__ W, const float* __restrict__ b, int Nout,
-                                                  float* __restrict__ out) {
-  extern __shared__ float sx[];
-  const int f = blockIdx.y;
-  for (int i = threadIdx.x; i < K; i += blockDim.x) {
-    float v = x[(size_t)f * ldx + off + i];
-    sx[i] = ACT ? silu(v) : v;
-  }
-  __syncthreads();
-  const int j = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  const int lane = threadIdx.x & 31;
-  if (j >= Nout) return;
-  const float* w = W + (size_t)j * K;
-  float acc = 0.f;
-  for (int i = lane; i < K; i += 32) acc += w[i] * sx[i];
-  acc = warp_sum(acc);
-  if (lane == 0) out[(size_t)f * Nout + j] = acc + (b ? b[j] : 0.f);
-}
-template <int ACT>
-__global__ void frame_linear_kernel(const float* __restrict__ x, int ldx, int off, int K,
-                                    const float* __restrict__ W, const float* __restrict__ b, int Nout,
-                                    float* __restrict__ out) {
-  frame_linear_body<ACT>(x, ldx, off, K, W, b, Nout, out);
-}
-// all (block, cross-attention) pairs of the per-clip conditioning in one launch each: blockIdx.z = descriptor
-__global__ void cond_mlp_batched_kernel(const float* __restrict__ cond, int cond_ld, const CondDesc* __restrict__ descs) {
-  const CondDesc d = descs[blockIdx.z];
-  if ((int)blockIdx.x * 8 >= d.n1) return;
-  frame_linear_body<1>(cond, cond_ld, d.off, d.K, d.mW, d.mB, d.n1, d.ctx);
-}
-__global__ void cond_kv_batched_kernel(const CondDesc* __restrict__ descs) {
-  const CondDesc d = descs[blockIdx.z];
-  frame_linear_body<0>(d.ctx, d.n1, 0, d.n1, d.Wkv, nullptr, 128, d.kv);
-}
-
-// v2 of the batched per-clip conditioning layers: a block owns FL_JT*8 = 32 outputs x FL_FT = 8 frames, so every weight row
-// is read once per 8 frames (v1: once per frame — 200 x 35 MB through L2 for the audio MLPs) and SiLU(cond) is evaluated
-// once per 32 outputs (v1: per 8).  Each (frame, output) keeps v1's arithmetic order exactly (lane-strided partial sums,
-// butterfly reduction), so the tables are bit-identical.
+// out[f][j] = b[j] + sum_i W[j][i] act(x[f][off + i]), act = SiLU when ACT = 1 (cond MLPs U:371-384, 440-442; to_kv U:524).
+// A block owns FL_JT*8 = 32 outputs x FL_FT = 8 frames, so every weight row is read once per 8 frames and act(x) is evaluated
+// once per 32 outputs; a warp computes FL_JT outputs with lane-strided partial sums and a butterfly reduction.
 constexpr int FL_FT = 8, FL_JT = 4;
 template <int ACT>
 __device__ __forceinline__ void frame_linear_tiled_body(const float* __restrict__ x, int ldx, int off, int K,
@@ -198,26 +159,11 @@ __global__ void __launch_bounds__(256) cond_kv_tiled_kernel(const CondDesc* __re
   frame_linear_tiled_body<0>(d.ctx, d.n1, 0, d.n1, d.Wkv, nullptr, 128, d.kv, F);
 }
 
-int launch_cond_mlp(const float* cond, int cond_ld, int off, int K, const float* W, const float* b, int Nout,
-                    int F, float* out, cudaStream_t st) {
-  dim3 grid((Nout + 7) / 8, F);
-  frame_linear_kernel<1><<<grid, 256, K * sizeof(float), st>>>(cond, cond_ld, off, K, W, b, Nout, out);
-  DAWN_LAUNCH_OK();
-  return 0;
-}
-int launch_linear_nobias(const float* x, int K, const float* W, int Nout, int F, float* out, cudaStream_t st) {
-  dim3 grid((Nout + 7) / 8, F);
-  frame_linear_kernel<0><<<grid, 256, K * sizeof(float), st>>>(x, K, 0, K, W, nullptr, Nout, out);
-  DAWN_LAUNCH_OK();
-  return 0;
-}
-
 // =========================================================================== cross-attention per-frame tables
 // With exactly two keys (null, real) per query the attention output of head h is
 //   o_h = nv + w_h (v_h - nv),  so  to_out(o) = u_0 + sum_h w_h u_h  with per-frame vectors
 //   u_0 = Wout * rep(nv),  u_h = Wout[:, h] (v_h - nv)   (U:530-559).
 // The output LayerNorm (U:511-514) of that combination needs only the centred vectors and their Gram matrix.
-template <bool V2>
 __device__ __forceinline__ void ca_tables_body(const CaTableArgs& a, int f) {
   extern __shared__ float sm[];
   float* u = sm;                       // [9][co]
@@ -243,41 +189,26 @@ __device__ __forceinline__ void ca_tables_body(const CaTableArgs& a, int f) {
     const float inv = 1.0f / fmaxf(sqrtf(n2), 1e-12f);
     a.nkq[a.ca * 8 + tid] = s_nk[tid] * inv * a.ks[tid] * a.qs[tid];
   }
-  // u vectors.  V2: a thread owns output channel c, reads its 64-float Wout row once (16 x LDG.128) and forms all nine
-  // combinations from registers — v1 re-read the row for each of the 9 vectors with a 256-byte lane stride.  Same sums, same order.
-  if (V2) {
-    for (int c = tid; c < co; c += blockDim.x) {
-      float w[64];
-      const float4* wr = reinterpret_cast<const float4*>(a.Wout + (size_t)c * 64);
+  // u vectors: a thread owns output channel c, reads its 64-float Wout row once (16 x LDG.128) and forms all nine
+  // combinations from registers
+  for (int c = tid; c < co; c += blockDim.x) {
+    float w[64];
+    const float4* wr = reinterpret_cast<const float4*>(a.Wout + (size_t)c * 64);
 #pragma unroll
-      for (int i = 0; i < 16; ++i) { const float4 t = __ldg(wr + i); w[4 * i] = t.x; w[4 * i + 1] = t.y; w[4 * i + 2] = t.z; w[4 * i + 3] = t.w; }
-      float acc0 = 0.f;
+    for (int i = 0; i < 16; ++i) { const float4 t = __ldg(wr + i); w[4 * i] = t.x; w[4 * i + 1] = t.y; w[4 * i + 2] = t.z; w[4 * i + 3] = t.w; }
+    float acc0 = 0.f;
 #pragma unroll
-      for (int h = 0; h < 8; ++h)
+    for (int h = 0; h < 8; ++h)
 #pragma unroll
-        for (int d = 0; d < 8; ++d) acc0 += w[h * 8 + d] * s_nv[d];
-      u[c] = acc0;
+      for (int d = 0; d < 8; ++d) acc0 += w[h * 8 + d] * s_nv[d];
+    u[c] = acc0;
 #pragma unroll
-      for (int h = 0; h < 8; ++h) {
-        float acc = 0.f;
+    for (int h = 0; h < 8; ++h) {
+      float acc = 0.f;
 #pragma unroll
-        for (int d = 0; d < 8; ++d) acc += w[h * 8 + d] * (s_kv[64 + h * 8 + d] - s_nv[d]);
-        u[(h + 1) * co + c] = acc;
-      }
-    }
-  } else
-  for (int idx = tid; idx < 9 * co; idx += blockDim.x) {
-    const int r = idx / co, c = idx - r * co;
-    const float* w = a.Wout + (size_t)c * 64;
-    float acc = 0.f;
-    if (r == 0) {
-      for (int h = 0; h < 8; ++h)
-        for (int d = 0; d < 8; ++d) acc += w[h * 8 + d] * s_nv[d];
-    } else {
-      const int h = r - 1;
       for (int d = 0; d < 8; ++d) acc += w[h * 8 + d] * (s_kv[64 + h * 8 + d] - s_nv[d]);
+      u[(h + 1) * co + c] = acc;
     }
-    u[idx] = acc;
   }
   __syncthreads();
   // centre each vector over channels
@@ -307,51 +238,26 @@ __device__ __forceinline__ void ca_tables_body(const CaTableArgs& a, int f) {
   }
 }
 
-__global__ void ca_tables_kernel(CaTableArgs a) { ca_tables_body<false>(a, blockIdx.x); }
-__global__ void ca_tables_batched_kernel(const CondDesc* __restrict__ descs) { ca_tables_body<false>(descs[blockIdx.y].t, blockIdx.x); }
-__global__ void __launch_bounds__(256) ca_tables_batched_v2_kernel(const CondDesc* __restrict__ descs) { ca_tables_body<true>(descs[blockIdx.y].t, blockIdx.x); }
+// grid (F, descriptors): one block per (frame, conditioned block x cross-attention)
+__global__ void __launch_bounds__(256) ca_tables_batched_kernel(const CondDesc* __restrict__ descs) { ca_tables_body(descs[blockIdx.y].t, blockIdx.x); }
 
 int launch_cond_batched(const float* cond, int cond_ld, const CondDesc* descs_dev, int ndesc, int max_n1, int max_k, int max_co, int F,
                         cudaStream_t st) {
+  const size_t sm1 = (size_t)FL_FT * max_k * sizeof(float), sm2 = (size_t)FL_FT * max_n1 * sizeof(float);
+  const size_t smem_t = (size_t)9 * max_co * sizeof(float);
   static size_t attr = 0;
-  static const bool v1 = [] { const char* e = getenv("DAWN_PREP_V1"); return e && e[0] == '1'; }();
-  const size_t smem_kv = (size_t)max_n1 * sizeof(float), smem_t = (size_t)9 * max_co * sizeof(float);
-  if (!v1) {
-    const size_t sm1 = (size_t)FL_FT * max_k * sizeof(float), sm2 = (size_t)FL_FT * max_n1 * sizeof(float);
-    static size_t attr2 = 0;
-    if (std::max({sm1, sm2, smem_t}) > 48 * 1024 && std::max({sm1, sm2, smem_t}) > attr2) {
-      attr2 = std::max({sm1, sm2, smem_t});
-      DAWN_CUDA_OK(cudaFuncSetAttribute(cond_mlp_tiled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attr2));
-      DAWN_CUDA_OK(cudaFuncSetAttribute(cond_kv_tiled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attr2));
-      DAWN_CUDA_OK(cudaFuncSetAttribute(ca_tables_batched_v2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attr2));
-    }
-    const int ft = (F + FL_FT - 1) / FL_FT, jb = 8 * FL_JT;
-    cond_mlp_tiled_kernel<<<dim3((max_n1 + jb - 1) / jb, ft, ndesc), 256, sm1, st>>>(cond, cond_ld, descs_dev, F);
-    DAWN_LAUNCH_OK();
-    cond_kv_tiled_kernel<<<dim3((128 + jb - 1) / jb, ft, ndesc), 256, sm2, st>>>(descs_dev, F);
-    DAWN_LAUNCH_OK();
-    ca_tables_batched_v2_kernel<<<dim3(F, ndesc), 256, smem_t, st>>>(descs_dev);
-    DAWN_LAUNCH_OK();
-    return 0;
+  if (std::max({sm1, sm2, smem_t}) > 48 * 1024 && std::max({sm1, sm2, smem_t}) > attr) {
+    attr = std::max({sm1, sm2, smem_t});
+    DAWN_CUDA_OK(cudaFuncSetAttribute(cond_mlp_tiled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attr));
+    DAWN_CUDA_OK(cudaFuncSetAttribute(cond_kv_tiled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attr));
+    DAWN_CUDA_OK(cudaFuncSetAttribute(ca_tables_batched_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attr));
   }
-  if (smem_kv > 48 * 1024 || smem_t > 48 * 1024) {
-    if (std::max(smem_kv, smem_t) > attr) {
-      DAWN_CUDA_OK(cudaFuncSetAttribute(cond_kv_batched_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max(smem_kv, smem_t)));
-      DAWN_CUDA_OK(cudaFuncSetAttribute(ca_tables_batched_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max(smem_kv, smem_t)));
-      attr = std::max(smem_kv, smem_t);
-    }
-  }
-  cond_mlp_batched_kernel<<<dim3((max_n1 + 7) / 8, F, ndesc), 256, (size_t)max_k * sizeof(float), st>>>(cond, cond_ld, descs_dev);
+  const int ft = (F + FL_FT - 1) / FL_FT, jb = 8 * FL_JT;
+  cond_mlp_tiled_kernel<<<dim3((max_n1 + jb - 1) / jb, ft, ndesc), 256, sm1, st>>>(cond, cond_ld, descs_dev, F);
   DAWN_LAUNCH_OK();
-  cond_kv_batched_kernel<<<dim3(16, F, ndesc), 256, smem_kv, st>>>(descs_dev);
+  cond_kv_tiled_kernel<<<dim3((128 + jb - 1) / jb, ft, ndesc), 256, sm2, st>>>(descs_dev, F);
   DAWN_LAUNCH_OK();
   ca_tables_batched_kernel<<<dim3(F, ndesc), 256, smem_t, st>>>(descs_dev);
-  DAWN_LAUNCH_OK();
-  return 0;
-}
-
-int launch_ca_tables(const CaTableArgs& a, int F, cudaStream_t st) {
-  ca_tables_kernel<<<F, 256, 9 * a.co * sizeof(float), st>>>(a);
   DAWN_LAUNCH_OK();
   return 0;
 }

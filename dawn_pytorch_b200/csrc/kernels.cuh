@@ -14,12 +14,6 @@ int launch_gn_apply(const float* Y, int ldy, int C, int M, const double* stats, 
                     const float* Res, int ldr, float* Out, int ldo, cudaStream_t st);
 
 // ---------------------------------------------------------------- conditioning tables (clip invariants)
-// ctx[f][j] = b[j] + sum_i W[j][i] * silu(cond[f][off + i])         U:371-384, 440-442
-int launch_cond_mlp(const float* cond, int cond_ld, int off, int K, const float* W, const float* b, int Nout,
-                    int F, float* out /*[F][Nout]*/, cudaStream_t st);
-// plain y[f][j] = sum_i W[j][i] x[f][i]  (no bias, no activation)    U:524 to_kv
-int launch_linear_nobias(const float* x, int K, const float* W, int Nout, int F, float* out, cudaStream_t st);
-
 struct CaTableArgs {
   const float* kv;     // [F][128]  (k | v) of this cross-attention
   const float* nkv;    // [2][8] null key / value
@@ -43,8 +37,6 @@ struct CondDesc {
 };
 int launch_cond_batched(const float* cond, int cond_ld, const CondDesc* descs_dev, int ndesc, int max_n1, int max_k, int max_co, int F,
                         cudaStream_t st);
-
-int launch_ca_tables(const CaTableArgs& a, int F, cudaStream_t st);
 
 // Wt[m][ca*9 + {0, 1+h}] = rstd_ca(m) * {1, gate(m,ca,h)}           U:511-514 (to_out LayerNorm) via Gram form
 int launch_ca_rstd(const float* gates, const float* G, int M, int P, float* Wt /*[M][32]*/, cudaStream_t st);

@@ -51,7 +51,7 @@ struct CCfg {
 // two dense fp16 planes (hi | lo, written by the producing kernel's epilogue) and ONE thread fetches the halo tile of a 64-channel chunk with
 // two cp.async.bulk.tensor loads (4-D tiled map {C, W, H, F}, box {64, 10, 18, 1}, 128-byte swizzle, out-of-image rows zero-filled by the
 // TMA unit): the smem image is byte-identical to what the producers write (row = hy * 10 + hx of 128 B, absolute-address swizzle).
-template <int BN, bool TMA, bool TR>
+template <int BN, bool TMA>
 __global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const GemmParams p, const float* __restrict__ Bimg,
                                                                           int tiles_y, int tiles_x, int tiles_n,
                                                                           const __grid_constant__ CUtensorMap tm_hi,
@@ -221,8 +221,6 @@ __global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const G
       }
       pending = 0;
     };
-    const bool tre = TR && (p.trace != nullptr) && blockIdx.x == 0 && etid == 0 && wg == 0;
-    long long te_final = 0, te0 = 0, te_bias = 0, te_store = 0, te1 = 0;
     constexpr uint32_t SBO_HALO = HW * 128;                    // 10 pixel rows of 128 B between 8-row groups
     constexpr uint32_t H2 = 8 * HW * 128;                      // output rows 64-127 start 8 halo rows further down
     const int dt = (p.drain == 1 || p.drain == 3) ? p.drain : 9;   // taps accumulated in registers before a drain
@@ -289,7 +287,6 @@ __global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const G
         }
       }
       __syncwarp();
-      if (tre) te0 = clock64();
 #pragma unroll
       for (int i = 0; i < 64; ++i) acc[i] *= p.tc_scale;
       const int oy = y0 + (row_in_tile >> 3), ox = x0 + (row_in_tile & 7);
@@ -317,9 +314,7 @@ __global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const G
           acc[4 * i] += b.x; acc[4 * i + 1] += b.y; acc[4 * i + 2] += b.z; acc[4 * i + 3] += b.w;
         }
       }
-      if (tre) { te1 = clock64(); te_bias += te1 - te0; }
       store_rows_coalesced(wbuf, acc, p.Out, opix, p.ldo, ocol, rv, lane);
-      if (tre) te_store += clock64() - te1;
       if (defer_stats) {
         if (rv) {
 #pragma unroll
@@ -355,13 +350,9 @@ __global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const G
           if (grp >= glo && grp <= ghi) atomicAdd(&p.stats[etid], (double)s_st[etid]);
         }
       }
-      if (tre) te_final += clock64() - te0;
       asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");     // the staged tile is rewritten by the next tile's first drain
     }
     if (defer_stats && pending > 0) flush_stats();
-    if (tre) {
-      p.trace[10] = (unsigned long long)te_final; p.trace[13] = (unsigned long long)te_bias; p.trace[14] = (unsigned long long)te_store;
-    }
   }
 }
 
@@ -402,9 +393,8 @@ int launch_c3(const GemmParams& p, const float* Bimg, cudaStream_t st) {
   static bool attr_set = false;
   static int num_sms = 0;
   if (!attr_set) {
-    DAWN_CUDA_OK(cudaFuncSetAttribute(tc_conv3_kernel<BN, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_DYN));
-    DAWN_CUDA_OK(cudaFuncSetAttribute(tc_conv3_kernel<BN, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_DYN));
-    DAWN_CUDA_OK(cudaFuncSetAttribute(tc_conv3_kernel<BN, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_DYN));
+    DAWN_CUDA_OK(cudaFuncSetAttribute(tc_conv3_kernel<BN, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_DYN));
+    DAWN_CUDA_OK(cudaFuncSetAttribute(tc_conv3_kernel<BN, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_DYN));
     int dev = 0;
     DAWN_CUDA_OK(cudaGetDevice(&dev));
     DAWN_CUDA_OK(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
@@ -416,12 +406,11 @@ int launch_c3(const GemmParams& p, const float* Bimg, cudaStream_t st) {
   if (p.A16h != nullptr && p.A16l != nullptr) {
     CUtensorMap mh, ml;
     if (halo_tensor_map(p.A16h, p.Cin, p.IW, p.IH, F, &mh) != 0 || halo_tensor_map(p.A16l, p.Cin, p.IW, p.IH, F, &ml) != 0) return -2;
-    tc_conv3_kernel<BN, true, false><<<grid, C::NTHREADS, C::SMEM_DYN, st>>>(p, Bimg, tiles_y, tiles_x, tiles_n, mh, ml);
+    tc_conv3_kernel<BN, true><<<grid, C::NTHREADS, C::SMEM_DYN, st>>>(p, Bimg, tiles_y, tiles_x, tiles_n, mh, ml);
   } else {
     CUtensorMap dummy;
     memset(&dummy, 0, sizeof(dummy));
-    if (p.trace) tc_conv3_kernel<BN, false, true><<<grid, C::NTHREADS, C::SMEM_DYN, st>>>(p, Bimg, tiles_y, tiles_x, tiles_n, dummy, dummy);
-    else tc_conv3_kernel<BN, false, false><<<grid, C::NTHREADS, C::SMEM_DYN, st>>>(p, Bimg, tiles_y, tiles_x, tiles_n, dummy, dummy);
+    tc_conv3_kernel<BN, false><<<grid, C::NTHREADS, C::SMEM_DYN, st>>>(p, Bimg, tiles_y, tiles_x, tiles_n, dummy, dummy);
   }
   DAWN_LAUNCH_OK();
   return 0;

@@ -87,7 +87,6 @@ __global__ void __launch_bounds__(Cfg<BN>::NTHREADS, 1) tc_gemm_kernel(const Gem
     float ln_s[4] = {0.f, 0.f, 0.f, 0.f}, ln_ss[4] = {0.f, 0.f, 0.f, 0.f};   // LayerNorm partial sums of this thread's 4 rows
     float ln_pv[4] = {0.f, 0.f, 0.f, 0.f};                                    // per-row shift (the row's first element)
     uint32_t it = 0;
-    long long tp_wait = 0, tp_work = 0, tp_load = 0;       // trace accumulators (registers; written once at the end)
 
     // row table of this CTA's T-th tile (ring of 3: prefetch runs at most 2 items = 2 tiles ahead of the stores)
     auto ensure_table = [&](int T) {
@@ -112,8 +111,6 @@ __global__ void __launch_bounds__(Cfg<BN>::NTHREADS, 1) tc_gemm_kernel(const Gem
       last_table = T;
     };
     auto load_item = [&](float4 (&v)[8], int g) {
-      const bool trl = (p.trace != nullptr) && blockIdx.x == 0 && tid == 0;
-      const long long tl0 = trl ? clock64() : 0;
       const int T = g / KC, kc = g - T * KC;
       ensure_table(T);
       const RowInfo* rows = s_rows[T % 3];
@@ -134,16 +131,11 @@ __global__ void __launch_bounds__(Cfg<BN>::NTHREADS, 1) tc_gemm_kernel(const Gem
           v[2 * q + 1] = make_float4(0.f, 0.f, 0.f, 0.f);
         }
       }
-      if (trl) tp_load += clock64() - tl0;
     };
     auto store_item = [&](const float4 (&v)[8]) {
       const int s = it % STAGES;
       const uint32_t round = it / STAGES;
-      const bool tr = (p.trace != nullptr) && blockIdx.x == 0 && tid == 0;
-      long long t0 = 0;
-      if (tr) t0 = clock64();
       mbar_wait(&slot_free[s], (round & 1) ^ 1);
-      if (tr) { const long long t1 = clock64(); p.trace[6] += (unsigned long long)(t1 - t0); t0 = t1; }
       uint8_t* a_hi = smem + s * STAGE_BYTES;
       uint8_t* a_lo = a_hi + A_PANEL;
       const int Ts = (int)(it / (uint32_t)KC), kcs = (int)(it - (uint32_t)Ts * KC);
@@ -193,7 +185,6 @@ __global__ void __launch_bounds__(Cfg<BN>::NTHREADS, 1) tc_gemm_kernel(const Gem
       // retire in order through the same shared-memory pipe; the consumers run the proxy fence after acquiring a_full
       // (they have no loads in flight), before the async-proxy reads of wgmma.
       mbar_arrive_relaxed(&a_full[s]);
-      if (tr) p.trace[7] += (unsigned long long)(clock64() - t0);
       ++it;
     };
 
@@ -255,30 +246,21 @@ __global__ void __launch_bounds__(Cfg<BN>::NTHREADS, 1) tc_gemm_kernel(const Gem
         }
       }
     }
-    if (p.trace != nullptr && blockIdx.x == 0 && tid == 0) {
-      p.trace[6] = (unsigned long long)tp_wait; p.trace[7] = (unsigned long long)tp_work; p.trace[11] = (unsigned long long)tp_load;
-    }
   } else if (warp == LOAD_WARP) {
     // =============================================================== weight loader (pre-swizzled hi|lo images)
     if (lane == 0) {
       uint32_t it = 0;
-      long long tl_wait = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         const int nt = tile % tiles_n;
         const uint8_t* src = reinterpret_cast<const uint8_t*>(Bimg) + (size_t)nt * KC * (2 * B_PANEL);
         for (int kc = 0; kc < KC; ++kc, ++it) {
           const int s = it % STAGES;
           const uint32_t round = it / STAGES;
-          const bool tr = (p.trace != nullptr) && blockIdx.x == 0;
-          long long t0 = 0;
-          if (tr) t0 = clock64();
           mbar_wait(&slot_free[s], (round & 1) ^ 1);
-          if (tr) tl_wait += clock64() - t0;
           mbar_arrive_expect_tx(&b_full[s], 2 * B_PANEL);
           bulk_copy_g2s(smem + s * STAGE_BYTES + 2 * A_PANEL, src + (size_t)kc * (2 * B_PANEL), 2 * B_PANEL, &b_full[s]);
         }
       }
-      if (p.trace != nullptr && blockIdx.x == 0) p.trace[8] = (unsigned long long)tl_wait;
     }
   } else {
     // =============================================================== consumers (warps 8 .. 8+4*NWG-1): MMA + epilogue
@@ -301,7 +283,6 @@ __global__ void __launch_bounds__(Cfg<BN>::NTHREADS, 1) tc_gemm_kernel(const Gem
     }
     const int CH = (p.drain > 0 && p.drain < CHUNK) ? p.drain : CHUNK;
     uint32_t it = 0;
-    long long te_final = 0, te_store = 0, te_pre = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       ++Te;
       const int m0 = (tile / tiles_n) * BM, n0 = (tile % tiles_n) * BN + wg * EN;
@@ -358,8 +339,6 @@ __global__ void __launch_bounds__(Cfg<BN>::NTHREADS, 1) tc_gemm_kernel(const Gem
       __syncwarp();
 
       // ---------------------------------------------------------- final epilogue: this thread owns row m
-      const bool tr_e = (p.trace != nullptr) && blockIdx.x == 0 && etid == 0;
-      const long long te0 = tr_e ? clock64() : 0;
       const int m = m0 + row_in_tile;
       bool rv = m < p.M;
       const int mc = rv ? m : (p.M - 1);
@@ -404,12 +383,7 @@ __global__ void __launch_bounds__(Cfg<BN>::NTHREADS, 1) tc_gemm_kernel(const Gem
             acc[4 * i] += r.x; acc[4 * i + 1] += r.y; acc[4 * i + 2] += r.z; acc[4 * i + 3] += r.w;
           }
         }
-        {
-          const long long ts0 = tr_e ? clock64() : 0;
-          if (tr_e) te_pre += ts0 - te0;
-          if (!(p.exp_shift & 64)) store_rows_coalesced(wbuf, acc, p.Out, opix, p.ldo, n0, rv, lane);     // bit 6 of the debug field: skip the stores (timing experiment)
-          if (tr_e) te_store += clock64() - ts0;
-        }
+        store_rows_coalesced(wbuf, acc, p.Out, opix, p.ldo, n0, rv, lane);
         if (p.stats != nullptr) {
           // GroupNorm partial statistics (U:230): per 8-column sub-block, reduced over the warp's 32 rows
           if (etid < 16) s_st[etid] = 0.f;
@@ -503,16 +477,10 @@ __global__ void __launch_bounds__(Cfg<BN>::NTHREADS, 1) tc_gemm_kernel(const Gem
             if (rv) p.gates[(size_t)m * 24 + ca * 8 + hd] = er / (er + en);
           }
         } else {
-          const long long ts0 = tr_e ? clock64() : 0;
-          if (!(p.exp_shift & 64)) store_rows_coalesced(wbuf, acc, p.Out, opix, p.ldo, n0, rv, lane);     // bit 6 of the debug field: skip the stores (timing experiment)
-          if (tr_e) te_store += clock64() - ts0;
+          store_rows_coalesced(wbuf, acc, p.Out, opix, p.ldo, n0, rv, lane);
         }
       }
-      if (tr_e) te_final += clock64() - te0;
       asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");     // the staged tile is rewritten by the next tile's first drain
-    }
-    if (p.trace != nullptr && blockIdx.x == 0 && etid == 0 && wg == 0) {
-      p.trace[10] = (unsigned long long)te_final; p.trace[14] = (unsigned long long)te_store; p.trace[13] = (unsigned long long)te_pre;
     }
   }
 }

@@ -186,16 +186,6 @@ struct dawn_unet {
   int cond_dim = 0, tdim = 0;
   std::unordered_map<std::string, HostParam> raw;
   bool committed = false;
-  bool use_tc = true;                          // wgmma contraction path (DAWN_TC=0 falls back to mma.sync)
-  bool use_conv3 = true;                       // halo-tile wgmma 3x3 conv (DAWN_TC_CONV3=0 falls back to the per-tap GEMM)
-  bool use_presplit = true;                    // fp16 hi|lo pre-split of A for multi-n-tile 3x3 convs (DAWN_PRESPLIT=0: off)
-  bool use_fused_ca = true;                    // fused cross-attention gate kernel for ci <= 128 (DAWN_FUSED_CA=0: unfused)
-  bool use_fused_sla = true;                   // fused SLA context on 64-channel levels (DAWN_FUSED_SLA=0: unfused)
-  int conv3_tma = 1;                           // halo conv fed by TMA from fp16 hi|lo planes: 1 (default) = second conv of a ResBlock, whose input the
-                                               // GroupNorm/cross-attention kernel writes pre-split; 2 = every halo conv through a split pass
-                                               // (measurement only); 0 = off (DAWN_CONV3_TMA)
-  bool use_fused_ta = true;                    // fused per-pixel temporal attention on 64-channel levels (DAWN_FUSED_TA=0: unfused)
-  bool use_attn_tc = true;                     // tensor-core attention core (DAWN_ATTN_TC=0 falls back to SIMT)
 
   // packed weights
   std::vector<void*> owned;                    // weight allocations
@@ -222,11 +212,10 @@ struct dawn_unet {
   std::vector<int> lH, lW;
   float* MAPPART = nullptr;                    // k partial maps of the per-clip init conv (one per kernel row)
   int* VARY = nullptr;                         // device flag of the general entry: 1 = feature channels differ between frames
-  bool prep_v1 = false;                        // DAWN_PREP_V1=1: the original per-clip table kernels
   float *X288 = nullptr, *FEA288 = nullptr, *MAP = nullptr, *XR = nullptr, *S0 = nullptr;
   std::vector<float*> bufA, bufB, CAT, DS;
   float *Y = nullptr, *A1 = nullptr, *QKV = nullptr, *O = nullptr, *ROWSTATS = nullptr, *GATES = nullptr, *WT = nullptr;
-  float *BF = nullptr, *HF = nullptr, *HO = nullptr, *ROT = nullptr, *TSILU = nullptr, *CTX = nullptr, *KV = nullptr;
+  float *BF = nullptr, *HF = nullptr, *HO = nullptr, *ROT = nullptr, *TSILU = nullptr;
   double* STATS = nullptr; int n_stats = 0;
   int64_t* T_HOSTSIDE = nullptr;               // device int64 for forward_host
   float *H_XT = nullptr, *H_FEA = nullptr, *H_COND = nullptr, *H_OUT = nullptr;   // device staging for forward_host
@@ -289,7 +278,7 @@ inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
 // wgmma weight image of a [K][ldb] weight matrix (only for shapes the wgmma kernel accepts)
 int upload_tc_image(dawn_unet* h, const std::vector<float>& m, int K, int N, int ldb, float** img, float* scale) {
   *img = nullptr; *scale = 1.f;
-  if (!h->use_tc || N % 64 != 0 || K % 64 != 0) return 0;
+  if (N % 64 != 0 || K % 64 != 0) return 0;
   std::vector<float> im;
   tc_pack_weights(m.data(), K, N, ldb, im, scale);
   return dev_upload(h, im, img);
@@ -622,26 +611,14 @@ int Ctx::gemm(const GemmParams& p, int epi, int cat) {
   if (p.Res) bytes += 4.0 * p.M * p.N;
   if (p.Y) bytes += 4.0 * p.M * p.N;
   if (epi == EPI_CA_GATE) bytes = 4.0 * p.M * (p.Cin + 24.0);
-  if (h->use_tc && h->use_conv3 && h->conv3_tma == 2 && p.Bimg != nullptr && tc_conv3_supported(p, epi) && p.A16h == nullptr && p.lda == p.Cin) {
-    // measurement mode (DAWN_CONV3_TMA=2): every halo conv fed by TMA; the planes come from a stand-alone split pass (timed under "misc")
-    GemmParams q = p;
-    unsigned short* hi = reinterpret_cast<unsigned short*>(h->O);
-    q.A16h = hi; q.A16l = hi + (size_t)p.M * p.Cin;
-    {
-      ProfScope ps0(*this, PC_MISC, 0, 8.0 * p.M * p.Cin);
-      DAWN_TRY(launch_split_rows(p.A, p.lda, p.Cin, p.M, (void*)q.A16h, (void*)q.A16l, st));
-    }
-    ProfScope ps(*this, cat, flops, bytes);
-    return launch_tc_conv3(q, q.Bimg, st);
-  }
   ProfScope ps(*this, cat, flops, bytes);
-  if (h->use_tc && h->use_conv3 && p.Bimg != nullptr && tc_conv3_supported(p, epi)) return launch_tc_conv3(p, p.Bimg, st);
-  if (h->use_tc && p.Bimg != nullptr && tc_gemm_supported(p, epi)) {
+  if (p.Bimg != nullptr && tc_conv3_supported(p, epi)) return launch_tc_conv3(p, p.Bimg, st);
+  if (p.Bimg != nullptr && tc_gemm_supported(p, epi)) {
     // several n-tiles re-convert the same A panels (per-tap gather of the small levels' 3x3 convolutions): split once instead
     const long long in_rows = (long long)(p.M / (p.OHs * p.OWs)) * p.IH * p.IW;
     const size_t need = (size_t)in_rows * p.Cin * 4;                                   // two fp16 planes
     const size_t have = (size_t)(h->F + 2 * h->cfg.win_width) * h->lH[0] * h->lW[0] * 256 * sizeof(float);
-    if (h->use_presplit && ((p.ntaps == 9 && p.N >= 256 && !p.perm_in) || p.want_split) && p.Cin % 64 == 0 && need <= have) {
+    if (((p.ntaps == 9 && p.N >= 256 && !p.perm_in) || p.want_split) && p.Cin % 64 == 0 && need <= have) {
       GemmParams q = p;
       unsigned short* hi = reinterpret_cast<unsigned short*>(h->O);
       q.A16h = hi; q.A16l = hi + (size_t)in_rows * p.Cin;
@@ -661,8 +638,8 @@ int tap(Ctx& c, const std::string& name, const Act& a);
 int ln_gemm(Ctx& c, GemmParams& p, int epi, int cat, const float* x, int ldx, int C, int rows) {
   dawn_unet* h = c.h;
   p.ln_inline = 0; p.rowstats = h->ROWSTATS;
-  const bool tc_ok = h->use_tc && p.Bimg != nullptr && tc_gemm_supported(p, epi) && p.ntaps == 1;
-  if (tc_ok && h->use_presplit && (p.N >= 384 || (p.N == 192 && p.Cin >= 256)) && p.Cin % 64 == 0) {
+  const bool tc_ok = p.Bimg != nullptr && tc_gemm_supported(p, epi) && p.ntaps == 1;
+  if (tc_ok && (p.N >= 384 || (p.N == 192 && p.Cin >= 256)) && p.Cin % 64 == 0) {
     // N = 768 is six 128-column tiles, each re-gathering and re-splitting the same A panels: split once (cp.async producers),
     // row statistics from the stand-alone kernel
     p.want_split = 1;
@@ -713,7 +690,7 @@ int resblock(Ctx& c, const ResBlockW& r, const Act& x, const Act& out) {
   DAWN_CHECK(x.C == r.ci && out.C == r.co, "resblock channel mismatch: " + r.name);
   Act y{h->Y, r.co, r.co, x.H, x.W}, a1{h->A1, r.co, r.co, x.H, x.W};
   const double count = (double)h->sh_Fglobal * P * (r.co / 8);     // GroupNorm statistics span the WHOLE clip (U:230)
-  if (r.cond && h->use_fused_ca && r.fWq && ca_fused_supported(r.ci, P)) {
+  if (r.cond && r.fWq && ca_fused_supported(r.ci, P)) {
     CaFusedArgs a{};
     a.x = x.p; a.ldx = x.ld; a.F = F; a.P = P; a.Wq = r.fWq; a.inv_wscale = r.f_inv_wscale;
     a.kq = r.kq; a.nkq = r.nkq; a.G = r.G; a.Wt = h->WT;
@@ -733,7 +710,7 @@ int resblock(Ctx& c, const ResBlockW& r, const Act& x, const Act& out) {
   // a1 is consumed by the second conv only: when that conv runs on the halo-tile wgmma kernel, a1 is written as two fp16 planes
   // (hi | lo, the same bytes as the fp32 row) and the conv fetches its tiles by TMA
   const unsigned short *a1h = nullptr, *a1l = nullptr;
-  if (r.cond && h->use_fused_ca && gn_hcond_supported(r.co, P) && h->conv3_tma >= 1 && h->use_tc && h->use_conv3 && r.c2.img != nullptr) {
+  if (r.cond && gn_hcond_supported(r.co, P) && r.c2.img != nullptr) {
     GemmParams q; base_params(q, a1, F);
     set_weights(q, r.c2); set_square_taps(q, 3, 1);
     q.Out = y.p; q.ldo = y.ld; q.stats = h->STATS + 16 * r.st2; q.cpg = r.co / 8;
@@ -742,7 +719,7 @@ int resblock(Ctx& c, const ResBlockW& r, const Act& x, const Act& out) {
       a1l = a1h + (size_t)M * r.co;
     }
   }
-  if (r.cond && h->use_fused_ca && gn_hcond_supported(r.co, P)) {
+  if (r.cond && gn_hcond_supported(r.co, P)) {
     GnHcondArgs a{};
     a.Wt = h->WT; a.T = r.T; a.ldbT = r.ldbT; a.Y = y.p; a.ldy = y.ld; a.Out = a1.p; a.ldo = a1.ld;
     a.Out16h = const_cast<unsigned short*>(a1h); a.Out16l = const_cast<unsigned short*>(a1l);
@@ -818,7 +795,7 @@ int temporal_attn(Ctx& c, const AttnW& w, const Act& x, const Act& dst, const st
     DAWN_NCCL_OK(g_nccl.GroupEnd());
     xe = Act{h->XE, x.C, x.C, x.H, x.W};
   }
-  const bool fused_ok = h->use_fused_ta && w.fq && temporal_fused_supported(x.C, Fe, h->cfg.win_width, hl, hl + F);
+  const bool fused_ok = w.fq && temporal_fused_supported(x.C, Fe, h->cfg.win_width, hl, hl + F);
   if (fused_ok) {
     TemporalFusedArgs a{};
     a.x = xe.p; a.ldx = xe.ld; a.res = x.p; a.ldr = x.ld; a.out = dst.p; a.ldo = dst.ld;
@@ -850,7 +827,7 @@ int temporal_attn(Ctx& c, const AttnW& w, const Act& x, const Act& dst, const st
     double pairs = 0;
     for (int i = hl; i < hl + F; ++i) pairs += std::min(Fe - 1, i + a.band) - std::max(0, i - a.band) + 1;
     ProfScope ps(c, PC_ATTN_CORE, 4.0 * 32 * 8 * P * pairs, 4.0 * Me * 1024);
-    if (h->use_attn_tc && attention_tc_supported(a)) DAWN_TRY(launch_attention_tc(a, c.st));
+    if (attention_tc_supported(a)) DAWN_TRY(launch_attention_tc(a, c.st));
     else DAWN_TRY(launch_attention(a, c.st));
   }
   {
@@ -882,7 +859,7 @@ int mid_spatial_attn(Ctx& c, const AttnW& w, const Act& x, const std::string& na
     a.nseq = F; a.L = P; a.seq_base_stride = P; a.elem_stride = 1;
     a.band = 1 << 30; a.bias = nullptr; a.q_lo = 0; a.q_hi = P;
     ProfScope ps(c, PC_ATTN_CORE, 4.0 * 32 * 8 * (double)F * P * P, 4.0 * M * 1024);
-    if (h->use_attn_tc && attention_tc_supported(a)) DAWN_TRY(launch_attention_tc(a, c.st));
+    if (attention_tc_supported(a)) DAWN_TRY(launch_attention_tc(a, c.st));
     else DAWN_TRY(launch_attention(a, c.st));
   }
   {
@@ -900,7 +877,7 @@ int sla(Ctx& c, const SlaW& w, const Act& x, const std::string& name) {
   dawn_unet* h = c.h;
   const int F = h->F, P = x.H * x.W, M = F * P;
   const int ldb = round_up(x.C, 64);
-  const bool fused = h->use_fused_sla && w.fkv && sla_fused_supported(x.C, P) &&
+  const bool fused = w.fkv && sla_fused_supported(x.C, P) &&
                      sla_fused_part_floats(F, P) <= (size_t)(F + 2 * h->cfg.win_width) * h->lH[0] * h->lW[0] * 256;
   const int qld = fused ? 256 : 768;
   if (fused) {
@@ -955,7 +932,7 @@ int downsample(Ctx& c, const ConvW& w, const Act& x, const Act& out, const std::
 }
 
 int upsample(Ctx& c, const UpW& u, const Act& x, const Act& out, const std::string& name) {       // U:165-167
-  if (c.h->use_tc && c.h->use_conv3 && u.all.img != nullptr) {
+  if (u.all.img != nullptr) {
     GemmParams p; base_params(p, x, c.h->F);
     set_weights(p, u.all); set_square_taps(p, 3, 1);
     p.up2 = 1; p.Out = out.p; p.ldo = out.ld;
@@ -996,30 +973,13 @@ int tap(Ctx& c, const std::string& name, const Act& a) {
 }
 
 // ------------------------------------------------------------------------------------------ per-clip tables
+// three launches for all (conditioned block, cross-attention) pairs
 int prep_cond(dawn_unet* h, const float* cond, cudaStream_t st) {
-  const int F = h->F;
+  if (h->n_cond == 0) return 0;                  // a grid dimension of 0 is a launch error
   Ctx c{h, st};
-  if (h->n_cond > 0 && !h->prof_on) {
-    // three launches for all (block, cross-attention) pairs; the per-pair path below is kept for profiling
-    h->launches += 3;
-    return launch_cond_batched(cond, h->cond_dim, h->cond_descs, h->n_cond, h->cond_max_n1, h->cond_max_k, h->cond_max_co, F, st);
-  }
-  const int off[3] = {h->cfg.cond_aud, 0, h->cfg.cond_aud + h->cfg.cond_pose};          // pose, aud, eye slices (U:425-428)
-  const int kd[3] = {h->cfg.cond_pose, h->cfg.cond_aud, h->cfg.cond_eye};
-  for (auto& r : h->rb) {
-    if (!r.cond) continue;
-    for (int a = 0; a < 3; ++a) {
-      ProfScope ps(c, PC_PREP, 0, 0);
-      h->launches += 2;
-      DAWN_TRY(launch_cond_mlp(cond, h->cond_dim, off[a], kd[a], r.mW[a], r.mB[a], 2 * r.co, F, h->CTX, st));
-      DAWN_TRY(launch_linear_nobias(h->CTX, 2 * r.co, r.ca[a].Wkv, 128, F, h->KV, st));
-      CaTableArgs t{};
-      t.kv = h->KV; t.nkv = r.ca[a].nkv; t.qs = r.ca[a].qs; t.ks = r.ca[a].ks; t.Wout = r.ca[a].Wout; t.gout = r.ca[a].gout;
-      t.co = r.co; t.ldbT = r.ldbT; t.ca = a; t.kq = r.kq; t.nkq = r.nkq; t.T = r.T; t.G = r.G;
-      DAWN_TRY(launch_ca_tables(t, F, st));
-    }
-  }
-  return 0;
+  ProfScope ps(c, PC_PREP, 0, 0);
+  h->launches += 2;
+  return launch_cond_batched(cond, h->cond_dim, h->cond_descs, h->n_cond, h->cond_max_n1, h->cond_max_k, h->cond_max_co, h->F, st);
 }
 
 // Per-clip constant part of the init conv (SURVEY a2) from ONE frame of the feature channels (fea: channel c at
@@ -1158,15 +1118,6 @@ int dawn_unet_create(const dawn_unet_cfg* cfg, dawn_unet** out) {
   DAWN_CHECK(cfg->win_width >= 1 && cfg->win_width <= 120, "win_width out of range");
   dawn_unet* h = new dawn_unet();
   h->cfg = *cfg;
-  { const char* e = getenv("DAWN_TC"); h->use_tc = !(e && e[0] == '0'); }
-  { const char* e = getenv("DAWN_ATTN_TC"); h->use_attn_tc = !(e && e[0] == '0'); }
-  { const char* e = getenv("DAWN_FUSED_TA"); h->use_fused_ta = !(e && e[0] == '0'); }
-  { const char* e = getenv("DAWN_CONV3_TMA"); h->conv3_tma = (e && e[0] >= '0' && e[0] <= '2') ? e[0] - '0' : 1; }
-  { const char* e = getenv("DAWN_FUSED_SLA"); h->use_fused_sla = !(e && e[0] == '0'); }
-  { const char* e = getenv("DAWN_FUSED_CA"); h->use_fused_ca = !(e && e[0] == '0'); }
-  { const char* e = getenv("DAWN_PRESPLIT"); h->use_presplit = !(e && e[0] == '0'); }
-  { const char* e = getenv("DAWN_TC_CONV3"); h->use_conv3 = !(e && e[0] == '0'); }
-  { const char* e = getenv("DAWN_PREP_V1"); h->prep_v1 = (e && e[0] == '1'); }
   h->nlev = cfg->n_levels;
   h->dims.push_back(cfg->dim);
   for (int i = 0; i < cfg->n_levels; ++i) h->dims.push_back(cfg->dim * cfg->dim_mults[i]);
@@ -1330,8 +1281,6 @@ int dawn_unet_set_num_frames(dawn_unet* h, int F, int height, int width) {
   DAWN_TRY(dev_alloc(own, M0 * dim, &h->HO, cnt));
   DAWN_TRY(dev_alloc(own, (size_t)(F + 2 * h->cfg.win_width) * 32, &h->ROT, cnt));
   DAWN_TRY(dev_alloc(own, h->tdim, &h->TSILU, cnt));
-  DAWN_TRY(dev_alloc(own, (size_t)F * 2048, &h->CTX, cnt));
-  DAWN_TRY(dev_alloc(own, (size_t)F * 128, &h->KV, cnt));
   {
     float* s; DAWN_TRY(dev_alloc(own, (size_t)h->n_stats * 32, &s, cnt)); h->STATS = (double*)s;
     float* t; DAWN_TRY(dev_alloc(own, 4, &t, cnt)); h->T_HOSTSIDE = (int64_t*)t;
@@ -1392,24 +1341,8 @@ int dawn_unet_set_clip_invariants(dawn_unet* h, const float* fea, const float* c
   DAWN_CHECK(h && fea && cond, "null argument");
   DAWN_CHECK(h->F > 0, "set_num_frames must precede set_clip_invariants");
   cudaStream_t st = (cudaStream_t)stream;
-  Ctx c{h, st};
-  const int H0 = h->lH[0], W0 = h->lW[0], dim = h->cfg.dim, k = h->cfg.init_kernel_size;
   // per-clip constant part of the init conv: conv(cat[0, fea]) + bias  (linearity; SURVEY a2)
-  if (!h->prep_v1) {
-    DAWN_TRY(init_map(h, fea, (long long)H0 * W0, st, nullptr, 0));
-  } else {
-  {
-    ProfScope ps(c, PC_PREP, 0, 0);
-    DAWN_TRY(launch_ncf_to_nhwc(fea, h->cfg.channels - 3, 1, H0 * W0, h->cin_pad, 3, h->FEA288, st));
-  }
-  {
-    Act in{h->FEA288, h->cin_pad, h->cin_pad, H0, W0};
-    GemmParams p; base_params(p, in, 1);
-    set_weights(p, h->init_full); set_square_taps(p, k, k / 2);
-    p.Out = h->MAP; p.ldo = dim;
-    DAWN_TRY(c.gemm(p, EPI_PLAIN, PC_PREP));
-  }
-  }
+  DAWN_TRY(init_map(h, fea, (long long)h->lH[0] * h->lW[0], st, nullptr, 0));
   DAWN_TRY(prep_cond(h, cond, st));
   h->have_invariants = true;
   return 0;
@@ -1427,11 +1360,10 @@ int dawn_unet_forward(dawn_unet* h, const float* x, const int64_t* t, const floa
   // Path selection on the device, no host synchronisation: one pass over x decides whether channels 3.. are the same in every
   // frame (the reference's sampler tiles them, U:1167); both paths are enqueued and the kernels of the one not taken return
   // at once.  invariant -> hoisted init conv (map from frame 0 + 3 live channels); varying -> full k x k conv over all channels.
-  const int* vary = nullptr;
-  if (!h->prep_v1) {
+  const int* vary = h->VARY;
+  {
     ProfScope ps(c, PC_MISC, 0, 4.0 * h->F * H0 * W0 * h->cfg.channels);
     DAWN_TRY(launch_frame_invariance(x, 3, h->cfg.channels, h->F, H0 * W0, h->VARY, st));
-    vary = h->VARY;
   }
   {
     ProfScope ps(c, PC_MISC, 0, 8.0 * h->F * H0 * W0 * h->cin_pad);
@@ -1446,8 +1378,8 @@ int dawn_unet_forward(dawn_unet* h, const float* x, const int64_t* t, const floa
     ProfScope ps(c, PC_CONV_OTHER, 2.0 * p.M * (double)p.N * p.K, 4.0 * p.M * ((double)p.Cin + p.N));
     DAWN_TRY(launch_gemm(p, EPI_PLAIN, st));      // Cin = 288 is not a wgmma-kernel shape: always the mma.sync kernel (it has the skip flag)
   }
-  if (vary) {
-    DAWN_TRY(init_map(h, x + (size_t)3 * h->F * H0 * W0, (long long)h->F * H0 * W0, st, vary, 1));
+  DAWN_TRY(init_map(h, x + (size_t)3 * h->F * H0 * W0, (long long)h->F * H0 * W0, st, vary, 1));
+  {
     const double k2 = (double)k * k;
     ProfScope ps(c, PC_MISC, 2.0 * h->F * H0 * W0 * dim * 3 * k2, 4.0 * h->F * H0 * W0 * (dim + 3));
     DAWN_TRY(launch_init_conv_x3(x, h->F, H0, W0, h->init_w3, h->MAP, dim, h->XR + dim, 2 * dim, k, st, vary, 1));
@@ -1728,86 +1660,6 @@ int dawn_selftest_attention(int nseq, int L, int temporal, float* max_abs_diff, 
     *max_abs_diff = md; *max_abs_ref = mr;
   }
   free_all(own);
-  return rc;
-}
-
-// random k x k conv through both contraction kernels; reports max |wgmma - mma.sync| over outputs and GN statistics
-int dawn_selftest_tc_gemm(int F, int H, int W, int Cin, int N, int ksize, int with_stats, float* max_abs_diff, float* max_abs_ref) {
-  DAWN_CHECK(max_abs_diff && max_abs_ref, "null argument");
-  const int M = F * H * W, K = ksize * ksize * Cin, ldb = round_up(N, 64);
-  std::vector<float> hA((size_t)M * Cin), hB((size_t)K * ldb, 0.f), hb(ldb, 0.f);
-  uint32_t seed = 12345u;
-  auto rnd = [&]() { seed = seed * 1664525u + 1013904223u; return ((seed >> 8) & 0xFFFF) / 32768.0f - 1.0f; };
-  for (auto& v : hA) v = rnd();
-  for (int k = 0; k < K; ++k) for (int n = 0; n < N; ++n) hB[(size_t)k * ldb + n] = rnd() * 0.05f;
-  for (int n = 0; n < N; ++n) hb[n] = rnd();
-  std::vector<float> img;
-  float img_scale = 1.f;
-  tc_pack_weights(hB.data(), K, N, ldb, img, &img_scale);
-  std::vector<void*> own;
-  float *dA, *dB, *db, *dImg, *dO1, *dO2, *dS;
-  auto cleanup = [&]() { free_all(own); };
-  if (dev_alloc(own, hA.size(), &dA) || dev_alloc(own, hB.size(), &dB) || dev_alloc(own, hb.size(), &db) ||
-      dev_alloc(own, img.size(), &dImg) || dev_alloc(own, (size_t)M * N, &dO1) || dev_alloc(own, (size_t)M * N, &dO2) ||
-      dev_alloc(own, 64, &dS)) { cleanup(); return -2; }
-  cudaMemcpy(dA, hA.data(), hA.size() * 4, cudaMemcpyHostToDevice);
-  cudaMemcpy(dB, hB.data(), hB.size() * 4, cudaMemcpyHostToDevice);
-  cudaMemcpy(db, hb.data(), hb.size() * 4, cudaMemcpyHostToDevice);
-  cudaMemcpy(dImg, img.data(), img.size() * 4, cudaMemcpyHostToDevice);
-  cudaMemset(dS, 0, 64 * 4);
-  Act in{dA, Cin, Cin, H, W};
-  GemmParams p; base_params(p, in, F);
-  p.B = dB; p.Bimg = dImg; p.tc_scale = 1.0f / (kTcActScale * img_scale); p.ldb = ldb; p.N = N; p.K = K; p.bias = db;
-  set_square_taps(p, ksize, ksize / 2);
-  if (with_stats) { p.stats = (double*)dS; p.cpg = N / 8; }
-  p.Out = dO1; p.ldo = N;
-  int rc = launch_gemm(p, EPI_PLAIN, 0);
-  if (rc == 0) {
-    if (with_stats) p.stats = (double*)dS + 16;
-    p.Out = dO2;
-    if (!tc_gemm_supported(p, EPI_PLAIN)) { cleanup(); set_last_error("selftest: shape not supported by tc_gemm"); return -1; }
-    if (getenv("DAWN_TC_SHIFT")) p.exp_shift = atoi(getenv("DAWN_TC_SHIFT"));
-    unsigned long long* dT = nullptr;
-    if (getenv("DAWN_TC_TRACE")) {
-      float* t; if (dev_alloc(own, 64, &t)) { cleanup(); return -2; }
-      cudaMemset(t, 0, 256); dT = (unsigned long long*)t; p.trace = dT;
-    }
-    if (getenv("DAWN_SELFTEST_CONV3") && tc_conv3_supported(p, EPI_PLAIN)) { rc = launch_tc_conv3(p, dImg, 0); printf("  (halo-tile conv3 kernel)\n"); }
-    else rc = launch_tc_gemm(p, dImg, EPI_PLAIN, 0);
-    if (rc == 0 && dT) {
-      unsigned long long tr[16];
-      cudaMemcpy(tr, dT, sizeof(tr), cudaMemcpyDeviceToHost);
-      const double n = (double)std::max<unsigned long long>(tr[1], 1);
-      printf("  trace (CTA 0, cycles/stage over %llu stages): total %.0f | MMA thread: wait acc_free %.0f, wait A %.0f, wait B %.0f, issue+commit %.0f | "
-             "producer t0: load issue %.0f, wait slot %.0f, split+store %.0f | loader wait slot %.0f | epilogue t0: wait acc_full %.0f, drain %.0f, final epilogue %.0f "
-             "(scale+bias %.0f, store %.0f)%s\n",
-             tr[1], tr[0] / n, tr[2] / n, tr[3] / n, tr[4] / n, tr[5] / n, tr[11] / n, tr[6] / n, tr[7] / n, tr[8] / n, tr[9] / n, tr[12] / n, tr[10] / n,
-             tr[13] / n, tr[14] / n, (p.exp_shift & 64) ? "  [stores SKIPPED]" : "");
-    }
-  }
-  if (rc == 0 && cudaDeviceSynchronize() != cudaSuccess) { set_last_error(std::string("selftest: ") + cudaGetErrorString(cudaGetLastError())); rc = -2; }
-  if (rc == 0) {
-    std::vector<float> o1((size_t)M * N), o2((size_t)M * N);
-    cudaMemcpy(o1.data(), dO1, o1.size() * 4, cudaMemcpyDeviceToHost);
-    cudaMemcpy(o2.data(), dO2, o2.size() * 4, cudaMemcpyDeviceToHost);
-    float md = 0.f, mr = 0.f;
-    // a NaN difference must win the max (std::max keeps its first argument when the comparison is false)
-    for (size_t i = 0; i < o1.size(); ++i) {
-      const float d = std::fabs(o1[i] - o2[i]);
-      md = (d > md || d != d) ? d : md;
-      mr = std::max(mr, std::fabs(o1[i]));
-    }
-    if (with_stats) {
-      double st[32];
-      cudaMemcpy(st, dS, sizeof(st), cudaMemcpyDeviceToHost);
-      for (int i = 0; i < 16; ++i) {
-        const float d = (float)(std::fabs(st[i] - st[16 + i]) / std::max(1.0, std::fabs(st[i])));
-        md = (d > md || d != d) ? d : md;
-      }
-    }
-    *max_abs_diff = md; *max_abs_ref = mr;
-  }
-  cleanup();
   return rc;
 }
 

@@ -137,10 +137,6 @@ int dawn_unet_sampler_capture(dawn_unet* h, float* x, float* eps, const float* n
                               const float* coef, int nsteps, float q, void* scratch);
 int dawn_unet_sampler_launch(dawn_unet* h, void* stream);
 
-/* self-test of the wgmma contraction kernel against the mma.sync kernel on a random k x k convolution
- * (F frames of H x W, Cin -> N channels); reports max |difference| (outputs and, if requested, GroupNorm sums). */
-int dawn_selftest_tc_gemm(int F, int H, int W, int Cin, int N, int ksize, int with_stats, float* max_abs_diff, float* max_abs_ref);
-
 /* One contraction through exactly one kernel path, for per-kernel tests against a high-precision reference.
  * Out[m, n] = epilogue( sum_{tap, c} A[pixel(m, tap), c] * B[tap*Cin + c, n] ) with the product's GemmParams semantics
  * (dawn_pytorch_b200/csrc/gemm.cuh): rows m = (f, i, j) over an F x OHs x OWs output sub-grid (M = F*OHs*OWs), input pixel
