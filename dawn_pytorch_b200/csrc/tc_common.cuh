@@ -2,6 +2,7 @@
 // shared-memory matrix descriptors, the fp16 hi/lo split and the coalesced row store.
 #pragma once
 #include <cuda_fp16.h>
+#include <type_traits>
 #include "common.cuh"
 
 namespace dawn {
@@ -9,6 +10,29 @@ namespace tc {
 
 // ---------------------------------------------------------------- PTX wrappers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+
+// The dynamic shared-memory base rounded up to 1024 bytes (the 128-byte swizzle repeats every 1024 B).  Offsetting the
+// __shared__ pointer itself keeps its address space visible to the compiler, so stores through it compile to STS; a
+// round trip through uintptr_t turned them into generic stores.
+__device__ __forceinline__ uint8_t* smem_align1024(uint8_t* base) { return base + ((1024u - (smem_u32(base) & 1023u)) & 1023u); }
+
+// Per-warpgroup register budgets (all four warps of the warpgroup execute the same instruction).  The kernel launches with
+// the even split its __launch_bounds__ allows; .dec may only lower a warp's count and returns the rest to the CTA's pool, .inc
+// may only raise it and waits until the pool holds enough.  ptxas allocates the code after each instruction within its budget.
+template <uint32_t R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <uint32_t R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+
+// f(integral_constant<int, I>) for I = 0 .. N-1, expanded at compile time: the MMA loops below branch only on constants,
+// so no runtime control-flow merge carries accumulator registers that a wgmma may still be writing
+template <int I, int N, class F>
+__device__ __forceinline__ void static_for(F&& f) {
+  if constexpr (I < N) {
+    f(std::integral_constant<int, I>{});
+    static_for<I + 1, N>(f);
+  }
+}
 
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));

@@ -7,8 +7,17 @@
 // may start at any 128-byte row and use any row-multiple stride between its 8-row groups:
 //     window(dy,dx): start = halo + ((dy+1)*10 + (dx+1))*128 B,  stride between 8-pixel rows (SBO) = 10*128 B.
 // Everything else follows tc_gemm.cu: FP16x3 split precision, register accumulators drained into an RN fp32 tile in shared
-// memory (once per 64-channel chunk), persistent warp-specialised CTA (8 producer warps, 1/2 consumer warpgroups, weight
-// loader), row-per-thread epilogue with bias + GroupNorm partial statistics.
+// memory (every 9, 3 or 1 taps), row-per-thread epilogue with bias + GroupNorm partial statistics.
+//
+// Persistent warp-specialised CTA of whole warpgroups, each with its own register budget (setmaxnreg, see CCfg):
+//   * warpgroups 0-1: A producers (gather + split + swizzled store of the halo tile), or one TMA thread;
+//   * BN = 64: one MMA warpgroup and one epilogue warpgroup.  The MMA warpgroup drains tile t into staging tile t & 1, signals
+//     the epilogue warpgroup through an mbarrier and goes on with tile t+1; before its first drain into a staging tile it waits
+//     until the epilogue has released that tile.  The tensor cores keep working while the epilogue of the previous tile runs;
+//   * BN = 128: two warpgroups, each issuing the MMAs of 64 columns and then running their epilogue from their own staging tile;
+//   * last warpgroup: the weight loader (one thread; the other three warps exit).
+// The taps of a chunk are expanded at compile time for each drain interval, so the only wgmma waits are wait_group 1 between
+// taps (one tap's MMAs stay in flight while the next tap is issued) and wait_group 0 before a drain.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cstdlib>
@@ -32,19 +41,33 @@ constexpr int HROWS = HH * HW;                 // 180 halo pixels = 180 rows of 
 constexpr int A_HALO = 23 * 1024;              // 180 * 128 = 23040 B, padded to 23 KB (keeps 1024-byte alignment)
 constexpr int NPROD = 256;
 
-// B stages: what fits in 227 KB next to the halo stages and the consumers' 128 x 64 fp32 staging tiles (34 KB each)
+// B stages: what fits in 227 KB next to the halo stages and two 128 x 64 fp32 staging tiles (34 KB each).
+// BN = 64: one MMA warpgroup and one epilogue warpgroup; the staging tiles are a double buffer between them, so the epilogue
+// of tile t runs while the MMAs of tile t+1 are issued.  BN = 128: two warpgroups, each issuing the MMAs of 64 columns and
+// then running their epilogue from its own staging tile.
+// Warpgroups: 0-1 A producers | MMA (| epilogue) | weight loader.  Registers per thread: every warp starts with the 96 that 640
+// threads allow, and setmaxnreg.inc can only take what other warpgroups of the CTA released.  The producers keep 96, the loader
+// gives 72 back and the MMA and epilogue warpgroups take them (5 x 96 = 480 at launch):
+//   BN =  64: 2 x 96 + 24 + 136 + 128 = 480        BN = 128: 2 x 96 + 24 + 2 x 128 = 472
 template <int BN>
 struct CCfg {
-  static constexpr int NWG = BN / 64;
+  static constexpr int NWG = BN / 64;                          // MMA warpgroups (64 output columns each)
+  static constexpr bool SPLIT_EPI = (BN == 64);                // separate epilogue warpgroup
   static constexpr int B_PANEL = BN * 128;                     // one (tap, chunk) weight panel, hi or lo
   static constexpr int A_STAGES = 2;
   static constexpr int B_STAGES = (BN == 64) ? 4 : 2;
   static constexpr int A_BYTES = A_STAGES * 2 * A_HALO;        // hi + lo
   static constexpr int B_BYTES = B_STAGES * 2 * B_PANEL;
-  static constexpr int ACC_STAGE = NWG * 128 * kStageLd * 4;
+  static constexpr int ACC_STAGE = 2 * 128 * kStageLd * 4;
   static constexpr int SMEM_DYN = A_BYTES + B_BYTES + ACC_STAGE + 1024;
-  static constexpr int NTHREADS = NPROD + 128 * NWG + 32;      // producers | consumers | loader warp
-  static constexpr int LOAD_WARP = (NPROD + 128 * NWG) / 32;
+  static constexpr int EPI_WARP = NPROD / 32 + 4 * NWG;        // first warp of the epilogue warpgroup (SPLIT_EPI)
+  static constexpr int LOAD_WARP = EPI_WARP + (SPLIT_EPI ? 4 : 0);
+  static constexpr int NTHREADS = 32 * LOAD_WARP + 128;        // the weight loader is a whole warpgroup (one thread works)
+  static constexpr uint32_t REG_LAUNCH = (65536 / NTHREADS) & ~7u;   // what ptxas allots each thread at launch (__launch_bounds__)
+  static constexpr uint32_t REG_LOAD = 24, REG_MMA = SPLIT_EPI ? 136 : 128, REG_EPI = 128;
+  // setmaxnreg.dec may only lower a warp's count and setmaxnreg.inc only raise it
+  static_assert(REG_LOAD < REG_LAUNCH && REG_MMA > REG_LAUNCH && REG_EPI > REG_LAUNCH, "register budgets");
+  static_assert(2 * REG_LAUNCH + REG_LOAD + NWG * REG_MMA + (SPLIT_EPI ? REG_EPI : 0) <= NTHREADS / 128 * REG_LAUNCH, "CTA register pool");
 };
 
 // A-operand source: TMA = false: fp32 activations, gathered / split / swizzled by the 8 producer warps.  TMA = true: the activation exists as
@@ -58,23 +81,25 @@ __global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const G
                                                                           const __grid_constant__ CUtensorMap tm_lo) {
   using C = CCfg<BN>;
   constexpr int B_PANEL = C::B_PANEL, A_STAGES = C::A_STAGES, B_STAGES = C::B_STAGES, NWG = C::NWG;
-  constexpr int LOAD_WARP = C::LOAD_WARP;
+  constexpr bool SPLIT = C::SPLIT_EPI;
   extern __shared__ uint8_t smem_raw[];
   __shared__ uint64_t a_full[A_STAGES], a_free[A_STAGES], b_full[B_STAGES], b_free[B_STAGES];
+  __shared__ uint64_t st_full[2], st_free[2];           // SPLIT: staging tile b handed from the MMA warpgroup to the epilogue and back
   __shared__ float s_stat[NWG][16];
   __shared__ __align__(16) float s_bias[NWG][64];       // bias of this epilogue warpgroup's 64 columns (single n-tile: constant for the whole launch)
 
   const int tid = threadIdx.x, lane = tid & 31;
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);          // warp-uniform by construction
-  uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+  uint8_t* smem = smem_align1024(smem_raw);
   uint8_t* smemA = smem;
   uint8_t* smemB = smem + C::A_BYTES;
-  uint8_t* smemE = smemB + C::B_BYTES;
+  float* stage_base = reinterpret_cast<float*>(smemB + C::B_BYTES);   // two [128][kStageLd] fp32 staging tiles
 
   if (tid == 0) {
-    // a_free / b_free: one arrive per consumer warp once its MMAs on the slot have completed
+    // a_free / b_free: one arrive per MMA warp once its MMAs on the slot have completed; st_full / st_free: one arrive per thread
     for (int s = 0; s < A_STAGES; ++s) { mbar_init(&a_full[s], TMA ? 1 : NPROD); mbar_init(&a_free[s], 4 * NWG); }
     for (int s = 0; s < B_STAGES; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_free[s], 4 * NWG); }
+    for (int s = 0; s < 2; ++s) { mbar_init(&st_full[s], 128); mbar_init(&st_free[s], 128); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -92,78 +117,83 @@ __global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const G
     y0 = (r / tiles_x) * TH; x0 = (r % tiles_x) * TW;
   };
 
-  if (TMA && warp < 8) {
-    // =============================================================== TMA producer: one thread, two tensor loads per (tile, chunk)
-    if (tid == 0) {
-      const uint64_t mh = reinterpret_cast<uint64_t>(&tm_hi), ml = reinterpret_cast<uint64_t>(&tm_lo);
+  if (warp < 8) {                                              // keeps the launch register budget
+    if (TMA) {
+      // ============================================================= TMA producer: one thread, two tensor loads per (tile, chunk)
+      if (tid == 0) {
+        const uint64_t mh = reinterpret_cast<uint64_t>(&tm_hi), ml = reinterpret_cast<uint64_t>(&tm_lo);
+        uint32_t ait = 0;
+        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+          int f, y0, x0, nt;
+          decode(tile, f, y0, x0, nt);
+          for (int cc = 0; cc < NCH; ++cc, ++ait) {
+            const int s = ait % A_STAGES;
+            mbar_wait(&a_free[s], ((ait / A_STAGES) & 1) ^ 1);
+            mbar_arrive_expect_tx(&a_full[s], 2 * HROWS * 128);
+            const uint32_t dst = smem_u32(smemA + s * 2 * A_HALO), bar = smem_u32(&a_full[s]);
+            const int c0 = cc * 64, c1 = x0 - 1, c2 = y0 - 1;
+            asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
+                         ::"r"(dst), "l"(mh), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(f) : "memory");
+            asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
+                         ::"r"(dst + A_HALO), "l"(ml), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(f) : "memory");
+          }
+        }
+      }
+    } else {
+      // ============================================================= producers: halo tile of one 64-channel chunk
+      const int c16 = tid & 7;
+      const int r0 = tid >> 3;                                 // halo rows r0 + 32 q, q = 0..5 (< 180)
       uint32_t ait = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         int f, y0, x0, nt;
         decode(tile, f, y0, x0, nt);
+        const float* img = p.A + (size_t)f * H * W * p.lda;
         for (int cc = 0; cc < NCH; ++cc, ++ait) {
           const int s = ait % A_STAGES;
-          mbar_wait(&a_free[s], ((ait / A_STAGES) & 1) ^ 1);
-          mbar_arrive_expect_tx(&a_full[s], 2 * HROWS * 128);
-          const uint32_t dst = smem_u32(smemA + s * 2 * A_HALO), bar = smem_u32(&a_full[s]);
-          const int c0 = cc * 64, c1 = x0 - 1, c2 = y0 - 1;
-          asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-                       ::"r"(dst), "l"(mh), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(f) : "memory");
-          asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-                       ::"r"(dst + A_HALO), "l"(ml), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(f) : "memory");
+          const uint32_t round = ait / A_STAGES;
+          float4 v[12];
+#pragma unroll
+          for (int q = 0; q < 6; ++q) {
+            const int r = r0 + 32 * q;
+            const int hy = r / HW, hx = r - hy * HW;
+            const int iy = y0 + hy - 1, ix = x0 + hx - 1;
+            const bool ok = (r < HROWS) && (iy >= 0) && (iy < H) && (ix >= 0) && (ix < W);
+            if (ok) {
+              const float4* src = reinterpret_cast<const float4*>(img + (size_t)(iy * W + ix) * p.lda + cc * 64) + 2 * c16;
+              v[2 * q] = __ldg(src);
+              v[2 * q + 1] = __ldg(src + 1);
+            } else {
+              v[2 * q] = make_float4(0.f, 0.f, 0.f, 0.f);
+              v[2 * q + 1] = make_float4(0.f, 0.f, 0.f, 0.f);
+            }
+          }
+          mbar_wait(&a_free[s], (round & 1) ^ 1);
+          uint8_t* a_hi = smemA + s * 2 * A_HALO;
+          uint8_t* a_lo = a_hi + A_HALO;
+#pragma unroll
+          for (int q = 0; q < 6; ++q) {
+            const int r = r0 + 32 * q;
+            if (r < HROWS) {
+              uint32_t h[4], l[4];
+              split_f16x2(v[2 * q].x, v[2 * q].y, h[0], l[0]);
+              split_f16x2(v[2 * q].z, v[2 * q].w, h[1], l[1]);
+              split_f16x2(v[2 * q + 1].x, v[2 * q + 1].y, h[2], l[2]);
+              split_f16x2(v[2 * q + 1].z, v[2 * q + 1].w, h[3], l[3]);
+              const uint32_t off = swz(r, c16);                // absolute-row swizzle (halo base is 1024-byte aligned)
+              *reinterpret_cast<uint4*>(a_hi + off) = make_uint4(h[0], h[1], h[2], h[3]);
+              *reinterpret_cast<uint4*>(a_lo + off) = make_uint4(l[0], l[1], l[2], l[3]);
+            }
+          }
+          mbar_arrive_relaxed(&a_full[s]);                     // proxy fence runs on the consumer side (see tc_gemm.cu)
         }
       }
     }
-  } else if (warp < 8) {
-    // =============================================================== producers: halo tile of one 64-channel chunk
-    const int c16 = tid & 7;
-    const int r0 = tid >> 3;                                   // halo rows r0 + 32 q, q = 0..5 (< 180)
-    uint32_t ait = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      int f, y0, x0, nt;
-      decode(tile, f, y0, x0, nt);
-      const float* img = p.A + (size_t)f * H * W * p.lda;
-      for (int cc = 0; cc < NCH; ++cc, ++ait) {
-        const int s = ait % A_STAGES;
-        const uint32_t round = ait / A_STAGES;
-        float4 v[12];
-#pragma unroll
-        for (int q = 0; q < 6; ++q) {
-          const int r = r0 + 32 * q;
-          const int hy = r / HW, hx = r - hy * HW;
-          const int iy = y0 + hy - 1, ix = x0 + hx - 1;
-          const bool ok = (r < HROWS) && (iy >= 0) && (iy < H) && (ix >= 0) && (ix < W);
-          if (ok) {
-            const float4* src = reinterpret_cast<const float4*>(img + (size_t)(iy * W + ix) * p.lda + cc * 64) + 2 * c16;
-            v[2 * q] = __ldg(src);
-            v[2 * q + 1] = __ldg(src + 1);
-          } else {
-            v[2 * q] = make_float4(0.f, 0.f, 0.f, 0.f);
-            v[2 * q + 1] = make_float4(0.f, 0.f, 0.f, 0.f);
-          }
-        }
-        mbar_wait(&a_free[s], (round & 1) ^ 1);
-        uint8_t* a_hi = smemA + s * 2 * A_HALO;
-        uint8_t* a_lo = a_hi + A_HALO;
-#pragma unroll
-        for (int q = 0; q < 6; ++q) {
-          const int r = r0 + 32 * q;
-          if (r < HROWS) {
-            uint32_t h[4], l[4];
-            split_f16x2(v[2 * q].x, v[2 * q].y, h[0], l[0]);
-            split_f16x2(v[2 * q].z, v[2 * q].w, h[1], l[1]);
-            split_f16x2(v[2 * q + 1].x, v[2 * q + 1].y, h[2], l[2]);
-            split_f16x2(v[2 * q + 1].z, v[2 * q + 1].w, h[3], l[3]);
-            const uint32_t off = swz(r, c16);                  // absolute-row swizzle (halo base is 1024-byte aligned)
-            *reinterpret_cast<uint4*>(a_hi + off) = make_uint4(h[0], h[1], h[2], h[3]);
-            *reinterpret_cast<uint4*>(a_lo + off) = make_uint4(l[0], l[1], l[2], l[3]);
-          }
-        }
-        mbar_arrive_relaxed(&a_full[s]);                       // proxy fence runs on the consumer side (see tc_gemm.cu)
-      }
-    }
-  } else if (warp == LOAD_WARP) {
+    return;
+  }
+  if (warp >= C::LOAD_WARP) {
     // =============================================================== weight loader: one (tap, chunk) panel pair per slot
-    if (lane == 0) {
+    setmaxnreg_dec<C::REG_LOAD>();
+    if (warp == C::LOAD_WARP && lane == 0) {
       uint32_t bit = 0;
       const int KC = 9 * NCH;                                  // panels per n-tile in the weight image: kc = tap*NCH + cc
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
@@ -180,179 +210,237 @@ __global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const G
           }
       }
     }
-  } else {
-    // =============================================================== consumers: MMA (two m64n64 per k-step: output rows 0-63 and
-    // 64-127 of this warpgroup's 64 columns) + row-per-thread epilogue read back from the staged fp32 tile
-    const int wg = (warp - 8) >> 2, ew = (warp - 8) & 3;
-    const int row_in_tile = ew * 32 + lane;
-    const int etid = (tid - NPROD) & 127;
-    float* s_st = s_stat[wg];
-    const int bar_id = 2 + wg;
-    float* stage = reinterpret_cast<float*>(smemE) + wg * 128 * kStageLd;
-    float* wbuf = stage + ew * 32 * kStageLd;                 // this warp's own staged rows, free once they are read back
-    // GroupNorm partial sums (U:230).  Reducing them per tile (16 warp reductions, shared and global atomics, two barriers) costs more
-    // than half of a 64 -> 64 tile.  With a single n-tile every epilogue thread owns the same
-    // 64 columns for the whole persistent loop, so it keeps fp32 running sums per 8-column block and the warps reduce them (in fp64) only
-    // every 8 tiles and at the end: at most 64 values per fp32 partial sum.
-    const bool defer_stats = (p.stats != nullptr) && tiles_n == 1;
-    float gs[8], gss[8];
-    int pending = 0;
+    return;
+  }
+
+  // ================================================================= MMA (two m64n64 per k-step: output rows 0-63 and 64-127 of the
+  // warpgroup's 64 columns) and row-per-thread epilogue read back from the staged fp32 tile
+  const int wg = SPLIT ? 0 : (warp - 8) >> 2;                  // 64-column block of this MMA / epilogue warpgroup
+  const int ew = (warp - 8) & 3;
+  const int etid = ew * 32 + lane;                             // thread in the warpgroup = its tile row in the epilogue
+  const int bar_id = 2 + wg;
+  constexpr uint32_t SBO_HALO = HW * 128;                      // 10 pixel rows of 128 B between 8-row groups
+  constexpr uint32_t H2 = 8 * HW * 128;                        // output rows 64-127 start 8 halo rows further down
+  const int dt = (p.drain == 1 || p.drain == 3) ? p.drain : 9; // taps accumulated in registers before a drain
+
+  // All MMAs of one tile into `stage`.  The nine taps of a chunk are expanded at compile time for a drain interval DT of 1, 3
+  // or 9 taps, so the only waits are the wait_group 1 that keeps one tap's MMAs in flight and the wait_group 0 before a drain.
+  // claim() runs once, before the tile's first drain writes the staging tile.
+  auto mma_tile = [&](auto DTc, float* stage, uint32_t& ait, uint32_t& bit, auto&& claim) {
+    constexpr int DT = decltype(DTc)::value;
+    float d0[32], d1[32];
+    bool first_drain = true;
+    for (int cc = 0; cc < NCH; ++cc, ++ait) {
+      const int sa = ait % A_STAGES;
+      mbar_wait(&a_full[sa], (ait / A_STAGES) & 1);
+      fence_proxy_async();
+      const uint32_t a_hi = smem_u32(smemA + sa * 2 * A_HALO), a_lo = a_hi + A_HALO;
+      static_for<0, 9>([&](auto TAPc) {
+        constexpr int tap = decltype(TAPc)::value;
+        constexpr bool group_first = tap % DT == 0, group_last = tap % DT == DT - 1;
+        constexpr uint32_t woff = (uint32_t)(((tap / 3) * HW + tap % 3) * 128);   // window start: halo pixel (ky, kx)
+        const int sb = bit % B_STAGES;
+        const int sprev = (bit + B_STAGES - 1) % B_STAGES;     // previous tap's B stage, released once its MMAs completed
+        mbar_wait(&b_full[sb], (bit / B_STAGES) & 1);
+        const uint64_t ahi = make_desc(a_hi + woff, SBO_HALO), alo = make_desc(a_lo + woff, SBO_HALO);
+        const uint64_t ahi2 = make_desc(a_hi + woff + H2, SBO_HALO), alo2 = make_desc(a_lo + woff + H2, SBO_HALO);
+        const uint32_t sbaddr = smem_u32(smemB + sb * 2 * B_PANEL) + wg * 64 * 128;
+        const uint64_t bhi = make_desc(sbaddr), blo = make_desc(sbaddr + B_PANEL);
+        wgmma_fence();
 #pragma unroll
-    for (int i = 0; i < 8; ++i) { gs[i] = 0.f; gss[i] = 0.f; }
-    // with one n-tile the 64 bias values never change: fetch them once instead of 16 L2 round trips per tile
-    const bool bias_smem = (p.bias != nullptr) && tiles_n == 1;
+        for (int j = 0; j < 4; ++j) {
+          const uint64_t o = (uint64_t)(j * 2);
+          const uint32_t acc = (group_first && j == 0) ? 0u : 1u;
+          wgmma_m64n64k16(d0, alo + o, bhi + o, acc);
+          wgmma_m64n64k16(d1, alo2 + o, bhi + o, acc);
+          wgmma_m64n64k16(d0, ahi + o, blo + o, 1u);
+          wgmma_m64n64k16(d1, ahi2 + o, blo + o, 1u);
+          wgmma_m64n64k16(d0, ahi + o, bhi + o, 1u);
+          wgmma_m64n64k16(d1, ahi2 + o, bhi + o, 1u);
+        }
+        wgmma_commit();
+        if constexpr (group_last) {
+          wgmma_wait<0>();
+          wgmma_fence_acc(d0); wgmma_fence_acc(d1);
+          if (lane == 0) { if (!group_first) mbar_arrive(&b_free[sprev]); mbar_arrive(&b_free[sb]); }
+          if (first_drain) claim();
+          stage_fragment(stage, 0, d0, first_drain, etid);
+          stage_fragment(stage, 64, d1, first_drain, etid);
+          first_drain = false;
+        } else {
+          wgmma_wait<1>();
+          wgmma_fence_acc(d0); wgmma_fence_acc(d1);
+          if (lane == 0 && !group_first) mbar_arrive(&b_free[sprev]);
+        }
+        ++bit;
+      });
+      if (lane == 0) mbar_arrive(&a_free[sa]);                 // 9 % DT == 0: every MMA of the chunk has completed
+    }
+  };
+
+  // GroupNorm partial sums (U:230).  Reducing them per tile (16 warp reductions, shared and global atomics, two barriers) costs more
+  // than half of a 64 -> 64 tile.  With a single n-tile every epilogue thread owns the same
+  // 64 columns for the whole persistent loop, so it keeps fp32 running sums per 8-column block and the warps reduce them (in fp64) only
+  // every 8 tiles and at the end: at most 64 values per fp32 partial sum.
+  const bool defer_stats = (p.stats != nullptr) && tiles_n == 1;
+  // with one n-tile the 64 bias values never change: fetch them once instead of 16 L2 round trips per tile
+  const bool bias_smem = (p.bias != nullptr) && tiles_n == 1;
+  auto load_bias = [&]() {
     if (bias_smem) {
       if (etid < 64) s_bias[wg][etid] = __ldg(p.bias + wg * 64 + etid);
       asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
     }
-    auto flush_stats = [&]() {
-      const int n0f = wg * 64;                                    // tiles_n == 1: this thread's columns never change
+  };
+  auto flush_stats = [&](float (&gs)[8], float (&gss)[8]) {
+    const int n0f = wg * 64;                                      // tiles_n == 1: this thread's columns never change
 #pragma unroll
-      for (int b8 = 0; b8 < 8; ++b8) {
-        double s = (double)gs[b8], ss = (double)gss[b8];
+    for (int b8 = 0; b8 < 8; ++b8) {
+      double s = (double)gs[b8], ss = (double)gss[b8];
 #pragma unroll
-        for (int o = 16; o > 0; o >>= 1) { s += __shfl_xor_sync(0xffffffffu, s, o); ss += __shfl_xor_sync(0xffffffffu, ss, o); }
-        if (lane == 0) {
-          const int grp = (n0f + b8 * 8) / p.cpg;
-          atomicAdd(&p.stats[2 * grp], s);
-          atomicAdd(&p.stats[2 * grp + 1], ss);
-        }
-        gs[b8] = 0.f; gss[b8] = 0.f;
+      for (int o = 16; o > 0; o >>= 1) { s += __shfl_xor_sync(0xffffffffu, s, o); ss += __shfl_xor_sync(0xffffffffu, ss, o); }
+      if (lane == 0) {
+        const int grp = (n0f + b8 * 8) / p.cpg;
+        atomicAdd(&p.stats[2 * grp], s);
+        atomicAdd(&p.stats[2 * grp + 1], ss);
       }
-      pending = 0;
-    };
-    constexpr uint32_t SBO_HALO = HW * 128;                    // 10 pixel rows of 128 B between 8-row groups
-    constexpr uint32_t H2 = 8 * HW * 128;                      // output rows 64-127 start 8 halo rows further down
-    const int dt = (p.drain == 1 || p.drain == 3) ? p.drain : 9;   // taps accumulated in registers before a drain
-    uint32_t ait = 0, bit = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      int f, y0, x0, nt;
-      decode(tile, f, y0, x0, nt);
-      const int n0 = nt * BN + wg * 64;
-      float d0[32], d1[32];
-      bool first_drain = true;
-      for (int cc = 0; cc < NCH; ++cc, ++ait) {
-        const int sa = ait % A_STAGES;
-        mbar_wait(&a_full[sa], (ait / A_STAGES) & 1);
-        fence_proxy_async();
-        const uint32_t a_hi = smem_u32(smemA + sa * 2 * A_HALO), a_lo = a_hi + A_HALO;
-        int in_group = 0, pend = -1;                           // B stage whose MMAs are still in flight
-        for (int tap = 0; tap < 9; ++tap, ++bit) {
-          const int sb = bit % B_STAGES;
-          mbar_wait(&b_full[sb], (bit / B_STAGES) & 1);
-          const int ky = tap / 3, kx = tap - ky * 3;          // window start: halo pixel (ky, kx)
-          const uint32_t woff = (uint32_t)((ky * HW + kx) * 128);
-          const uint64_t ahi = make_desc(a_hi + woff, SBO_HALO), alo = make_desc(a_lo + woff, SBO_HALO);
-          const uint64_t ahi2 = make_desc(a_hi + woff + H2, SBO_HALO), alo2 = make_desc(a_lo + woff + H2, SBO_HALO);
-          const uint32_t sbaddr = smem_u32(smemB + sb * 2 * B_PANEL) + wg * 64 * 128;
-          const uint64_t bhi = make_desc(sbaddr), blo = make_desc(sbaddr + B_PANEL);
-          wgmma_fence();
+      gs[b8] = 0.f; gss[b8] = 0.f;
+    }
+  };
+  // epilogue of one tile: thread etid owns tile row etid; its warp's 32 staged rows serve as the store buffer once read back
+  auto epilogue_tile = [&](int tile, float* stage, float (&gs)[8], float (&gss)[8], int& pending) {
+    int f, y0, x0, nt;
+    decode(tile, f, y0, x0, nt);
+    const int n0 = nt * BN + wg * 64;
+    const int row_in_tile = etid;
+    float* s_st = s_stat[wg];
+    float* wbuf = stage + ew * 32 * kStageLd;
+    float acc[64];
+    {
+      const float4* src = reinterpret_cast<const float4*>(stage + row_in_tile * kStageLd);
 #pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const uint64_t o = (uint64_t)(j * 2);
-            const uint32_t acc = (in_group == 0 && j == 0) ? 0u : 1u;
-            wgmma_m64n64k16(d0, alo + o, bhi + o, acc);
-            wgmma_m64n64k16(d1, alo2 + o, bhi + o, acc);
-            wgmma_m64n64k16(d0, ahi + o, blo + o, 1u);
-            wgmma_m64n64k16(d1, ahi2 + o, blo + o, 1u);
-            wgmma_m64n64k16(d0, ahi + o, bhi + o, 1u);
-            wgmma_m64n64k16(d1, ahi2 + o, bhi + o, 1u);
-          }
-          wgmma_commit();
-          if (++in_group == dt) {
-            wgmma_wait<0>();
-            wgmma_fence_acc(d0); wgmma_fence_acc(d1);
-            if (lane == 0) { if (pend >= 0) mbar_arrive(&b_free[pend]); mbar_arrive(&b_free[sb]); }
-            pend = -1;
-            stage_fragment(stage, 0, d0, first_drain, etid);
-            stage_fragment(stage, 64, d1, first_drain, etid);
-            first_drain = false;
-            in_group = 0;
-          } else {
-            wgmma_wait<1>();
-            if (lane == 0 && pend >= 0) mbar_arrive(&b_free[pend]);
-            pend = sb;
-          }
-        }
-        if (lane == 0) mbar_arrive(&a_free[sa]);               // 9 % dt == 0: every MMA of the chunk has completed
+      for (int i = 0; i < 16; ++i) {
+        const float4 v = src[i];
+        acc[4 * i] = v.x; acc[4 * i + 1] = v.y; acc[4 * i + 2] = v.z; acc[4 * i + 3] = v.w;
       }
-      asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
-      float acc[64];
-      {
-        const float4* src = reinterpret_cast<const float4*>(stage + row_in_tile * kStageLd);
+    }
+    __syncwarp();
 #pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const float4 v = src[i];
-          acc[4 * i] = v.x; acc[4 * i + 1] = v.y; acc[4 * i + 2] = v.z; acc[4 * i + 3] = v.w;
-        }
+    for (int i = 0; i < 64; ++i) acc[i] *= p.tc_scale;
+    const int oy = y0 + (row_in_tile >> 3), ox = x0 + (row_in_tile & 7);
+    const bool rv = (oy < H) && (ox < W);
+    size_t opix = (size_t)f * H * W + (size_t)(rv ? oy * W + ox : 0);
+    int ocol = n0;
+    if (p.up2) {
+      // transposed conv as one 3x3 conv with 4 x 64 output columns: column block = output parity class (py, px)
+      const int cls = n0 >> 6, py = cls >> 1, px = cls & 1;
+      opix = (size_t)f * 4 * H * W + (size_t)(rv ? (2 * oy + py) * 2 * W + 2 * ox + px : 0);
+      ocol = n0 & 63;
+    }
+    if (bias_smem) {
+      const float4* bp = reinterpret_cast<const float4*>(s_bias[wg]);
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        const float4 b = bp[i];
+        acc[4 * i] += b.x; acc[4 * i + 1] += b.y; acc[4 * i + 2] += b.z; acc[4 * i + 3] += b.w;
       }
-      __syncwarp();
+    } else if (p.bias) {
+      const float4* bp = reinterpret_cast<const float4*>(p.bias + n0);
 #pragma unroll
-      for (int i = 0; i < 64; ++i) acc[i] *= p.tc_scale;
-      const int oy = y0 + (row_in_tile >> 3), ox = x0 + (row_in_tile & 7);
-      const bool rv = (oy < H) && (ox < W);
-      size_t opix = (size_t)f * H * W + (size_t)(rv ? oy * W + ox : 0);
-      int ocol = n0;
-      if (p.up2) {
-        // transposed conv as one 3x3 conv with 4 x 64 output columns: column block = output parity class (py, px)
-        const int cls = n0 >> 6, py = cls >> 1, px = cls & 1;
-        opix = (size_t)f * 4 * H * W + (size_t)(rv ? (2 * oy + py) * 2 * W + 2 * ox + px : 0);
-        ocol = n0 & 63;
+      for (int i = 0; i < 16; ++i) {
+        const float4 b = __ldg(bp + i);
+        acc[4 * i] += b.x; acc[4 * i + 1] += b.y; acc[4 * i + 2] += b.z; acc[4 * i + 3] += b.w;
       }
-      if (bias_smem) {
-        const float4* bp = reinterpret_cast<const float4*>(s_bias[wg]);
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const float4 b = bp[i];
-          acc[4 * i] += b.x; acc[4 * i + 1] += b.y; acc[4 * i + 2] += b.z; acc[4 * i + 3] += b.w;
-        }
-      } else if (p.bias) {
-        const float4* bp = reinterpret_cast<const float4*>(p.bias + n0);
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const float4 b = __ldg(bp + i);
-          acc[4 * i] += b.x; acc[4 * i + 1] += b.y; acc[4 * i + 2] += b.z; acc[4 * i + 3] += b.w;
-        }
-      }
-      store_rows_coalesced(wbuf, acc, p.Out, opix, p.ldo, ocol, rv, lane);
-      if (defer_stats) {
-        if (rv) {
-#pragma unroll
-          for (int b8 = 0; b8 < 8; ++b8) {
-            float s = 0.f, ss = 0.f;
-#pragma unroll
-            for (int i = 0; i < 8; ++i) { const float x = acc[b8 * 8 + i]; s += x; ss += x * x; }
-            gs[b8] += s; gss[b8] += ss;
-          }
-        }
-        if (++pending == 8) flush_stats();
-      } else if (p.stats != nullptr) {
-        if (etid < 16) s_st[etid] = 0.f;
-        asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
+    }
+    store_rows_coalesced(wbuf, acc, p.Out, opix, p.ldo, ocol, rv, lane);
+    if (defer_stats) {
+      if (rv) {
 #pragma unroll
         for (int b8 = 0; b8 < 8; ++b8) {
           float s = 0.f, ss = 0.f;
-          if (rv) {
 #pragma unroll
-            for (int i = 0; i < 8; ++i) { const float x = acc[b8 * 8 + i]; s += x; ss += x * x; }
-          }
-          s = warp_sum(s); ss = warp_sum(ss);
-          if (lane == 0) {
-            const int grp = (n0 + b8 * 8) / p.cpg;
-            atomicAdd(&s_st[2 * grp], s);
-            atomicAdd(&s_st[2 * grp + 1], ss);
-          }
-        }
-        asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
-        if (etid < 16) {
-          const int grp = etid >> 1;
-          const int glo = n0 / p.cpg, ghi = (n0 + 63) / p.cpg;
-          if (grp >= glo && grp <= ghi) atomicAdd(&p.stats[etid], (double)s_st[etid]);
+          for (int i = 0; i < 8; ++i) { const float x = acc[b8 * 8 + i]; s += x; ss += x * x; }
+          gs[b8] += s; gss[b8] += ss;
         }
       }
-      asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");     // the staged tile is rewritten by the next tile's first drain
+      if (++pending == 8) { flush_stats(gs, gss); pending = 0; }
+    } else if (p.stats != nullptr) {
+      if (etid < 16) s_st[etid] = 0.f;
+      asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
+#pragma unroll
+      for (int b8 = 0; b8 < 8; ++b8) {
+        float s = 0.f, ss = 0.f;
+        if (rv) {
+#pragma unroll
+          for (int i = 0; i < 8; ++i) { const float x = acc[b8 * 8 + i]; s += x; ss += x * x; }
+        }
+        s = warp_sum(s); ss = warp_sum(ss);
+        if (lane == 0) {
+          const int grp = (n0 + b8 * 8) / p.cpg;
+          atomicAdd(&s_st[2 * grp], s);
+          atomicAdd(&s_st[2 * grp + 1], ss);
+        }
+      }
+      asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
+      if (etid < 16) {
+        const int grp = etid >> 1;
+        const int glo = n0 / p.cpg, ghi = (n0 + 63) / p.cpg;
+        if (grp >= glo && grp <= ghi) atomicAdd(&p.stats[etid], (double)s_st[etid]);
+      }
     }
-    if (defer_stats && pending > 0) flush_stats();
+  };
+  // the MMA tile loop, expanded once per legal drain interval
+  auto with_drain = [&](auto&& run) {
+    if (dt == 1) run(std::integral_constant<int, 1>{});
+    else if (dt == 3) run(std::integral_constant<int, 3>{});
+    else run(std::integral_constant<int, 9>{});
+  };
+
+  if (SPLIT && warp >= C::EPI_WARP) {
+    // =============================================================== epilogue warpgroup: tile t from staging tile t & 1
+    setmaxnreg_inc<C::REG_EPI>();
+    float gs[8], gss[8];
+    int pending = 0;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) { gs[i] = 0.f; gss[i] = 0.f; }
+    load_bias();
+    uint32_t lt = 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++lt) {
+      const int b = lt & 1;
+      mbar_wait(&st_full[b], (lt >> 1) & 1);
+      epilogue_tile(tile, stage_base + b * 128 * kStageLd, gs, gss, pending);
+      mbar_arrive(&st_free[b]);                                // after the last read and the last store-buffer use of the tile
+    }
+    if (defer_stats && pending > 0) flush_stats(gs, gss);
+  } else if (SPLIT) {
+    // =============================================================== MMA warpgroup: drains tile t into staging tile t & 1, hands it
+    // to the epilogue warpgroup and goes on with tile t+1
+    setmaxnreg_inc<C::REG_MMA>();
+    with_drain([&](auto DTc) {
+      uint32_t ait = 0, bit = 0, lt = 0;
+      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++lt) {
+        const int b = lt & 1;
+        mma_tile(DTc, stage_base + b * 128 * kStageLd, ait, bit, [&]() { mbar_wait(&st_free[b], ((lt >> 1) & 1) ^ 1); });
+        mbar_arrive(&st_full[b]);                              // this thread's drained fragments are in the tile
+      }
+    });
+  } else {
+    // =============================================================== BN = 128: each warpgroup runs the MMAs and then the epilogue
+    // of its 64 columns
+    setmaxnreg_inc<C::REG_MMA>();
+    float gs[8], gss[8];
+    int pending = 0;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) { gs[i] = 0.f; gss[i] = 0.f; }
+    load_bias();
+    float* stage = stage_base + wg * 128 * kStageLd;
+    uint32_t ait = 0, bit = 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      with_drain([&](auto DTc) { mma_tile(DTc, stage, ait, bit, []() {}); });
+      asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
+      epilogue_tile(tile, stage, gs, gss, pending);
+      asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");   // the staged tile is rewritten by the next tile's first drain
+    }
+    if (defer_stats && pending > 0) flush_stats(gs, gss);
   }
 }
 

@@ -10,9 +10,13 @@
 //   * The tensor core adds into its accumulator with truncation; chained over a long K that is a biased error
 //     (1.4e-4 at K=14112).  So the register accumulator only spans CHUNK panels (first MMA overwrites) and is then
 //     added into an fp32 tile in shared memory with ordinary round-to-nearest adds.
-//   * persistent CTAs, warp roles: 0-7 A producers (gather + split + swizzled st.shared, global loads prefetched
-//     two panels ahead in registers), then BN/64 consumer warpgroups (wgmma on 128 rows x 64 columns each, then the
-//     epilogue with one output row per thread, read back from the staged tile), last a weight loader (one thread).
+//   * persistent CTAs of whole warpgroups: 0-1 A producers (gather + split + swizzled st.shared, global loads prefetched
+//     two panels ahead in registers for BN = 64, one for BN = 128), then BN/64 consumer warpgroups (wgmma on 128 rows x 64
+//     columns each, then the epilogue with one output row per thread, read back from the staged tile), last the weight
+//     loader (one thread; the other three warps exit).  setmaxnreg moves registers from the loader warpgroup to the
+//     consumers (budgets in Cfg), so the consumers' accumulators and the producers' prefetch do not spill.
+//   * each chunk of CHUNK (or `drain`) panels is expanded at compile time: wait_group 1 between panels keeps one panel's
+//     MMAs in flight while the next is issued, wait_group 0 comes only before the drain.
 #include <cuda_fp16.h>
 #include "common.cuh"
 #include "gemm.cuh"
@@ -37,8 +41,16 @@ struct Cfg {
   static constexpr int B_PANEL = BN * 128;
   static constexpr int STAGE_BYTES = 2 * A_PANEL + 2 * B_PANEL;
   static constexpr int STAGES = (BN == 64) ? 3 : 2;
-  static constexpr int NTHREADS = NPROD + 128 * NWG + 32;    // producers | consumers | loader warp
   static constexpr int LOAD_WARP = (NPROD + 128 * NWG) / 32;
+  static constexpr int NTHREADS = 32 * LOAD_WARP + 128;      // producers | consumers | loader warpgroup (one thread works)
+  // registers per thread by warpgroup.  Every warp starts with what NTHREADS allows (BN = 64: 128, BN = 128: 96), and
+  // setmaxnreg.inc can only take what other warpgroups of the CTA released: the producers keep their count, the loader gives
+  // all but 24 back and the consumers take them.  BN = 64: 2 x 128 + 24 + 232 = 512, BN = 128: 2 x 96 + 24 + 2 x 128 = 472 (of 480)
+  static constexpr uint32_t REG_LAUNCH = (65536 / NTHREADS) & ~7u;
+  static constexpr uint32_t REG_LOAD = 24, REG_MMA = (BN == 64) ? 232 : 128;
+  // setmaxnreg.dec may only lower a warp's count and setmaxnreg.inc only raise it
+  static_assert(REG_LOAD < REG_LAUNCH && REG_MMA > REG_LAUNCH, "register budgets");
+  static_assert(2 * REG_LAUNCH + REG_LOAD + NWG * REG_MMA <= NTHREADS / 128 * REG_LAUNCH, "CTA register pool");
   static constexpr int ACC_STAGE = NWG * BM * tc::kStageLd * 4;
   static constexpr int SMEM_DYN = STAGES * STAGE_BYTES + ACC_STAGE + 1024;
 };
@@ -62,7 +74,7 @@ __global__ void __launch_bounds__(Cfg<BN>::NTHREADS, 1) tc_gemm_kernel(const Gem
 
   const int tid = threadIdx.x, lane = tid & 31;
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);          // warp-uniform by construction
-  uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+  uint8_t* smem = smem_align1024(smem_raw);
 
   if (tid == 0) {
     // slot_free: one arrive per consumer warp once its MMAs on the slot have completed
@@ -76,7 +88,7 @@ __global__ void __launch_bounds__(Cfg<BN>::NTHREADS, 1) tc_gemm_kernel(const Gem
   const int chunks_per_tap = p.Cin / BKP;
 
   if (warp < 8) {
-    // =============================================================== A producers
+    // =============================================================== A producers (keep the launch register budget)
     // Work items are (tile, k-panel) pairs flattened over this CTA's tiles, so the register prefetch keeps running
     // across tile boundaries (with K = 64 a tile is a single panel: per-tile prologues exposed the full load latency).
     const int c16 = tid & 7;            // 16-byte chunk inside the 128-byte row
@@ -246,9 +258,10 @@ __global__ void __launch_bounds__(Cfg<BN>::NTHREADS, 1) tc_gemm_kernel(const Gem
         }
       }
     }
-  } else if (warp == LOAD_WARP) {
+  } else if (warp >= LOAD_WARP) {
     // =============================================================== weight loader (pre-swizzled hi|lo images)
-    if (lane == 0) {
+    setmaxnreg_dec<C::REG_LOAD>();
+    if (warp == LOAD_WARP && lane == 0) {
       uint32_t it = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         const int nt = tile % tiles_n;
@@ -266,6 +279,7 @@ __global__ void __launch_bounds__(Cfg<BN>::NTHREADS, 1) tc_gemm_kernel(const Gem
     // =============================================================== consumers (warps 8 .. 8+4*NWG-1): MMA + epilogue
     // warpgroup wg owns output columns [64 wg, 64 wg + 64) of the tile (two m64n64 MMAs per k-step: rows 0-63 and 64-127);
     // in the epilogue thread etid owns tile row etid (row-per-thread layout, read back from the staged fp32 tile)
+    setmaxnreg_inc<C::REG_MMA>();
     const int wg = (warp - 8) >> 2;
     const int ew = (warp - 8) & 3;
     const int row_in_tile = ew * 32 + lane;
@@ -282,17 +296,17 @@ __global__ void __launch_bounds__(Cfg<BN>::NTHREADS, 1) tc_gemm_kernel(const Gem
       asm volatile("bar.sync 4, %0;" ::"n"(128 * NWG) : "memory");
     }
     const int CH = (p.drain > 0 && p.drain < CHUNK) ? p.drain : CHUNK;
-    uint32_t it = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      ++Te;
-      const int m0 = (tile / tiles_n) * BM, n0 = (tile % tiles_n) * BN + wg * EN;
+    // NP consecutive K panels into the register accumulator, then one drain into the staged tile (`first`: the tile's first
+    // chunk stores, later chunks add).  The panels are expanded at compile time, so the only waits are the wait_group 1 that
+    // keeps one panel's MMAs in flight and the wait_group 0 before the drain.
+    auto mma_chunk = [&](auto NPc, float* stage, uint32_t& it, bool first) {
+      constexpr int NP = decltype(NPc)::value;
       float d0[32], d1[32];
-      int pend = -1;                                       // stage whose MMAs are still in flight (released one panel later)
-      for (int kc = 0; kc < KC; ++kc, ++it) {
+      static_for<0, NP>([&](auto Ic) {
+        constexpr int i = decltype(Ic)::value;
         const int s = it % STAGES;
+        const int sprev = (it + STAGES - 1) % STAGES;        // previous panel's stage, released once its MMAs completed
         const uint32_t round = it / STAGES;
-        const bool chunk_first = (kc % CH) == 0;
-        const bool chunk_last = ((kc % CH) == CH - 1) || (kc == KC - 1);
         mbar_wait(&a_full[s], round & 1);
         mbar_wait(&b_full[s], round & 1);
         fence_proxy_async();          // generic-proxy operand writes of the producers -> async proxy (see store_item)
@@ -304,7 +318,7 @@ __global__ void __launch_bounds__(Cfg<BN>::NTHREADS, 1) tc_gemm_kernel(const Gem
 #pragma unroll
         for (int j = 0; j < BKP / 16; ++j) {
           const uint64_t o = (uint64_t)(j * 2);               // +32 bytes per k-step, in 16-byte units
-          const uint32_t acc = (chunk_first && j == 0) ? 0u : 1u;
+          const uint32_t acc = (i == 0 && j == 0) ? 0u : 1u;
           wgmma_m64n64k16(d0, alo + o, bhi + o, acc);
           wgmma_m64n64k16(d1, alo + H2 + o, bhi + o, acc);
           wgmma_m64n64k16(d0, ahi + o, blo + o, 1u);
@@ -313,18 +327,31 @@ __global__ void __launch_bounds__(Cfg<BN>::NTHREADS, 1) tc_gemm_kernel(const Gem
           wgmma_m64n64k16(d1, ahi + H2 + o, bhi + o, 1u);
         }
         wgmma_commit();
-        if (chunk_last) {
+        if constexpr (i == NP - 1) {
           wgmma_wait<0>();
           wgmma_fence_acc(d0); wgmma_fence_acc(d1);
-          if (lane == 0) { if (pend >= 0) mbar_arrive(&slot_free[pend]); mbar_arrive(&slot_free[s]); }
-          pend = -1;
-          stage_fragment(stage, 0, d0, kc < CH, etid);
-          stage_fragment(stage, 64, d1, kc < CH, etid);
+          if (lane == 0) { if (i > 0) mbar_arrive(&slot_free[sprev]); mbar_arrive(&slot_free[s]); }
+          stage_fragment(stage, 0, d0, first, etid);
+          stage_fragment(stage, 64, d1, first, etid);
         } else {
           wgmma_wait<1>();
-          if (lane == 0 && pend >= 0) mbar_arrive(&slot_free[pend]);
-          pend = s;
+          wgmma_fence_acc(d0); wgmma_fence_acc(d1);
+          if (lane == 0 && i > 0) mbar_arrive(&slot_free[sprev]);
         }
+        ++it;
+      });
+    };
+    static_assert(CHUNK == 4, "the chunk dispatch below expands 1 .. 4 panels");
+    uint32_t it = 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      ++Te;
+      const int m0 = (tile / tiles_n) * BM, n0 = (tile % tiles_n) * BN + wg * EN;
+      for (int kc = 0; kc < KC; kc += CH) {                 // chunks of CH panels, the last one possibly shorter
+        const int np = min(CH, KC - kc);
+        if (np == 4) mma_chunk(std::integral_constant<int, 4>{}, stage, it, kc == 0);
+        else if (np == 3) mma_chunk(std::integral_constant<int, 3>{}, stage, it, kc == 0);
+        else if (np == 2) mma_chunk(std::integral_constant<int, 2>{}, stage, it, kc == 0);
+        else mma_chunk(std::integral_constant<int, 1>{}, stage, it, kc == 0);
       }
       asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
       float acc[EN];
