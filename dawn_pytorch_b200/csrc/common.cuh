@@ -19,6 +19,18 @@ void set_last_error(const std::string& s);
     }                                                                                   \
   } while (0)
 #define DAWN_LAUNCH_OK() DAWN_CUDA_OK(cudaGetLastError())
+#define DAWN_CHECK(cond, msg)                 \
+  do {                                        \
+    if (!(cond)) {                            \
+      ::dawn::set_last_error(msg);            \
+      return -1;                              \
+    }                                         \
+  } while (0)
+#define DAWN_TRY(expr)           \
+  do {                           \
+    int _rc = (expr);            \
+    if (_rc != 0) return _rc;    \
+  } while (0)
 
 // ---------------------------------------------------------------- small device helpers
 __device__ __forceinline__ float silu(float x) { return x / (1.0f + expf(-x)); }

@@ -22,7 +22,7 @@ struct GemmParams {
   const float* A; int lda; int Cin;
   // optional pre-split copy of A (fp16 hi and lo planes, dense rows of Cin halfs): the wgmma-kernel producers then only copy
   const unsigned short* A16h = nullptr; const unsigned short* A16l = nullptr;
-  int want_split = 0;      // host side: ask Ctx::gemm to build the pre-split copy
+  int want_split = 0;      // host side: ask choose_path (contraction.cuh) for the pre-split copy
   int up2 = 0;             // halo conv3 kernel only: 64-column block j of the output is parity class j of a 2x upsampled grid
   int IH, IW;              // input frame dims
   int OHs, OWs;            // output sub-grid dims; rows m = (f, i, j)

@@ -7,14 +7,13 @@
 #include <cstring>
 #include <map>
 #include <string>
-#include <unordered_map>
 #include <vector>
 
 #include "../../include/dawn_unet.h"
 #include "common.cuh"
+#include "contraction.cuh"
 #include "gemm.cuh"
 #include "kernels.cuh"
-#include "tc_gemm.cuh"
 #include "temporal_fused.cuh"
 #include "sla_fused.cuh"
 #include "ca_fused.cuh"
@@ -24,19 +23,6 @@ namespace dawn {
 
 static thread_local std::string g_last_error;
 void set_last_error(const std::string& s) { g_last_error = s; }
-
-#define DAWN_CHECK(cond, msg)                 \
-  do {                                        \
-    if (!(cond)) {                            \
-      ::dawn::set_last_error(msg);            \
-      return -1;                              \
-    }                                         \
-  } while (0)
-#define DAWN_TRY(expr)           \
-  do {                           \
-    int _rc = (expr);            \
-    if (_rc != 0) return _rc;    \
-  } while (0)
 
 // ------------------------------------------------------------------ NCCL, resolved at run time (torch ships libnccl.so.2)
 typedef struct ncclComm* ncclComm_t;
@@ -82,17 +68,9 @@ static int load_nccl() {
     if (_r != 0) { ::dawn::set_last_error(std::string(#expr) + ": " + g_nccl.GetErrorString(_r)); return -2; } \
   } while (0)
 
-struct HostParam {
-  std::vector<float> data;
-  std::vector<int64_t> shape;
-  int64_t numel() const { int64_t n = 1; for (auto s : shape) n *= s; return n; }
-};
-
 struct Act {          // channels-last activation view: pixel stride ld, C channels, frame size H x W
   float* p = nullptr; int ld = 0; int C = 0; int H = 0; int W = 0;
 };
-
-struct ConvW { float* w = nullptr; float* b = nullptr; float* img = nullptr; float img_scale = 1.f; int K = 0, N = 0, ldb = 0; };
 
 struct CrossAttnW { float *Wkv, *nkv, *qs, *ks, *Wout, *gout; };
 
@@ -100,12 +78,11 @@ struct ResBlockW {
   std::string name;
   int ci = 0, co = 0;
   bool cond = false, res = false;
-  ConvW c1, c2, cres;
+  PackedWeight c1, c2, cres;
   float *gn1w = nullptr, *gn1b = nullptr, *gn2w = nullptr, *gn2b = nullptr;
   float *tW = nullptr, *tB = nullptr;
   float *mW[3] = {nullptr, nullptr, nullptr}, *mB[3] = {nullptr, nullptr, nullptr};   // pose, aud, eye MLPs
-  float Wq_scale = 1.f;
-  float *Wq = nullptr, *wsumq = nullptr, *Wq_img = nullptr;                              // [ci][192], [192]
+  PackedWeight wq; float* wsumq = nullptr;                                                // [ci][192], [192]
   uint16_t* fWq = nullptr; float f_inv_wscale = 1.f;                                      // ca_fused.cu image (ci <= 128)
   CrossAttnW ca[3];
   // per-clip (depend on F / cond)
@@ -115,18 +92,16 @@ struct ResBlockW {
 };
 
 struct AttnW {     // temporal attention / mid spatial attention (U:648-725)
-  int C = 0; float Wqkv_scale = 1.f; float *Wqkv = nullptr, *wsum = nullptr, *Wqkv_img = nullptr; ConvW out;
+  int C = 0; PackedWeight qkv, out; float* wsum = nullptr;
   // fused per-pixel kernel (temporal_fused.cu), 64-channel levels only
   uint16_t *fq = nullptr, *fo = nullptr; float f_inv_wscale = 1.f, f_inv_oscale = 1.f;
 };
 struct SlaW {      // spatial linear attention (U:602-627)
-  int C = 0; float Wqkv_scale = 1.f; float *Wqkv = nullptr, *wsum = nullptr, *Wqkv_img = nullptr, *WoutT = nullptr, *bout = nullptr;
-  // fused context kernel (sla_fused.cu), 64-channel levels: q-only projection + K/V weights as fp16 hi|lo images
-  float *Wq = nullptr, *wsum_q = nullptr, *Wq_img = nullptr; float Wq_scale = 1.f;
+  int C = 0; PackedWeight qkv; float *wsum = nullptr, *WoutT = nullptr, *bout = nullptr;
+  // fused context and output kernels (sla_fused.cu), 64-channel levels: K/V and q weights as fp16 hi|lo images
   uint16_t* fkv = nullptr; float f_inv_wscale = 1.f;
   uint16_t* fq = nullptr; float fq_inv_wscale = 1.f;
 };
-struct UpW { ConvW cls[4]; ConvW all; };      // all: the four parity classes as one 3x3 conv with 4*C outputs (C = 64)
 
 }  // namespace dawn
 
@@ -184,14 +159,14 @@ struct dawn_unet {
   std::vector<int> dims;                       // [dim, dim*m0, ...]
   std::vector<std::pair<int, int>> in_out;
   int cond_dim = 0, tdim = 0;
-  std::unordered_map<std::string, HostParam> raw;
+  HostParams raw;
   bool committed = false;
 
   // packed weights
   std::vector<void*> owned;                    // weight allocations
   std::vector<void*> ws_owned;                 // workspace allocations
   int64_t ws_bytes = 0;
-  ConvW init_full;                             // 7x7 over channels padded to cin_pad
+  PackedWeight init_full;                      // 7x7 over channels padded to cin_pad
   float* init_w3 = nullptr;                    // [k*k*3][dim] for the 3 noisy channels
   int cin_pad = 0;
   float *time_freqs = nullptr, *tW1 = nullptr, *tb1 = nullptr, *tW2 = nullptr, *tb2 = nullptr;
@@ -201,8 +176,8 @@ struct dawn_unet {
   AttnW init_ta, mid_sa, mid_ta;
   std::vector<AttnW> down_ta, up_ta;
   std::vector<SlaW> down_sla, up_sla;
-  std::vector<ConvW> down_conv;
-  std::vector<UpW> up_conv;
+  std::vector<PackedWeight> down_conv;
+  std::vector<UpConv> up_conv;
   float *headW[2] = {nullptr, nullptr}, *headB[2] = {nullptr, nullptr};
   FilmDesc* film_descs = nullptr; int n_film = 0;
   CondDesc* cond_descs = nullptr; int n_cond = 0, cond_max_n1 = 0, cond_max_k = 0, cond_max_co = 0;   // batched per-clip prep
@@ -254,60 +229,11 @@ struct dawn_unet {
 
 namespace {
 
-// ------------------------------------------------------------------------------------------ allocation helpers
-int dev_alloc(std::vector<void*>& owner, size_t nfloats, float** out, int64_t* counter = nullptr) {
-  void* p = nullptr;
-  size_t bytes = std::max<size_t>(nfloats, 4) * sizeof(float);
-  DAWN_CUDA_OK(cudaMalloc(&p, bytes));
-  owner.push_back(p);
-  if (counter) *counter += (int64_t)bytes;
-  *out = (float*)p;
-  return 0;
-}
-int dev_upload(dawn_unet* h, const std::vector<float>& v, float** out) {
-  DAWN_TRY(dev_alloc(h->owned, v.size(), out));
-  DAWN_CUDA_OK(cudaMemcpy(*out, v.data(), v.size() * sizeof(float), cudaMemcpyHostToDevice));
-  return 0;
-}
-void free_all(std::vector<void*>& v) {
-  for (void* p : v) cudaFree(p);
-  v.clear();
-}
-inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
-
-// wgmma weight image of a [K][ldb] weight matrix (only for shapes the wgmma kernel accepts)
-int upload_tc_image(dawn_unet* h, const std::vector<float>& m, int K, int N, int ldb, float** img, float* scale) {
-  *img = nullptr; *scale = 1.f;
-  if (N % 64 != 0 || K % 64 != 0) return 0;
-  std::vector<float> im;
-  tc_pack_weights(m.data(), K, N, ldb, im, scale);
-  return dev_upload(h, im, img);
-}
-
-const HostParam* find(dawn_unet* h, const std::string& name) {
-  auto it = h->raw.find(name);
-  return it == h->raw.end() ? nullptr : &it->second;
-}
-int need(dawn_unet* h, const std::string& name, std::vector<int64_t> shape, const HostParam** out) {
-  const HostParam* p = find(h, name);
-  if (!p) { set_last_error("missing parameter: " + name); return -1; }
-  if (p->shape != shape) {
-    std::string s = "parameter " + name + " has shape (";
-    for (auto d : p->shape) s += std::to_string(d) + ",";
-    s += ") expected (";
-    for (auto d : shape) s += std::to_string(d) + ",";
-    set_last_error(s + ")");
-    return -1;
-  }
-  *out = p;
-  return 0;
-}
-
 // conv weight (co, ci, 1, kh, kw) -> [ (ky*kw+kx)*ci_pad + c ][ldb]
-int pack_conv(dawn_unet* h, const std::string& prefix, int co, int ci, int kh, int kw, int ci_pad, bool bias, ConvW* out) {
+int pack_conv(dawn_unet* h, const std::string& prefix, int co, int ci, int kh, int kw, int ci_pad, bool bias, PackedWeight* out) {
   const HostParam* w; const HostParam* b = nullptr;
-  DAWN_TRY(need(h, prefix + ".weight", {co, ci, 1, kh, kw}, &w));
-  if (bias) DAWN_TRY(need(h, prefix + ".bias", {co}, &b));
+  DAWN_TRY(h->raw.need(prefix + ".weight", {co, ci, 1, kh, kw}, &w));
+  if (bias) DAWN_TRY(h->raw.need(prefix + ".bias", {co}, &b));
   const int ldb = round_up(co, 64);
   const int K = kh * kw * ci_pad;
   std::vector<float> m((size_t)K * ldb, 0.f);
@@ -315,22 +241,13 @@ int pack_conv(dawn_unet* h, const std::string& prefix, int co, int ci, int kh, i
     for (int c = 0; c < ci; ++c)
       for (int t = 0; t < kh * kw; ++t)
         m[((size_t)t * ci_pad + c) * ldb + n] = w->data[((size_t)n * ci + c) * kh * kw + t];
-  DAWN_TRY(dev_upload(h, m, &out->w));
-  DAWN_TRY(upload_tc_image(h, m, K, co, ldb, &out->img, &out->img_scale));
-  out->b = nullptr;
-  if (bias) {
-    std::vector<float> bb(ldb, 0.f);
-    std::copy(b->data.begin(), b->data.end(), bb.begin());
-    DAWN_TRY(dev_upload(h, bb, &out->b));
-  }
-  out->K = K; out->N = co; out->ldb = ldb;
-  return 0;
+  return upload_weight(h->owned, m, K, co, ldb, b ? b->data : std::vector<float>{}, out);
 }
 
 // Linear weight (N, K) [+ optional per-input gain, + per-output-row scale for the first `nscale` rows]
 // -> [K][ldb], plus column sums for the LayerNorm fold
-int pack_linear(dawn_unet* h, const HostParam* w, int N, int K, const float* gain, float qscale, int nscale,
-                float** Wout, float** wsum, int* ldb_out, float** img = nullptr, float* img_scale = nullptr) {
+int pack_linear(dawn_unet* h, const HostParam* w, int N, int K, const float* gain, float qscale, int nscale, PackedWeight* out,
+                float** wsum) {
   const int ldb = round_up(N, 64);
   std::vector<float> m((size_t)K * ldb, 0.f), s(ldb, 0.f);
   for (int n = 0; n < N; ++n) {
@@ -345,17 +262,15 @@ int pack_linear(dawn_unet* h, const HostParam* w, int N, int K, const float* gai
     }
     s[n] = (float)acc;
   }
-  DAWN_TRY(dev_upload(h, m, Wout));
-  if (img) DAWN_TRY(upload_tc_image(h, m, K, N, ldb, img, img_scale));
-  if (wsum) DAWN_TRY(dev_upload(h, s, wsum));
-  if (ldb_out) *ldb_out = ldb;
+  DAWN_TRY(upload_weight(h->owned, m, K, N, ldb, {}, out));
+  if (wsum) DAWN_TRY(dev_upload(h->owned, s, wsum));
   return 0;
 }
 
 int upload_raw(dawn_unet* h, const std::string& name, std::vector<int64_t> shape, float** out) {
   const HostParam* p;
-  DAWN_TRY(need(h, name, shape, &p));
-  return dev_upload(h, p->data, out);
+  DAWN_TRY(h->raw.need(name, shape, &p));
+  return dev_upload(h->owned, p->data, out);
 }
 
 int pack_resblock(dawn_unet* h, const std::string& name, int ci, int co, bool cond, int* stat_counter) {
@@ -384,8 +299,8 @@ int pack_resblock(dawn_unet* h, const std::string& name, int ci, int co, bool co
       DAWN_TRY(upload_raw(h, name + "." + mlp[a] + ".1.bias", {2 * co}, &r.mB[a]));
       const std::string p = name + "." + can[a];
       const HostParam *g, *q;
-      DAWN_TRY(need(h, p + ".norm.g", {ci}, &g));
-      DAWN_TRY(need(h, p + ".to_q.weight", {64, ci}, &q));
+      DAWN_TRY(h->raw.need(p + ".norm.g", {ci}, &g));
+      DAWN_TRY(h->raw.need(p + ".to_q.weight", {64, ci}, &q));
       for (int j = 0; j < 64; ++j) {
         double acc = 0.0;
         for (int k = 0; k < ci; ++k) {
@@ -402,17 +317,12 @@ int pack_resblock(dawn_unet* h, const std::string& name, int ci, int co, bool co
       DAWN_TRY(upload_raw(h, p + ".to_out.0.weight", {co, 64}, &r.ca[a].Wout));
       DAWN_TRY(upload_raw(h, p + ".to_out.1.g", {co}, &r.ca[a].gout));
     }
-    DAWN_TRY(dev_upload(h, wq, &r.Wq));
-    DAWN_TRY(upload_tc_image(h, wq, ci, 192, 192, &r.Wq_img, &r.Wq_scale));
-    DAWN_TRY(dev_upload(h, wsum, &r.wsumq));
+    DAWN_TRY(upload_weight(h->owned, wq, ci, 192, 192, {}, &r.wq));
+    DAWN_TRY(dev_upload(h->owned, wsum, &r.wsumq));
     if (ci == 64 || ci == 128) {
       std::vector<uint16_t> W;
       ca_fused_pack(wq.data(), ci, W, &r.f_inv_wscale);
-      std::vector<float> tmp(W.size() / 2);
-      memcpy(tmp.data(), W.data(), W.size() * 2);
-      float* d = nullptr;
-      DAWN_TRY(dev_upload(h, tmp, &d));
-      r.fWq = reinterpret_cast<uint16_t*>(d);
+      DAWN_TRY(dev_upload(h->owned, W, &r.fWq));
     }
   }
   h->rb_index[name] = (int)h->rb.size();
@@ -422,63 +332,50 @@ int pack_resblock(dawn_unet* h, const std::string& name, int ci, int co, bool co
 
 int pack_attn(dawn_unet* h, const std::string& norm_name, const std::string& fn, int C, AttnW* a) {
   const HostParam *g, *qkv, *o;
-  DAWN_TRY(need(h, norm_name + ".gamma", {1, C, 1, 1, 1}, &g));
-  DAWN_TRY(need(h, fn + ".to_qkv.weight", {768, C}, &qkv));
-  DAWN_TRY(need(h, fn + ".to_out.weight", {C, 256}, &o));
+  DAWN_TRY(h->raw.need(norm_name + ".gamma", {1, C, 1, 1, 1}, &g));
+  DAWN_TRY(h->raw.need(fn + ".to_qkv.weight", {768, C}, &qkv));
+  DAWN_TRY(h->raw.need(fn + ".to_out.weight", {C, 256}, &o));
   a->C = C;
   const float scale = 1.0f / sqrtf(32.0f);                                   // q * dim_head^-0.5 (U:657, 687)
-  DAWN_TRY(pack_linear(h, qkv, 768, C, g->data.data(), scale, 256, &a->Wqkv, &a->wsum, nullptr, &a->Wqkv_img, &a->Wqkv_scale));
-  int ldb = 0;
-  DAWN_TRY(pack_linear(h, o, C, 256, nullptr, 1.f, 0, &a->out.w, nullptr, &ldb, &a->out.img, &a->out.img_scale));
-  a->out.b = nullptr; a->out.K = 256; a->out.N = C; a->out.ldb = ldb;
+  DAWN_TRY(pack_linear(h, qkv, 768, C, g->data.data(), scale, 256, &a->qkv, &a->wsum));
+  DAWN_TRY(pack_linear(h, o, C, 256, nullptr, 1.f, 0, &a->out, nullptr));
   if (C == 64) {
     std::vector<float> wq((size_t)768 * C);
     for (int n = 0; n < 768; ++n)
       for (int k = 0; k < C; ++k) wq[(size_t)n * C + k] = qkv->data[(size_t)n * C + k] * g->data[k] * (n < 256 ? scale : 1.0f);
     std::vector<uint16_t> Wq, Wo;
     temporal_fused_pack(wq.data(), o->data.data(), Wq, Wo, &a->f_inv_wscale, &a->f_inv_oscale);
-    float *dq = nullptr, *dout = nullptr;
-    std::vector<float> tq(Wq.size() / 2), to(Wo.size() / 2);
-    memcpy(tq.data(), Wq.data(), Wq.size() * 2); memcpy(to.data(), Wo.data(), Wo.size() * 2);
-    DAWN_TRY(dev_upload(h, tq, &dq)); DAWN_TRY(dev_upload(h, to, &dout));
-    a->fq = reinterpret_cast<uint16_t*>(dq); a->fo = reinterpret_cast<uint16_t*>(dout);
+    DAWN_TRY(dev_upload(h->owned, Wq, &a->fq));
+    DAWN_TRY(dev_upload(h->owned, Wo, &a->fo));
   }
   return 0;
 }
 
 int pack_sla(dawn_unet* h, const std::string& p, int C, SlaW* s) {        // p = "downs.L.2.fn"
   const HostParam *g, *qkv, *o, *b;
-  DAWN_TRY(need(h, p + ".norm.gamma", {1, C, 1, 1, 1}, &g));
-  DAWN_TRY(need(h, p + ".fn.to_qkv.weight", {768, C, 1, 1}, &qkv));
-  DAWN_TRY(need(h, p + ".fn.to_out.weight", {C, 256, 1, 1}, &o));
-  DAWN_TRY(need(h, p + ".fn.to_out.bias", {C}, &b));
+  DAWN_TRY(h->raw.need(p + ".norm.gamma", {1, C, 1, 1, 1}, &g));
+  DAWN_TRY(h->raw.need(p + ".fn.to_qkv.weight", {768, C, 1, 1}, &qkv));
+  DAWN_TRY(h->raw.need(p + ".fn.to_out.weight", {C, 256, 1, 1}, &o));
+  DAWN_TRY(h->raw.need(p + ".fn.to_out.bias", {C}, &b));
   s->C = C;
-  DAWN_TRY(pack_linear(h, qkv, 768, C, g->data.data(), 1.f, 0, &s->Wqkv, &s->wsum, nullptr, &s->Wqkv_img, &s->Wqkv_scale));
+  DAWN_TRY(pack_linear(h, qkv, 768, C, g->data.data(), 1.f, 0, &s->qkv, &s->wsum));
   if (C == 64) {
-    DAWN_TRY(pack_linear(h, qkv, 256, C, g->data.data(), 1.f, 0, &s->Wq, &s->wsum_q, nullptr, &s->Wq_img, &s->Wq_scale));
     std::vector<float> wf((size_t)768 * C);
     for (int n = 0; n < 768; ++n)
       for (int k = 0; k < C; ++k) wf[(size_t)n * C + k] = qkv->data[(size_t)n * C + k] * g->data[k];
     std::vector<uint16_t> W;
     sla_fused_pack(wf.data(), W, &s->f_inv_wscale);
-    std::vector<float> tmp(W.size() / 2);
-    memcpy(tmp.data(), W.data(), W.size() * 2);
-    float* d = nullptr;
-    DAWN_TRY(dev_upload(h, tmp, &d));
-    s->fkv = reinterpret_cast<uint16_t*>(d);
+    DAWN_TRY(dev_upload(h->owned, W, &s->fkv));
     sla_out_pack(wf.data(), W, &s->fq_inv_wscale);
-    tmp.assign(W.size() / 2, 0.f);
-    memcpy(tmp.data(), W.data(), W.size() * 2);
-    DAWN_TRY(dev_upload(h, tmp, &d));
-    s->fq = reinterpret_cast<uint16_t*>(d);
+    DAWN_TRY(dev_upload(h->owned, W, &s->fq));
   }
   std::vector<float> wt((size_t)256 * C);
   for (int c = 0; c < C; ++c)
     for (int k = 0; k < 256; ++k) wt[(size_t)k * C + c] = o->data[(size_t)c * 256 + k];
-  DAWN_TRY(dev_upload(h, wt, &s->WoutT));
+  DAWN_TRY(dev_upload(h->owned, wt, &s->WoutT));
   std::vector<float> bb(round_up(C, 64), 0.f);
   std::copy(b->data.begin(), b->data.end(), bb.begin());
-  DAWN_TRY(dev_upload(h, bb, &s->bout));
+  DAWN_TRY(dev_upload(h->owned, bb, &s->bout));
   return 0;
 }
 
@@ -486,75 +383,17 @@ int pack_sla(dawn_unet* h, const std::string& p, int C, SlaW* s) {        // p =
 // out[y] gets in[(y+1-ky)/2]: y even -> ky in {1 (dy 0), 3 (dy -1)}; y odd -> ky in {0 (dy +1), 2 (dy 0)}.   (U:165-167)
 static const int kUpK[2][2] = {{1, 3}, {0, 2}};
 static const int kUpD[2][2] = {{0, -1}, {1, 0}};
-int pack_up(dawn_unet* h, const std::string& name, int C, UpW* u) {
+int pack_up(dawn_unet* h, const std::string& name, int C, UpConv* u) {
   const HostParam *w, *b;
-  DAWN_TRY(need(h, name + ".weight", {C, C, 1, 4, 4}, &w));
-  DAWN_TRY(need(h, name + ".bias", {C}, &b));
-  const int ldb = round_up(C, 64);
-  std::vector<float> bb(ldb, 0.f);
-  std::copy(b->data.begin(), b->data.end(), bb.begin());
-  float* bdev;
-  DAWN_TRY(dev_upload(h, bb, &bdev));
-  for (int py = 0; py < 2; ++py)
-    for (int px = 0; px < 2; ++px) {
-      std::vector<float> m((size_t)4 * C * ldb, 0.f);
-      for (int ty = 0; ty < 2; ++ty)
-        for (int tx = 0; tx < 2; ++tx) {
-          const int ky = kUpK[py][ty], kx = kUpK[px][tx];
-          for (int c = 0; c < C; ++c)
-            for (int n = 0; n < C; ++n)
-              m[((size_t)(ty * 2 + tx) * C + c) * ldb + n] = w->data[(((size_t)c * C + n) * 4 + ky) * 4 + kx];
-        }
-      ConvW& cw = u->cls[py * 2 + px];
-      DAWN_TRY(dev_upload(h, m, &cw.w));
-      DAWN_TRY(upload_tc_image(h, m, 4 * C, C, ldb, &cw.img, &cw.img_scale));
-      cw.b = bdev; cw.K = 4 * C; cw.N = C; cw.ldb = ldb;
-    }
-  if (C == 64) {
-    // one 3x3 conv over the input grid producing all four output parities: weight rows (tap, cin), columns (class, cout);
-    // taps a class does not touch stay zero (2.25x the MACs, one launch of the halo-tile kernel instead of four gather GEMMs)
-    const int N4 = 4 * C;
-    std::vector<float> m((size_t)9 * C * N4, 0.f), b4(N4, 0.f);
-    for (int py = 0; py < 2; ++py)
-      for (int px = 0; px < 2; ++px) {
-        const int cls = py * 2 + px;
-        for (int n = 0; n < C; ++n) b4[cls * C + n] = b->data[n];
-        for (int ty = 0; ty < 2; ++ty)
-          for (int tx = 0; tx < 2; ++tx) {
-            const int ky = kUpK[py][ty], kx = kUpK[px][tx];
-            const int tap = (kUpD[py][ty] + 1) * 3 + (kUpD[px][tx] + 1);
-            for (int c = 0; c < C; ++c)
-              for (int n = 0; n < C; ++n)
-                m[((size_t)tap * C + c) * N4 + cls * C + n] = w->data[(((size_t)c * C + n) * 4 + ky) * 4 + kx];
-          }
-      }
-    DAWN_TRY(dev_upload(h, m, &u->all.w));
-    DAWN_TRY(upload_tc_image(h, m, 9 * C, N4, N4, &u->all.img, &u->all.img_scale));
-    DAWN_TRY(dev_upload(h, b4, &u->all.b));
-    u->all.K = 9 * C; u->all.N = N4; u->all.ldb = N4;
-  }
-  return 0;
+  DAWN_TRY(h->raw.need(name + ".weight", {C, C, 1, 4, 4}, &w));
+  DAWN_TRY(h->raw.need(name + ".bias", {C}, &b));
+  return dawn::pack_up(h->owned, C, C, kUpD, b->data, [&](int py, int px, int ty, int tx, int c, int n) {
+    return w->data[(((size_t)c * C + n) * 4 + kUpK[py][ty]) * 4 + kUpK[px][tx]];
+  }, u);
 }
 
 // ------------------------------------------------------------------------------------------ GEMM wrappers
-void base_params(GemmParams& p, const Act& in, int F) {
-  memset(&p, 0, sizeof(p));
-  p.A = in.p; p.lda = in.ld; p.Cin = in.C;
-  p.IH = in.H; p.IW = in.W; p.OHs = in.H; p.OWs = in.W; p.in_stride = 1;
-  p.ntaps = 1; p.dy[0] = 0; p.dx[0] = 0;
-  p.M = F * in.H * in.W; p.rows_per_batch = p.M;
-  p.OH = in.H; p.OW = in.W; p.out_stride = 1; p.oy0 = 0; p.ox0 = 0;
-  p.P = in.H * in.W;
-  p.q_post_scale = 1.f;
-}
-void set_weights(GemmParams& p, const ConvW& w) {
-  p.B = w.w; p.Bimg = w.img; p.tc_scale = 1.0f / (kTcActScale * w.img_scale); p.ldb = w.ldb; p.b_batch_stride = 0; p.N = w.N; p.K = w.K; p.bias = w.b;
-}
-void set_square_taps(GemmParams& p, int k, int pad) {
-  p.ntaps = k * k;
-  for (int ky = 0; ky < k; ++ky)
-    for (int kx = 0; kx < k; ++kx) { p.dy[ky * k + kx] = (signed char)(ky - pad); p.dx[ky * k + kx] = (signed char)(kx - pad); }
-}
+void base_params(GemmParams& p, const Act& in, int F) { dawn::base_params(p, in.p, in.ld, in.C, F, in.H, in.W); }
 
 
 // profile categories (dawn_unet_profile_read)
@@ -605,30 +444,20 @@ struct ProfScope {
 };
 
 int Ctx::gemm(const GemmParams& p, int epi, int cat) {
-  // algorithmic work: 2*M*N*K flops (1x, not the 3 split passes); bytes: A once + output write (+ residual/Y read)
-  const double flops = 2.0 * p.M * (double)p.N * p.K;
+  // algorithmic work: 2*M*N*K flops (1x, not the 3 split passes; an up2 conv's classes use 4 of its 9 taps);
+  // bytes: A once + output write (+ residual/Y read)
+  const double flops = 2.0 * p.M * (double)p.N * (p.up2 ? p.K / 9 * 4 : p.K);
   double bytes = 4.0 * p.M * ((double)p.Cin * (p.in_stride == 1 ? 1 : 4) + p.N);
   if (p.Res) bytes += 4.0 * p.M * p.N;
   if (p.Y) bytes += 4.0 * p.M * p.N;
   if (epi == EPI_CA_GATE) bytes = 4.0 * p.M * (p.Cin + 24.0);
   ProfScope ps(*this, cat, flops, bytes);
-  if (p.Bimg != nullptr && tc_conv3_supported(p, epi)) return launch_tc_conv3(p, p.Bimg, st);
-  if (p.Bimg != nullptr && tc_gemm_supported(p, epi)) {
-    // several n-tiles re-convert the same A panels (per-tap gather of the small levels' 3x3 convolutions): split once instead
-    const long long in_rows = (long long)(p.M / (p.OHs * p.OWs)) * p.IH * p.IW;
-    const size_t need = (size_t)in_rows * p.Cin * 4;                                   // two fp16 planes
-    const size_t have = (size_t)(h->F + 2 * h->cfg.win_width) * h->lH[0] * h->lW[0] * 256 * sizeof(float);
-    if (((p.ntaps == 9 && p.N >= 256 && !p.perm_in) || p.want_split) && p.Cin % 64 == 0 && need <= have) {
-      GemmParams q = p;
-      unsigned short* hi = reinterpret_cast<unsigned short*>(h->O);
-      q.A16h = hi; q.A16l = hi + (size_t)in_rows * p.Cin;
-      h->launches++;
-      DAWN_TRY(launch_split_rows(p.A, p.lda, p.Cin, in_rows, (void*)q.A16h, (void*)q.A16l, st));
-      return launch_tc_gemm(q, q.Bimg, epi, st);
-    }
-    return launch_tc_gemm(p, p.Bimg, epi, st);
-  }
-  return launch_gemm(p, epi, st);
+  // the attention output buffer O doubles as the scratch of the pre-split planes
+  const size_t scratch = (size_t)(h->F + 2 * h->cfg.win_width) * h->lH[0] * h->lW[0] * 256 * sizeof(float);
+  int kernels = 0;
+  const int rc = launch_path(p, epi, choose_path(p, epi, scratch), h->O, st, &kernels);
+  h->launches += kernels - 1;                     // ProfScope counted one
+  return rc;
 }
 
 int tap(Ctx& c, const std::string& name, const Act& a);
@@ -638,7 +467,7 @@ int tap(Ctx& c, const std::string& name, const Act& a);
 int ln_gemm(Ctx& c, GemmParams& p, int epi, int cat, const float* x, int ldx, int C, int rows) {
   dawn_unet* h = c.h;
   p.ln_inline = 0; p.rowstats = h->ROWSTATS;
-  const bool tc_ok = p.Bimg != nullptr && tc_gemm_supported(p, epi) && p.ntaps == 1;
+  const bool tc_ok = path_ok(p, epi, DAWN_PATH_TC_GEMM, 0) && p.ntaps == 1;
   if (tc_ok && (p.N >= 384 || (p.N == 192 && p.Cin >= 256)) && p.Cin % 64 == 0) {
     // N = 768 is six 128-column tiles, each re-gathering and re-splitting the same A panels: split once (cp.async producers),
     // row statistics from the stand-alone kernel
@@ -655,15 +484,16 @@ int ln_gemm(Ctx& c, GemmParams& p, int epi, int cat, const float* x, int ldx, in
 }
 
 // conv k x k, stride 1, same padding, + bias, optional GroupNorm statistics slot
-int conv_same(Ctx& c, const Act& in, const ConvW& w, int k, const Act& out, int stat_slot, const unsigned short* in16h = nullptr,
-              const unsigned short* in16l = nullptr) {
+GemmParams conv_same_params(Ctx& c, const Act& in, const PackedWeight& w, int k, const Act& out, int stat_slot) {
   GemmParams p; base_params(p, in, c.h->F);
   set_weights(p, w); set_square_taps(p, k, k / 2);
   p.Out = out.p; p.ldo = out.ld;
-  p.A16h = in16h; p.A16l = in16l;               // the input exists as fp16 hi | lo planes (and NOT as fp32): halo conv by TMA
   if (stat_slot >= 0) { p.stats = c.h->STATS + 16 * stat_slot; p.cpg = w.N / 8; }
-  const bool l0 = in.H == c.h->lH[0] && in.C == c.h->cfg.dim && w.N == c.h->cfg.dim;
-  return c.gemm(p, EPI_PLAIN, k == 3 ? (l0 ? PC_CONV3_L0 : PC_CONV3) : PC_CONV_OTHER);
+  return p;
+}
+int conv_same(Ctx& c, const GemmParams& p) {
+  const bool l0 = p.IH == c.h->lH[0] && p.Cin == c.h->cfg.dim && p.N == c.h->cfg.dim;
+  return c.gemm(p, EPI_PLAIN, p.ntaps == 9 ? (l0 ? PC_CONV3_L0 : PC_CONV3) : PC_CONV_OTHER);
 }
 
 // GroupNorm statistics span all frames of the clip: with frame sharding the 16 partial sums are all-reduced (fp64)
@@ -699,30 +529,25 @@ int resblock(Ctx& c, const ResBlockW& r, const Act& x, const Act& out) {
   } else if (r.cond) {
     // cross-attention gates from the raw block input (U:454-463): LayerNorm_img folded into the q projection
     GemmParams p; base_params(p, x, F);
-    p.B = r.Wq; p.Bimg = r.Wq_img; p.tc_scale = 1.0f / (kTcActScale * r.Wq_scale); p.ldb = 192; p.N = 192; p.K = r.ci;
+    set_weights(p, r.wq);
     p.wsum = r.wsumq; p.kq = r.kq; p.nkq = r.nkq; p.gates = h->GATES;
     DAWN_TRY(ln_gemm(c, p, EPI_CA_GATE, PC_CA_GATE, x.p, x.ld, x.C, M));
     ProfScope ps(c, PC_CA_RSTD, 0, 4.0 * M * 56);
     DAWN_TRY(launch_ca_rstd(h->GATES, r.G, M, P, h->WT, c.st));
   }
-  DAWN_TRY(conv_same(c, x, r.c1, 3, y, r.st1));
+  DAWN_TRY(conv_same(c, conv_same_params(c, x, r.c1, 3, y, r.st1)));
   DAWN_TRY(gn_allreduce(c, r.st1));
   // a1 is consumed by the second conv only: when that conv runs on the halo-tile wgmma kernel, a1 is written as two fp16 planes
-  // (hi | lo, the same bytes as the fp32 row) and the conv fetches its tiles by TMA
-  const unsigned short *a1h = nullptr, *a1l = nullptr;
-  if (r.cond && gn_hcond_supported(r.co, P) && r.c2.img != nullptr) {
-    GemmParams q; base_params(q, a1, F);
-    set_weights(q, r.c2); set_square_taps(q, 3, 1);
-    q.Out = y.p; q.ldo = y.ld; q.stats = h->STATS + 16 * r.st2; q.cpg = r.co / 8;
-    if (tc_conv3_supported(q, EPI_PLAIN)) {
-      a1h = reinterpret_cast<const unsigned short*>(h->A1);
-      a1l = a1h + (size_t)M * r.co;
-    }
+  // (hi | lo, the same bytes as the fp32 row, and no fp32 copy) and the conv fetches its tiles by TMA
+  GemmParams conv2 = conv_same_params(c, a1, r.c2, 3, y, r.st2);
+  if (r.cond && gn_hcond_supported(r.co, P) && path_ok(conv2, EPI_PLAIN, DAWN_PATH_TC_CONV3, 0)) {
+    conv2.A16h = reinterpret_cast<const unsigned short*>(h->A1);
+    conv2.A16l = conv2.A16h + (size_t)M * r.co;
   }
   if (r.cond && gn_hcond_supported(r.co, P)) {
     GnHcondArgs a{};
     a.Wt = h->WT; a.T = r.T; a.ldbT = r.ldbT; a.Y = y.p; a.ldy = y.ld; a.Out = a1.p; a.ldo = a1.ld;
-    a.Out16h = const_cast<unsigned short*>(a1h); a.Out16l = const_cast<unsigned short*>(a1l);
+    a.Out16h = const_cast<unsigned short*>(conv2.A16h); a.Out16l = const_cast<unsigned short*>(conv2.A16l);
     a.F = F; a.P = P; a.co = r.co;
     a.gn_stats = h->STATS + 16 * r.st1; a.gn_count = count; a.cpg = r.co / 8;
     a.gn_w = r.gn1w; a.gn_b = r.gn1b; a.film = r.film;
@@ -743,14 +568,11 @@ int resblock(Ctx& c, const ResBlockW& r, const Act& x, const Act& out) {
     DAWN_TRY(launch_gn_apply(y.p, y.ld, r.co, M, h->STATS + 16 * r.st1, count, r.co / 8, r.gn1w, r.gn1b, nullptr,
                              nullptr, 0, a1.p, a1.ld, c.st));
   }
-  DAWN_TRY(conv_same(c, a1, r.c2, 3, y, r.st2, a1h, a1l));
+  DAWN_TRY(conv_same(c, conv2));
   DAWN_TRY(gn_allreduce(c, r.st2));
   const float* res = x.p; int ldr = x.ld;
   if (r.res) {
-    GemmParams p; base_params(p, x, F);
-    set_weights(p, r.cres);
-    p.Out = out.p; p.ldo = out.ld;
-    DAWN_TRY(c.gemm(p, EPI_PLAIN, PC_CONV_OTHER));
+    DAWN_TRY(conv_same(c, conv_same_params(c, x, r.cres, 1, out, -1)));
     res = out.p; ldr = out.ld;
   }
   {
@@ -811,7 +633,7 @@ int temporal_attn(Ctx& c, const AttnW& w, const Act& x, const Act& dst, const st
   }
   {
     GemmParams p; base_params(p, xe, Fe);
-    p.B = w.Wqkv; p.Bimg = w.Wqkv_img; p.tc_scale = 1.0f / (kTcActScale * w.Wqkv_scale); p.ldb = 768; p.N = 768; p.K = x.C;
+    set_weights(p, w.qkv);
     p.wsum = w.wsum; p.rot = h->ROT;
     p.Out = h->QKV; p.ldo = 768;
     p.perm_pb = pb; p.perm_F = Fe; p.perm_in = 1; p.perm_out = 0;
@@ -848,7 +670,7 @@ int mid_spatial_attn(Ctx& c, const AttnW& w, const Act& x, const std::string& na
   const int F = h->F, P = x.H * x.W, M = F * P;
   {
     GemmParams p; base_params(p, x, F);
-    p.B = w.Wqkv; p.Bimg = w.Wqkv_img; p.tc_scale = 1.0f / (kTcActScale * w.Wqkv_scale); p.ldb = 768; p.N = 768; p.K = x.C;
+    set_weights(p, w.qkv);
     p.wsum = w.wsum;
     p.Out = h->QKV; p.ldo = 768;
     DAWN_TRY(ln_gemm(c, p, EPI_QKV_MID, PC_QKV, x.p, x.ld, x.C, M));
@@ -897,7 +719,7 @@ int sla(Ctx& c, const SlaW& w, const Act& x, const std::string& name) {
     return tap(c, name, x);
   } else {
     GemmParams p; base_params(p, x, F);
-    p.B = w.Wqkv; p.Bimg = w.Wqkv_img; p.tc_scale = 1.0f / (kTcActScale * w.Wqkv_scale); p.ldb = 768; p.N = 768; p.K = x.C;
+    set_weights(p, w.qkv);
     p.wsum = w.wsum; p.q_post_scale = 1.0f / sqrtf(32.0f);
     p.Out = h->QKV; p.ldo = 768;
     DAWN_TRY(ln_gemm(c, p, EPI_QKV_SLA, PC_QKV, x.p, x.ld, x.C, M));
@@ -917,13 +739,11 @@ int sla(Ctx& c, const SlaW& w, const Act& x, const std::string& name) {
   return tap(c, name, x);
 }
 
-int downsample(Ctx& c, const ConvW& w, const Act& x, const Act& out, const std::string& name) {   // U:175-176
+int downsample(Ctx& c, const PackedWeight& w, const Act& x, const Act& out, const std::string& name) {   // U:175-176
   GemmParams p; base_params(p, x, c.h->F);
   set_weights(p, w);
   p.OHs = out.H; p.OWs = out.W; p.in_stride = 2;
-  p.ntaps = 16;
-  for (int ky = 0; ky < 4; ++ky)
-    for (int kx = 0; kx < 4; ++kx) { p.dy[ky * 4 + kx] = (signed char)(ky - 1); p.dx[ky * 4 + kx] = (signed char)(kx - 1); }
+  set_square_taps(p, 4, 1);
   p.M = c.h->F * out.H * out.W; p.rows_per_batch = p.M;
   p.OH = out.H; p.OW = out.W; p.P = out.H * out.W;
   p.Out = out.p; p.ldo = out.ld;
@@ -931,28 +751,9 @@ int downsample(Ctx& c, const ConvW& w, const Act& x, const Act& out, const std::
   return tap(c, name, out);
 }
 
-int upsample(Ctx& c, const UpW& u, const Act& x, const Act& out, const std::string& name) {       // U:165-167
-  if (u.all.img != nullptr) {
-    GemmParams p; base_params(p, x, c.h->F);
-    set_weights(p, u.all); set_square_taps(p, 3, 1);
-    p.up2 = 1; p.Out = out.p; p.ldo = out.ld;
-    if (tc_conv3_supported(p, EPI_PLAIN)) {
-      ProfScope ps(c, PC_CONV_OTHER, 2.0 * p.M * 4.0 * x.C * x.C * 4, 4.0 * p.M * (x.C + 4.0 * x.C));
-      DAWN_TRY(launch_tc_conv3(p, p.Bimg, c.st));
-      return tap(c, name, out);
-    }
-  }
-  for (int py = 0; py < 2; ++py)
-    for (int px = 0; px < 2; ++px) {
-      GemmParams p; base_params(p, x, c.h->F);
-      set_weights(p, u.cls[py * 2 + px]);
-      p.ntaps = 4;
-      for (int ty = 0; ty < 2; ++ty)
-        for (int tx = 0; tx < 2; ++tx) { p.dy[ty * 2 + tx] = (signed char)kUpD[py][ty]; p.dx[ty * 2 + tx] = (signed char)kUpD[px][tx]; }
-      p.OH = out.H; p.OW = out.W; p.out_stride = 2; p.oy0 = py; p.ox0 = px;
-      p.Out = out.p; p.ldo = out.ld;
-      DAWN_TRY(c.gemm(p, EPI_PLAIN, PC_CONV_OTHER));
-    }
+int upsample(Ctx& c, const UpConv& u, const Act& x, const Act& out, const std::string& name) {   // U:165-167
+  GemmParams p; base_params(p, x, c.h->F);
+  DAWN_TRY(run_up(p, u, out.p, out.ld, [&](const GemmParams& q) { return c.gemm(q, EPI_PLAIN, PC_CONV_OTHER); }));
   return tap(c, name, out);
 }
 
@@ -1004,7 +805,7 @@ int init_map(dawn_unet* h, const float* fea, long long cstride, cudaStream_t st,
     p.Out = h->MAPPART; p.ldo = dim;
     p.skip_flag = skip_flag; p.skip_if = skip_if;
     ProfScope ps(c, PC_PREP, 0, 0);
-    DAWN_TRY(launch_gemm(p, EPI_PLAIN, st));
+    DAWN_TRY(launch_path(p, EPI_PLAIN, DAWN_PATH_MMA_SYNC, nullptr, st));      // per-batch B and the skip flag: mma.sync only
   }
   ProfScope ps(c, PC_PREP, 0, 0);
   return launch_map_reduce(h->MAPPART, k, (long long)H0 * W0 * dim, h->init_full.b, dim, h->MAP, st, skip_flag, skip_if);
@@ -1146,10 +947,7 @@ void dawn_unet_destroy(dawn_unet* h) {
 
 int dawn_unet_set_param(dawn_unet* h, const char* name, const float* host, const int64_t* shape, int ndim) {
   DAWN_CHECK(h && name && host && (shape || ndim == 0), "null argument");
-  HostParam p;
-  p.shape.assign(shape, shape + ndim);
-  p.data.assign(host, host + p.numel());
-  h->raw[name] = std::move(p);
+  h->raw.set(name, host, shape, ndim);
   h->committed = false;
   return 0;
 }
@@ -1170,12 +968,12 @@ int dawn_unet_commit_params(dawn_unet* h) {
   DAWN_TRY(pack_conv(h, "init_conv", dim, cfg.channels, k, k, h->cin_pad, true, &h->init_full));
   {
     const HostParam* w;
-    DAWN_TRY(need(h, "init_conv.weight", {dim, cfg.channels, 1, k, k}, &w));
+    DAWN_TRY(h->raw.need("init_conv.weight", {dim, cfg.channels, 1, k, k}, &w));
     std::vector<float> w3((size_t)k * k * 3 * dim);
     for (int t = 0; t < k * k; ++t)
       for (int c = 0; c < 3; ++c)
         for (int n = 0; n < dim; ++n) w3[((size_t)t * 3 + c) * dim + n] = w->data[((size_t)n * cfg.channels + c) * k * k + t];
-    DAWN_TRY(dev_upload(h, w3, &h->init_w3));
+    DAWN_TRY(dev_upload(h->owned, w3, &h->init_w3));
   }
   DAWN_TRY(upload_raw(h, "aux.time_freqs", {dim / 2}, &h->time_freqs));
   DAWN_TRY(upload_raw(h, "aux.rel_bias", {8, 2 * cfg.win_width + 1}, &h->rel_bias));
@@ -1194,7 +992,7 @@ int dawn_unet_commit_params(dawn_unet* h) {
     SlaW s; DAWN_TRY(pack_sla(h, pre + ".2.fn", co, &s)); h->down_sla.push_back(s);
     AttnW a; DAWN_TRY(pack_attn(h, pre + ".3.fn.norm", pre + ".3.fn.fn.fn", co, &a)); h->down_ta.push_back(a);
     if (L < nlev - 1) {
-      ConvW d; DAWN_TRY(pack_conv(h, pre + ".4", co, co, 4, 4, co, true, &d)); h->down_conv.push_back(d);
+      PackedWeight d; DAWN_TRY(pack_conv(h, pre + ".4", co, co, 4, 4, co, true, &d)); h->down_conv.push_back(d);
     }
   }
   const int mid = h->dims.back();
@@ -1211,7 +1009,7 @@ int dawn_unet_commit_params(dawn_unet* h) {
     SlaW s; DAWN_TRY(pack_sla(h, pre + ".2.fn", ci, &s)); h->up_sla.push_back(s);
     AttnW a; DAWN_TRY(pack_attn(h, pre + ".3.fn.norm", pre + ".3.fn.fn.fn", ci, &a)); h->up_ta.push_back(a);
     if (K < nlev - 1) {
-      UpW u; DAWN_TRY(pack_up(h, pre + ".4", ci, &u)); h->up_conv.push_back(u);
+      UpConv u; DAWN_TRY(pack_up(h, pre + ".4", ci, &u)); h->up_conv.push_back(u);
     }
   }
   // heads: ResnetBlock_ca_mul without time/cond MLPs (their cross-attention parameters exist but never run, U:862, 875)
@@ -1376,7 +1174,7 @@ int dawn_unet_forward(dawn_unet* h, const float* x, const int64_t* t, const floa
     p.Out = h->XR + dim; p.ldo = 2 * dim;
     p.skip_flag = vary; p.skip_if = 0;
     ProfScope ps(c, PC_CONV_OTHER, 2.0 * p.M * (double)p.N * p.K, 4.0 * p.M * ((double)p.Cin + p.N));
-    DAWN_TRY(launch_gemm(p, EPI_PLAIN, st));      // Cin = 288 is not a wgmma-kernel shape: always the mma.sync kernel (it has the skip flag)
+    DAWN_TRY(launch_path(p, EPI_PLAIN, DAWN_PATH_MMA_SYNC, nullptr, st));      // only the mma.sync kernel has the skip flag
   }
   DAWN_TRY(init_map(h, x + (size_t)3 * h->F * H0 * W0, (long long)h->F * H0 * W0, st, vary, 1));
   {

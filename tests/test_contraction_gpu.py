@@ -1,7 +1,9 @@
 """GPU: every wgmma / mma.sync contraction path, one kernel at a time, against a float64 reference of the same operation.
 
-`dawn_test_contraction` (include/dawn_unet.h) runs one contraction through exactly one kernel path with the weight image and
-accumulator scale the network builds; a path that refuses the geometry returns -1 and launches nothing.  Each reference is
+`dawn_test_contraction` (include/dawn_unet.h) runs one contraction through exactly one kernel path with the code the UNet and
+the LFG decoder run (csrc/contraction.cu): the same weight upload builds the weight image and accumulator scale, the same
+path check accepts or refuses the geometry, and the same launcher enqueues the split pass and the kernel.  A path that
+refuses the geometry returns -1 and launches nothing.  Each reference is
 defined from the operation (conv2d, conv_transpose2d, LayerNorm, rotary, softmax, cosine-similarity gate, GroupNorm) in
 float64, on the GPU for the large cases and on the CPU for the small ones.
 

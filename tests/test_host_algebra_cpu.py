@@ -1,6 +1,7 @@
 """CPU: the algebraic rewrites the CUDA paths rely on, checked with plain torch ops (host-side logic, no GPU):
  * nearest-2x upsample + 3x3 conv == four output-parity 2x2 convs over the low-resolution grid with summed taps
-   (csrc/lfg.cu::pack_up, reference UpBlock2d LFG/modules/util.py:106-111);
+   (the summed taps in csrc/lfg.cu::pack_up, the class convs in csrc/contraction.cu::pack_up / run_up,
+   reference UpBlock2d LFG/modules/util.py:106-111);
  * a k x k conv == the sum of k row-convolutions (1 x k) over vertically shifted copies of the input
    (csrc/unet.cu::init_map, the per-clip part of the 7x7 init conv, reference U:776-777);
  * the init conv is linear in its input channels: conv(cat[x_t, fea]) == conv3(x_t) + map(fea)  (SURVEY a2, U:1167, 1177);
