@@ -1,5 +1,6 @@
 // DDIM update around the denoising UNet (reference U:1169-1205): x0 prediction, dynamic thresholding with the exact
 // 0.9-quantile of |x0| over the whole clip (torch.quantile semantics, linear interpolation), and the eta-noise update.
+// The ancestral (DDPM) update of p_sample (U:1087-1121) shares the same threshold.
 // Everything stays on the device: no host synchronisation inside a sampling step.
 #include "common.cuh"
 #include "sampler.cuh"
@@ -109,6 +110,78 @@ __global__ void ddim_update_kernel(float* __restrict__ x, const float* __restric
   }
 }
 
+// coefficients of this launch: the by-value set, or the table row of the timestep in the device slot (step graph)
+__device__ __forceinline__ DdpmCoef ddpm_coef(const DdpmCoef& c, const DdpmCoef* tab, const int64_t* t_slot, int num_t) {
+  if (!tab) return c;
+  const long long t = *t_slot;
+  return tab[t < 0 ? 0 : (t >= num_t ? num_t - 1 : t)];
+}
+
+// keys[i] = |x0| rounded like the reference's two products and one difference (U:1072-1076; no fused multiply-add: at
+// t = 999 the products are ~6e4 times x, so a contraction would move x0 by far more than an ulp of it)
+__global__ void ddpm_x0_abs_kernel(const float* __restrict__ x, const float* __restrict__ eps, DdpmCoef c,
+                                   const DdpmCoef* __restrict__ tab, const int64_t* __restrict__ t_slot, int num_t, long long n,
+                                   uint32_t* __restrict__ keys) {
+  const DdpmCoef k = ddpm_coef(c, tab, t_slot, num_t);
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    keys[i] = __float_as_uint(fabsf(__fsub_rn(__fmul_rn(k.ca, x[i]), __fmul_rn(k.cb, eps[i]))));
+}
+
+// x = c1 * clamp(x0, -s, s)/s + c2 * x + sigma * noise  (U:1078-1085, 1107, 1118-1121), each operation rounded as torch does;
+// clamp == 0: x0 is used as predicted (clip_denoised=False)
+__global__ void ddpm_update_kernel(float* __restrict__ x, const float* __restrict__ eps, const float* __restrict__ noise,
+                                   const float* __restrict__ s_ptr, DdpmCoef c, const DdpmCoef* __restrict__ tab,
+                                   const int64_t* __restrict__ t_slot, int num_t, long long n, int clamp) {
+  const DdpmCoef k = ddpm_coef(c, tab, t_slot, num_t);
+  const float s = s_ptr ? *s_ptr : 1.0f;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const float xi = x[i];
+    float x0 = __fsub_rn(__fmul_rn(k.ca, xi), __fmul_rn(k.cb, eps[i]));
+    if (clamp) x0 = __fdiv_rn(fminf(fmaxf(x0, -s), s), s);
+    float v = __fadd_rn(__fmul_rn(k.c1, x0), __fmul_rn(k.c2, xi));
+    if (noise) v = __fadd_rn(v, __fmul_rn(k.sigma, noise[i]));
+    x[i] = v;
+  }
+}
+
+// the step graph's last node: the next replay runs timestep t - 1
+__global__ void ddpm_advance_kernel(int64_t* t_slot) { *t_slot -= 1; }
+
+// s = max(1, q-quantile of the n_global keys) by exact radix select, written to scratch word 263 (*s_ptr points there).
+// write_keys(keys) enqueues the kernel that fills this rank's n keys at scratch word 512 once the select state is reset.
+// scratch layout (32-bit words): [0,4) select state | [4,260) histogram | [260,262) count_le (u64) | 262 min_gt | 263 s | [512, 512+n) keys
+template <class WriteKeys>
+int clip_threshold(void* scratch, long long n, int64_t n_global, float q, int blocks, cudaStream_t st, const DdimReduce* red,
+                   float** s_ptr, WriteKeys write_keys) {
+  const int threads = 256;
+  uint32_t* base = (uint32_t*)scratch;
+  uint32_t* state = base;
+  unsigned int* hist = base + 4;
+  unsigned long long* count_le = (unsigned long long*)(base + 260);
+  unsigned int* min_gt = base + 262;
+  float* s_out = (float*)(base + 263);
+  uint32_t* keys = base + 512;
+  // torch.quantile: ranks = q * (n - 1) evaluated in fp32 (ATen quantile_compute), lerp between floor and ceil
+  const float rank_f = q * (float)(n_global - 1);
+  const long long lo = (long long)floorf(rank_f), hi = (long long)ceilf(rank_f);
+  const float w = rank_f - floorf(rank_f);
+  select_init_kernel<<<1, 256, 0, st>>>(state, hist, count_le, min_gt, (unsigned long long)lo);
+  write_keys(keys);
+  for (int shift = 24; shift >= 0; shift -= 8) {
+    radix_hist_kernel<<<blocks, 256, 0, st>>>(keys, n, state, shift, hist);
+    if (red) DAWN_TRY(red->sum_u32(red->ctx, hist, 256, st));
+    radix_pick_kernel<<<1, 32, 0, st>>>(state, shift, hist);
+  }
+  next_stat_kernel<<<blocks, threads, 0, st>>>(keys, n, state, count_le, min_gt);
+  if (red) {
+    DAWN_TRY(red->sum_u64(red->ctx, count_le, 1, st));
+    DAWN_TRY(red->min_u32(red->ctx, min_gt, 1, st));
+  }
+  threshold_kernel<<<1, 1, 0, st>>>(state, count_le, min_gt, lo, hi, w, s_out);
+  *s_ptr = s_out;
+  return 0;
+}
+
 }  // namespace
 
 // One DDIM update in place on x (n_local floats of this rank's frames of the (3, F, h, w) latent).  The dynamic threshold
@@ -122,35 +195,39 @@ int ddim_step_impl(float* x, const float* eps, const float* noise, int64_t n_loc
   const int threads = 256;
   int blocks = (int)std::min<long long>((n + threads - 1) / threads, 148LL * 8);
   float* s_ptr = nullptr;
-  if (q > 0.f) {
-    // scratch layout (32-bit words): [0,4) select state | [4,260) histogram | [260,262) count_le (u64) | 262 min_gt | 263 s | [512, 512+n) keys
-    uint32_t* base = (uint32_t*)scratch;
-    uint32_t* state = base;
-    unsigned int* hist = base + 4;
-    unsigned long long* count_le = (unsigned long long*)(base + 260);
-    unsigned int* min_gt = base + 262;
-    float* s_out = (float*)(base + 263);
-    uint32_t* keys = base + 512;
-    // torch.quantile: ranks = q * (n - 1) evaluated in fp32 (ATen quantile_compute), lerp between floor and ceil
-    const float rank_f = q * (float)(n_global - 1);
-    const long long lo = (long long)floorf(rank_f), hi = (long long)ceilf(rank_f);
-    const float w = rank_f - floorf(rank_f);
-    select_init_kernel<<<1, 256, 0, st>>>(state, hist, count_le, min_gt, (unsigned long long)lo);
-    x0_abs_kernel<<<blocks, threads, 0, st>>>(x, eps, ca, cb, n, keys);
-    for (int shift = 24; shift >= 0; shift -= 8) {
-      radix_hist_kernel<<<blocks, 256, 0, st>>>(keys, n, state, shift, hist);
-      if (red) DAWN_TRY(red->sum_u32(red->ctx, hist, 256, st));
-      radix_pick_kernel<<<1, 32, 0, st>>>(state, shift, hist);
-    }
-    next_stat_kernel<<<blocks, threads, 0, st>>>(keys, n, state, count_le, min_gt);
-    if (red) {
-      DAWN_TRY(red->sum_u64(red->ctx, count_le, 1, st));
-      DAWN_TRY(red->min_u32(red->ctx, min_gt, 1, st));
-    }
-    threshold_kernel<<<1, 1, 0, st>>>(state, count_le, min_gt, lo, hi, w, s_out);
-    s_ptr = s_out;
-  }
+  if (q > 0.f)
+    DAWN_TRY(clip_threshold(scratch, n, n_global, q, blocks, st, red, &s_ptr, [&](uint32_t* keys) {
+      x0_abs_kernel<<<blocks, threads, 0, st>>>(x, eps, ca, cb, n, keys);
+    }));
   ddim_update_kernel<<<blocks, threads, 0, st>>>(x, eps, noise, s_ptr, ca, cb, sqrt_an, c, sigma, n, q < 0.f ? 0 : 1);
+  DAWN_LAUNCH_OK();
+  return 0;
+}
+
+// One ancestral update in place on x, same threshold and sharding as ddim_step_impl; the step graph passes `tab` and `t_slot`
+// so that one captured step serves every timestep.
+int ddpm_step_impl(float* x, const float* eps, const float* noise, int64_t n_local, int64_t n_global, DdpmCoef c,
+                   const DdpmCoef* tab, const int64_t* t_slot, int num_t, float q, void* scratch, cudaStream_t st,
+                   const DdimReduce* red) {
+  if (!x || !eps || !scratch || n_local <= 0 || n_global < n_local || (tab && (!t_slot || num_t < 1))) {
+    set_last_error("dawn_ddpm_step: bad argument");
+    return -1;
+  }
+  const long long n = n_local;
+  const int threads = 256;
+  int blocks = (int)std::min<long long>((n + threads - 1) / threads, 148LL * 8);
+  float* s_ptr = nullptr;
+  if (q > 0.f)
+    DAWN_TRY(clip_threshold(scratch, n, n_global, q, blocks, st, red, &s_ptr, [&](uint32_t* keys) {
+      ddpm_x0_abs_kernel<<<blocks, threads, 0, st>>>(x, eps, c, tab, t_slot, num_t, n, keys);
+    }));
+  ddpm_update_kernel<<<blocks, threads, 0, st>>>(x, eps, noise, s_ptr, c, tab, t_slot, num_t, n, q < 0.f ? 0 : 1);
+  DAWN_LAUNCH_OK();
+  return 0;
+}
+
+int ddpm_advance_slot(int64_t* t_slot, cudaStream_t st) {
+  ddpm_advance_kernel<<<1, 1, 0, st>>>(t_slot);
   DAWN_LAUNCH_OK();
   return 0;
 }
@@ -165,6 +242,13 @@ extern "C" {
 int dawn_ddim_step(float* x, const float* eps, const float* noise, int64_t n, float ca, float cb, float sqrt_an, float c,
                    float sigma, float q, void* scratch, void* stream) {
   return ddim_step_impl(x, eps, noise, n, n, ca, cb, sqrt_an, c, sigma, q, scratch, (cudaStream_t)stream, nullptr);
+}
+
+// single-GPU entry (see include/dawn_unet.h); dawn_unet_ddpm_step in unet.cu is the frame-sharded one
+int dawn_ddpm_step(float* x, const float* eps, const float* noise, int64_t n, float ca, float cb, float c1, float c2, float sigma,
+                   float q, void* scratch, void* stream) {
+  return ddpm_step_impl(x, eps, noise, n, n, DdpmCoef{ca, cb, c1, c2, sigma}, nullptr, nullptr, 0, q, scratch,
+                        (cudaStream_t)stream, nullptr);
 }
 
 }  // extern "C"

@@ -214,6 +214,10 @@ struct dawn_unet {
   cudaGraphExec_t samp_exec = nullptr;
   cudaStream_t samp_stream = nullptr;          // capture origin (the legacy default stream cannot be captured)
   int64_t samp_launches = 0;
+  // one ancestral step (forward_x3 + DDPM update + timestep advance) captured for T replays (dawn_unet_ddpm_capture); held
+  // beside samp_exec (neither capture drops the other) and invalidated by the same geometry changes
+  cudaGraphExec_t ddpm_exec = nullptr;
+  int64_t ddpm_launches = 0;
 
   // per-category kernel timing (CUDA events on the launching stream), see dawn_unet_profile_*
   bool prof_on = false;
@@ -936,6 +940,7 @@ void dawn_unet_destroy(dawn_unet* h) {
   if (!h) return;
   for (cudaEvent_t e : h->prof_ev) cudaEventDestroy(e);
   if (h->samp_exec) cudaGraphExecDestroy(h->samp_exec);
+  if (h->ddpm_exec) cudaGraphExecDestroy(h->ddpm_exec);
   if (h->samp_stream) cudaStreamDestroy(h->samp_stream);
   if (h->sh_comm && g_nccl.ok) g_nccl.CommDestroy(h->sh_comm);
   for (int r = 0; r < kP2pMaxRanks; ++r)
@@ -955,10 +960,18 @@ int dawn_unet_set_param(dawn_unet* h, const char* name, const float* host, const
 static void drop_sampler_graph(dawn_unet* h) {
   if (h->samp_exec) { cudaGraphExecDestroy(h->samp_exec); h->samp_exec = nullptr; }
 }
+static void drop_ddpm_graph(dawn_unet* h) {
+  if (h->ddpm_exec) { cudaGraphExecDestroy(h->ddpm_exec); h->ddpm_exec = nullptr; }
+}
+// a new geometry, parameter set or sharding invalidates both captured sampler graphs
+static void drop_graphs(dawn_unet* h) {
+  drop_sampler_graph(h);
+  drop_ddpm_graph(h);
+}
 
 int dawn_unet_commit_params(dawn_unet* h) {
   DAWN_CHECK(h, "null handle");
-  drop_sampler_graph(h);
+  drop_graphs(h);
   free_all(h->owned);
   h->rb.clear(); h->rb_index.clear();
   h->down_ta.clear(); h->up_ta.clear(); h->down_sla.clear(); h->up_sla.clear(); h->down_conv.clear(); h->up_conv.clear();
@@ -1029,7 +1042,7 @@ int dawn_unet_commit_params(dawn_unet* h) {
 
 int dawn_unet_set_num_frames(dawn_unet* h, int F, int height, int width) {
   DAWN_CHECK(h, "null handle");
-  drop_sampler_graph(h);
+  drop_graphs(h);
   DAWN_CHECK(h->committed, "commit_params must precede set_num_frames");
   DAWN_CHECK(F >= 1 && F <= 65535, "F out of range");
   const int nlev = h->nlev, dim = h->cfg.dim;
@@ -1262,7 +1275,7 @@ int dawn_unet_init_shard(dawn_unet* h, const char* id128, int nranks, int rank, 
   DAWN_CHECK(nranks >= 1 && rank >= 0 && rank < nranks, "bad rank");
   DAWN_CHECK(F_global == h->F * nranks, "F_global must equal nranks * local frames (equal contiguous frame ranges)");
   DAWN_CHECK(nranks == 1 || h->F >= h->cfg.win_width, "each rank must own at least win_width frames (only neighbours exchange halos)");
-  drop_sampler_graph(h);
+  drop_graphs(h);
   if (nranks > 1) {
     DAWN_TRY(load_nccl());
     if (h->sh_comm) { g_nccl.CommDestroy(h->sh_comm); h->sh_comm = nullptr; }
@@ -1317,7 +1330,7 @@ int dawn_unet_shard_ipc_import(dawn_unet* h, const char* handles) {
     h->p2p_peer[r] = reinterpret_cast<P2pMail*>(ptr);
   }
   h->p2p_ready = true;
-  drop_sampler_graph(h);
+  drop_graphs(h);
   return 0;
 }
 
@@ -1385,6 +1398,62 @@ int dawn_unet_sampler_launch(dawn_unet* h, void* stream) {
   DAWN_CHECK(h->have_invariants, "set_clip_invariants must precede sampler_launch");
   DAWN_CUDA_OK(cudaGraphLaunch(h->samp_exec, (cudaStream_t)stream));
   h->launches = h->samp_launches;
+  return 0;
+}
+
+// Ancestral update of this handle's frames (see sampler.cu); frame-sharded handles select the quantile over the whole clip
+// exactly as dawn_unet_ddim_step does.
+static int ddpm_step_handle(dawn_unet* h, float* x, const float* eps, const float* noise, int64_t n_local, DdpmCoef c,
+                            const DdpmCoef* tab, const int64_t* t_slot, int num_t, float q, void* scratch, cudaStream_t st) {
+  if (h->sh_nranks <= 1 || !h->sh_comm)
+    return ddpm_step_impl(x, eps, noise, n_local, n_local, c, tab, t_slot, num_t, q, scratch, st, nullptr);
+  DdimReduce red{(void*)h->sh_comm, red_sum_u32, red_sum_u64, red_min_u32};
+  return ddpm_step_impl(x, eps, noise, n_local, n_local * h->sh_nranks, c, tab, t_slot, num_t, q, scratch, st, &red);
+}
+
+int dawn_unet_ddpm_step(dawn_unet* h, float* x, const float* eps, const float* noise, int64_t n_local, float ca, float cb,
+                        float c1, float c2, float sigma, float q, void* scratch, void* stream) {
+  DAWN_CHECK(h, "null handle");
+  return ddpm_step_handle(h, x, eps, noise, n_local, DdpmCoef{ca, cb, c1, c2, sigma}, nullptr, nullptr, 0, q, scratch,
+                          (cudaStream_t)stream);
+}
+
+// One ancestral step as a CUDA graph: forward_x3(x, *t_slot) -> eps, the DDPM update with row *t_slot of the coefficient
+// table, then *t_slot -= 1.  Replayed num_timesteps times per clip instead of capturing the whole loop (at T = 1000 that graph
+// would hold ~235k nodes and a pre-drawn noise slab of T clips).
+int dawn_unet_ddpm_capture(dawn_unet* h, float* x, float* eps, const float* noise, int64_t* t_slot, const float* coef,
+                           int num_timesteps, float q, void* scratch) {
+  static_assert(sizeof(DdpmCoef) == 5 * sizeof(float), "a coefficient table row is 5 floats");
+  DAWN_CHECK(h && x && eps && noise && t_slot && coef && scratch && num_timesteps >= 1, "bad argument");
+  DAWN_CHECK(h->F > 0 && h->have_invariants, "set_clip_invariants must precede ddpm_capture");
+  DAWN_CHECK(!h->prof_on, "disable profiling before capturing the ancestral step graph");
+  drop_ddpm_graph(h);
+  if (!h->samp_stream) DAWN_CUDA_OK(cudaStreamCreateWithFlags(&h->samp_stream, cudaStreamNonBlocking));
+  const int64_t n = (int64_t)(h->cfg.out_grid_dim + h->cfg.out_conf_dim) * h->F * h->H * h->W;
+  cudaStream_t st = h->samp_stream;
+  DAWN_CUDA_OK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+  int rc = dawn_unet_forward_x3(h, x, t_slot, eps, st);
+  const int64_t launches = h->launches;
+  if (rc == 0)
+    rc = ddpm_step_handle(h, x, eps, noise, n, DdpmCoef{}, reinterpret_cast<const DdpmCoef*>(coef), t_slot, num_timesteps, q,
+                          scratch, st);
+  if (rc == 0) rc = ddpm_advance_slot(t_slot, st);
+  cudaGraph_t graph = nullptr;
+  const cudaError_t e = cudaStreamEndCapture(st, &graph);
+  if (rc != 0) { if (graph) cudaGraphDestroy(graph); return rc; }
+  DAWN_CUDA_OK(e);
+  const cudaError_t ei = cudaGraphInstantiate(&h->ddpm_exec, graph, 0);
+  cudaGraphDestroy(graph);
+  DAWN_CUDA_OK(ei);
+  h->ddpm_launches = launches;
+  return 0;
+}
+
+int dawn_unet_ddpm_launch(dawn_unet* h, void* stream) {
+  DAWN_CHECK(h && h->ddpm_exec, "ddpm_capture must precede ddpm_launch (a geometry change drops the graph)");
+  DAWN_CHECK(h->have_invariants, "set_clip_invariants must precede ddpm_launch");
+  DAWN_CUDA_OK(cudaGraphLaunch(h->ddpm_exec, (cudaStream_t)stream));
+  h->launches = h->ddpm_launches;
   return 0;
 }
 

@@ -1,12 +1,14 @@
 """Drop-in replacement for the reference's `GaussianDiffusion` / `DynamicNfGaussianDiffusion` sampler
 (DM_3/modules/video_flow_diffusion_multiGPU_v0_crema_plus_faceemb_ca_multi_test.py:988-1313) around the CUDA UNet:
 same constructor keywords, the same 12 schedule buffers (so `diffusion.load_state_dict(checkpoint['diffusion'])`,
-unified_video_generator.py:527-528, fills `denoise_fn.*` and the buffers), `sample(fea, bbox_mask, cond, cond_scale)`
-and `ddim_sample`.  Training entry points (`forward`, `p_losses`) are out of scope and raise.
+unified_video_generator.py:527-528, fills `denoise_fn.*` and the buffers), `sample(fea, bbox_mask, cond, cond_scale)`,
+`ddim_sample` and the ancestral `p_sample_loop` / `p_sample`.  Training entry points (`forward`, `p_losses`) are out of
+scope and raise.
 
-The sampling loop keeps the clip on the device: the 272 feature channels and the conditioning are handed to the UNet
-once per clip (`set_clip_invariants`), each step is `forward_x3` + one fused `dawn_ddim_step` (x0, exact clip-wide
-0.9-quantile dynamic threshold, eta-noise update) with no host synchronisation.
+The sampling loops keep the clip on the device: the 272 feature channels and the conditioning are handed to the UNet
+once per clip (`set_clip_invariants`), each step is `forward_x3` + one fused update (`dawn_ddim_step`, or
+`dawn_ddpm_step` for the ancestral loop: x0, exact clip-wide 0.9-quantile dynamic threshold, noise update) with no host
+synchronisation.
 """
 import ctypes
 
@@ -88,11 +90,23 @@ class GaussianDiffusion(nn.Module):
     @torch.no_grad()
     def sample(self, fea, bbox_mask, cond=None, cond_scale=1., batch_size=16):
         batch_size = cond.shape[0] if cond is not None else batch_size
-        if not self.is_ddim_sampling:
-            raise NotImplementedError("only DDIM sampling (sampling_timesteps < timesteps) is implemented, as DAWN configures it")
+        sample_fn = self.p_sample_loop if not self.is_ddim_sampling else self.ddim_sample      # U:1150
         fea = torch.cat([fea, bbox_mask], dim=1)
-        return self.ddim_sample(fea, (batch_size, self.channels, self.num_frames, fea.shape[-1], fea.shape[-1]), cond=cond,
-                                cond_scale=cond_scale)
+        return sample_fn(fea, (batch_size, self.channels, self.num_frames, fea.shape[-1], fea.shape[-1]), cond=cond,
+                         cond_scale=cond_scale)
+
+    def _clip_q(self, clip_denoised):
+        # q > 0: dynamic threshold; q = 0: static clamp to [-1, 1]; q < 0: no clamp at all (clip_denoised=False, U:1094, 1183)
+        return (float(self.dynamic_thres_percentile) if self.use_dynamic_thres else 0.0) if clip_denoised else -1.0
+
+    def _check_sample_shape(self, what, fea, shape, cond):
+        b, ch, Fr, h, w = shape
+        if tuple(shape[1:]) != (self.channels,) + tuple(shape[2:]) or fea.shape[0] != b or (cond is not None and cond.shape[0] != b):
+            raise ValueError(f"{what}: shape {tuple(shape)} does not match fea {tuple(fea.shape)} / cond "
+                             f"{None if cond is None else tuple(cond.shape)} (batch) or channels {self.channels}")
+        if tuple(fea.shape[-2:]) != (h, w) or (cond is not None and cond.shape[1] != Fr):
+            raise ValueError(f"{what}: fea {tuple(fea.shape)} / cond {None if cond is None else tuple(cond.shape)} do not "
+                             f"match the sample shape {tuple(shape)}")
 
     @torch.no_grad()
     def ddim_sample(self, fea, shape, cond=None, cond_scale=1., clip_denoised=True, noise_fn=None, pairs=None,
@@ -113,14 +127,8 @@ class GaussianDiffusion(nn.Module):
         draw = noise_fn if noise_fn is not None else self._default_noise(unet, device, seed)
         img = draw(-1, shape).to(device).contiguous()
         n = ch * Fr * h * w
-        # q > 0: dynamic threshold; q = 0: static clamp to [-1, 1]; q < 0: no clamp at all (clip_denoised=False, U:1183)
-        q = (float(self.dynamic_thres_percentile) if self.use_dynamic_thres else 0.0) if clip_denoised else -1.0
-        if tuple(shape[1:]) != (self.channels,) + tuple(shape[2:]) or fea.shape[0] != b or (cond is not None and cond.shape[0] != b):
-            raise ValueError(f"ddim_sample: shape {tuple(shape)} does not match fea {tuple(fea.shape)} / cond "
-                             f"{None if cond is None else tuple(cond.shape)} (batch) or channels {self.channels}")
-        if tuple(fea.shape[-2:]) != (h, w) or (cond is not None and cond.shape[1] != Fr):
-            raise ValueError(f"ddim_sample: fea {tuple(fea.shape)} / cond {None if cond is None else tuple(cond.shape)} do not "
-                             f"match the sample shape {tuple(shape)}")
+        q = self._clip_q(clip_denoised)
+        self._check_sample_shape("ddim_sample", fea, shape, cond)
         st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
         guided = cond_scale != 1 and getattr(unet, "has_cond", True)
         if use_graph:
@@ -207,6 +215,153 @@ class GaussianDiffusion(nn.Module):
             for k in range(ns - 1):
                 g["noise"][k].copy_(draw(k, (ch, Fr, h, w)))
             check(lib.dawn_unet_sampler_launch(unet._handle, st), "dawn_unet_sampler_launch")
+            img[i].copy_(g["x"])
+        return img
+
+    # ------------------------------------------------------------------ ancestral sampling (reference :1087-1134)
+    def ddpm_table(self):
+        """(num_timesteps, 5) fp32 host table, row t = {ca, cb, c1, c2, sigma} of one ancestral update (U:1072-1085,
+        1118-1121): sqrt_recip_alphas_cumprod[t], sqrt_recipm1_alphas_cumprod[t], posterior_mean_coef1[t],
+        posterior_mean_coef2[t] read from the registered buffers, and sigma = [t > 0] * exp(0.5 * posterior_log_variance_clipped[t])
+        evaluated per t on a one-element fp32 tensor, as the reference evaluates it for a one-clip batch."""
+        bufs = (self.sqrt_recip_alphas_cumprod, self.sqrt_recipm1_alphas_cumprod, self.posterior_mean_coef1,
+                self.posterior_mean_coef2, self.posterior_log_variance_clipped)
+        key = tuple((b.data_ptr(), b._version, b.device) for b in bufs)
+        cached = getattr(self, "_host_ddpm", None)
+        if cached is None or cached[0] != key:
+            ca, cb, c1, c2, lv = (b.detach().float().cpu() for b in bufs)
+            sigma = torch.empty_like(lv)
+            for t in range(lv.shape[0]):
+                nonzero_mask = 1 - (torch.full((1,), t) == 0).float()
+                sigma[t] = (nonzero_mask * (0.5 * lv[t:t + 1]).exp())[0]
+            cached = (key, torch.stack([ca, cb, c1, c2, sigma], dim=1).contiguous())
+            self._host_ddpm = cached
+        return cached[1]
+
+    def ddpm_coefficients(self, t):
+        """(ca, cb, c1, c2, sigma) of the ancestral update at timestep t, as Python floats (see ddpm_table)."""
+        return tuple(float(v) for v in self.ddpm_table()[t])
+
+    def _ddpm_step(self, unet, fea_i, cond_i, x, t, cond_scale, guided, eps, eps_null, noise, q, scratch, st):
+        """One ancestral step in place on x (3, F, h, w), this handle's frames of one clip (U:1087-1121).  Without guidance
+        the caller has set the clip invariants of (fea_i, cond_i)."""
+        t_dev = torch.full((1,), t, device=x.device, dtype=torch.long)
+        if guided:
+            # forward_with_cond_scale (U:879-890): null + (cond - null) * cond_scale, the null condition being all zeros
+            # (learn_null_cond=False, U:920); two hoisted forwards, each after rebuilding the per-clip conditioning tables
+            unet.set_clip_invariants(fea_i, cond_i)
+            unet.forward_x3(x, t_dev, eps)
+            unet.set_clip_invariants(fea_i, torch.zeros_like(cond_i))
+            unet.forward_x3(x, t_dev, eps_null)
+            eps.sub_(eps_null).mul_(float(cond_scale)).add_(eps_null)
+        else:
+            unet.forward_x3(x, t_dev, eps)
+        ca, cb, c1, c2, sigma = self.ddpm_coefficients(t)
+        check(lib.dawn_unet_ddpm_step(unet._handle, ctypes.c_void_p(x.data_ptr()), ctypes.c_void_p(eps.data_ptr()),
+                                      ctypes.c_void_p(noise.data_ptr()) if noise is not None else None, x.numel(),
+                                      ca, cb, c1, c2, sigma, q, ctypes.c_void_p(scratch.data_ptr()), st), "dawn_unet_ddpm_step")
+
+    @torch.no_grad()
+    def p_sample(self, x, t, fea, cond=None, cond_scale=1., clip_denoised=True, noise=None):
+        """reference p_sample (U:1112-1121): one ancestral step of x (b, 3, F, h, w) at timestep t (an int, or the reference's
+        (b,) tensor holding one value); fea (b, 272, h, w); cond (b, F, cond_dim).  noise (b, 3, F, h, w) is the draw the
+        reference takes with torch.randn_like(x) (default: `_default_noise`); at t = 0 it is multiplied by 0.  Returns the
+        new sample.  On a frame-sharded UNet x, cond and noise hold this rank's frames."""
+        if torch.is_tensor(t):
+            if t.numel() == 0 or bool((t != t.flatten()[0]).any()):
+                raise ValueError("p_sample: t must hold one timestep for the whole batch")
+            t = int(t.flatten()[0])
+        t = int(t)
+        if not 0 <= t < self.num_timesteps:
+            raise ValueError(f"p_sample: t = {t} is outside [0, {self.num_timesteps})")
+        device = self.betas.device
+        b, ch, Fr, h, w = x.shape
+        self._check_sample_shape("p_sample", fea, tuple(x.shape), cond)
+        unet = self.denoise_fn
+        if noise is None:
+            noise = self._default_noise(unet, device, None)(0, tuple(x.shape))
+        if tuple(noise.shape) != tuple(x.shape):
+            raise ValueError(f"p_sample: noise {tuple(noise.shape)} does not match x {tuple(x.shape)}")
+        img = x.to(device=device, dtype=torch.float32).contiguous().clone()
+        noise = noise.to(device=device, dtype=torch.float32).contiguous()
+        guided = cond_scale != 1 and getattr(unet, "has_cond", True)
+        st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+        scratch = torch.empty(ch * Fr * h * w + 512, dtype=torch.int32, device=device)
+        eps = torch.empty((ch, Fr, h, w), device=device)
+        eps_null = torch.empty_like(eps) if guided else None
+        q = self._clip_q(clip_denoised)
+        for i in range(b):
+            unet.update_num_frames(Fr)
+            if not guided:
+                unet.set_clip_invariants(fea[i], cond[i])
+            self._ddpm_step(unet, fea[i], cond[i], img[i], t, cond_scale, guided, eps, eps_null, noise[i], q, scratch, st)
+        return img
+
+    @torch.no_grad()
+    def p_sample_loop(self, fea, shape, cond=None, cond_scale=1., clip_denoised=True, noise_fn=None, use_graph=False, seed=None):
+        """reference p_sample_loop (U:1123-1134): num_timesteps ancestral steps, t = num_timesteps-1 down to 0.
+        fea (b, 272, h, w); cond (b, F, cond_dim); shape (b, 3, F, h, w).
+
+        noise_fn(k, shape) -> tensor lets tests inject the noise the reference draws: k = -1 is the start image (torch.randn,
+        U:1128), k >= 0 the draw of step k, t = num_timesteps-1-k (torch.randn_like, U:1118; drawn at t = 0 too, where it is
+        multiplied by 0).
+        use_graph: capture one step (UNet forward + update + timestep advance) as a CUDA graph (`dawn_unet_ddpm_capture`,
+        cached on the module) and replay it num_timesteps times per clip; the noise is copied into the graph's buffer before
+        each replay.  Frame-sharded UNet: as ddim_sample (clip-wide quantile; default noise = this rank's slice of one
+        clip-wide seeded stream)."""
+        device = self.betas.device
+        b, ch, Fr, h, w = shape
+        unet = self.denoise_fn
+        self._check_sample_shape("p_sample_loop", fea, shape, cond)
+        draw = noise_fn if noise_fn is not None else self._default_noise(unet, device, seed)
+        img = draw(-1, shape).to(device).contiguous()
+        q = self._clip_q(clip_denoised)
+        st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+        guided = cond_scale != 1 and getattr(unet, "has_cond", True)
+        if use_graph:
+            if guided:
+                raise NotImplementedError("use_graph captures the cond_scale = 1 step (DAWN's shipped setting); "
+                                          "classifier-free guidance runs eagerly")
+            return self._p_sample_loop_graph(unet, fea, cond, img, draw, q, st)
+        scratch = torch.empty(ch * Fr * h * w + 512, dtype=torch.int32, device=device)
+        eps = torch.empty((ch, Fr, h, w), device=device)
+        eps_null = torch.empty_like(eps) if guided else None
+        T = self.num_timesteps
+        for i in range(b):
+            unet.update_num_frames(Fr)
+            if not guided:
+                unet.set_clip_invariants(fea[i], cond[i])
+            for k in range(T):
+                noise = draw(k, (ch, Fr, h, w)).to(device).contiguous()
+                self._ddpm_step(unet, fea[i], cond[i], img[i], T - 1 - k, cond_scale, guided, eps, eps_null, noise, q, scratch, st)
+        return img
+
+    def _p_sample_loop_graph(self, unet, fea, cond, img, draw, q, st):
+        b, ch, Fr, h, w = img.shape
+        device, n, T = img.device, ch * Fr * h * w, self.num_timesteps
+        key = (Fr, h, w, T, q, device.index)
+        g = getattr(self, "_ddpm_graph", None)
+        unet.update_num_frames(Fr)
+        if g is None or g["key"] != key or g["gen"] != unet.graph_generation():
+            g = dict(key=key, x=torch.empty((ch, Fr, h, w), device=device), eps=torch.empty((ch, Fr, h, w), device=device),
+                     noise=torch.empty((ch, Fr, h, w), device=device), t=torch.empty(1, dtype=torch.long, device=device),
+                     coef=torch.empty((T, 5), device=device), scratch=torch.empty(n + 512, dtype=torch.int32, device=device))
+            unet.set_clip_invariants(fea[0], cond[0])
+            torch.cuda.synchronize(device)
+            check(lib.dawn_unet_ddpm_capture(unet._handle, ctypes.c_void_p(g["x"].data_ptr()), ctypes.c_void_p(g["eps"].data_ptr()),
+                                             ctypes.c_void_p(g["noise"].data_ptr()), ctypes.c_void_p(g["t"].data_ptr()),
+                                             ctypes.c_void_p(g["coef"].data_ptr()), T, q, ctypes.c_void_p(g["scratch"].data_ptr())),
+                  "dawn_unet_ddpm_capture")
+            g["gen"] = unet.graph_generation()
+            self._ddpm_graph = g
+        g["coef"].copy_(self.ddpm_table())          # the schedule buffers may have been reloaded since the capture
+        for i in range(b):
+            unet.set_clip_invariants(fea[i], cond[i])
+            g["x"].copy_(img[i])
+            g["t"].fill_(T - 1)
+            for k in range(T):
+                g["noise"].copy_(draw(k, (ch, Fr, h, w)))
+                check(lib.dawn_unet_ddpm_launch(unet._handle, st), "dawn_unet_ddpm_launch")
             img[i].copy_(g["x"])
         return img
 

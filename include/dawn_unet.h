@@ -137,6 +137,34 @@ int dawn_unet_sampler_capture(dawn_unet* h, float* x, float* eps, const float* n
                               const float* coef, int nsteps, float q, void* scratch);
 int dawn_unet_sampler_launch(dawn_unet* h, void* stream);
 
+/* One ancestral (DDPM) update around the UNet (reference GaussianDiffusion.p_sample :1087-1121), in place on x (device,
+ * n floats), each operation rounded as the reference's fp32 torch arithmetic (no fused multiply-add):
+ *   x0 = ca*x - cb*eps;  s and the clamp exactly as dawn_ddim_step (q > 0 dynamic threshold, q = 0 clamp to [-1, 1],
+ *   q < 0 no clip: the reference's clip_denoised=False);
+ *   x = c1*(clamp(x0,-s,s)/s) + c2*x + sigma*noise      (noise may be NULL)
+ * with ca = sqrt_recip_alphas_cumprod[t], cb = sqrt_recipm1_alphas_cumprod[t], c1/c2 = posterior_mean_coef1/2[t] and
+ * sigma = [t > 0] * exp(0.5 * posterior_log_variance_clipped[t]).  scratch as dawn_ddim_step.  No host synchronisation. */
+int dawn_ddpm_step(float* x, const float* eps, const float* noise, int64_t n, float ca, float cb, float c1, float c2,
+                   float sigma, float q, void* scratch, void* stream);
+
+/* The same update for the frames a handle owns.  Unsharded handle: identical to dawn_ddpm_step.  After dawn_unet_init_shard
+ * the quantile spans the whole clip, as in dawn_unet_ddim_step; every rank passes the same coefficients and its slice of
+ * the clip's noise. */
+int dawn_unet_ddpm_step(dawn_unet* h, float* x, const float* eps, const float* noise, int64_t n_local, float ca, float cb,
+                        float c1, float c2, float sigma, float q, void* scratch, void* stream);
+
+/* One step of the ancestral loop (reference p_sample_loop :1123-1134) captured as a CUDA graph and replayed once per
+ * timestep: forward_x3(x, t = *t_slot) -> eps, the DDPM update with row *t_slot of coef, then *t_slot -= 1.  All
+ * addresses are fixed at capture: x (3,F,h,w) in/out, eps (3,F,h,w) scratch, noise (3,F,h,w; refill it on the stream
+ * before every replay), t_slot (one int64, device), coef (device, num_timesteps x {ca, cb, c1, c2, sigma}; the slot is
+ * clamped to [0, num_timesteps) when the row is read), scratch (as dawn_ddim_step).  Per clip: fill x, set *t_slot =
+ * num_timesteps - 1, call dawn_unet_set_clip_invariants, then dawn_unet_ddpm_launch(stream) num_timesteps times.
+ * set_num_frames / commit_params / init_shard drop the graph.  It is held beside the dawn_unet_sampler_capture graph:
+ * capturing either one leaves the other in place. */
+int dawn_unet_ddpm_capture(dawn_unet* h, float* x, float* eps, const float* noise, int64_t* t_slot, const float* coef,
+                           int num_timesteps, float q, void* scratch);
+int dawn_unet_ddpm_launch(dawn_unet* h, void* stream);
+
 /* One contraction through exactly one kernel path, for per-kernel tests against a high-precision reference.
  * Out[m, n] = epilogue( sum_{tap, c} A[pixel(m, tap), c] * B[tap*Cin + c, n] ) with the product's GemmParams semantics
  * (dawn_pytorch_b200/csrc/gemm.cuh): rows m = (f, i, j) over an F x OHs x OWs output sub-grid (M = F*OHs*OWs), input pixel
