@@ -44,6 +44,22 @@ class DawnContractionCase(ctypes.Structure):
                 ("Y", _p), ("ldy", _i), ("gn_stats", _p), ("gn_w", _p), ("gn_b", _p), ("film", _p), ("gn_count", ctypes.c_double)]
 
 
+FUSED_TEMPORAL, FUSED_ATTN_TC, FUSED_ATTN_SIMT, FUSED_SLA_CTX, FUSED_SLA_OUT, FUSED_SLA_CTX_UNFUSED, FUSED_CA_WT, \
+    FUSED_CA_RSTD, FUSED_GN_HCOND = range(9)
+
+
+class DawnFusedCase(ctypes.Structure):
+    """include/dawn_unet.h: dawn_fused_case (pointers are device addresses)"""
+    _i, _p = ctypes.c_int, ctypes.c_void_p
+    _fields_ = [("kernel", _i), ("F", _i), ("P", _i), ("C", _i), ("band", _i), ("q_lo", _i), ("q_hi", _i),
+                ("nseq", _i), ("L", _i), ("pb", _i), ("seq_base_stride", ctypes.c_longlong), ("elem_stride", ctypes.c_longlong),
+                ("ldx", _i), ("ldr", _i), ("ldo", _i), ("ld", _i), ("ldb", _i), ("ldy", _i), ("ldbT", _i),
+                ("x", _p), ("res", _p), ("out", _p), ("gamma", _p), ("w_qkv", _p), ("w_out", _p), ("rot", _p), ("bias", _p),
+                ("qkv", _p), ("Bf", _p), ("out_bias", _p), ("kq", _p), ("nkq", _p), ("G", _p), ("gates", _p), ("Wt", _p),
+                ("T", _p), ("Y", _p), ("out16h", _p), ("out16l", _p),
+                ("gn_stats", _p), ("gn_count", ctypes.c_double), ("cpg", _i), ("gn_w", _p), ("gn_b", _p), ("film", _p)]
+
+
 class DawnError(RuntimeError):
     pass
 
@@ -75,8 +91,8 @@ def _load():
     lib.dawn_unet_last_launch_count.restype = ctypes.c_int64
     lib.dawn_unet_workspace_bytes.argtypes = [vp]
     lib.dawn_unet_workspace_bytes.restype = ctypes.c_int64
-    lib.dawn_selftest_attention.argtypes = [ctypes.c_int] * 3 + [ctypes.POINTER(ctypes.c_float)] * 2
     lib.dawn_test_contraction.argtypes = [ctypes.POINTER(DawnContractionCase), vp]
+    lib.dawn_test_fused.argtypes = [ctypes.POINTER(DawnFusedCase), vp]
     lib.dawn_nccl_unique_id.argtypes = [ctypes.c_char_p]
     lib.dawn_unet_init_shard.argtypes = [vp, ctypes.c_char_p, ctypes.c_int, ctypes.c_int, ctypes.c_int]
     lib.dawn_unet_shard_ipc_export.argtypes = [vp, ctypes.c_char_p]
@@ -118,7 +134,7 @@ EXPORTS = ["dawn_unet_create", "dawn_unet_destroy", "dawn_unet_set_param", "dawn
            "dawn_unet_forward_x3", "dawn_unet_forward_host", "dawn_unet_set_tap", "dawn_unet_tap_shape",
            "dawn_unet_profile_enable", "dawn_unet_profile_read", "dawn_unet_last_launch_count", "dawn_unet_workspace_bytes", "dawn_ddim_step", "dawn_unet_ddim_step", "dawn_unet_sampler_capture", "dawn_unet_sampler_launch",
            "dawn_ddpm_step", "dawn_unet_ddpm_step", "dawn_unet_ddpm_capture", "dawn_unet_ddpm_launch",
-           "dawn_test_contraction", "dawn_selftest_attention", "dawn_last_error", "dawn_build_info"]
+           "dawn_test_contraction", "dawn_test_fused", "dawn_last_error", "dawn_build_info"]
 
 
 LFG_EXPORTS = ["dawn_lfg_create", "dawn_lfg_destroy", "dawn_lfg_set_param", "dawn_lfg_commit_params", "dawn_lfg_set_geometry",

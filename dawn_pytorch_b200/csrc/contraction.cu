@@ -81,6 +81,42 @@ int upload_weight(std::vector<void*>& owner, const std::vector<float>& m, int K,
   return 0;
 }
 
+std::vector<float> fold_linear(const float* w, int N, int K, const float* gain, float qscale, int nscale) {
+  std::vector<float> m((size_t)N * K);
+  for (int n = 0; n < N; ++n) {
+    const float sc = (n < nscale) ? qscale : 1.0f;
+    for (int k = 0; k < K; ++k) {
+      float v = w[(size_t)n * K + k];
+      if (gain) v *= gain[k];
+      m[(size_t)n * K + k] = v * sc;
+    }
+  }
+  return m;
+}
+
+std::vector<float> row_sums(const std::vector<float>& w, int N, int K) {
+  std::vector<float> s(N);
+  for (int n = 0; n < N; ++n) {
+    double acc = 0.0;
+    for (int k = 0; k < K; ++k) acc += w[(size_t)n * K + k];
+    s[n] = (float)acc;
+  }
+  return s;
+}
+
+void fold_ca_q(const float* const to_q[3], const float* const gain[3], int ci, std::vector<float>& wq, std::vector<float>& wsum) {
+  wq.assign((size_t)ci * 192, 0.f);
+  wsum.assign(192, 0.f);
+  for (int a = 0; a < 3; ++a) {
+    const std::vector<float> m = fold_linear(to_q[a], 64, ci, gain[a], 1.f, 0);
+    const std::vector<float> s = row_sums(m, 64, ci);
+    for (int j = 0; j < 64; ++j) {
+      for (int k = 0; k < ci; ++k) wq[(size_t)k * 192 + a * 64 + j] = m[(size_t)j * ci + k];
+      wsum[a * 64 + j] = s[j];
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------------------ GemmParams
 void base_params(GemmParams& p, const float* A, int lda, int Cin, int frames, int H, int W) {
   memset(&p, 0, sizeof(p));

@@ -42,6 +42,14 @@ struct PackedWeight {
 int upload_weight(std::vector<void*>& owner, const std::vector<float>& m, int K, int N, int ldb, const std::vector<float>& bias,
                   PackedWeight* out);
 
+// Folds shared by the network's weight upload and dawn_test_fused.  Linear weight w [N][K] (row-major) with a per-input gain
+// (a LayerNorm gamma, may be null) folded into its columns and rows [0, nscale) scaled by qscale: (w[n][k] * gain[k]) * sc.
+std::vector<float> fold_linear(const float* w, int N, int K, const float* gain, float qscale, int nscale);
+// per-row sums of a folded [N][K] matrix (fp64 accumulation): the column sums of B that the LayerNorm fold subtracts
+std::vector<float> row_sums(const std::vector<float>& w, int N, int K);
+// the three cross-attentions' to_q [64][ci] with their LayerNorm_img gains folded, as one k-major [ci][192] matrix and its wsum
+void fold_ca_q(const float* const to_q[3], const float* const gain[3], int ci, std::vector<float>& wq, std::vector<float>& wsum);
+
 // ---------------------------------------------------------------- GemmParams
 // 1x1 contraction of (frames, H, W, Cin) rows of stride lda onto the same grid
 void base_params(GemmParams& p, const float* A, int lda, int Cin, int frames, int H, int W);

@@ -436,21 +436,26 @@ constexpr size_t kSmemOut = (size_t)(2 * 256 * LD + 2 * C * BLD + 2 * OCH * LD) 
 
 }  // namespace
 
-bool sla_fused_supported(int C_, int P) { return C_ == C && P % 16 == 0 && P >= 64; }
-
-int sla_fused_splits(int P) {
+// Pixels per context CTA: the largest power of two from 512 down to 64 that divides P (64 if none does), or -1 when that needs
+// more than 16 splits.  The kernel only consumes whole 16-pixel groups, so every split but the last must be a multiple of 16:
+// ceil(P / nsplit) is not (P = 80 would give splits of 40 and drop 16 pixels).
+int sla_fused_run(int P) {
   int px = 512;
   while (px > 64 && P % px != 0) px >>= 1;
-  int n = (P + px - 1) / px;
-  return n > 16 ? -1 : n;
+  return (P + px - 1) / px > 16 ? -1 : px;
 }
+int sla_fused_splits(int P) {
+  const int px = sla_fused_run(P);
+  return px < 0 ? -1 : (P + px - 1) / px;
+}
+bool sla_fused_supported(int C_, int P) { return C_ == C && P % 16 == 0 && P >= 64 && sla_fused_run(P) > 0; }
 size_t sla_fused_part_floats(int F, int P) { return (size_t)F * std::max(1, sla_fused_splits(P)) * 8 * PART; }
 
 int launch_sla_ctx_fused(const SlaCtxArgs& a_in, const float* WoutT, float* Bf, int ldb, cudaStream_t st) {
   SlaCtxArgs a = a_in;
   const int nsplit = sla_fused_splits(a.P);
   if (!sla_fused_supported(C, a.P) || nsplit < 1) { set_last_error("sla_fused: unsupported shape"); return -1; }
-  a.px_per_cta = (a.P + nsplit - 1) / nsplit;
+  a.px_per_cta = sla_fused_run(a.P);
   static bool attr = false;
   if (!attr) {
     DAWN_CUDA_OK(cudaFuncSetAttribute(sla_ctx_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmem));

@@ -253,19 +253,11 @@ int pack_conv(dawn_unet* h, const std::string& prefix, int co, int ci, int kh, i
 int pack_linear(dawn_unet* h, const HostParam* w, int N, int K, const float* gain, float qscale, int nscale, PackedWeight* out,
                 float** wsum) {
   const int ldb = round_up(N, 64);
-  std::vector<float> m((size_t)K * ldb, 0.f), s(ldb, 0.f);
-  for (int n = 0; n < N; ++n) {
-    double acc = 0.0;
-    const float sc = (n < nscale) ? qscale : 1.0f;
-    for (int k = 0; k < K; ++k) {
-      float v = w->data[(size_t)n * K + k];
-      if (gain) v *= gain[k];
-      v *= sc;
-      m[(size_t)k * ldb + n] = v;
-      acc += v;
-    }
-    s[n] = (float)acc;
-  }
+  const std::vector<float> f = fold_linear(w->data.data(), N, K, gain, qscale, nscale);
+  std::vector<float> m((size_t)K * ldb, 0.f), s = row_sums(f, N, K);
+  for (int n = 0; n < N; ++n)
+    for (int k = 0; k < K; ++k) m[(size_t)k * ldb + n] = f[(size_t)n * K + k];
+  s.resize(ldb, 0.f);
   DAWN_TRY(upload_weight(h->owned, m, K, N, ldb, {}, out));
   if (wsum) DAWN_TRY(dev_upload(h->owned, s, wsum));
   return 0;
@@ -297,7 +289,8 @@ int pack_resblock(dawn_unet* h, const std::string& name, int ci, int co, bool co
     const char* mlp[3] = {"pose_mlp", "audio_mlp", "eye_mlp"};
     const int kdim[3] = {h->cfg.cond_pose, h->cfg.cond_aud, h->cfg.cond_eye};
     const char* can[3] = {"cross_attn_pose", "cross_attn_aud", "cross_attn_eye"};
-    std::vector<float> wq((size_t)ci * 192, 0.f), wsum(192, 0.f);
+    const float* to_q[3];
+    const float* gain[3];
     for (int a = 0; a < 3; ++a) {
       DAWN_TRY(upload_raw(h, name + "." + mlp[a] + ".1.weight", {2 * co, kdim[a]}, &r.mW[a]));
       DAWN_TRY(upload_raw(h, name + "." + mlp[a] + ".1.bias", {2 * co}, &r.mB[a]));
@@ -305,15 +298,7 @@ int pack_resblock(dawn_unet* h, const std::string& name, int ci, int co, bool co
       const HostParam *g, *q;
       DAWN_TRY(h->raw.need(p + ".norm.g", {ci}, &g));
       DAWN_TRY(h->raw.need(p + ".to_q.weight", {64, ci}, &q));
-      for (int j = 0; j < 64; ++j) {
-        double acc = 0.0;
-        for (int k = 0; k < ci; ++k) {
-          const float v = q->data[(size_t)j * ci + k] * g->data[k];     // LayerNorm_img gain folded (U:203, 519)
-          wq[(size_t)k * 192 + a * 64 + j] = v;
-          acc += v;
-        }
-        wsum[a * 64 + j] = (float)acc;
-      }
+      to_q[a] = q->data.data(); gain[a] = g->data.data();                 // LayerNorm_img gain folded (U:203, 519)
       DAWN_TRY(upload_raw(h, p + ".to_kv.weight", {128, 2 * co}, &r.ca[a].Wkv));
       DAWN_TRY(upload_raw(h, p + ".null_kv", {2, 8}, &r.ca[a].nkv));
       DAWN_TRY(upload_raw(h, p + ".q_scale", {8}, &r.ca[a].qs));
@@ -321,6 +306,8 @@ int pack_resblock(dawn_unet* h, const std::string& name, int ci, int co, bool co
       DAWN_TRY(upload_raw(h, p + ".to_out.0.weight", {co, 64}, &r.ca[a].Wout));
       DAWN_TRY(upload_raw(h, p + ".to_out.1.g", {co}, &r.ca[a].gout));
     }
+    std::vector<float> wq, wsum;
+    fold_ca_q(to_q, gain, ci, wq, wsum);
     DAWN_TRY(upload_weight(h->owned, wq, ci, 192, 192, {}, &r.wq));
     DAWN_TRY(dev_upload(h->owned, wsum, &r.wsumq));
     if (ci == 64 || ci == 128) {
@@ -344,9 +331,7 @@ int pack_attn(dawn_unet* h, const std::string& norm_name, const std::string& fn,
   DAWN_TRY(pack_linear(h, qkv, 768, C, g->data.data(), scale, 256, &a->qkv, &a->wsum));
   DAWN_TRY(pack_linear(h, o, C, 256, nullptr, 1.f, 0, &a->out, nullptr));
   if (C == 64) {
-    std::vector<float> wq((size_t)768 * C);
-    for (int n = 0; n < 768; ++n)
-      for (int k = 0; k < C; ++k) wq[(size_t)n * C + k] = qkv->data[(size_t)n * C + k] * g->data[k] * (n < 256 ? scale : 1.0f);
+    const std::vector<float> wq = fold_linear(qkv->data.data(), 768, C, g->data.data(), scale, 256);
     std::vector<uint16_t> Wq, Wo;
     temporal_fused_pack(wq.data(), o->data.data(), Wq, Wo, &a->f_inv_wscale, &a->f_inv_oscale);
     DAWN_TRY(dev_upload(h->owned, Wq, &a->fq));
@@ -364,9 +349,7 @@ int pack_sla(dawn_unet* h, const std::string& p, int C, SlaW* s) {        // p =
   s->C = C;
   DAWN_TRY(pack_linear(h, qkv, 768, C, g->data.data(), 1.f, 0, &s->qkv, &s->wsum));
   if (C == 64) {
-    std::vector<float> wf((size_t)768 * C);
-    for (int n = 0; n < 768; ++n)
-      for (int k = 0; k < C; ++k) wf[(size_t)n * C + k] = qkv->data[(size_t)n * C + k] * g->data[k];
+    const std::vector<float> wf = fold_linear(qkv->data.data(), 768, C, g->data.data(), 1.f, 0);
     std::vector<uint16_t> W;
     sla_fused_pack(wf.data(), W, &s->f_inv_wscale);
     DAWN_TRY(dev_upload(h->owned, W, &s->fkv));
@@ -1485,49 +1468,5 @@ int dawn_unet_profile_read(dawn_unet* h, double* ms, double* flops, double* byte
   return 0;
 }
 int64_t dawn_unet_workspace_bytes(dawn_unet* h) { return h ? h->ws_bytes : 0; }
-
-// random qkv through both attention kernels (temporal: nseq pixel sequences of L frames, band 40 + bias;
-// spatial: nseq frames of L tokens, full attention); reports max |tensor-core - SIMT|
-int dawn_selftest_attention(int nseq, int L, int temporal, float* max_abs_diff, float* max_abs_ref) {
-  DAWN_CHECK(max_abs_diff && max_abs_ref, "null argument");
-  const size_t rows = (size_t)nseq * L;
-  std::vector<float> hq(rows * 768), hb(8 * 81);
-  uint32_t seed = 777u;
-  auto rnd = [&]() { seed = seed * 1664525u + 1013904223u; return ((seed >> 8) & 0xFFFF) / 32768.0f - 1.0f; };
-  for (auto& v : hq) v = rnd() * 1.5f;
-  for (auto& v : hb) v = rnd() * 2.0f;
-  std::vector<void*> own;
-  float *dq, *db, *o1, *o2;
-  if (dev_alloc(own, hq.size(), &dq) || dev_alloc(own, hb.size(), &db) || dev_alloc(own, rows * 256, &o1) || dev_alloc(own, rows * 256, &o2)) {
-    free_all(own); return -2;
-  }
-  cudaMemcpy(dq, hq.data(), hq.size() * 4, cudaMemcpyHostToDevice);
-  cudaMemcpy(db, hb.data(), hb.size() * 4, cudaMemcpyHostToDevice);
-  cudaMemset(o1, 0, rows * 256 * 4); cudaMemset(o2, 0, rows * 256 * 4);
-  AttnArgs a{};
-  a.qkv = dq; a.ld = 768; a.ldo = 256; a.nseq = nseq; a.L = L;
-  if (temporal) { a.seq_base_stride = 1; a.elem_stride = nseq; a.band = 40; a.bias = db; }
-  else { a.seq_base_stride = L; a.elem_stride = 1; a.band = 1 << 30; a.bias = nullptr; }
-  a.q_lo = 0; a.q_hi = L;
-  a.out = o1;
-  int rc = launch_attention(a, 0);
-  a.out = o2;
-  if (rc == 0) rc = launch_attention_tc(a, 0);
-  if (rc == 0 && cudaDeviceSynchronize() != cudaSuccess) { set_last_error(std::string("selftest: ") + cudaGetErrorString(cudaGetLastError())); rc = -2; }
-  if (rc == 0) {
-    std::vector<float> r1(rows * 256), r2(rows * 256);
-    cudaMemcpy(r1.data(), o1, r1.size() * 4, cudaMemcpyDeviceToHost);
-    cudaMemcpy(r2.data(), o2, r2.size() * 4, cudaMemcpyDeviceToHost);
-    float md = 0.f, mr = 0.f;
-    for (size_t i = 0; i < r1.size(); ++i) {
-      const float d = std::fabs(r1[i] - r2[i]);
-      md = (d > md || d != d) ? d : md;
-      mr = std::max(mr, std::fabs(r1[i]));
-    }
-    *max_abs_diff = md; *max_abs_ref = mr;
-  }
-  free_all(own);
-  return rc;
-}
 
 }  // extern "C"

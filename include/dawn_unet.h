@@ -204,9 +204,47 @@ typedef struct {
 } dawn_contraction_case;
 int dawn_test_contraction(const dawn_contraction_case* c, void* stream);
 
-/* self-test of the tensor-core attention core against the SIMT fp32 kernel on random q/k/v:
- * temporal != 0: nseq pixel sequences of L frames, band 40 with bias; else nseq frames of L tokens, full attention */
-int dawn_selftest_attention(int nseq, int L, int temporal, float* max_abs_diff, float* max_abs_ref);
+/* One fused attention / cross-attention kernel, for per-kernel tests against a high-precision reference.  Weights arrive
+ * as fp32 device matrices in the reference's layout; the harness builds the fp16 hi|lo images, scales and column sums with
+ * the host code the network's weight upload runs.  Rows are f*P + pixel (channels last).  Every table (rotary, relative
+ * bias, cross-attention keys and Gram forms, GroupNorm sums, FiLM) is a caller input.  Returns -1 and launches nothing
+ * when the kernel's own shape predicate refuses the geometry (it never falls back to another kernel), -2 on a CUDA error;
+ * synchronises the stream before it returns. */
+enum {
+  DAWN_FUSED_TEMPORAL = 0,         /* temporal_fused_kernel: out = res + to_out(banded attention(rotary(LN-folded q|k|v of x)))
+                                      over an on-chip sequence of F frames; rows [q_lo, q_hi) of it are written to out / read
+                                      from res at row (f - q_lo)*P + pixel */
+  DAWN_FUSED_ATTN_TC = 1,          /* attention_tc_kernel: softmax attention core over qkv rows [q | k | v] (256 each) */
+  DAWN_FUSED_ATTN_SIMT = 2,        /* attention_kernel: the same operation on the fp32 SIMT kernel */
+  DAWN_FUSED_SLA_CTX = 3,          /* sla_ctx_kernel + sla_merge_kernel: Bf[f] = per-head softmax_px(k) v^T composed with to_out */
+  DAWN_FUSED_SLA_OUT = 4,          /* sla_out_kernel: out = x + out_bias + sum_h softmax_d(q_h) 32^-1/2 Bf[f][h] */
+  DAWN_FUSED_SLA_CTX_UNFUSED = 5,  /* sla_context_kernel: Bf from a qkv buffer (ld 768) */
+  DAWN_FUSED_CA_WT = 6,            /* ca_wt_kernel<C>: Wt = rstd * [1, gates] of the three cross-attentions */
+  DAWN_FUSED_CA_RSTD = 7,          /* ca_rstd_kernel: Wt from given gates [F*P][24] */
+  DAWN_FUSED_GN_HCOND = 8          /* gn_hcond_kernel: SiLU(FiLM(GN(Y))) + Wt T_f, fp32 rows, or fp16 hi|lo planes if out16h */
+};
+typedef struct {
+  int kernel;                      /* DAWN_FUSED_* */
+  int F, P, C;                     /* frames, pixels per frame, channels (ca: ci; gn_hcond: co) */
+  int band, q_lo, q_hi;            /* temporal and attention cores: |key - query| <= band attend (attention: band >= L is full) */
+  int nseq, L, pb;                 /* attention cores: element e of sequence s is row ((s / pb) * L + e) * pb + s % pb if pb > 0, */
+  long long seq_base_stride, elem_stride;   /* else s * seq_base_stride + e * elem_stride */
+  int ldx, ldr, ldo, ld, ldb, ldy, ldbT;
+  /* device pointers owned by the caller */
+  const float* x; const float* res; float* out;
+  const float* gamma;              /* [C] PreNorm gamma; ca: [3][C] LayerNorm_img gains */
+  const float* w_qkv;              /* [768][C] to_qkv; ca: [3][64][C] to_q */
+  const float* w_out;              /* [C][256] to_out */
+  const float* rot;                /* [F][16][2] (cos, sin) */
+  const float* bias;               /* [8][2*band+1] relative bias, rel = key - query; NULL for none (attention cores) */
+  const float* qkv;                /* attention cores, unfused SLA context */
+  float* Bf;                       /* [F][256][ldb] SLA context output / SLA output input */
+  const float* out_bias;           /* [C] SLA to_out bias */
+  const float* kq; const float* nkq; const float* G; const float* gates; float* Wt;
+  const float* T; const float* Y; unsigned short* out16h; unsigned short* out16l;
+  const double* gn_stats; double gn_count; int cpg; const float* gn_w; const float* gn_b; const float* film;
+} dawn_fused_case;
+int dawn_test_fused(const dawn_fused_case* c, void* stream);
 
 const char* dawn_last_error(void);
 const char* dawn_build_info(void);
