@@ -77,6 +77,7 @@ def _load():
     lib.dawn_unet_set_param.argtypes = [vp, cp, fp, i64p, ctypes.c_int]
     lib.dawn_unet_commit_params.argtypes = [vp]
     lib.dawn_unet_set_num_frames.argtypes = [vp, ctypes.c_int, ctypes.c_int, ctypes.c_int]
+    lib.dawn_unet_set_geometry.argtypes = [vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int]
     lib.dawn_unet_set_clip_invariants.argtypes = [vp, fp, fp, vp]
     lib.dawn_unet_forward.argtypes = [vp, fp, vp, fp, fp, vp]
     lib.dawn_unet_forward_x3.argtypes = [vp, fp, vp, fp, vp]
@@ -130,7 +131,7 @@ def _load():
 lib = _load()
 
 EXPORTS = ["dawn_unet_create", "dawn_unet_destroy", "dawn_unet_set_param", "dawn_unet_commit_params",
-           "dawn_unet_set_num_frames", "dawn_nccl_unique_id", "dawn_unet_init_shard", "dawn_unet_shard_ipc_export", "dawn_unet_shard_ipc_import", "dawn_unet_set_clip_invariants", "dawn_unet_forward",
+           "dawn_unet_set_num_frames", "dawn_unet_set_geometry", "dawn_nccl_unique_id", "dawn_unet_init_shard", "dawn_unet_shard_ipc_export", "dawn_unet_shard_ipc_import", "dawn_unet_set_clip_invariants", "dawn_unet_forward",
            "dawn_unet_forward_x3", "dawn_unet_forward_host", "dawn_unet_set_tap", "dawn_unet_tap_shape",
            "dawn_unet_profile_enable", "dawn_unet_profile_read", "dawn_unet_last_launch_count", "dawn_unet_workspace_bytes", "dawn_ddim_step", "dawn_unet_ddim_step", "dawn_unet_sampler_capture", "dawn_unet_sampler_launch",
            "dawn_ddpm_step", "dawn_unet_ddpm_step", "dawn_unet_ddpm_capture", "dawn_unet_ddpm_launch",

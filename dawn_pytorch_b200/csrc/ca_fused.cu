@@ -319,14 +319,17 @@ __global__ void __launch_bounds__(NTH, 3) gn_hcond_kernel(GnHcondArgs a) {
       Th[c * TLD + k] = __float2half_rn(h);
       Tl[c * TLD + k] = __float2half_rn(v - h);
     }
+    const int clip = a.clips > 1 ? f % a.clips : 0;
+    const double* gs = a.gn_stats + 16 * clip;
+    const float* film = a.film ? a.film + (size_t)clip * 2 * co : nullptr;
     for (int c = tid; c < co; c += NTH) {
       const int grp = c / a.cpg;
-      const double sm = a.gn_stats[2 * grp], ss = a.gn_stats[2 * grp + 1];
+      const double sm = gs[2 * grp], ss = gs[2 * grp + 1];
       const double mean = sm / a.gn_count;
       const double var = ss / a.gn_count - mean * mean;
       const float rstd = (float)(1.0 / sqrt(var + 1e-5));
       float al = rstd * a.gn_w[c], be = a.gn_b[c] - (float)mean * al;
-      if (a.film) { const float sc = a.film[c] + 1.f; al *= sc; be = be * sc + a.film[co + c]; }
+      if (film) { const float sc = film[c] + 1.f; al *= sc; be = be * sc + film[co + c]; }
       s_al[c] = al; s_be[c] = be;
     }
   }

@@ -26,9 +26,10 @@ struct GnHcondArgs {
   unsigned short *Out16h, *Out16l; // a1 as two dense fp16 planes [F*P][co] (hi | lo of the wgmma-kernel split): the consuming 3x3 conv then
                                   // fetches its halo tiles by TMA with no conversion pass; same bytes as the fp32 row
   int F, P, co;
-  const double* gn_stats; double gn_count; int cpg;     // clip-wide GroupNorm sums (sum, sumsq per group)
-  const float *gn_w, *gn_b, *film;                     // film: [2*co] (scale | shift) or nullptr
+  const double* gn_stats; double gn_count; int cpg;     // clip-wide GroupNorm sums (sum, sumsq per group), [clips][16]
+  const float *gn_w, *gn_b, *film;                     // film: [clips][2*co] (scale | shift) or nullptr
   int px_per_cta;                 // set by the launcher
+  int clips = 1;                  // frame f belongs to clip f % clips
 };
 bool gn_hcond_supported(int co, int P);
 int launch_gn_hcond(const GnHcondArgs& a, cudaStream_t st);

@@ -32,6 +32,10 @@ void set_last_error(const std::string& s);
     if (_rc != 0) return _rc;    \
   } while (0)
 
+// Clips of one batched pass.  Activations hold frame f of clip b as frame f * clips + b; per-clip GroupNorm statistics (16 doubles),
+// FiLM tables and init-conv maps are one slice per clip, found from a row's frame index.
+constexpr int kMaxClips = 16;
+
 // ---------------------------------------------------------------- small device helpers
 __device__ __forceinline__ float silu(float x) { return x / (1.0f + expf(-x)); }
 

@@ -127,6 +127,7 @@ void base_params(GemmParams& p, const float* A, int lda, int Cin, int frames, in
   p.OH = H; p.OW = W; p.out_stride = 1;
   p.P = H * W;
   p.q_post_scale = 1.f;
+  p.clips = 1;
 }
 void set_weights(GemmParams& p, const PackedWeight& w) {
   p.B = w.w; p.Bimg = w.img; p.tc_scale = 1.0f / w.img_scale; p.ldb = w.ldb; p.N = w.N; p.K = w.K; p.bias = w.b;
@@ -267,7 +268,7 @@ int test_contraction(const dawn_contraction_case& c, cudaStream_t st) {
   p.B = c.B; p.ldb = c.ldb; p.b_batch_stride = c.b_batch_stride;
   p.Out = c.Out; p.ldo = c.ldo; p.OH = c.OH; p.OW = c.OW; p.out_stride = c.out_stride; p.oy0 = c.oy0; p.ox0 = c.ox0;
   p.bias = c.bias; p.Res = c.Res; p.ldr = c.ldr;
-  p.stats = c.stats; p.cpg = c.cpg;
+  p.stats = c.stats; p.cpg = c.cpg; p.clips = 1;
   p.rowstats = c.rowstats; p.ln_inline = c.ln_inline; p.wsum = c.wsum; p.rot = c.rot; p.P = c.P;
   p.q_post_scale = c.q_post_scale;
   p.kq = c.kq; p.nkq = c.nkq; p.gates = c.gates;

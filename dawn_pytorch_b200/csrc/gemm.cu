@@ -25,7 +25,7 @@ __global__ void __launch_bounds__(THREADS, 2) gemm_kernel(const GemmParams p) {
   float* As = smem;
   float* Bs = smem + STAGES * BM * A_LD;
   __shared__ float s_stat[16];
-  __shared__ float s_gn[16];
+  __shared__ float s_gn[16 * kMaxClips];
 
   if (p.skip_flag && *p.skip_flag == p.skip_if) return;
   const int tid = threadIdx.x;
@@ -43,7 +43,7 @@ __global__ void __launch_bounds__(THREADS, 2) gemm_kernel(const GemmParams p) {
   const float* Bmat = p.B + (long long)batch * p.b_batch_stride;
 
   if (tid < 16) s_stat[tid] = 0.f;
-  if (EPI == EPI_GN_APPLY && tid < 8) {
+  if (EPI == EPI_GN_APPLY && tid < 8 * p.clips) {     // (mean, rstd) of every clip's 8 groups
     double s = p.gn_stats[2 * tid], ss = p.gn_stats[2 * tid + 1];
     double mean = s / p.gn_count;
     double var = ss / p.gn_count - mean * mean;
@@ -156,6 +156,8 @@ __global__ void __launch_bounds__(THREADS, 2) gemm_kernel(const GemmParams p) {
   // thread owns rows r(mt,h) = m0 + wm*32 + mt*16 + g + 8h, cols n0 + wn*32 + nt*8 + 2*t4 (+1)
   const int ncol0 = n0 + wn * 32 + 2 * t4;
   float st_s[4] = {0.f, 0.f, 0.f, 0.f}, st_ss[4] = {0.f, 0.f, 0.f, 0.f};
+  // GroupNorm statistics are per clip: a tile whose rows span frames of several clips adds each row's sums to its own clip's slot
+  const bool mixed_clips = p.clips > 1 && m0 / Ps != (min(m0 + BM, m_end) - 1) / Ps;
 
 #pragma unroll
   for (int mt = 0; mt < 2; ++mt)
@@ -183,6 +185,7 @@ __global__ void __launch_bounds__(THREADS, 2) gemm_kernel(const GemmParams p) {
       }
 
       if (EPI == EPI_PLAIN) {
+        float rs_[4] = {0.f, 0.f, 0.f, 0.f}, rss_[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
         for (int nt = 0; nt < 4; ++nt) {
           const int n = ncol0 + nt * 8;
@@ -196,24 +199,42 @@ __global__ void __launch_bounds__(THREADS, 2) gemm_kernel(const GemmParams p) {
                 x0 += r.x; x1 += r.y;
               }
               *reinterpret_cast<float2*>(p.Out + opix * p.ldo + n) = make_float2(x0, x1);
-              st_s[nt] += x0 + x1;
-              st_ss[nt] += x0 * x0 + x1 * x1;
+              rs_[nt] = x0 + x1;
+              rss_[nt] = x0 * x0 + x1 * x1;
+              st_s[nt] += rs_[nt];
+              st_ss[nt] += rss_[nt];
+            }
+          }
+        }
+        if (p.stats != nullptr && mixed_clips) {
+          double* cs = p.stats + 16 * (f % p.clips);
+#pragma unroll
+          for (int nt = 0; nt < 4; ++nt) {
+            const float s = quad_sum(rs_[nt]), ss = quad_sum(rss_[nt]);
+            const int n = n0 + wn * 32 + nt * 8;
+            if (t4 == 0 && rv && n < p.N) {
+              const int grp = n / p.cpg;
+              atomicAdd(&cs[2 * grp], (double)s);
+              atomicAdd(&cs[2 * grp + 1], (double)ss);
             }
           }
         }
       } else if (EPI == EPI_GN_APPLY) {
+        const int clip = p.clips > 1 ? f % p.clips : 0;
+        const float* gn = s_gn + 16 * clip;
+        const float* film = p.film ? p.film + (size_t)clip * 2 * p.N : nullptr;
 #pragma unroll
         for (int nt = 0; nt < 4; ++nt) {
           const int n = ncol0 + nt * 8;
           if (n < p.N && rv) {
             const float2 y = *reinterpret_cast<const float2*>(p.Y + opix * p.ldy + n);
             const int grp = n / p.cpg;
-            const float mean = s_gn[2 * grp], rstd = s_gn[2 * grp + 1];
+            const float mean = gn[2 * grp], rstd = gn[2 * grp + 1];
             float t0 = (y.x - mean) * rstd * p.gn_w[n] + p.gn_b[n];
             float t1 = (y.y - mean) * rstd * p.gn_w[n + 1] + p.gn_b[n + 1];
-            if (p.film) {
-              t0 = t0 * (p.film[n] + 1.f) + p.film[p.N + n];
-              t1 = t1 * (p.film[n + 1] + 1.f) + p.film[p.N + n + 1];
+            if (film) {
+              t0 = t0 * (film[n] + 1.f) + film[p.N + n];
+              t1 = t1 * (film[n + 1] + 1.f) + film[p.N + n + 1];
             }
             *reinterpret_cast<float2*>(p.Out + opix * p.ldo + n) =
                 make_float2(silu(t0) + v[nt][0], silu(t1) + v[nt][1]);
@@ -292,8 +313,9 @@ __global__ void __launch_bounds__(THREADS, 2) gemm_kernel(const GemmParams p) {
       }
     }
 
-  if (EPI == EPI_PLAIN && p.stats != nullptr) {
+  if (EPI == EPI_PLAIN && p.stats != nullptr && !mixed_clips) {
     // GroupNorm partial statistics of the values just written (U:230: statistics span the clip)
+    double* cs = p.clips > 1 ? p.stats + 16 * ((m0 / Ps) % p.clips) : p.stats;
 #pragma unroll
     for (int nt = 0; nt < 4; ++nt) {
       float s = warp_sum(st_s[nt]), ss = warp_sum(st_ss[nt]);
@@ -308,7 +330,7 @@ __global__ void __launch_bounds__(THREADS, 2) gemm_kernel(const GemmParams p) {
     if (tid < 16) {
       const int grp = tid >> 1;
       const int glo = n0 / p.cpg, ghi = (min(n0 + BN, p.N) - 1) / p.cpg;
-      if (grp >= glo && grp <= ghi) atomicAdd(&p.stats[tid], (double)s_stat[tid]);
+      if (grp >= glo && grp <= ghi) atomicAdd(&cs[tid], (double)s_stat[tid]);
     }
   }
 }

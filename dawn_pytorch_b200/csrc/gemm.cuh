@@ -44,6 +44,7 @@ struct GemmParams {
   const float* bias;
   const float* Res; int ldr;
   double* stats; int cpg;  // GroupNorm accumulators [groups][2], channels per group
+  int clips;               // >= 1 clips interleaved by frame (frame index = f * clips + clip): stats and gn_stats are [clips][16], film [clips][2N]
   // LayerNorm fold
   const float* rowstats;   // [M][2] (mu, rstd); null on the wgmma path when ln_inline is set
   int ln_inline;           // wgmma 1x1 GEMMs: the producers accumulate each row's sum / sum of squares while they stream it

@@ -50,12 +50,12 @@ int launch_rowstats(const float* x, int ld, int C, int M, float eps, float* out,
 
 // =========================================================================== GroupNorm apply (elementwise)
 __global__ void gn_apply_kernel(const float* __restrict__ Y, int ldy, int C, long long nvec_total,
-                                const double* __restrict__ stats, double count, int cpg,
+                                const double* __restrict__ stats, double count, int cpg, int P, int clips,
                                 const float* __restrict__ gw, const float* __restrict__ gb,
                                 const float* __restrict__ film, const float* Res, int ldr,
                                 float* Out, int ldo) {
-  __shared__ float s_gn[16];
-  if (threadIdx.x < 8) {
+  __shared__ float s_gn[16 * kMaxClips];
+  if (threadIdx.x < 8 * clips) {                 // (mean, rstd) of every clip's 8 groups
     const double s = stats[2 * threadIdx.x], ss = stats[2 * threadIdx.x + 1];
     const double mean = s / count;
     const double var = ss / count - mean * mean;
@@ -68,9 +68,10 @@ __global__ void gn_apply_kernel(const float* __restrict__ Y, int ldy, int C, lon
        idx += (long long)gridDim.x * blockDim.x) {
     const long long row = idx / vpr;
     const int c = (int)(idx - row * vpr) * 4;
+    const int clip = clips > 1 ? (int)((row / P) % clips) : 0;
     const float4 y = *reinterpret_cast<const float4*>(Y + row * ldy + c);
     const int grp = c / cpg;
-    const float mean = s_gn[2 * grp], rstd = s_gn[2 * grp + 1];
+    const float mean = s_gn[16 * clip + 2 * grp], rstd = s_gn[16 * clip + 2 * grp + 1];
     const float4 w = *reinterpret_cast<const float4*>(gw + c);
     const float4 b = *reinterpret_cast<const float4*>(gb + c);
     float t0 = (y.x - mean) * rstd * w.x + b.x;
@@ -78,8 +79,9 @@ __global__ void gn_apply_kernel(const float* __restrict__ Y, int ldy, int C, lon
     float t2 = (y.z - mean) * rstd * w.z + b.z;
     float t3 = (y.w - mean) * rstd * w.w + b.w;
     if (film) {
-      const float4 sc = *reinterpret_cast<const float4*>(film + c);
-      const float4 sh = *reinterpret_cast<const float4*>(film + C + c);
+      const float* fc = film + (size_t)clip * 2 * C;
+      const float4 sc = *reinterpret_cast<const float4*>(fc + c);
+      const float4 sh = *reinterpret_cast<const float4*>(fc + C + c);
       t0 = t0 * (sc.x + 1.f) + sh.x; t1 = t1 * (sc.y + 1.f) + sh.y;
       t2 = t2 * (sc.z + 1.f) + sh.z; t3 = t3 * (sc.w + 1.f) + sh.w;
     }
@@ -92,14 +94,15 @@ __global__ void gn_apply_kernel(const float* __restrict__ Y, int ldy, int C, lon
   }
 }
 
-int launch_gn_apply(const float* Y, int ldy, int C, int M, const double* stats, double count, int cpg,
+int launch_gn_apply(const float* Y, int ldy, int C, int M, const double* stats, double count, int cpg, int P, int clips,
                     const float* gw, const float* gb, const float* film, const float* Res, int ldr,
                     float* Out, int ldo, cudaStream_t st) {
+  if (clips < 1 || clips > kMaxClips || P < 1) { set_last_error("gn_apply: bad clip geometry"); return -1; }
   const long long nvec = (long long)M * (C >> 2);
   const int threads = 256;
   long long blocks = (nvec + threads - 1) / threads;
   if (blocks > 148LL * 16) blocks = 148LL * 16;
-  gn_apply_kernel<<<(int)blocks, threads, 0, st>>>(Y, ldy, C, nvec, stats, count, cpg, gw, gb, film, Res, ldr, Out, ldo);
+  gn_apply_kernel<<<(int)blocks, threads, 0, st>>>(Y, ldy, C, nvec, stats, count, cpg, P, clips, gw, gb, film, Res, ldr, Out, ldo);
   DAWN_LAUNCH_OK();
   return 0;
 }
@@ -109,16 +112,20 @@ int launch_gn_apply(const float* Y, int ldy, int C, int M, const double* stats, 
 // A block owns FL_JT*8 = 32 outputs x FL_FT = 8 frames, so every weight row is read once per 8 frames and act(x) is evaluated
 // once per 32 outputs; a warp computes FL_JT outputs with lane-strided partial sums and a butterfly reduction.
 constexpr int FL_FT = 8, FL_JT = 4;
+// Output row i (table order: frame f of clip b is i = f * clips + b) reads input row b * (F / clips) + f (clips back to back).
 template <int ACT>
 __device__ __forceinline__ void frame_linear_tiled_body(const float* __restrict__ x, int ldx, int off, int K,
                                                         const float* __restrict__ W, const float* __restrict__ b, int Nout,
-                                                        float* __restrict__ out, int F) {
+                                                        float* __restrict__ out, int F, int clips) {
   extern __shared__ float sx[];                 // [FL_FT][K]
   const int f0 = blockIdx.y * FL_FT;
   for (int i = threadIdx.x; i < FL_FT * K; i += blockDim.x) {
     const int ft = i / K, k = i - ft * K;
     float v = 0.f;
-    if (f0 + ft < F) { v = x[(size_t)(f0 + ft) * ldx + off + k]; v = ACT ? silu(v) : v; }
+    if (f0 + ft < F) {
+      const int ti = f0 + ft, src = (ti % clips) * (F / clips) + ti / clips;
+      v = x[(size_t)src * ldx + off + k]; v = ACT ? silu(v) : v;
+    }
     sx[i] = v;
   }
   __syncthreads();
@@ -149,14 +156,15 @@ __device__ __forceinline__ void frame_linear_tiled_body(const float* __restrict_
       if (lane == 0 && j0 + jj < Nout && f0 + ft < F) out[(size_t)(f0 + ft) * Nout + j0 + jj] = r + (b ? b[j0 + jj] : 0.f);
     }
 }
-__global__ void __launch_bounds__(256) cond_mlp_tiled_kernel(const float* __restrict__ cond, int cond_ld, const CondDesc* __restrict__ descs, int F) {
+__global__ void __launch_bounds__(256) cond_mlp_tiled_kernel(const float* __restrict__ cond, int cond_ld, const CondDesc* __restrict__ descs, int F,
+                                                             int clips) {
   const CondDesc d = descs[blockIdx.z];
   if ((int)blockIdx.x * 8 * FL_JT >= d.n1) return;
-  frame_linear_tiled_body<1>(cond, cond_ld, d.off, d.K, d.mW, d.mB, d.n1, d.ctx, F);
+  frame_linear_tiled_body<1>(cond, cond_ld, d.off, d.K, d.mW, d.mB, d.n1, d.ctx, F, clips);
 }
 __global__ void __launch_bounds__(256) cond_kv_tiled_kernel(const CondDesc* __restrict__ descs, int F) {
   const CondDesc d = descs[blockIdx.z];
-  frame_linear_tiled_body<0>(d.ctx, d.n1, 0, d.n1, d.Wkv, nullptr, 128, d.kv, F);
+  frame_linear_tiled_body<0>(d.ctx, d.n1, 0, d.n1, d.Wkv, nullptr, 128, d.kv, F, 1);
 }
 
 // =========================================================================== cross-attention per-frame tables
@@ -242,7 +250,8 @@ __device__ __forceinline__ void ca_tables_body(const CaTableArgs& a, int f) {
 __global__ void __launch_bounds__(256) ca_tables_batched_kernel(const CondDesc* __restrict__ descs) { ca_tables_body(descs[blockIdx.y].t, blockIdx.x); }
 
 int launch_cond_batched(const float* cond, int cond_ld, const CondDesc* descs_dev, int ndesc, int max_n1, int max_k, int max_co, int F,
-                        cudaStream_t st) {
+                        int clips, cudaStream_t st) {
+  if (clips < 1 || F % clips != 0) { set_last_error("cond tables: frames must be a multiple of the clip count"); return -1; }
   const size_t sm1 = (size_t)FL_FT * max_k * sizeof(float), sm2 = (size_t)FL_FT * max_n1 * sizeof(float);
   const size_t smem_t = (size_t)9 * max_co * sizeof(float);
   static size_t attr = 0;
@@ -253,7 +262,7 @@ int launch_cond_batched(const float* cond, int cond_ld, const CondDesc* descs_de
     DAWN_CUDA_OK(cudaFuncSetAttribute(ca_tables_batched_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attr));
   }
   const int ft = (F + FL_FT - 1) / FL_FT, jb = 8 * FL_JT;
-  cond_mlp_tiled_kernel<<<dim3((max_n1 + jb - 1) / jb, ft, ndesc), 256, sm1, st>>>(cond, cond_ld, descs_dev, F);
+  cond_mlp_tiled_kernel<<<dim3((max_n1 + jb - 1) / jb, ft, ndesc), 256, sm1, st>>>(cond, cond_ld, descs_dev, F, clips);
   DAWN_LAUNCH_OK();
   cond_kv_tiled_kernel<<<dim3((128 + jb - 1) / jb, ft, ndesc), 256, sm2, st>>>(descs_dev, F);
   DAWN_LAUNCH_OK();
@@ -332,12 +341,13 @@ int launch_split_rows(const float* x, int ld, int C, long long M, void* hi, void
 __global__ void time_mlp_kernel(const int64_t* __restrict__ t, const float* __restrict__ freqs, int dim,
                                 const float* __restrict__ W1, const float* __restrict__ b1,
                                 const float* __restrict__ W2, const float* __restrict__ b2,
-                                float* __restrict__ t_silu) {
+                                float* __restrict__ t_silu, int t_stride) {
   extern __shared__ float sm[];
   float* emb = sm;             // [dim]
   float* hid = sm + dim;       // [4 dim]
   const int tdim = 4 * dim, half = dim / 2;
-  const float tv = (float)t[0];
+  const float tv = (float)t[(size_t)blockIdx.x * t_stride];     // block = clip
+  t_silu += (size_t)blockIdx.x * tdim;
   for (int i = threadIdx.x; i < half; i += blockDim.x) {
     const float a = tv * freqs[i];
     emb[i] = sinf(a);
@@ -357,9 +367,9 @@ __global__ void time_mlp_kernel(const int64_t* __restrict__ t, const float* __re
   }
 }
 
-int launch_time_mlp(const int64_t* t_dev, const float* freqs, int dim, const float* W1, const float* b1,
+int launch_time_mlp(const int64_t* t_dev, int t_stride, int clips, const float* freqs, int dim, const float* W1, const float* b1,
                     const float* W2, const float* b2, float* t_silu, cudaStream_t st) {
-  time_mlp_kernel<<<1, 256, 5 * dim * sizeof(float), st>>>(t_dev, freqs, dim, W1, b1, W2, b2, t_silu);
+  time_mlp_kernel<<<clips, 256, 5 * dim * sizeof(float), st>>>(t_dev, freqs, dim, W1, b1, W2, b2, t_silu, t_stride);
   DAWN_LAUNCH_OK();
   return 0;
 }
@@ -367,16 +377,17 @@ int launch_time_mlp(const int64_t* t_dev, const float* freqs, int dim, const flo
 __global__ void film_kernel(const FilmDesc* __restrict__ descs, const float* __restrict__ t_silu, int tdim) {
   const FilmDesc d = descs[blockIdx.y];
   const int j = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  const int lane = threadIdx.x & 31;
+  const int lane = threadIdx.x & 31, clip = blockIdx.z;
   if (j >= d.n) return;
+  t_silu += (size_t)clip * tdim;
   float acc = 0.f;
   for (int i = lane; i < tdim; i += 32) acc += d.W[(size_t)j * tdim + i] * t_silu[i];
   acc = warp_sum(acc);
-  if (lane == 0) d.out[j] = acc + d.b[j];
+  if (lane == 0) d.out[(size_t)clip * d.n + j] = acc + d.b[j];
 }
 
-int launch_film(const FilmDesc* descs_dev, int ndesc, const float* t_silu, int tdim, cudaStream_t st) {
-  dim3 grid(1024 / 8, ndesc);       // n <= 1024 outputs per block descriptor
+int launch_film(const FilmDesc* descs_dev, int ndesc, int clips, const float* t_silu, int tdim, cudaStream_t st) {
+  dim3 grid(1024 / 8, ndesc, clips);       // n <= 1024 outputs per block descriptor
   film_kernel<<<grid, 256, 0, st>>>(descs_dev, t_silu, tdim);
   DAWN_LAUNCH_OK();
   return 0;
@@ -617,11 +628,13 @@ int launch_sla_context(const float* qkv, int ld, int F, int P, const float* Wout
 
 // =========================================================================== layout transforms / init conv / heads
 // x[c][f][p] -> out[f][p][c_dst0 + c] (Cpad channels per pixel).  Channels outside [c_dst0, c_dst0+C) are zeroed.
+// x holds `clips` such tensors back to back; output frame f * clips + b is frame f of clip b
 __global__ void ncf_to_nhwc_kernel(const float* __restrict__ x, int C, int F, int HW, int Cpad, int c_dst0,
-                                   float* __restrict__ out, const int* __restrict__ skip_flag, int skip_if) {
+                                   float* __restrict__ out, const int* __restrict__ skip_flag, int skip_if, int clips) {
   __shared__ float tile[32][33];
   if (skip_flag && *skip_flag == skip_if) return;
-  const int f = blockIdx.z;
+  const int fo = blockIdx.z, f = fo / clips;
+  x += (size_t)(fo % clips) * C * F * HW;
   const int p0 = blockIdx.x * 32, c0 = blockIdx.y * 32;       // c0 indexes destination channels
   const int tx = threadIdx.x, ty = threadIdx.y;               // (32, 8)
   for (int k = ty; k < 32; k += 8) {
@@ -633,13 +646,13 @@ __global__ void ncf_to_nhwc_kernel(const float* __restrict__ x, int C, int F, in
   __syncthreads();
   for (int k = ty; k < 32; k += 8) {
     const int p = p0 + k, cd = c0 + tx;
-    if (p < HW && cd < Cpad) out[((size_t)f * HW + p) * Cpad + cd] = tile[tx][k];
+    if (p < HW && cd < Cpad) out[((size_t)fo * HW + p) * Cpad + cd] = tile[tx][k];
   }
 }
 int launch_ncf_to_nhwc(const float* x, int C, int F, int HW, int Cpad, int c_dst0, float* out, cudaStream_t st,
-                       const int* skip_flag, int skip_if) {
-  dim3 grid((HW + 31) / 32, (Cpad + 31) / 32, F);
-  ncf_to_nhwc_kernel<<<grid, dim3(32, 8), 0, st>>>(x, C, F, HW, Cpad, c_dst0, out, skip_flag, skip_if);
+                       const int* skip_flag, int skip_if, int clips) {
+  dim3 grid((HW + 31) / 32, (Cpad + 31) / 32, F * clips);
+  ncf_to_nhwc_kernel<<<grid, dim3(32, 8), 0, st>>>(x, C, F, HW, Cpad, c_dst0, out, skip_flag, skip_if, clips);
   DAWN_LAUNCH_OK();
   return 0;
 }
@@ -647,12 +660,14 @@ int launch_ncf_to_nhwc(const float* x, int C, int F, int HW, int Cpad, int c_dst
 // Per-clip constant part of the k x k init conv as k row-convolutions that run side by side: copy s of the feature frame is
 // the frame shifted by (s - pad) rows (zero outside), so row ky of the kernel becomes a 1 x k conv over copy ky and the k
 // partial maps only need adding.  One frame of 64x64 pixels is 32 row tiles of the contraction kernel: k copies = k x 32 CTAs.
-// x[c][p] -> out[s][p][c_dst0 + c], Cpad channels per pixel, other channels zero.
-__global__ void fea_shift_nhwc_kernel(const float* __restrict__ x, long long cstride, int C, int H, int W, int Cpad, int c_dst0, int pad,
-                                      float* __restrict__ out, const int* __restrict__ skip_flag, int skip_if) {
+// x[c][p] -> out[s][p][c_dst0 + c], Cpad channels per pixel, other channels zero.  With several clips (clip b's frame at
+// x + b * clip_stride) copy s of clip b is out[s * clips + b].
+__global__ void fea_shift_nhwc_kernel(const float* __restrict__ x, long long cstride, long long clip_stride, int clips, int C, int H, int W,
+                                      int Cpad, int c_dst0, int pad, float* __restrict__ out, const int* __restrict__ skip_flag, int skip_if) {
   __shared__ float tile[32][33];
   if (skip_flag && *skip_flag == skip_if) return;
-  const int s = blockIdx.z, HW = H * W, shift = (s - pad) * W;
+  const int so = blockIdx.z, s = so / clips, HW = H * W, shift = (s - pad) * W;
+  x += (size_t)(so % clips) * clip_stride;
   const int p0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
   const int tx = threadIdx.x, ty = threadIdx.y;               // (32, 8)
   for (int k = ty; k < 32; k += 8) {
@@ -664,13 +679,13 @@ __global__ void fea_shift_nhwc_kernel(const float* __restrict__ x, long long cst
   __syncthreads();
   for (int k = ty; k < 32; k += 8) {
     const int p = p0 + k, cd = c0 + tx;
-    if (p < HW && cd < Cpad) out[((size_t)s * HW + p) * Cpad + cd] = tile[tx][k];
+    if (p < HW && cd < Cpad) out[((size_t)so * HW + p) * Cpad + cd] = tile[tx][k];
   }
 }
-int launch_fea_shift_nhwc(const float* x, long long cstride, int C, int H, int W, int Cpad, int c_dst0, int k, float* out, cudaStream_t st,
-                          const int* skip_flag, int skip_if) {
-  dim3 grid((H * W + 31) / 32, (Cpad + 31) / 32, k);
-  fea_shift_nhwc_kernel<<<grid, dim3(32, 8), 0, st>>>(x, cstride, C, H, W, Cpad, c_dst0, k / 2, out, skip_flag, skip_if);
+int launch_fea_shift_nhwc(const float* x, long long cstride, long long clip_stride, int clips, int C, int H, int W, int Cpad, int c_dst0,
+                          int k, float* out, cudaStream_t st, const int* skip_flag, int skip_if) {
+  dim3 grid((H * W + 31) / 32, (Cpad + 31) / 32, k * clips);
+  fea_shift_nhwc_kernel<<<grid, dim3(32, 8), 0, st>>>(x, cstride, clip_stride, clips, C, H, W, Cpad, c_dst0, k / 2, out, skip_flag, skip_if);
   DAWN_LAUNCH_OK();
   return 0;
 }
@@ -694,38 +709,45 @@ int launch_map_reduce(const float* part, int nsplit, long long n, const float* b
 // flag = 1 iff some channel c in [c0, C) of x (C, F, HW) differs between frame 0 and any other frame (bit compare: NaNs and
 // signed zeros count as different -> the general path).  The reference's sampler tiles the per-clip features over the frames
 // (U:1167 `fea.repeat`), so the general entry can take the hoisted init conv whenever this finds no difference.
-__global__ void frame_invariance_kernel(const float* __restrict__ x, int c0, int C, int F, int HW, int* __restrict__ flag) {
-  const long long per_c = (long long)(F - 1) * HW, total = (long long)(C - c0) * per_c;
-  bool diff = false;
+// Per clip (x holds `clips` (C, F, HW) tensors back to back): flag[b] for clip b, and flag[clips] counts the clips whose flag is set.
+__global__ void frame_invariance_kernel(const float* __restrict__ x, int c0, int C, int F, int HW, int clips, int* __restrict__ flag) {
+  const long long per_c = (long long)(F - 1) * HW, per_clip = (long long)(C - c0) * per_c, total = per_clip * clips;
+  unsigned int diff = 0;                         // bit b: clip b differs
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-    const int c = c0 + (int)(i / per_c);
-    const long long r = i - (long long)(c - c0) * per_c;
+    const int b = (int)(i / per_clip);
+    const long long ic = i - (long long)b * per_clip;
+    const int c = c0 + (int)(ic / per_c);
+    const long long r = ic - (long long)(c - c0) * per_c;
     const int p = (int)(r % HW);
-    const float* base = x + (size_t)c * F * HW;
-    diff |= __float_as_uint(base[HW + r]) != __float_as_uint(base[p]);
+    const float* base = x + ((size_t)b * C + c) * F * HW;
+    if (__float_as_uint(base[HW + r]) != __float_as_uint(base[p])) diff |= 1u << b;
   }
-  if (__any_sync(0xffffffffu, diff) && (threadIdx.x & 31) == 0) atomicOr(flag, 1);
+  diff = __reduce_or_sync(0xffffffffu, diff);
+  if ((threadIdx.x & 31) == 0)
+    for (int b = 0; b < clips; ++b)
+      if (((diff >> b) & 1u) && atomicOr(flag + b, 1) == 0) atomicAdd(flag + clips, 1);
 }
-int launch_frame_invariance(const float* x, int c0, int C, int F, int HW, int* flag, cudaStream_t st) {
-  DAWN_CUDA_OK(cudaMemsetAsync(flag, 0, sizeof(int), st));
+int launch_frame_invariance(const float* x, int c0, int C, int F, int HW, int clips, int* flag, cudaStream_t st) {
+  DAWN_CUDA_OK(cudaMemsetAsync(flag, 0, sizeof(int) * (clips + 1), st));
   if (F > 1 && C > c0) {
-    frame_invariance_kernel<<<148 * 8, 256, 0, st>>>(x, c0, C, F, HW, flag);
+    frame_invariance_kernel<<<148 * 8, 256, 0, st>>>(x, c0, C, F, HW, clips, flag);
     DAWN_LAUNCH_OK();
   }
   return 0;
 }
 
-// hoisted init conv: only the 3 noisy channels change per step; the 272 feature channels are a per-clip map
-__global__ void init_conv_x3_kernel(const float* __restrict__ xt, int F, int H, int W,
+// hoisted init conv: only the 3 noisy channels change per step; the 272 feature channels are a per-clip map.
+// Clip b's channels 0..2 start at xt + b * clip_stride, map holds one (H, W, Co) map per clip; output frame f * clips + b is frame f
+// of clip b, and skip_flag (optional) is per clip: clip b is left alone when skip_flag[b] == skip_if.
+__global__ void init_conv_x3_kernel(const float* __restrict__ xt, long long clip_stride, int F, int H, int W, int clips,
                                     const float* __restrict__ w3, const float* __restrict__ map, int Co,
                                     float* __restrict__ out, int ldo, int ksz, const int* __restrict__ skip_flag, int skip_if) {
   extern __shared__ float sw[];                 // [ksz*ksz*3][Co]
-  if (skip_flag && *skip_flag == skip_if) return;
   const int ntap = ksz * ksz * 3;
   for (int i = threadIdx.x; i < ntap * Co; i += blockDim.x) sw[i] = w3[i];
   __syncthreads();
   const int cg = Co >> 2;                       // float4 groups per pixel
-  const long long total = (long long)F * H * W * cg;
+  const long long total = (long long)F * clips * H * W * cg;
   const int pad = ksz / 2;
   for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
        idx += (long long)gridDim.x * blockDim.x) {
@@ -733,8 +755,10 @@ __global__ void init_conv_x3_kernel(const float* __restrict__ xt, int F, int H, 
     const long long pix = idx / cg;
     const int x0 = (int)(pix % W);
     const int y0 = (int)((pix / W) % H);
-    const int f = (int)(pix / ((long long)W * H));
-    float4 acc = *reinterpret_cast<const float4*>(map + ((size_t)y0 * W + x0) * Co + c4);
+    const int fo = (int)(pix / ((long long)W * H)), f = fo / clips, b = fo % clips;
+    if (skip_flag && skip_flag[b] == skip_if) continue;
+    const float* xc = xt + (size_t)b * clip_stride;
+    float4 acc = *reinterpret_cast<const float4*>(map + (((size_t)b * H + y0) * W + x0) * Co + c4);
     for (int ky = 0; ky < ksz; ++ky) {
       const int iy = y0 + ky - pad;
       if (iy < 0 || iy >= H) continue;
@@ -743,7 +767,7 @@ __global__ void init_conv_x3_kernel(const float* __restrict__ xt, int F, int H, 
         if (ix < 0 || ix >= W) continue;
 #pragma unroll
         for (int c = 0; c < 3; ++c) {
-          const float xv = xt[(((size_t)c * F + f) * H + iy) * W + ix];
+          const float xv = xc[(((size_t)c * F + f) * H + iy) * W + ix];
           const float4 wv = *reinterpret_cast<const float4*>(&sw[((ky * ksz + kx) * 3 + c) * Co + c4]);
           acc.x += xv * wv.x; acc.y += xv * wv.y; acc.z += xv * wv.z; acc.w += xv * wv.w;
         }
@@ -756,17 +780,21 @@ __global__ void init_conv_x3_kernel(const float* __restrict__ xt, int F, int H, 
 // channels (32 accumulators).  One (channel, ky) input row segment of 4 + KS - 1 values feeds KS x 32 FMAs, so shared-memory traffic
 // per FMA drops ~4x against the one-pixel-per-thread kernel above, which was bound by its weight reads.
 template <int KS>
-__global__ void __launch_bounds__(128) init_conv_x3_tiled_kernel(const float* __restrict__ xt, int F, int H, int W,
+__global__ void __launch_bounds__(128) init_conv_x3_tiled_kernel(const float* __restrict__ xt, long long clip_stride, int F, int H, int W,
+                                                                 int clips,
                                                                  const float* __restrict__ w3, const float* __restrict__ map,
                                                                  float* __restrict__ out, int ldo, const int* __restrict__ skip_flag,
                                                                  int skip_if) {
   constexpr int PAD = KS / 2, TW = 64, TR = 8, IR = TR + KS - 1, ILD = 72, NW = KS * KS * 3 * 64;
   extern __shared__ __align__(16) float sm_ic[];
-  if (skip_flag && *skip_flag == skip_if) return;
+  const int fo = blockIdx.z, f = fo / clips, b = fo % clips;
+  if (skip_flag && skip_flag[b] == skip_if) return;
   float* sw = sm_ic;                            // [KS*KS*3][64]
   float* sx = sm_ic + NW;                       // [3][IR][ILD]
   const int tid = threadIdx.x;
-  const int f = blockIdx.z, y0 = blockIdx.y * TR, x0 = blockIdx.x * TW;
+  const int y0 = blockIdx.y * TR, x0 = blockIdx.x * TW;
+  xt += (size_t)b * clip_stride;
+  map += (size_t)b * H * W * 64;
   for (int i = tid; i < NW / 4; i += 128) reinterpret_cast<float4*>(sw)[i] = __ldg(reinterpret_cast<const float4*>(w3) + i);
   for (int i = tid; i < 3 * IR * ILD; i += 128) {
     const int c = i / (IR * ILD), rem = i - c * IR * ILD, r = rem / ILD, col = rem - r * ILD;
@@ -819,7 +847,7 @@ __global__ void __launch_bounds__(128) init_conv_x3_tiled_kernel(const float* __
     for (int i = 0; i < 4; ++i) {
       const int x = x0 + pxg * 4 + i;
       if (x < W) {
-        float* dst = out + ((size_t)f * H * W + (size_t)y * W + x) * ldo + cg * 8;
+        float* dst = out + ((size_t)fo * H * W + (size_t)y * W + x) * ldo + cg * 8;
         *reinterpret_cast<float4*>(dst) = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
         *reinterpret_cast<float4*>(dst + 4) = make_float4(acc[i][4], acc[i][5], acc[i][6], acc[i][7]);
       }
@@ -827,7 +855,7 @@ __global__ void __launch_bounds__(128) init_conv_x3_tiled_kernel(const float* __
   }
 }
 
-int launch_init_conv_x3(const float* xt, int F, int H, int W, const float* w3, const float* map, int Co,
+int launch_init_conv_x3(const float* xt, long long clip_stride, int F, int H, int W, int clips, const float* w3, const float* map, int Co,
                         float* out, int ldo, int ksz, cudaStream_t st, const int* skip_flag, int skip_if) {
   if (ksz == 7 && Co == 64) {
     constexpr size_t smem_t = (size_t)(7 * 7 * 3 * 64 + 3 * (8 + 6) * 72) * sizeof(float);
@@ -836,7 +864,8 @@ int launch_init_conv_x3(const float* xt, int F, int H, int W, const float* w3, c
       DAWN_CUDA_OK(cudaFuncSetAttribute(init_conv_x3_tiled_kernel<7>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_t));
       attr_t = true;
     }
-    init_conv_x3_tiled_kernel<7><<<dim3((W + 63) / 64, (H + 7) / 8, F), 128, smem_t, st>>>(xt, F, H, W, w3, map, out, ldo, skip_flag, skip_if);
+    init_conv_x3_tiled_kernel<7><<<dim3((W + 63) / 64, (H + 7) / 8, F * clips), 128, smem_t, st>>>(xt, clip_stride, F, H, W, clips, w3, map, out, ldo,
+                                                                                                  skip_flag, skip_if);
     DAWN_LAUNCH_OK();
     return 0;
   }
@@ -847,21 +876,29 @@ int launch_init_conv_x3(const float* xt, int F, int H, int W, const float* w3, c
     attr = true;
   }
   if (smem > 100 * 1024) { set_last_error("init_conv_x3: kernel too large for shared memory"); return -1; }
-  const long long total = (long long)F * H * W * (Co >> 2);
+  const long long total = (long long)F * clips * H * W * (Co >> 2);
   long long blocks = (total + 255) / 256;
   if (blocks > 148 * 8) blocks = 148 * 8;
-  init_conv_x3_kernel<<<(int)blocks, 256, smem, st>>>(xt, F, H, W, w3, map, Co, out, ldo, ksz, skip_flag, skip_if);
+  init_conv_x3_kernel<<<(int)blocks, 256, smem, st>>>(xt, clip_stride, F, H, W, clips, w3, map, Co, out, ldo, ksz, skip_flag, skip_if);
   DAWN_LAUNCH_OK();
   return 0;
 }
 
-// final 1x1 convs of both heads, written channel-major (the module's NCFHW output)
-__global__ void heads_out_kernel(const float* __restrict__ hf, const float* __restrict__ ho, int C, int M,
+// final 1x1 convs of both heads, written channel-major (the module's NCFHW output), clip by clip: row m is pixel p of frame
+// fo = f * clips + b, written to out[b][j][f][p]
+__global__ void heads_out_kernel(const float* __restrict__ hf, const float* __restrict__ ho, int C, int M, int HW, int clips,
                                  const float* __restrict__ Wf, const float* __restrict__ bf, int ng,
                                  const float* __restrict__ Wo, const float* __restrict__ bo, int nc,
                                  float* __restrict__ out) {
   const int m = blockIdx.x * blockDim.x + threadIdx.x;
   if (m >= M) return;
+  size_t mc = m, Mc = M;                                       // row within the clip, rows per clip
+  if (clips > 1) {
+    const int fo = m / HW, b = fo % clips;
+    Mc = M / clips;
+    mc = (size_t)(fo / clips) * HW + (m - fo * HW);
+    out += (size_t)b * (ng + nc) * Mc;
+  }
   for (int j = 0; j < ng + nc; ++j) {
     const float* src = (j < ng ? hf : ho) + (size_t)m * C;
     const float* w = (j < ng) ? Wf + (size_t)j * C : Wo + (size_t)(j - ng) * C;
@@ -871,12 +908,12 @@ __global__ void heads_out_kernel(const float* __restrict__ hf, const float* __re
       const float4 b = *reinterpret_cast<const float4*>(w + c);
       acc += a.x * b.x + a.y * b.y + a.z * b.z + a.w * b.w;
     }
-    out[(size_t)j * M + m] = acc;
+    out[j * Mc + mc] = acc;
   }
 }
-int launch_heads_out(const float* hf, const float* ho, int C, int M, const float* Wf, const float* bf, int ng,
+int launch_heads_out(const float* hf, const float* ho, int C, int M, int HW, int clips, const float* Wf, const float* bf, int ng,
                      const float* Wo, const float* bo, int nc, float* out, cudaStream_t st) {
-  heads_out_kernel<<<(M + 127) / 128, 128, 0, st>>>(hf, ho, C, M, Wf, bf, ng, Wo, bo, nc, out);
+  heads_out_kernel<<<(M + 127) / 128, 128, 0, st>>>(hf, ho, C, M, HW, clips, Wf, bf, ng, Wo, bo, nc, out);
   DAWN_LAUNCH_OK();
   return 0;
 }

@@ -9,8 +9,9 @@ namespace dawn {
 int launch_rowstats(const float* x, int ld, int C, int M, float eps, float* out_mu_rstd, cudaStream_t st);
 
 // Out = SiLU(FiLM(GroupNorm(Y))) (+ Res).  U:235-248, 478-479
-int launch_gn_apply(const float* Y, int ldy, int C, int M, const double* stats, double count, int cpg,
-                    const float* gw, const float* gb, const float* film /*[2C] or null*/,
+// Per clip (row r is in frame r / P, clip (r / P) % clips): stats [clips][16], film [clips][2C].
+int launch_gn_apply(const float* Y, int ldy, int C, int M, const double* stats, double count, int cpg, int P, int clips,
+                    const float* gw, const float* gb, const float* film /*[clips][2C] or null*/,
                     const float* Res, int ldr, float* Out, int ldo, cudaStream_t st);
 
 // ---------------------------------------------------------------- conditioning tables (clip invariants)
@@ -35,17 +36,19 @@ struct CondDesc {
   float* ctx; float* kv;                              // scratch [F][n1], [F][128]
   CaTableArgs t;
 };
+// F table frames of `clips` clips: table frame f * clips + b is built from cond row b * (F / clips) + f
 int launch_cond_batched(const float* cond, int cond_ld, const CondDesc* descs_dev, int ndesc, int max_n1, int max_k, int max_co, int F,
-                        cudaStream_t st);
+                        int clips, cudaStream_t st);
 
 // Wt[m][ca*9 + {0, 1+h}] = rstd_ca(m) * {1, gate(m,ca,h)}           U:511-514 (to_out LayerNorm) via Gram form
 int launch_ca_rstd(const float* gates, const float* G, int M, int P, float* Wt /*[M][32]*/, cudaStream_t st);
 
 // ---------------------------------------------------------------- time embedding  U:150-162, 788-794, 366-369
-struct FilmDesc { const float* W; const float* b; float* out; int n; };   // out[n] = W[n][256] silu(t256) + b
-int launch_time_mlp(const int64_t* t_dev, const float* freqs /*[dim/2]*/, int dim, const float* W1, const float* b1,
-                    const float* W2, const float* b2, float* t_silu /*[4*dim]*/, cudaStream_t st);
-int launch_film(const FilmDesc* descs_dev, int ndesc, const float* t_silu, int tdim, cudaStream_t st);
+// one timestep per clip: clip b uses t_dev[b * t_stride] (t_stride 0: one shared timestep) and writes t_silu[b], out[b]
+struct FilmDesc { const float* W; const float* b; float* out; int n; };   // out[clip][n] = W[n][256] silu(t256[clip]) + b
+int launch_time_mlp(const int64_t* t_dev, int t_stride, int clips, const float* freqs /*[dim/2]*/, int dim, const float* W1, const float* b1,
+                    const float* W2, const float* b2, float* t_silu /*[clips][4*dim]*/, cudaStream_t st);
+int launch_film(const FilmDesc* descs_dev, int ndesc, int clips, const float* t_silu, int tdim, cudaStream_t st);
 
 // rotary cos/sin table [F][16][2] from freqs[16], position = pos0 + f
 int launch_rotary_table(const float* freqs, int F, int pos0, float* out, cudaStream_t st);
@@ -80,22 +83,25 @@ int launch_sla_context(const float* qkv, int ld, int F, int P, const float* Wout
                        float* Bf, int ldb, cudaStream_t st);
 
 // ---------------------------------------------------------------- layout / heads / init conv
-// x (C, F, H*W) channel-major -> (F, H*W, Cpad) channels-last, zero padding channels [C, Cpad)
-// skip_flag (device int, optional): the kernel returns at once when *skip_flag == skip_if (device-side path selection)
+// x (clips, C, F, H*W) channel-major -> (F * clips, H*W, Cpad) channels-last (frame f of clip b at f * clips + b), zero padding
+// channels [C, Cpad).  skip_flag (device int, optional): the kernel returns at once when *skip_flag == skip_if (device-side path
+// selection)
 int launch_ncf_to_nhwc(const float* x, int C, int F, int HW, int Cpad, int c_dst0, float* out, cudaStream_t st,
-                       const int* skip_flag = nullptr, int skip_if = 0);
-// *flag = 1 iff channels [c0, C) of x (C, F, HW) are not identical in every frame
-int launch_frame_invariance(const float* x, int c0, int C, int F, int HW, int* flag, cudaStream_t st);
-// k vertically shifted channels-last copies of one (C, H, W) frame and the reduction of the k partial maps (per-clip init-conv map)
-int launch_fea_shift_nhwc(const float* x, long long cstride, int C, int H, int W, int Cpad, int c_dst0, int k, float* out, cudaStream_t st,
-                          const int* skip_flag = nullptr, int skip_if = 0);
+                       const int* skip_flag = nullptr, int skip_if = 0, int clips = 1);
+// x (clips, C, F, HW): flag[b] = 1 iff channels [c0, C) of clip b are not identical in every frame; flag[clips] = number of such clips
+int launch_frame_invariance(const float* x, int c0, int C, int F, int HW, int clips, int* flag, cudaStream_t st);
+// k vertically shifted channels-last copies of one (C, H, W) frame per clip (clip b's frame at x + b * clip_stride; copy s of clip b
+// is output frame s * clips + b) and the reduction of the k partial maps (per-clip init-conv maps)
+int launch_fea_shift_nhwc(const float* x, long long cstride, long long clip_stride, int clips, int C, int H, int W, int Cpad, int c_dst0,
+                          int k, float* out, cudaStream_t st, const int* skip_flag = nullptr, int skip_if = 0);
 int launch_map_reduce(const float* part, int nsplit, long long n, const float* bias, int Co, float* map, cudaStream_t st,
                       const int* skip_flag = nullptr, int skip_if = 0);
-// out[f][p][co0..] = map[p][:] + conv7x7(x_t[3][F][H][W]; w3[49*3][64])   (hoisted init conv, SURVEY a2)
-int launch_init_conv_x3(const float* xt, int F, int H, int W, const float* w3, const float* map, int Co,
+// out[f*clips+b][p][co0..] = map[b][p][:] + conv7x7(x_t[b][3][F][H][W]; w3[49*3][64])   (hoisted init conv, SURVEY a2), clip b's
+// channels 0..2 at xt + b * clip_stride; skip_flag (optional) per clip: clip b is skipped when skip_flag[b] == skip_if
+int launch_init_conv_x3(const float* xt, long long clip_stride, int F, int H, int W, int clips, const float* w3, const float* map, int Co,
                         float* out, int ldo, int ksz, cudaStream_t st, const int* skip_flag = nullptr, int skip_if = 0);
-// eps[c][f][p] = head 1x1 convs: c<ng from flow features, else occlusion features   U:863, 876, 956
-int launch_heads_out(const float* hf, const float* ho, int C, int M, const float* Wf, const float* bf, int ng,
-                     const float* Wo, const float* bo, int nc, float* out /*[(ng+nc)][M]*/, cudaStream_t st);
+// eps[b][c][f][p] = head 1x1 convs of row (f*clips+b)*HW + p: c<ng from flow features, else occlusion features   U:863, 876, 956
+int launch_heads_out(const float* hf, const float* ho, int C, int M, int HW, int clips, const float* Wf, const float* bf, int ng,
+                     const float* Wo, const float* bo, int nc, float* out /*[clips][(ng+nc)][M/clips]*/, cudaStream_t st);
 
 }  // namespace dawn

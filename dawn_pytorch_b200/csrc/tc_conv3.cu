@@ -109,11 +109,15 @@ __global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const G
   const int NCH = p.Cin / 64;                                  // 64-channel chunks
   const int tiles_sp = tiles_y * tiles_x;
   const int total_tiles = F * tiles_sp * tiles_n;              // n fastest: CTAs of one patch share its activations in L2
+  // Tiles are visited clip by clip (image f * clips + b is the (f, b) frame): a CTA's consecutive tiles then stay in one clip, so the
+  // deferred GroupNorm partial sums below are flushed every 8 tiles and not at every change of clip.
+  const int fpc = F / p.clips;                                 // frames per clip
   auto decode = [&](int tile, int& f, int& y0, int& x0, int& nt) {
     nt = tile % tiles_n;
     const int sp = tile / tiles_n;
-    f = sp / tiles_sp;
-    const int r = sp - f * tiles_sp;
+    const int seq = sp / tiles_sp;                             // clip-major image sequence number
+    const int r = sp - seq * tiles_sp;
+    f = p.clips == 1 ? seq : (seq % fpc) * p.clips + seq / fpc;
     y0 = (r / tiles_x) * TH; x0 = (r % tiles_x) * TW;
   };
 
@@ -291,8 +295,11 @@ __global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const G
       asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
     }
   };
-  auto flush_stats = [&](float (&gs)[8], float (&gss)[8]) {
+  // A tile covers one frame, so one clip (frame % clips): the running sums belong to the clip of the tiles they hold and are flushed
+  // before a tile of another clip is added.
+  auto flush_stats = [&](float (&gs)[8], float (&gss)[8], int clip) {
     const int n0f = wg * 64;                                      // tiles_n == 1: this thread's columns never change
+    double* cs = p.stats + 16 * clip;
 #pragma unroll
     for (int b8 = 0; b8 < 8; ++b8) {
       double s = (double)gs[b8], ss = (double)gss[b8];
@@ -300,16 +307,17 @@ __global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const G
       for (int o = 16; o > 0; o >>= 1) { s += __shfl_xor_sync(0xffffffffu, s, o); ss += __shfl_xor_sync(0xffffffffu, ss, o); }
       if (lane == 0) {
         const int grp = (n0f + b8 * 8) / p.cpg;
-        atomicAdd(&p.stats[2 * grp], s);
-        atomicAdd(&p.stats[2 * grp + 1], ss);
+        atomicAdd(&cs[2 * grp], s);
+        atomicAdd(&cs[2 * grp + 1], ss);
       }
       gs[b8] = 0.f; gss[b8] = 0.f;
     }
   };
   // epilogue of one tile: thread etid owns tile row etid; its warp's 32 staged rows serve as the store buffer once read back
-  auto epilogue_tile = [&](int tile, float* stage, float (&gs)[8], float (&gss)[8], int& pending) {
+  auto epilogue_tile = [&](int tile, float* stage, float (&gs)[8], float (&gss)[8], int& pending, int& pclip) {
     int f, y0, x0, nt;
     decode(tile, f, y0, x0, nt);
+    const int clip = p.clips > 1 ? f % p.clips : 0;
     const int n0 = nt * BN + wg * 64;
     const int row_in_tile = etid;
     float* s_st = s_stat[wg];
@@ -353,6 +361,8 @@ __global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const G
     }
     store_rows_coalesced(wbuf, acc, p.Out, opix, p.ldo, ocol, rv, lane);
     if (defer_stats) {
+      if (pending > 0 && clip != pclip) { flush_stats(gs, gss, pclip); pending = 0; }
+      pclip = clip;
       if (rv) {
 #pragma unroll
         for (int b8 = 0; b8 < 8; ++b8) {
@@ -362,7 +372,7 @@ __global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const G
           gs[b8] += s; gss[b8] += ss;
         }
       }
-      if (++pending == 8) { flush_stats(gs, gss); pending = 0; }
+      if (++pending == 8) { flush_stats(gs, gss, clip); pending = 0; }
     } else if (p.stats != nullptr) {
       if (etid < 16) s_st[etid] = 0.f;
       asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
@@ -384,7 +394,7 @@ __global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const G
       if (etid < 16) {
         const int grp = etid >> 1;
         const int glo = n0 / p.cpg, ghi = (n0 + 63) / p.cpg;
-        if (grp >= glo && grp <= ghi) atomicAdd(&p.stats[etid], (double)s_st[etid]);
+        if (grp >= glo && grp <= ghi) atomicAdd(&p.stats[16 * clip + etid], (double)s_st[etid]);
       }
     }
   };
@@ -399,7 +409,7 @@ __global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const G
     // =============================================================== epilogue warpgroup: tile t from staging tile t & 1
     setmaxnreg_inc<C::REG_EPI>();
     float gs[8], gss[8];
-    int pending = 0;
+    int pending = 0, pclip = 0;
 #pragma unroll
     for (int i = 0; i < 8; ++i) { gs[i] = 0.f; gss[i] = 0.f; }
     load_bias();
@@ -407,10 +417,10 @@ __global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const G
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++lt) {
       const int b = lt & 1;
       mbar_wait(&st_full[b], (lt >> 1) & 1);
-      epilogue_tile(tile, stage_base + b * 128 * kStageLd, gs, gss, pending);
+      epilogue_tile(tile, stage_base + b * 128 * kStageLd, gs, gss, pending, pclip);
       mbar_arrive(&st_free[b]);                                // after the last read and the last store-buffer use of the tile
     }
-    if (defer_stats && pending > 0) flush_stats(gs, gss);
+    if (defer_stats && pending > 0) flush_stats(gs, gss, pclip);
   } else if (SPLIT) {
     // =============================================================== MMA warpgroup: drains tile t into staging tile t & 1, hands it
     // to the epilogue warpgroup and goes on with tile t+1
@@ -428,7 +438,7 @@ __global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const G
     // of its 64 columns
     setmaxnreg_inc<C::REG_MMA>();
     float gs[8], gss[8];
-    int pending = 0;
+    int pending = 0, pclip = 0;
 #pragma unroll
     for (int i = 0; i < 8; ++i) { gs[i] = 0.f; gss[i] = 0.f; }
     load_bias();
@@ -437,10 +447,10 @@ __global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const G
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       with_drain([&](auto DTc) { mma_tile(DTc, stage, ait, bit, []() {}); });
       asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
-      epilogue_tile(tile, stage, gs, gss, pending);
+      epilogue_tile(tile, stage, gs, gss, pending, pclip);
       asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");   // the staged tile is rewritten by the next tile's first drain
     }
-    if (defer_stats && pending > 0) flush_stats(gs, gss);
+    if (defer_stats && pending > 0) flush_stats(gs, gss, pclip);
   }
 }
 

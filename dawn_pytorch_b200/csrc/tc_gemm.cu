@@ -411,8 +411,34 @@ __global__ void __launch_bounds__(Cfg<BN>::NTHREADS, 1) tc_gemm_kernel(const Gem
           }
         }
         store_rows_coalesced(wbuf, acc, p.Out, opix, p.ldo, n0, rv, lane);
-        if (p.stats != nullptr) {
+        if (p.stats != nullptr && p.clips > 1 && m0 / Ps != (min(m0 + BM, p.M) - 1) / Ps) {
+          // the tile's rows belong to several clips (small levels of a batched pass): the warp reduces its 32 rows once per clip
+          // present among them and adds each clip's sums to that clip's slot
+          const int clip = f % p.clips;
+          unsigned rest = 0xffffffffu;
+          while (rest) {
+            const int c = __shfl_sync(0xffffffffu, clip, __ffs(rest) - 1);
+            rest &= ~__ballot_sync(0xffffffffu, clip == c);
+            const bool mine = rv && clip == c;
+            double* cs = p.stats + 16 * c;
+#pragma unroll
+            for (int b8 = 0; b8 < EN / 8; ++b8) {
+              float s = 0.f, ss = 0.f;
+              if (mine) {
+#pragma unroll
+                for (int i = 0; i < 8; ++i) { const float x = acc[b8 * 8 + i]; s += x; ss += x * x; }
+              }
+              s = warp_sum(s); ss = warp_sum(ss);
+              if (lane == 0) {
+                const int grp = (n0 + b8 * 8) / p.cpg;
+                atomicAdd(&cs[2 * grp], (double)s);
+                atomicAdd(&cs[2 * grp + 1], (double)ss);
+              }
+            }
+          }
+        } else if (p.stats != nullptr) {
           // GroupNorm partial statistics (U:230): per 8-column sub-block, reduced over the warp's 32 rows
+          double* cs = p.clips > 1 ? p.stats + 16 * ((m0 / Ps) % p.clips) : p.stats;
           if (etid < 16) s_st[etid] = 0.f;
           asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
 #pragma unroll
@@ -433,7 +459,7 @@ __global__ void __launch_bounds__(Cfg<BN>::NTHREADS, 1) tc_gemm_kernel(const Gem
           if (etid < 16) {
             const int grp = etid >> 1;
             const int glo = n0 / p.cpg, ghi = (n0 + EN - 1) / p.cpg;
-            if (grp >= glo && grp <= ghi) atomicAdd(&p.stats[etid], (double)s_st[etid]);
+            if (grp >= glo && grp <= ghi) atomicAdd(&cs[etid], (double)s_st[etid]);
           }
         }
       } else {

@@ -1,6 +1,7 @@
 // Host-side orchestration + C-ABI of the DAWN denoising UNet (reference U:728-965; see include/dawn_unet.h).
-// One handle = one GPU = one clip at a time.  Weights are repacked once into GEMM-friendly layouts;
-// activations live channels-last (F, H, W, C) in a workspace sized by dawn_unet_set_num_frames.
+// One handle = one GPU = a batch of B clips of F frames (dawn_unet_set_geometry).  Weights are repacked once into GEMM-friendly
+// layouts; activations live channels-last (F, B, H, W, C): frame f of clip b is frame f * B + b, so every per-frame operation
+// sees F * B images and every temporal operation B * H * W pixel sequences of length F.
 #include <dlfcn.h>
 #include <algorithm>
 #include <cmath>
@@ -182,11 +183,12 @@ struct dawn_unet {
   FilmDesc* film_descs = nullptr; int n_film = 0;
   CondDesc* cond_descs = nullptr; int n_cond = 0, cond_max_n1 = 0, cond_max_k = 0, cond_max_co = 0;   // batched per-clip prep
 
-  // workspace (per set_num_frames)
-  int F = 0, H = 0, W = 0;
+  // workspace (per set_geometry): B clips of F frames each
+  int B = 1, F = 0, H = 0, W = 0;
   std::vector<int> lH, lW;
   float* MAPPART = nullptr;                    // k partial maps of the per-clip init conv (one per kernel row)
-  int* VARY = nullptr;                         // device flag of the general entry: 1 = feature channels differ between frames
+  int* VARY = nullptr;                         // device flags of the general entry: [b] = 1 if clip b's feature channels differ
+                                               // between frames, [B] = number of such clips
   float *X288 = nullptr, *FEA288 = nullptr, *MAP = nullptr, *XR = nullptr, *S0 = nullptr;
   std::vector<float*> bufA, bufB, CAT, DS;
   float *Y = nullptr, *A1 = nullptr, *QKV = nullptr, *O = nullptr, *ROWSTATS = nullptr, *GATES = nullptr, *WT = nullptr;
@@ -440,7 +442,7 @@ int Ctx::gemm(const GemmParams& p, int epi, int cat) {
   if (epi == EPI_CA_GATE) bytes = 4.0 * p.M * (p.Cin + 24.0);
   ProfScope ps(*this, cat, flops, bytes);
   // the attention output buffer O doubles as the scratch of the pre-split planes
-  const size_t scratch = (size_t)(h->F + 2 * h->cfg.win_width) * h->lH[0] * h->lW[0] * 256 * sizeof(float);
+  const size_t scratch = (size_t)(h->F * h->B + 2 * h->cfg.win_width) * h->lH[0] * h->lW[0] * 256 * sizeof(float);
   int kernels = 0;
   const int rc = launch_path(p, epi, choose_path(p, epi, scratch), h->O, st, &kernels);
   h->launches += kernels - 1;                     // ProfScope counted one
@@ -470,12 +472,15 @@ int ln_gemm(Ctx& c, GemmParams& p, int epi, int cat, const float* x, int ldx, in
   return c.gemm(p, epi, cat);
 }
 
+// GroupNorm statistic slot: 16 doubles (8 groups x {sum, sum of squares}) per clip
+double* stats_slot(dawn_unet* h, int slot) { return h->STATS + (size_t)16 * h->B * slot; }
+
 // conv k x k, stride 1, same padding, + bias, optional GroupNorm statistics slot
 GemmParams conv_same_params(Ctx& c, const Act& in, const PackedWeight& w, int k, const Act& out, int stat_slot) {
-  GemmParams p; base_params(p, in, c.h->F);
+  GemmParams p; base_params(p, in, c.h->F * c.h->B);
   set_weights(p, w); set_square_taps(p, k, k / 2);
   p.Out = out.p; p.ldo = out.ld;
-  if (stat_slot >= 0) { p.stats = c.h->STATS + 16 * stat_slot; p.cpg = w.N / 8; }
+  if (stat_slot >= 0) { p.stats = stats_slot(c.h, stat_slot); p.cpg = w.N / 8; p.clips = c.h->B; }
   return p;
 }
 int conv_same(Ctx& c, const GemmParams& p) {
@@ -487,7 +492,7 @@ int conv_same(Ctx& c, const GemmParams& p) {
 int gn_allreduce(Ctx& c, int slot) {
   dawn_unet* h = c.h;
   if (h->sh_nranks <= 1) return 0;
-  double* st = h->STATS + 16 * slot;
+  double* st = stats_slot(h, slot);
   ProfScope ps(c, PC_COMM_AR, 0, 128.0 * h->sh_nranks);
   if (h->p2p_ready) {
     P2pPeers pp;
@@ -503,7 +508,7 @@ int gn_allreduce(Ctx& c, int slot) {
 // ResnetBlock_ca_mul (U:363-479)
 int resblock(Ctx& c, const ResBlockW& r, const Act& x, const Act& out) {
   dawn_unet* h = c.h;
-  const int F = h->F, M = F * x.H * x.W, P = x.H * x.W;
+  const int F = h->F * h->B, M = F * x.H * x.W, P = x.H * x.W;      // F: frames of all clips
   DAWN_CHECK(x.C == r.ci && out.C == r.co, "resblock channel mismatch: " + r.name);
   Act y{h->Y, r.co, r.co, x.H, x.W}, a1{h->A1, r.co, r.co, x.H, x.W};
   const double count = (double)h->sh_Fglobal * P * (r.co / 8);     // GroupNorm statistics span the WHOLE clip (U:230)
@@ -535,8 +540,8 @@ int resblock(Ctx& c, const ResBlockW& r, const Act& x, const Act& out) {
     GnHcondArgs a{};
     a.Wt = h->WT; a.T = r.T; a.ldbT = r.ldbT; a.Y = y.p; a.ldy = y.ld; a.Out = a1.p; a.ldo = a1.ld;
     a.Out16h = const_cast<unsigned short*>(conv2.A16h); a.Out16l = const_cast<unsigned short*>(conv2.A16l);
-    a.F = F; a.P = P; a.co = r.co;
-    a.gn_stats = h->STATS + 16 * r.st1; a.gn_count = count; a.cpg = r.co / 8;
+    a.F = F; a.P = P; a.co = r.co; a.clips = h->B;
+    a.gn_stats = stats_slot(h, r.st1); a.gn_count = count; a.cpg = r.co / 8;
     a.gn_w = r.gn1w; a.gn_b = r.gn1b; a.film = r.film;
     ProfScope ps(c, PC_GN_HCOND, 2.0 * M * 32 * r.co, 4.0 * M * (2.0 * r.co + 32));
     DAWN_TRY(launch_gn_hcond(a, c.st));
@@ -547,12 +552,12 @@ int resblock(Ctx& c, const ResBlockW& r, const Act& x, const Act& out) {
     p.B = r.T; p.ldb = r.ldbT; p.b_batch_stride = (long long)32 * r.ldbT; p.N = r.co; p.K = 32;
     p.rows_per_batch = P;
     p.Out = a1.p; p.ldo = a1.ld;
-    p.Y = y.p; p.ldy = y.ld; p.gn_stats = h->STATS + 16 * r.st1; p.gn_w = r.gn1w; p.gn_b = r.gn1b;
-    p.film = r.film; p.gn_count = count; p.cpg = r.co / 8;
+    p.Y = y.p; p.ldy = y.ld; p.gn_stats = stats_slot(h, r.st1); p.gn_w = r.gn1w; p.gn_b = r.gn1b;
+    p.film = r.film; p.gn_count = count; p.cpg = r.co / 8; p.clips = h->B;
     DAWN_TRY(c.gemm(p, EPI_GN_APPLY, PC_GN_HCOND));
   } else {
     ProfScope ps(c, PC_GN_APPLY, 0, 8.0 * M * r.co);
-    DAWN_TRY(launch_gn_apply(y.p, y.ld, r.co, M, h->STATS + 16 * r.st1, count, r.co / 8, r.gn1w, r.gn1b, nullptr,
+    DAWN_TRY(launch_gn_apply(y.p, y.ld, r.co, M, stats_slot(h, r.st1), count, r.co / 8, P, h->B, r.gn1w, r.gn1b, nullptr,
                              nullptr, 0, a1.p, a1.ld, c.st));
   }
   DAWN_TRY(conv_same(c, conv2));
@@ -564,7 +569,7 @@ int resblock(Ctx& c, const ResBlockW& r, const Act& x, const Act& out) {
   }
   {
   ProfScope ps(c, PC_GN_APPLY, 0, 12.0 * M * r.co);
-  DAWN_TRY(launch_gn_apply(y.p, y.ld, r.co, M, h->STATS + 16 * r.st2, count, r.co / 8, r.gn2w, r.gn2b, nullptr,
+  DAWN_TRY(launch_gn_apply(y.p, y.ld, r.co, M, stats_slot(h, r.st2), count, r.co / 8, P, h->B, r.gn2w, r.gn2b, nullptr,
                            res, ldr, out.p, out.ld, c.st));
   }
   return tap(c, r.name, out);
@@ -579,7 +584,7 @@ inline int seq_block(int P) { for (int b = 16; b > 1; --b) if (P % b == 0) retur
 // TLB/latency-bound; the QKV GEMM gathers its A rows through the permutation and the out-projection scatters back.
 int temporal_attn(Ctx& c, const AttnW& w, const Act& x, const Act& dst, const std::string& name) {
   dawn_unet* h = c.h;
-  const int F = h->F, P = x.H * x.W;
+  const int F = h->F, P = h->B * x.H * x.W;                                // B * H * W pixel sequences of F frames
   const int pb = seq_block(P);
   const int hl = h->sh_halo_l, hr = h->sh_halo_r, Fe = hl + F + hr;       // frames incl. neighbours' halos
   const int Me = Fe * P;
@@ -619,8 +624,9 @@ int temporal_attn(Ctx& c, const AttnW& w, const Act& x, const Act& dst, const st
     return tap(c, name, dst);
   }
   {
-    GemmParams p; base_params(p, xe, Fe);
+    GemmParams p; base_params(p, xe, Fe * h->B);
     set_weights(p, w.qkv);
+    p.P = P;
     p.wsum = w.wsum; p.rot = h->ROT;
     p.Out = h->QKV; p.ldo = 768;
     p.perm_pb = pb; p.perm_F = Fe; p.perm_in = 1; p.perm_out = 0;
@@ -654,7 +660,7 @@ int temporal_attn(Ctx& c, const AttnW& w, const Act& x, const Act& dst, const st
 // Residual(PreNorm(Attention over the h*w tokens of each frame)) (U:841-843), in place
 int mid_spatial_attn(Ctx& c, const AttnW& w, const Act& x, const std::string& name) {
   dawn_unet* h = c.h;
-  const int F = h->F, P = x.H * x.W, M = F * P;
+  const int F = h->F * h->B, P = x.H * x.W, M = F * P;
   {
     GemmParams p; base_params(p, x, F);
     set_weights(p, w.qkv);
@@ -684,7 +690,7 @@ int mid_spatial_attn(Ctx& c, const AttnW& w, const Act& x, const std::string& na
 // Residual(PreNorm(SpatialLinearAttention)) (U:602-627), in place
 int sla(Ctx& c, const SlaW& w, const Act& x, const std::string& name) {
   dawn_unet* h = c.h;
-  const int F = h->F, P = x.H * x.W, M = F * P;
+  const int F = h->F * h->B, P = x.H * x.W, M = F * P;
   const int ldb = round_up(x.C, 64);
   const bool fused = w.fkv && sla_fused_supported(x.C, P) &&
                      sla_fused_part_floats(F, P) <= (size_t)(F + 2 * h->cfg.win_width) * h->lH[0] * h->lW[0] * 256;
@@ -727,11 +733,11 @@ int sla(Ctx& c, const SlaW& w, const Act& x, const std::string& name) {
 }
 
 int downsample(Ctx& c, const PackedWeight& w, const Act& x, const Act& out, const std::string& name) {   // U:175-176
-  GemmParams p; base_params(p, x, c.h->F);
+  GemmParams p; base_params(p, x, c.h->F * c.h->B);
   set_weights(p, w);
   p.OHs = out.H; p.OWs = out.W; p.in_stride = 2;
   set_square_taps(p, 4, 1);
-  p.M = c.h->F * out.H * out.W; p.rows_per_batch = p.M;
+  p.M = c.h->F * c.h->B * out.H * out.W; p.rows_per_batch = p.M;
   p.OH = out.H; p.OW = out.W; p.P = out.H * out.W;
   p.Out = out.p; p.ldo = out.ld;
   DAWN_TRY(c.gemm(p, EPI_PLAIN, PC_CONV_OTHER));
@@ -739,7 +745,7 @@ int downsample(Ctx& c, const PackedWeight& w, const Act& x, const Act& out, cons
 }
 
 int upsample(Ctx& c, const UpConv& u, const Act& x, const Act& out, const std::string& name) {   // U:165-167
-  GemmParams p; base_params(p, x, c.h->F);
+  GemmParams p; base_params(p, x, c.h->F * c.h->B);
   DAWN_TRY(run_up(p, u, out.p, out.ld, [&](const GemmParams& q) { return c.gemm(q, EPI_PLAIN, PC_CONV_OTHER); }));
   return tap(c, name, out);
 }
@@ -767,27 +773,31 @@ int prep_cond(dawn_unet* h, const float* cond, cudaStream_t st) {
   Ctx c{h, st};
   ProfScope ps(c, PC_PREP, 0, 0);
   h->launches += 2;
-  return launch_cond_batched(cond, h->cond_dim, h->cond_descs, h->n_cond, h->cond_max_n1, h->cond_max_k, h->cond_max_co, h->F, st);
+  return launch_cond_batched(cond, h->cond_dim, h->cond_descs, h->n_cond, h->cond_max_n1, h->cond_max_k, h->cond_max_co, h->F * h->B,
+                             h->B, st);
 }
 
 // Per-clip constant part of the init conv (SURVEY a2) from ONE frame of the feature channels (fea: channel c at
-// fea + c * cstride, H0*W0 values): kernel row ky runs as a 1 x k conv over the frame shifted by ky - pad rows ("batch" ky of
-// the contraction kernel, weight rows [ky*k*cin_pad, (ky+1)*k*cin_pad) of the packed matrix) -> k x 32 CTAs instead of 32;
-// the k partial maps are then added in a fixed order.  skip_flag: device-side path selection of the general entry.
-int init_map(dawn_unet* h, const float* fea, long long cstride, cudaStream_t st, const int* skip_flag, int skip_if) {
+// fea + c * cstride, H0*W0 values; clip b's frame at fea + b * clip_stride): kernel row ky runs as a 1 x k conv over the frame
+// shifted by ky - pad rows ("batch" ky of the contraction kernel: the B clips' copies ky, weight rows [ky*k*cin_pad,
+// (ky+1)*k*cin_pad) of the packed matrix) -> k x 32 CTAs per clip instead of 32; the k partial maps are then added in a fixed
+// order.  skip_flag: device-side path selection of the general entry.
+int init_map(dawn_unet* h, const float* fea, long long cstride, long long clip_stride, cudaStream_t st, const int* skip_flag,
+             int skip_if) {
   Ctx c{h, st};
   const int H0 = h->lH[0], W0 = h->lW[0], dim = h->cfg.dim, k = h->cfg.init_kernel_size;
   {
     ProfScope ps(c, PC_PREP, 0, 0);
-    DAWN_TRY(launch_fea_shift_nhwc(fea, cstride, h->cfg.channels - 3, H0, W0, h->cin_pad, 3, k, h->FEA288, st, skip_flag, skip_if));
+    DAWN_TRY(launch_fea_shift_nhwc(fea, cstride, clip_stride, h->B, h->cfg.channels - 3, H0, W0, h->cin_pad, 3, k, h->FEA288, st,
+                                   skip_flag, skip_if));
   }
   {
     Act in{h->FEA288, h->cin_pad, h->cin_pad, H0, W0};
-    GemmParams p; base_params(p, in, k);                       // k "frames" = the shifted copies
+    GemmParams p; base_params(p, in, k * h->B);                // k x B "frames" = the shifted copies
     set_weights(p, h->init_full);
     p.ntaps = k;
     for (int kx = 0; kx < k; ++kx) { p.dy[kx] = 0; p.dx[kx] = (signed char)(kx - k / 2); }
-    p.K = k * h->cin_pad; p.rows_per_batch = H0 * W0; p.b_batch_stride = (long long)k * h->cin_pad * h->init_full.ldb;
+    p.K = k * h->cin_pad; p.rows_per_batch = h->B * H0 * W0; p.b_batch_stride = (long long)k * h->cin_pad * h->init_full.ldb;
     p.bias = nullptr;
     p.Out = h->MAPPART; p.ldo = dim;
     p.skip_flag = skip_flag; p.skip_if = skip_if;
@@ -795,18 +805,19 @@ int init_map(dawn_unet* h, const float* fea, long long cstride, cudaStream_t st,
     DAWN_TRY(launch_path(p, EPI_PLAIN, DAWN_PATH_MMA_SYNC, nullptr, st));      // per-batch B and the skip flag: mma.sync only
   }
   ProfScope ps(c, PC_PREP, 0, 0);
-  return launch_map_reduce(h->MAPPART, k, (long long)H0 * W0 * dim, h->init_full.b, dim, h->MAP, st, skip_flag, skip_if);
+  return launch_map_reduce(h->MAPPART, k, (long long)h->B * H0 * W0 * dim, h->init_full.b, dim, h->MAP, st, skip_flag, skip_if);
 }
 
-int forward_core(dawn_unet* h, const int64_t* t_dev, float* out, cudaStream_t st) {
+// t_dev: clip b's timestep at t_dev[b * t_stride] (t_stride 0: every clip at the same timestep)
+int forward_core(dawn_unet* h, const int64_t* t_dev, int t_stride, float* out, cudaStream_t st) {
   Ctx c{h, st};
-  const int F = h->F, nlev = h->nlev, dim = h->cfg.dim;
-  DAWN_CUDA_OK(cudaMemsetAsync(h->STATS, 0, sizeof(double) * 16 * h->n_stats, st));
+  const int F = h->F * h->B, nlev = h->nlev, dim = h->cfg.dim;
+  DAWN_CUDA_OK(cudaMemsetAsync(h->STATS, 0, sizeof(double) * 16 * h->B * h->n_stats, st));
   {
     ProfScope ps(c, PC_MISC, 0, 0);
     h->launches += 1;
-    DAWN_TRY(launch_time_mlp(t_dev, h->time_freqs, dim, h->tW1, h->tb1, h->tW2, h->tb2, h->TSILU, st));
-    DAWN_TRY(launch_film(h->film_descs, h->n_film, h->TSILU, h->tdim, st));
+    DAWN_TRY(launch_time_mlp(t_dev, t_stride, h->B, h->time_freqs, dim, h->tW1, h->tb1, h->tW2, h->tb2, h->TSILU, st));
+    DAWN_TRY(launch_film(h->film_descs, h->n_film, h->B, h->TSILU, h->tdim, st));
   }
 
   const int H0 = h->lH[0], W0 = h->lW[0];
@@ -866,7 +877,7 @@ int forward_core(dawn_unet* h, const int64_t* t_dev, float* out, cudaStream_t st
   DAWN_TRY(resblock(c, h->rb[h->rb_index["final_conv.0"]], xr, hf));
   DAWN_TRY(resblock(c, h->rb[h->rb_index["occlusion_map.0"]], xr, ho));
   ProfScope ps(c, PC_MISC, 0, 4.0 * F * H0 * W0 * (2 * dim + 3));
-  DAWN_TRY(launch_heads_out(h->HF, h->HO, dim, F * H0 * W0, h->headW[0], h->headB[0], h->cfg.out_grid_dim,
+  DAWN_TRY(launch_heads_out(h->HF, h->HO, dim, F * H0 * W0, H0 * W0, h->B, h->headW[0], h->headB[0], h->cfg.out_grid_dim,
                             h->headW[1], h->headB[1], h->cfg.out_conf_dim, out, st));
   return 0;
 }
@@ -1019,15 +1030,21 @@ int dawn_unet_commit_params(dawn_unet* h) {
   h->committed = true;
   // a changed parameter set invalidates per-clip tables
   h->have_invariants = false;
-  if (h->F > 0) return dawn_unet_set_num_frames(h, h->F, h->H, h->W);
+  if (h->F > 0) return dawn_unet_set_geometry(h, h->B, h->F, h->H, h->W);
   return 0;
 }
 
-int dawn_unet_set_num_frames(dawn_unet* h, int F, int height, int width) {
+int dawn_unet_set_num_frames(dawn_unet* h, int F, int height, int width) { return dawn_unet_set_geometry(h, 1, F, height, width); }
+
+int dawn_unet_set_geometry(dawn_unet* h, int B, int F, int height, int width) {
   DAWN_CHECK(h, "null handle");
   drop_graphs(h);
-  DAWN_CHECK(h->committed, "commit_params must precede set_num_frames");
+  DAWN_CHECK(h->committed, "commit_params must precede set_geometry");
   DAWN_CHECK(F >= 1 && F <= 65535, "F out of range");
+  DAWN_CHECK(B >= 1 && B <= kMaxClips, "the clip count B must be in [1, " + std::to_string(kMaxClips) + "]");
+  DAWN_CHECK((int64_t)B * F <= 65535, "B * F out of range");
+  DAWN_CHECK(B == 1 || h->sh_nranks <= 1, "a frame-sharded handle runs one clip at a time (B = 1)");
+  DAWN_CHECK(B == 1 || h->taps.empty(), "debugging taps need B = 1: clear them before setting B > 1");
   const int nlev = h->nlev, dim = h->cfg.dim;
   const int div = 1 << (nlev - 1);
   DAWN_CHECK(height % div == 0 && width % div == 0 && height >= div && width >= div,
@@ -1035,35 +1052,36 @@ int dawn_unet_set_num_frames(dawn_unet* h, int F, int height, int width) {
   free_all(h->ws_owned);
   h->ws_bytes = 0;
   h->have_invariants = false;
-  h->F = F; h->H = height; h->W = width;
+  h->B = B; h->F = F; h->H = height; h->W = width;
   h->lH.assign(nlev, 0); h->lW.assign(nlev, 0);
   for (int l = 0; l < nlev; ++l) { h->lH[l] = height >> l; h->lW[l] = width >> l; }
   auto& own = h->ws_owned;
-  const size_t P0 = (size_t)height * width, M0 = (size_t)F * P0;
+  const int NF = B * F;                                              // frames of all clips
+  const size_t P0 = (size_t)height * width, M0 = (size_t)NF * P0;
   int64_t* cnt = &h->ws_bytes;
   DAWN_TRY(dev_alloc(own, M0 * h->cin_pad, &h->X288, cnt));
-  DAWN_TRY(dev_alloc(own, P0 * h->cin_pad * h->cfg.init_kernel_size, &h->FEA288, cnt));   // k row-shifted copies
-  DAWN_TRY(dev_alloc(own, P0 * dim * h->cfg.init_kernel_size, &h->MAPPART, cnt));
-  { float* f; DAWN_TRY(dev_alloc(own, 4, &f, cnt)); h->VARY = (int*)f; }
-  DAWN_TRY(dev_alloc(own, P0 * dim, &h->MAP, cnt));
+  DAWN_TRY(dev_alloc(own, B * P0 * h->cin_pad * h->cfg.init_kernel_size, &h->FEA288, cnt));   // k row-shifted copies per clip
+  DAWN_TRY(dev_alloc(own, B * P0 * dim * h->cfg.init_kernel_size, &h->MAPPART, cnt));
+  { float* f; DAWN_TRY(dev_alloc(own, B + 4, &f, cnt)); h->VARY = (int*)f; }
+  DAWN_TRY(dev_alloc(own, B * P0 * dim, &h->MAP, cnt));
   DAWN_TRY(dev_alloc(own, M0 * 2 * dim, &h->XR, cnt));
   DAWN_TRY(dev_alloc(own, M0 * dim, &h->S0, cnt));
   h->bufA.assign(nlev, nullptr); h->bufB.assign(nlev, nullptr); h->CAT.assign(nlev, nullptr); h->DS.assign(nlev, nullptr);
   size_t max_mc = 0, max_bf = 0;
   for (int l = 0; l < nlev; ++l) {
-    const size_t Ml = (size_t)F * h->lH[l] * h->lW[l];
+    const size_t Ml = (size_t)NF * h->lH[l] * h->lW[l];
     const int ci = h->in_out[l].first, co = h->in_out[l].second;
     DAWN_TRY(dev_alloc(own, Ml * co, &h->bufA[l], cnt));
     DAWN_TRY(dev_alloc(own, Ml * co, &h->bufB[l], cnt));
     DAWN_TRY(dev_alloc(own, Ml * 2 * co, &h->CAT[l], cnt));
     if (l > 0) DAWN_TRY(dev_alloc(own, Ml * ci, &h->DS[l], cnt));
     max_mc = std::max(max_mc, Ml * co);
-    max_bf = std::max(max_bf, (size_t)F * 256 * round_up(co, 64));
+    max_bf = std::max(max_bf, (size_t)NF * 256 * round_up(co, 64));
   }
   max_mc = std::max(max_mc, M0 * dim);
   DAWN_TRY(dev_alloc(own, max_mc, &h->Y, cnt));
   DAWN_TRY(dev_alloc(own, max_mc, &h->A1, cnt));
-  const size_t Mext = (size_t)(F + 2 * h->cfg.win_width) * P0;      // rows incl. temporal halos of a sharded clip
+  const size_t Mext = (size_t)(NF + 2 * h->cfg.win_width) * P0;     // rows incl. temporal halos of a sharded clip
   DAWN_TRY(dev_alloc(own, Mext * 768, &h->QKV, cnt));
   DAWN_TRY(dev_alloc(own, Mext * 256, &h->O, cnt));
   DAWN_TRY(dev_alloc(own, Mext * 2, &h->ROWSTATS, cnt));
@@ -1074,9 +1092,9 @@ int dawn_unet_set_num_frames(dawn_unet* h, int F, int height, int width) {
   DAWN_TRY(dev_alloc(own, M0 * dim, &h->HF, cnt));
   DAWN_TRY(dev_alloc(own, M0 * dim, &h->HO, cnt));
   DAWN_TRY(dev_alloc(own, (size_t)(F + 2 * h->cfg.win_width) * 32, &h->ROT, cnt));
-  DAWN_TRY(dev_alloc(own, h->tdim, &h->TSILU, cnt));
+  DAWN_TRY(dev_alloc(own, (size_t)B * h->tdim, &h->TSILU, cnt));
   {
-    float* s; DAWN_TRY(dev_alloc(own, (size_t)h->n_stats * 32, &s, cnt)); h->STATS = (double*)s;
+    float* s; DAWN_TRY(dev_alloc(own, (size_t)h->n_stats * 32 * B, &s, cnt)); h->STATS = (double*)s;
     float* t; DAWN_TRY(dev_alloc(own, 4, &t, cnt)); h->T_HOSTSIDE = (int64_t*)t;
   }
   DAWN_TRY(dev_alloc(own, 3 * M0, &h->H_XT, cnt));
@@ -1088,12 +1106,12 @@ int dawn_unet_set_num_frames(dawn_unet* h, int F, int height, int width) {
   for (auto& r : h->rb) {
     if (!r.cond) continue;
     r.ldbT = round_up(r.co, 64);
-    DAWN_TRY(dev_alloc(own, 2 * r.co, &r.film, cnt));
-    DAWN_TRY(dev_alloc(own, (size_t)F * 3 * 64, &r.kq, cnt));
+    DAWN_TRY(dev_alloc(own, (size_t)B * 2 * r.co, &r.film, cnt));
+    DAWN_TRY(dev_alloc(own, (size_t)NF * 3 * 64, &r.kq, cnt));
     DAWN_TRY(dev_alloc(own, 24, &r.nkq, cnt));
-    DAWN_TRY(dev_alloc(own, (size_t)F * 32 * r.ldbT, &r.T, cnt));
-    DAWN_CUDA_OK(cudaMemset(r.T, 0, (size_t)F * 32 * r.ldbT * sizeof(float)));
-    DAWN_TRY(dev_alloc(own, (size_t)F * 3 * 81, &r.G, cnt));
+    DAWN_TRY(dev_alloc(own, (size_t)NF * 32 * r.ldbT, &r.T, cnt));
+    DAWN_CUDA_OK(cudaMemset(r.T, 0, (size_t)NF * 32 * r.ldbT * sizeof(float)));
+    DAWN_TRY(dev_alloc(own, (size_t)NF * 3 * 81, &r.G, cnt));
     descs.push_back(FilmDesc{r.tW, r.tB, r.film, 2 * r.co});
   }
   {
@@ -1112,8 +1130,8 @@ int dawn_unet_set_num_frames(dawn_unet* h, int F, int height, int width) {
       for (int a = 0; a < 3; ++a) {
         CondDesc d{};
         d.mW = r.mW[a]; d.mB = r.mB[a]; d.off = off[a]; d.K = kd[a]; d.n1 = 2 * r.co; d.Wkv = r.ca[a].Wkv;
-        DAWN_TRY(dev_alloc(own, (size_t)F * d.n1, &d.ctx, cnt));
-        DAWN_TRY(dev_alloc(own, (size_t)F * 128, &d.kv, cnt));
+        DAWN_TRY(dev_alloc(own, (size_t)NF * d.n1, &d.ctx, cnt));
+        DAWN_TRY(dev_alloc(own, (size_t)NF * 128, &d.kv, cnt));
         d.t.kv = d.kv; d.t.nkv = r.ca[a].nkv; d.t.qs = r.ca[a].qs; d.t.ks = r.ca[a].ks; d.t.Wout = r.ca[a].Wout; d.t.gout = r.ca[a].gout;
         d.t.co = r.co; d.t.ldbT = r.ldbT; d.t.ca = a; d.t.kq = r.kq; d.t.nkq = r.nkq; d.t.T = r.T; d.t.G = r.G;
         cd.push_back(d);
@@ -1136,7 +1154,8 @@ int dawn_unet_set_clip_invariants(dawn_unet* h, const float* fea, const float* c
   DAWN_CHECK(h->F > 0, "set_num_frames must precede set_clip_invariants");
   cudaStream_t st = (cudaStream_t)stream;
   // per-clip constant part of the init conv: conv(cat[0, fea]) + bias  (linearity; SURVEY a2)
-  DAWN_TRY(init_map(h, fea, (long long)h->lH[0] * h->lW[0], st, nullptr, 0));
+  const long long P0 = (long long)h->lH[0] * h->lW[0];
+  DAWN_TRY(init_map(h, fea, P0, (h->cfg.channels - 3) * P0, st, nullptr, 0));
   DAWN_TRY(prep_cond(h, cond, st));
   h->have_invariants = true;
   return 0;
@@ -1145,61 +1164,72 @@ int dawn_unet_set_clip_invariants(dawn_unet* h, const float* fea, const float* c
 int dawn_unet_forward(dawn_unet* h, const float* x, const int64_t* t, const float* cond, float* out, void* stream) {
   DAWN_CHECK(h && x && t && cond && out, "null argument");
   DAWN_CHECK(h->F > 0, "set_num_frames must precede forward");
+  DAWN_CHECK(h->B == 1 || h->taps.empty(), "debugging taps need B = 1");
   cudaStream_t st = (cudaStream_t)stream;
   h->launches = 0;
   Ctx c{h, st};
-  const int H0 = h->lH[0], W0 = h->lW[0], dim = h->cfg.dim, k = h->cfg.init_kernel_size;
+  const int H0 = h->lH[0], W0 = h->lW[0], dim = h->cfg.dim, k = h->cfg.init_kernel_size, B = h->B, NF = h->B * h->F;
   DAWN_TRY(prep_cond(h, cond, st));
   h->have_invariants = false;         // MAP is refreshed by this entry only when the features turn out frame-invariant
-  // Path selection on the device, no host synchronisation: one pass over x decides whether channels 3.. are the same in every
-  // frame (the reference's sampler tiles them, U:1167); both paths are enqueued and the kernels of the one not taken return
-  // at once.  invariant -> hoisted init conv (map from frame 0 + 3 live channels); varying -> full k x k conv over all channels.
+  // Path selection on the device, per clip, no host synchronisation: one pass over x decides for every clip whether channels
+  // 3.. are the same in every frame (the reference's sampler tiles them, U:1167); both paths are enqueued and the kernels of the
+  // one not taken return at once.  invariant -> hoisted init conv (map from frame 0 + 3 live channels); varying -> full k x k
+  // conv over all channels.  VARY[b] is clip b's flag, VARY[B] the number of varying clips: the full conv runs when any clip
+  // varies (the hoisted conv then rewrites the invariant clips' rows), the maps when any clip is invariant.
   const int* vary = h->VARY;
+  const int* n_vary = h->VARY + B;
   {
-    ProfScope ps(c, PC_MISC, 0, 4.0 * h->F * H0 * W0 * h->cfg.channels);
-    DAWN_TRY(launch_frame_invariance(x, 3, h->cfg.channels, h->F, H0 * W0, h->VARY, st));
+    ProfScope ps(c, PC_MISC, 0, 4.0 * NF * H0 * W0 * h->cfg.channels);
+    DAWN_TRY(launch_frame_invariance(x, 3, h->cfg.channels, h->F, H0 * W0, B, h->VARY, st));
   }
   {
-    ProfScope ps(c, PC_MISC, 0, 8.0 * h->F * H0 * W0 * h->cin_pad);
-    DAWN_TRY(launch_ncf_to_nhwc(x, h->cfg.channels, h->F, H0 * W0, h->cin_pad, 0, h->X288, st, vary, 0));
+    ProfScope ps(c, PC_MISC, 0, 8.0 * NF * H0 * W0 * h->cin_pad);
+    DAWN_TRY(launch_ncf_to_nhwc(x, h->cfg.channels, h->F, H0 * W0, h->cin_pad, 0, h->X288, st, n_vary, 0, B));
   }
   {
     Act in{h->X288, h->cin_pad, h->cin_pad, H0, W0};
-    GemmParams p; base_params(p, in, h->F);
+    GemmParams p; base_params(p, in, NF);
     set_weights(p, h->init_full); set_square_taps(p, k, k / 2);
     p.Out = h->XR + dim; p.ldo = 2 * dim;
-    p.skip_flag = vary; p.skip_if = 0;
+    p.skip_flag = n_vary; p.skip_if = 0;
     ProfScope ps(c, PC_CONV_OTHER, 2.0 * p.M * (double)p.N * p.K, 4.0 * p.M * ((double)p.Cin + p.N));
     DAWN_TRY(launch_path(p, EPI_PLAIN, DAWN_PATH_MMA_SYNC, nullptr, st));      // only the mma.sync kernel has the skip flag
   }
-  DAWN_TRY(init_map(h, x + (size_t)3 * h->F * H0 * W0, (long long)h->F * H0 * W0, st, vary, 1));
+  const long long clip_in = (long long)h->cfg.channels * h->F * H0 * W0;       // floats of one clip of x
+  DAWN_TRY(init_map(h, x + (size_t)3 * h->F * H0 * W0, (long long)h->F * H0 * W0, clip_in, st, n_vary, B));
   {
     const double k2 = (double)k * k;
-    ProfScope ps(c, PC_MISC, 2.0 * h->F * H0 * W0 * dim * 3 * k2, 4.0 * h->F * H0 * W0 * (dim + 3));
-    DAWN_TRY(launch_init_conv_x3(x, h->F, H0, W0, h->init_w3, h->MAP, dim, h->XR + dim, 2 * dim, k, st, vary, 1));
+    ProfScope ps(c, PC_MISC, 2.0 * NF * H0 * W0 * dim * 3 * k2, 4.0 * NF * H0 * W0 * (dim + 3));
+    DAWN_TRY(launch_init_conv_x3(x, clip_in, h->F, H0, W0, B, h->init_w3, h->MAP, dim, h->XR + dim, 2 * dim, k, st, vary, 1));
   }
-  return forward_core(h, t, out, st);
+  return forward_core(h, t, 1, out, st);
 }
 
-int dawn_unet_forward_x3(dawn_unet* h, const float* x_t, const int64_t* t, float* out, void* stream) {
+// forward_x3 with clip b's timestep at t[b * t_stride]
+static int forward_x3_impl(dawn_unet* h, const float* x_t, const int64_t* t, int t_stride, float* out, cudaStream_t st) {
   DAWN_CHECK(h && x_t && t && out, "null argument");
   DAWN_CHECK(h->F > 0 && h->have_invariants, "set_clip_invariants must precede forward_x3");
-  cudaStream_t st = (cudaStream_t)stream;
+  DAWN_CHECK(h->B == 1 || h->taps.empty(), "debugging taps need B = 1");
   h->launches = 0;
-  const int H0 = h->lH[0], W0 = h->lW[0], dim = h->cfg.dim;
+  const int H0 = h->lH[0], W0 = h->lW[0], dim = h->cfg.dim, NF = h->B * h->F;
   {
     Ctx c{h, st};
     const double k2 = (double)h->cfg.init_kernel_size * h->cfg.init_kernel_size;
-    ProfScope ps(c, PC_MISC, 2.0 * h->F * H0 * W0 * dim * 3 * k2, 4.0 * h->F * H0 * W0 * (dim + 3));
-    DAWN_TRY(launch_init_conv_x3(x_t, h->F, H0, W0, h->init_w3, h->MAP, dim, h->XR + dim, 2 * dim,
+    ProfScope ps(c, PC_MISC, 2.0 * NF * H0 * W0 * dim * 3 * k2, 4.0 * NF * H0 * W0 * (dim + 3));
+    DAWN_TRY(launch_init_conv_x3(x_t, 3LL * h->F * H0 * W0, h->F, H0, W0, h->B, h->init_w3, h->MAP, dim, h->XR + dim, 2 * dim,
                                  h->cfg.init_kernel_size, st));
   }
-  return forward_core(h, t, out, st);
+  return forward_core(h, t, t_stride, out, st);
+}
+
+int dawn_unet_forward_x3(dawn_unet* h, const float* x_t, const int64_t* t, float* out, void* stream) {
+  return forward_x3_impl(h, x_t, t, 1, out, (cudaStream_t)stream);
 }
 
 int dawn_unet_forward_host(dawn_unet* h, const float* x_t, const float* fea, const float* cond, int64_t t, float* out) {
   DAWN_CHECK(h && x_t && fea && cond && out, "null argument");
   DAWN_CHECK(h->F > 0, "set_num_frames must precede forward_host");
+  DAWN_CHECK(h->B == 1, "forward_host runs one clip: set_geometry with B = 1 (use the device entries for a batch)");
   cudaStream_t st = 0;
   const size_t M0 = (size_t)h->F * h->H * h->W, P0 = (size_t)h->H * h->W;
   const size_t nout = (size_t)(h->cfg.out_grid_dim + h->cfg.out_conf_dim) * M0;
@@ -1209,7 +1239,7 @@ int dawn_unet_forward_host(dawn_unet* h, const float* x_t, const float* fea, con
   DAWN_CUDA_OK(cudaMemcpyAsync(h->T_HOSTSIDE, &t, sizeof(int64_t), cudaMemcpyHostToDevice, st));
   DAWN_TRY(dawn_unet_set_clip_invariants(h, h->H_FEA, h->H_COND, st));
   const int64_t prep_launches = h->launches;
-  DAWN_TRY(dawn_unet_forward_x3(h, h->H_XT, h->T_HOSTSIDE, h->H_OUT, st));
+  DAWN_TRY(forward_x3_impl(h, h->H_XT, h->T_HOSTSIDE, 1, h->H_OUT, st));
   h->launches += prep_launches;
   DAWN_CUDA_OK(cudaMemcpyAsync(out, h->H_OUT, nout * sizeof(float), cudaMemcpyDeviceToHost, st));
   DAWN_CUDA_OK(cudaStreamSynchronize(st));
@@ -1239,6 +1269,7 @@ int dawn_unet_tap_shape(dawn_unet* h, const char* name, int* C, int* hl, int* wl
 
 int dawn_unet_set_tap(dawn_unet* h, const char* name, float* dst) {
   DAWN_CHECK(h && name, "null argument");
+  DAWN_CHECK(!dst || h->B == 1, "debugging taps need B = 1 (set_geometry with one clip)");
   if (dst) h->taps[name] = dst; else h->taps.erase(name);
   return 0;
 }
@@ -1258,6 +1289,7 @@ int dawn_unet_init_shard(dawn_unet* h, const char* id128, int nranks, int rank, 
   DAWN_CHECK(nranks >= 1 && rank >= 0 && rank < nranks, "bad rank");
   DAWN_CHECK(F_global == h->F * nranks, "F_global must equal nranks * local frames (equal contiguous frame ranges)");
   DAWN_CHECK(nranks == 1 || h->F >= h->cfg.win_width, "each rank must own at least win_width frames (only neighbours exchange halos)");
+  DAWN_CHECK(nranks == 1 || h->B == 1, "frame sharding runs one clip at a time: set_geometry with B = 1 before init_shard");
   drop_graphs(h);
   if (nranks > 1) {
     DAWN_TRY(load_nccl());
@@ -1332,8 +1364,15 @@ static int red_min_u32(void* ctx, unsigned int* b, size_t n, cudaStream_t st) {
 int dawn_unet_ddim_step(dawn_unet* h, float* x, const float* eps, const float* noise, int64_t n_local, float ca, float cb,
                         float sqrt_an, float c, float sigma, float q, void* scratch, void* stream) {
   DAWN_CHECK(h, "null handle");
-  if (h->sh_nranks <= 1 || !h->sh_comm)
-    return ddim_step_impl(x, eps, noise, n_local, n_local, ca, cb, sqrt_an, c, sigma, q, scratch, (cudaStream_t)stream, nullptr);
+  if (h->sh_nranks <= 1 || !h->sh_comm) {
+    // B clips back to back: each clip's quantile is its own (U:1184-1193), so one select per clip on the same scratch
+    DAWN_CHECK(n_local % h->B == 0, "n must be a multiple of the clip count");
+    const int64_t nc = n_local / h->B;
+    for (int b = 0; b < h->B; ++b)
+      DAWN_TRY(ddim_step_impl(x + b * nc, eps + b * nc, noise ? noise + b * nc : nullptr, nc, nc, ca, cb, sqrt_an, c, sigma, q, scratch,
+                              (cudaStream_t)stream, nullptr));
+    return 0;
+  }
   DdimReduce red{(void*)h->sh_comm, red_sum_u32, red_sum_u64, red_min_u32};
   return ddim_step_impl(x, eps, noise, n_local, n_local * h->sh_nranks, ca, cb, sqrt_an, c, sigma, q, scratch,
                         (cudaStream_t)stream, &red);
@@ -1352,13 +1391,13 @@ int dawn_unet_sampler_capture(dawn_unet* h, float* x, float* eps, const float* n
   DAWN_CHECK(!h->prof_on, "disable profiling before capturing the sampler graph");
   drop_sampler_graph(h);
   if (!h->samp_stream) DAWN_CUDA_OK(cudaStreamCreateWithFlags(&h->samp_stream, cudaStreamNonBlocking));
-  const int64_t n = (int64_t)(h->cfg.out_grid_dim + h->cfg.out_conf_dim) * h->F * h->H * h->W;
+  const int64_t n = (int64_t)(h->cfg.out_grid_dim + h->cfg.out_conf_dim) * h->B * h->F * h->H * h->W;
   cudaStream_t st = h->samp_stream;
   DAWN_CUDA_OK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
   int rc = 0;
   int64_t launches = 0;
   for (int k = 0; k < nsteps && rc == 0; ++k) {
-    rc = dawn_unet_forward_x3(h, x, t_all + k, eps, st);
+    rc = forward_x3_impl(h, x, t_all + k, 0, eps, st);               // every clip at step k's timestep
     launches += h->launches;
     const float* cf = coef + 5 * k;
     if (rc == 0)
@@ -1388,8 +1427,14 @@ int dawn_unet_sampler_launch(dawn_unet* h, void* stream) {
 // exactly as dawn_unet_ddim_step does.
 static int ddpm_step_handle(dawn_unet* h, float* x, const float* eps, const float* noise, int64_t n_local, DdpmCoef c,
                             const DdpmCoef* tab, const int64_t* t_slot, int num_t, float q, void* scratch, cudaStream_t st) {
-  if (h->sh_nranks <= 1 || !h->sh_comm)
-    return ddpm_step_impl(x, eps, noise, n_local, n_local, c, tab, t_slot, num_t, q, scratch, st, nullptr);
+  if (h->sh_nranks <= 1 || !h->sh_comm) {
+    DAWN_CHECK(n_local % h->B == 0, "n must be a multiple of the clip count");
+    const int64_t nc = n_local / h->B;
+    for (int b = 0; b < h->B; ++b)       // one select per clip: each clip's quantile is its own
+      DAWN_TRY(ddpm_step_impl(x + b * nc, eps + b * nc, noise ? noise + b * nc : nullptr, nc, nc, c, tab, t_slot, num_t, q, scratch, st,
+                              nullptr));
+    return 0;
+  }
   DdimReduce red{(void*)h->sh_comm, red_sum_u32, red_sum_u64, red_min_u32};
   return ddpm_step_impl(x, eps, noise, n_local, n_local * h->sh_nranks, c, tab, t_slot, num_t, q, scratch, st, &red);
 }
@@ -1412,10 +1457,10 @@ int dawn_unet_ddpm_capture(dawn_unet* h, float* x, float* eps, const float* nois
   DAWN_CHECK(!h->prof_on, "disable profiling before capturing the ancestral step graph");
   drop_ddpm_graph(h);
   if (!h->samp_stream) DAWN_CUDA_OK(cudaStreamCreateWithFlags(&h->samp_stream, cudaStreamNonBlocking));
-  const int64_t n = (int64_t)(h->cfg.out_grid_dim + h->cfg.out_conf_dim) * h->F * h->H * h->W;
+  const int64_t n = (int64_t)(h->cfg.out_grid_dim + h->cfg.out_conf_dim) * h->B * h->F * h->H * h->W;
   cudaStream_t st = h->samp_stream;
   DAWN_CUDA_OK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-  int rc = dawn_unet_forward_x3(h, x, t_slot, eps, st);
+  int rc = forward_x3_impl(h, x, t_slot, 0, eps, st);                // the one time slot applies to every clip
   const int64_t launches = h->launches;
   if (rc == 0)
     rc = ddpm_step_handle(h, x, eps, noise, n, DdpmCoef{}, reinterpret_cast<const DdpmCoef*>(coef), t_slot, num_timesteps, q,

@@ -99,6 +99,13 @@ class GaussianDiffusion(nn.Module):
         # q > 0: dynamic threshold; q = 0: static clamp to [-1, 1]; q < 0: no clamp at all (clip_denoised=False, U:1094, 1183)
         return (float(self.dynamic_thres_percentile) if self.use_dynamic_thres else 0.0) if clip_denoised else -1.0
 
+    @staticmethod
+    def _batched(unet, b, Fr, h, w):
+        """True when all b > 1 clips step together: an unsharded UNet whose native pass takes the whole batch (one forward and
+        one update per step, noise drawn as (b, ch, F, h, w) like the reference's randn_like over the batch).  Otherwise the
+        clips are sampled one after the other, as for b = 1."""
+        return b > 1 and hasattr(unet, "clips_per_pass") and unet.clips_per_pass(b, Fr, h, w) == b
+
     def _check_sample_shape(self, what, fea, shape, cond):
         b, ch, Fr, h, w = shape
         if tuple(shape[1:]) != (self.channels,) + tuple(shape[2:]) or fea.shape[0] != b or (cond is not None and cond.shape[0] != b):
@@ -136,6 +143,8 @@ class GaussianDiffusion(nn.Module):
                 raise NotImplementedError("use_graph captures the cond_scale = 1 loop (DAWN's shipped setting); "
                                           "classifier-free guidance runs eagerly")
             return self._ddim_sample_graph(unet, fea, cond, img, pairs, draw, q, st)
+        if self._batched(unet, b, Fr, h, w):
+            return self._ddim_sample_batched(unet, fea, cond, img, pairs, draw, q, st, guided, cond_scale)
         scratch = torch.empty(n + 512, dtype=torch.int32, device=device)
         eps = torch.empty((ch, Fr, h, w), device=device)
         eps_null = torch.empty_like(eps) if guided else None
@@ -165,6 +174,37 @@ class GaussianDiffusion(nn.Module):
                                               ctypes.c_void_p(scratch.data_ptr()), st), "dawn_unet_ddim_step")
         return img
 
+    def _ddim_sample_batched(self, unet, fea, cond, img, pairs, draw, q, st, guided, cond_scale):
+        """All b clips of an unsharded UNet step together (reference ddim_sample over the batch, U:1156-1208): one forward and
+        one update per step, each clip with its own timestep embedding slot and its own dynamic-threshold quantile.  Noise is
+        drawn as the reference draws it, noise_fn(k, (b, ch, F, h, w)) per step."""
+        b, ch, Fr, h, w = img.shape
+        device, n = img.device, ch * Fr * h * w
+        unet.update_num_frames(Fr)
+        scratch = torch.empty(n + 512, dtype=torch.int32, device=device)
+        eps = torch.empty_like(img)
+        eps_null = torch.empty_like(img) if guided else None
+        fea, cond = fea.contiguous(), cond.contiguous()
+        null = torch.zeros_like(cond) if guided else None
+        if not guided:
+            unet.set_clip_invariants(fea, cond)
+        for k, (t, t_next) in enumerate(pairs):
+            t_dev = torch.full((b,), t, device=device, dtype=torch.long)
+            if guided:                                   # cond, then all-zero null cond, per step (U:879-890, 920)
+                unet.set_clip_invariants(fea, cond)
+                unet.forward_x3(img, t_dev, eps)
+                unet.set_clip_invariants(fea, null)
+                unet.forward_x3(img, t_dev, eps_null)
+                torch.add(eps_null, eps - eps_null, alpha=float(cond_scale), out=eps)
+            else:
+                unet.forward_x3(img, t_dev, eps)
+            ca, cb, san, c, sigma = self.ddim_coefficients(t, t_next)
+            noise = draw(k, (b, ch, Fr, h, w)).to(device).contiguous() if t_next > 0 else None
+            check(lib.dawn_unet_ddim_step(unet._handle, ctypes.c_void_p(img.data_ptr()), ctypes.c_void_p(eps.data_ptr()),
+                                          ctypes.c_void_p(noise.data_ptr()) if noise is not None else None, b * n,
+                                          ca, cb, san, c, sigma, q, ctypes.c_void_p(scratch.data_ptr()), st), "dawn_unet_ddim_step")
+        return img
+
     @staticmethod
     def _default_noise(unet, device, seed):
         """torch.randn per step (:1166, 1201).  For a frame-sharded clip every rank draws the clip-wide tensor from the same
@@ -190,32 +230,36 @@ class GaussianDiffusion(nn.Module):
     def _ddim_sample_graph(self, unet, fea, cond, img, pairs, draw, q, st):
         b, ch, Fr, h, w = img.shape
         device, n, ns = img.device, ch * Fr * h * w, len(pairs)
-        key = (Fr, h, w, tuple(pairs), q, device.index)
+        # one graph launch runs the whole batch (leading clip dimension) or one clip
+        batched = self._batched(unet, b, Fr, h, w)
+        one = (b, ch, Fr, h, w) if batched else (ch, Fr, h, w)
+        key = (Fr, h, w, tuple(pairs), q, device.index, one)
         g = getattr(self, "_graph", None)
         unet.update_num_frames(Fr)
         if g is None or g["key"] != key or g["gen"] != unet.graph_generation():
-            g = dict(key=key, x=torch.empty((ch, Fr, h, w), device=device), eps=torch.empty((ch, Fr, h, w), device=device),
-                     noise=torch.empty((max(ns - 1, 1), ch, Fr, h, w), device=device),
+            g = dict(key=key, x=torch.empty(one, device=device), eps=torch.empty(one, device=device),
+                     noise=torch.empty((max(ns - 1, 1),) + one, device=device),
                      t_all=torch.tensor([p[0] for p in pairs], dtype=torch.long, device=device),
                      scratch=torch.empty(n + 512, dtype=torch.int32, device=device))
             coef = (ctypes.c_float * (5 * ns))()
             for k, (t, t_next) in enumerate(pairs):
                 coef[5 * k:5 * k + 5] = self.ddim_coefficients(t, t_next)
                 assert (t_next > 0) == (k < ns - 1), "only the last DDIM step ends at t = 0 (reference :1201)"
-            unet.set_clip_invariants(fea[0], cond[0])
+            unet.set_clip_invariants(*((fea, cond) if batched else (fea[0], cond[0])))
             torch.cuda.synchronize(device)
             check(lib.dawn_unet_sampler_capture(unet._handle, ctypes.c_void_p(g["x"].data_ptr()), ctypes.c_void_p(g["eps"].data_ptr()),
                                                 ctypes.c_void_p(g["noise"].data_ptr()), ctypes.c_void_p(g["t_all"].data_ptr()),
                                                 coef, ns, q, ctypes.c_void_p(g["scratch"].data_ptr())), "dawn_unet_sampler_capture")
             g["gen"] = unet.graph_generation()
             self._graph = g
-        for i in range(b):
-            unet.set_clip_invariants(fea[i], cond[i])
-            g["x"].copy_(img[i])
+        for i in range(1 if batched else b):
+            sel = slice(None) if batched else i
+            unet.set_clip_invariants(fea[sel], cond[sel])
+            g["x"].copy_(img[sel])
             for k in range(ns - 1):
-                g["noise"][k].copy_(draw(k, (ch, Fr, h, w)))
+                g["noise"][k].copy_(draw(k, one))
             check(lib.dawn_unet_sampler_launch(unet._handle, st), "dawn_unet_sampler_launch")
-            img[i].copy_(g["x"])
+            img[sel].copy_(g["x"])
         return img
 
     # ------------------------------------------------------------------ ancestral sampling (reference :1087-1134)
@@ -243,9 +287,9 @@ class GaussianDiffusion(nn.Module):
         return tuple(float(v) for v in self.ddpm_table()[t])
 
     def _ddpm_step(self, unet, fea_i, cond_i, x, t, cond_scale, guided, eps, eps_null, noise, q, scratch, st):
-        """One ancestral step in place on x (3, F, h, w), this handle's frames of one clip (U:1087-1121).  Without guidance
-        the caller has set the clip invariants of (fea_i, cond_i)."""
-        t_dev = torch.full((1,), t, device=x.device, dtype=torch.long)
+        """One ancestral step in place on x (3, F, h, w), this handle's frames of one clip, or on x (b, 3, F, h, w), a batch
+        run in one pass (U:1087-1121).  Without guidance the caller has set the clip invariants of (fea_i, cond_i)."""
+        t_dev = torch.full((x.shape[0] if x.dim() == 5 else 1,), t, device=x.device, dtype=torch.long)
         if guided:
             # forward_with_cond_scale (U:879-890): null + (cond - null) * cond_scale, the null condition being all zeros
             # (learn_null_cond=False, U:920); two hoisted forwards, each after rebuilding the per-clip conditioning tables
@@ -287,14 +331,16 @@ class GaussianDiffusion(nn.Module):
         guided = cond_scale != 1 and getattr(unet, "has_cond", True)
         st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
         scratch = torch.empty(ch * Fr * h * w + 512, dtype=torch.int32, device=device)
-        eps = torch.empty((ch, Fr, h, w), device=device)
+        batched = self._batched(unet, b, Fr, h, w)
+        eps = torch.empty(tuple(img.shape) if batched else (ch, Fr, h, w), device=device)
         eps_null = torch.empty_like(eps) if guided else None
         q = self._clip_q(clip_denoised)
-        for i in range(b):
+        for i in range(1 if batched else b):
+            sel = slice(None) if batched else i
             unet.update_num_frames(Fr)
             if not guided:
-                unet.set_clip_invariants(fea[i], cond[i])
-            self._ddpm_step(unet, fea[i], cond[i], img[i], t, cond_scale, guided, eps, eps_null, noise[i], q, scratch, st)
+                unet.set_clip_invariants(fea[sel], cond[sel])
+            self._ddpm_step(unet, fea[sel], cond[sel], img[sel], t, cond_scale, guided, eps, eps_null, noise[sel], q, scratch, st)
         return img
 
     @torch.no_grad()
@@ -324,29 +370,34 @@ class GaussianDiffusion(nn.Module):
                                           "classifier-free guidance runs eagerly")
             return self._p_sample_loop_graph(unet, fea, cond, img, draw, q, st)
         scratch = torch.empty(ch * Fr * h * w + 512, dtype=torch.int32, device=device)
-        eps = torch.empty((ch, Fr, h, w), device=device)
+        batched = self._batched(unet, b, Fr, h, w)
+        one = tuple(shape) if batched else (ch, Fr, h, w)
+        eps = torch.empty(one, device=device)
         eps_null = torch.empty_like(eps) if guided else None
         T = self.num_timesteps
-        for i in range(b):
+        for i in range(1 if batched else b):
+            sel = slice(None) if batched else i
             unet.update_num_frames(Fr)
             if not guided:
-                unet.set_clip_invariants(fea[i], cond[i])
+                unet.set_clip_invariants(fea[sel], cond[sel])
             for k in range(T):
-                noise = draw(k, (ch, Fr, h, w)).to(device).contiguous()
-                self._ddpm_step(unet, fea[i], cond[i], img[i], T - 1 - k, cond_scale, guided, eps, eps_null, noise, q, scratch, st)
+                noise = draw(k, one).to(device).contiguous()
+                self._ddpm_step(unet, fea[sel], cond[sel], img[sel], T - 1 - k, cond_scale, guided, eps, eps_null, noise, q, scratch, st)
         return img
 
     def _p_sample_loop_graph(self, unet, fea, cond, img, draw, q, st):
         b, ch, Fr, h, w = img.shape
         device, n, T = img.device, ch * Fr * h * w, self.num_timesteps
-        key = (Fr, h, w, T, q, device.index)
+        batched = self._batched(unet, b, Fr, h, w)
+        one = (b, ch, Fr, h, w) if batched else (ch, Fr, h, w)
+        key = (Fr, h, w, T, q, device.index, one)
         g = getattr(self, "_ddpm_graph", None)
         unet.update_num_frames(Fr)
         if g is None or g["key"] != key or g["gen"] != unet.graph_generation():
-            g = dict(key=key, x=torch.empty((ch, Fr, h, w), device=device), eps=torch.empty((ch, Fr, h, w), device=device),
-                     noise=torch.empty((ch, Fr, h, w), device=device), t=torch.empty(1, dtype=torch.long, device=device),
+            g = dict(key=key, x=torch.empty(one, device=device), eps=torch.empty(one, device=device),
+                     noise=torch.empty(one, device=device), t=torch.empty(1, dtype=torch.long, device=device),
                      coef=torch.empty((T, 5), device=device), scratch=torch.empty(n + 512, dtype=torch.int32, device=device))
-            unet.set_clip_invariants(fea[0], cond[0])
+            unet.set_clip_invariants(*((fea, cond) if batched else (fea[0], cond[0])))
             torch.cuda.synchronize(device)
             check(lib.dawn_unet_ddpm_capture(unet._handle, ctypes.c_void_p(g["x"].data_ptr()), ctypes.c_void_p(g["eps"].data_ptr()),
                                              ctypes.c_void_p(g["noise"].data_ptr()), ctypes.c_void_p(g["t"].data_ptr()),
@@ -355,14 +406,15 @@ class GaussianDiffusion(nn.Module):
             g["gen"] = unet.graph_generation()
             self._ddpm_graph = g
         g["coef"].copy_(self.ddpm_table())          # the schedule buffers may have been reloaded since the capture
-        for i in range(b):
-            unet.set_clip_invariants(fea[i], cond[i])
-            g["x"].copy_(img[i])
+        for i in range(1 if batched else b):
+            sel = slice(None) if batched else i
+            unet.set_clip_invariants(fea[sel], cond[sel])
+            g["x"].copy_(img[sel])
             g["t"].fill_(T - 1)
             for k in range(T):
-                g["noise"].copy_(draw(k, (ch, Fr, h, w)))
+                g["noise"].copy_(draw(k, one))
                 check(lib.dawn_unet_ddpm_launch(unet._handle, st), "dawn_unet_ddpm_launch")
-            img[i].copy_(g["x"])
+            img[sel].copy_(g["x"])
         return img
 
     def forward(self, *a, **k):

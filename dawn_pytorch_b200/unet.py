@@ -17,6 +17,11 @@ from torch import nn
 from . import _lib
 from ._lib import DawnUnetCfg, check, lib
 
+MAX_CLIPS = 16                  # clips per native pass the library accepts (kMaxClips, csrc/common.cuh)
+# Largest batched pass, in frames x latent pixels over all its clips: bounds the workspace of a pass (~9 KiB per pixel-frame,
+# ~19 GiB at the cap: two 200-frame 64x64 clips, ten 200-frame 32x32 clips).  Per-clip times: DESIGN.md section 5.
+BATCH_PIXEL_FRAMES = 1 << 21
+
 
 # ----------------------------------------------------------------------------- parameter holders
 class _Holder(nn.Module):
@@ -244,7 +249,20 @@ class Unet3D(nn.Module):
             except Exception:
                 pass
 
-    def _ensure(self, device, F, h, w):
+    def clips_per_pass(self, b, F, h, w):
+        """How many of b clips of F frames x h x w one native pass runs: all of them up to MAX_CLIPS and BATCH_PIXEL_FRAMES,
+        passes of equal size beyond that; one at a time on a frame-sharded handle."""
+        if getattr(self, "_shard", None) is not None:
+            return 1
+        n = max(1, min(b, MAX_CLIPS, BATCH_PIXEL_FRAMES // (F * h * w)))
+        passes = -(-b // n)
+        return -(-b // passes)
+
+    def clip_count(self):
+        """Clips (batch elements) the native handle runs per call for the current geometry."""
+        return getattr(self, "_clips", 1)
+
+    def _ensure(self, device, F, h, w, B=1):
         if device.type != "cuda":
             raise _lib.DawnError("the DAWN denoising UNet runs on CUDA (sm_90a) only; there is no CPU path")
         idx = device.index if device.index is not None else torch.cuda.current_device()
@@ -258,9 +276,9 @@ class Unet3D(nn.Module):
                 self._handle, self._device_index = hd, idx
             if self._dirty:
                 self.sync_parameters()
-            if self._geom != (F, h, w):
-                check(lib.dawn_unet_set_num_frames(self._handle, F, h, w), "dawn_unet_set_num_frames")
-                self._geom = (F, h, w)
+            if self._geom != (F, h, w) or self.clip_count() != B:
+                check(lib.dawn_unet_set_geometry(self._handle, B, F, h, w), "dawn_unet_set_geometry")
+                self._geom, self._clips = (F, h, w), B
                 self._gen = getattr(self, "_gen", 0) + 1
             lost = getattr(self, "_shard_lost", None)
             if lost is not None and not getattr(self, "_in_init_shard", False):
@@ -313,7 +331,8 @@ class Unet3D(nn.Module):
             raise ValueError(f"num_frames={self.num_frames} but x has {F} frames and cond {cond.shape[1]}: "
                              "call update_num_frames first (reference :925-926)")
         device = x.device
-        self._ensure(device, F, h, w)
+        n = self.clips_per_pass(b, F, h, w)
+        self._ensure(device, F, h, w, n)
         x = x.contiguous().float()
         time = time.to(device=device, dtype=torch.int64).contiguous()
         # classifier-free guidance plumbing (reference :917-926); learn_null_cond=False -> zeros
@@ -331,30 +350,44 @@ class Unet3D(nn.Module):
         out = torch.empty((b, self.out_dim, F, h, w), device=device, dtype=torch.float32)
         st = self._stream()
         with torch.cuda.device(device):
-            for i in range(b):
-                check(lib.dawn_unet_forward(self._handle, ctypes.c_void_p(x[i].data_ptr()),
-                                            ctypes.c_void_p(time[i:i + 1].data_ptr()),
-                                            ctypes.c_void_p(cond[i].data_ptr()),
-                                            ctypes.c_void_p(out[i].data_ptr()), st), "dawn_unet_forward")
+            # passes of n clips; a short last pass is filled up with copies of its last clip (their output is dropped), so the
+            # handle keeps one geometry
+            for i0 in range(0, b, n):
+                i1 = min(b, i0 + n)
+                xs, ts, cs, os_ = x[i0:i1], time[i0:i1], cond[i0:i1], out[i0:i1]
+                if i1 - i0 < n:
+                    pad = lambda a: torch.cat([a, a[-1:].expand((n - (i1 - i0),) + a.shape[1:])]).contiguous()   # noqa: E731
+                    xs, ts, cs = pad(xs), pad(ts), pad(cs)
+                    os_ = torch.empty((n,) + out.shape[1:], device=device, dtype=torch.float32)
+                check(lib.dawn_unet_forward(self._handle, ctypes.c_void_p(xs.data_ptr()), ctypes.c_void_p(ts.data_ptr()),
+                                            ctypes.c_void_p(cs.data_ptr()), ctypes.c_void_p(os_.data_ptr()), st),
+                      "dawn_unet_forward")
+                if os_.data_ptr() != out[i0:i1].data_ptr():
+                    out[i0:i1].copy_(os_[:i1 - i0])
         return out
 
     # ------------------------------------------------------------------ fast path used by our sampler
     def set_clip_invariants(self, fea, cond):
-        """fea (channels-3, h, w) and cond (F, cond_dim) of ONE clip: everything that is constant over the
-        DDIM steps (272 of the 275 init-conv input channels, all cross-attention keys/values)."""
-        if fea.dim() != 3 or cond.dim() != 2:
-            raise ValueError(f"set_clip_invariants: fea must be (channels-3, h, w) and cond (F, cond_dim); got {tuple(fea.shape)}, {tuple(cond.shape)}")
-        F, (h, w) = cond.shape[0], fea.shape[-2:]
-        if fea.shape[0] != self.channels - 3 or cond.shape[1] != (self.cond_dim or 0):
+        """fea (channels-3, h, w) and cond (F, cond_dim) of ONE clip, or fea (B, channels-3, h, w) and cond (B, F, cond_dim)
+        of B clips run together: everything that is constant over the DDIM steps (272 of the 275 init-conv input channels,
+        all cross-attention keys/values).  forward_x3 then takes the same number of clips."""
+        batched = fea.dim() == 4 and cond.dim() == 3 and fea.shape[0] == cond.shape[0]
+        if not batched and (fea.dim() != 3 or cond.dim() != 2):
+            raise ValueError(f"set_clip_invariants: fea must be (channels-3, h, w) and cond (F, cond_dim), or fea (B, channels-3, h, w) "
+                             f"and cond (B, F, cond_dim); got {tuple(fea.shape)}, {tuple(cond.shape)}")
+        B = fea.shape[0] if batched else 1
+        F, (h, w) = cond.shape[-2], fea.shape[-2:]
+        if fea.shape[-3] != self.channels - 3 or cond.shape[-1] != (self.cond_dim or 0):
             raise ValueError(f"set_clip_invariants: expected fea with {self.channels - 3} channels and cond with {self.cond_dim} "
                              f"features; got {tuple(fea.shape)}, {tuple(cond.shape)}")
         if F != self.num_frames:
             raise ValueError(f"num_frames={self.num_frames} but cond has {F} frames: call update_num_frames first (reference :925-926)")
         if not fea.is_cuda or cond.device != fea.device:
             raise _lib.DawnError("set_clip_invariants needs CUDA tensors on one device (no CPU fallback)")
-        self._ensure(fea.device, F, h, w)
+        self._ensure(fea.device, F, h, w, B)
         self._fea = fea.contiguous().float()
         self._cond = cond.contiguous().float()
+        self._inv_batched = batched
         with torch.cuda.device(fea.device):
             check(lib.dawn_unet_set_clip_invariants(self._handle, ctypes.c_void_p(self._fea.data_ptr()),
                                                     ctypes.c_void_p(self._cond.data_ptr()), self._stream()),
@@ -404,17 +437,22 @@ class Unet3D(nn.Module):
         return (id(self._handle), getattr(self, "_gen", 0))
 
     def forward_x3(self, x_t, time, out=None):
-        """x_t (3, F, h, w) of the clip whose invariants were set; time int64 tensor (1,) on the device."""
+        """x_t (3, F, h, w) of the clip whose invariants were set and time int64 (1,) on the device; after batched
+        invariants x_t (B, 3, F, h, w) and time (B,), one timestep per clip."""
         if self._geom is None or getattr(self, "_fea", None) is None:
             raise _lib.DawnError("forward_x3: call set_clip_invariants first")
-        if tuple(x_t.shape) != (3,) + tuple(self._geom) or x_t.dtype != torch.float32 or x_t.device != self._fea.device:
-            raise ValueError(f"forward_x3: x_t must be float32 (3, {self._geom[0]}, {self._geom[1]}, {self._geom[2]}) on "
+        lead = (self.clip_count(),) if getattr(self, "_inv_batched", False) else ()
+        if tuple(x_t.shape) != lead + (3,) + tuple(self._geom) or x_t.dtype != torch.float32 or x_t.device != self._fea.device:
+            raise ValueError(f"forward_x3: x_t must be float32 {lead + (3,) + tuple(self._geom)} on "
                              f"{self._fea.device}; got {x_t.dtype} {tuple(x_t.shape)} on {x_t.device}")
-        _, F, h, w = x_t.shape
+        if time.numel() != self.clip_count():
+            raise ValueError(f"forward_x3: one timestep per clip ({self.clip_count()}), got {time.numel()}")
+        F, h, w = x_t.shape[-3:]
+        oshape = lead + (self.out_dim, F, h, w)
         if out is None:
-            out = torch.empty((self.out_dim, F, h, w), device=x_t.device, dtype=torch.float32)
-        elif tuple(out.shape) != (self.out_dim, F, h, w) or out.dtype != torch.float32 or not out.is_contiguous() or out.device != x_t.device:
-            raise ValueError(f"forward_x3: out must be contiguous float32 ({self.out_dim}, {F}, {h}, {w}) on {x_t.device}")
+            out = torch.empty(oshape, device=x_t.device, dtype=torch.float32)
+        elif tuple(out.shape) != oshape or out.dtype != torch.float32 or not out.is_contiguous() or out.device != x_t.device:
+            raise ValueError(f"forward_x3: out must be contiguous float32 {oshape} on {x_t.device}")
         x_t = x_t.contiguous()
         with torch.cuda.device(x_t.device):
             check(lib.dawn_unet_forward_x3(self._handle, ctypes.c_void_p(x_t.data_ptr()), ctypes.c_void_p(time.data_ptr()),
@@ -424,7 +462,7 @@ class Unet3D(nn.Module):
     def forward_host(self, x_t, fea, cond, t, out=None):
         """End-to-end step with HOST tensors (pinned recommended): H2D of x_t/fea/cond, compute, D2H of eps."""
         _, F, h, w = x_t.shape
-        self._ensure(torch.device("cuda", torch.cuda.current_device()), F, h, w)
+        self._ensure(torch.device("cuda", torch.cuda.current_device()), F, h, w)      # one clip
         if out is None:
             out = torch.empty((self.out_dim, F, h, w), dtype=torch.float32, pin_memory=True)
         check(lib.dawn_unet_forward_host(self._handle, ctypes.c_void_p(x_t.data_ptr()), ctypes.c_void_p(fea.data_ptr()),
@@ -434,7 +472,7 @@ class Unet3D(nn.Module):
 
     # ------------------------------------------------------------------ debugging taps (sub-module parity tests)
     def request_taps(self, names, F, h, w, device):
-        self._ensure(device, F, h, w)
+        self._ensure(device, F, h, w)                          # taps run on one clip
         bufs = {}
         for n in names:
             C, hl, wl = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()

@@ -6,7 +6,9 @@
  * (..._flow_fast_init_cond_test.py:140).  The entry points below are what a binding for that seam needs;
  * dawn_pytorch_b200/unet.py is the ctypes binding that keeps the reference's Python signature on top of them.
  * Plain pointers and sizes only; no torch types.  One handle per GPU, not thread-safe, stream-ordered,
- * no hidden host synchronisation inside forward calls.  All tensors are fp32; one clip (batch element) per call.
+ * no hidden host synchronisation inside forward calls.  All tensors are fp32.  A handle runs a batch of B clips (batch
+ * elements) per call, B = 1 unless dawn_unet_set_geometry says otherwise; every per-clip tensor below then holds the B clips
+ * back to back (a leading batch dimension of B) and each clip is computed as it would be on its own.
  *
  * Return value: 0 ok; -1 bad argument / unsupported configuration / wrong call order; -2 CUDA error.
  * dawn_last_error() returns a human-readable description of the last failure on this thread.
@@ -56,6 +58,11 @@ int dawn_unet_commit_params(dawn_unet* h);
 /* replaces DynamicNfUnet3D.update_num_frames (reference :964-965) and fixes the latent size.
  * For a frame-sharded clip F is the LOCAL frame count of this rank. */
 int dawn_unet_set_num_frames(dawn_unet* h, int F, int height, int width);
+/* B clips of F frames each in one pass (reference batch dimension, U:892-956); set_num_frames(F, h, w) is set_geometry(1, F, h, w).
+ * Sizes the workspace for B*F frames and one GroupNorm statistics / FiLM / init-conv map / cross-attention table slice per clip;
+ * drops both captured sampler graphs.  1 <= B <= 16.  B > 1 is refused (-1) on a frame-sharded handle, with debugging taps set,
+ * by init_shard (with more than one rank), forward_host and set_tap. */
+int dawn_unet_set_geometry(dawn_unet* h, int B, int F, int height, int width);
 
 /* Exact frame sharding of ONE clip over `nranks` GPUs (no reference counterpart; SURVEY 8e): rank r owns the contiguous
  * global frames [r*F, (r+1)*F).  Every temporal attention exchanges its +-win_width boundary frames with the adjacent
@@ -73,15 +80,16 @@ int dawn_unet_shard_ipc_import(dawn_unet* h, const char* handles);
 
 /* Clip invariants (SURVEY §8 a2/a5): the 272 feature channels are identical for every frame and every
  * DDIM step (reference :1167 `fea.repeat`), and cross-attention keys/values depend only on `cond`.
- * fea: device (channels-3, height, width); cond: device (F, cond_dim).  Needed by dawn_unet_forward_x3. */
+ * fea: device (B, channels-3, height, width); cond: device (B, F, cond_dim).  Needed by dawn_unet_forward_x3. */
 int dawn_unet_set_clip_invariants(dawn_unet* h, const float* fea, const float* cond, void* stream);
 
 /* replaces Unet3D.forward / forward_with_cond_scale(cond_scale=1) (reference :879-956) for one clip:
- * x: device (channels, F, height, width); t: device int64[1]; cond: device (F, cond_dim);
- * out: device (out_grid_dim + out_conf_dim, F, height, width). */
+ * x: device (B, channels, F, height, width); t: device int64[B]; cond: device (B, F, cond_dim);
+ * out: device (B, out_grid_dim + out_conf_dim, F, height, width).  The frame-invariant path of the init conv is chosen per
+ * clip on the device. */
 int dawn_unet_forward(dawn_unet* h, const float* x, const int64_t* t, const float* cond, float* out, void* stream);
 
-/* same function when the caller knows the clip invariants: x_t: device (3, F, height, width) */
+/* same function when the caller knows the clip invariants: x_t: device (B, 3, F, height, width), t: device int64[B] */
 int dawn_unet_forward_x3(dawn_unet* h, const float* x_t, const int64_t* t, float* out, void* stream);
 
 /* end-to-end entry with HOST buffers (pinned recommended): copies x_t, fea, cond, t to the device,
@@ -119,7 +127,8 @@ int64_t dawn_unet_workspace_bytes(dawn_unet* h);
 int dawn_ddim_step(float* x, const float* eps, const float* noise, int64_t n, float ca, float cb, float sqrt_an, float c,
                    float sigma, float q, void* scratch, void* stream);
 
-/* The same update for the frames a handle owns.  Unsharded handle: identical to dawn_ddim_step.  After dawn_unet_init_shard
+/* The same update for the frames a handle owns.  Unsharded handle: x, eps, noise hold the B clips back to back (n = B * per-clip
+ * size) and each clip is updated as dawn_ddim_step would update it alone (its own quantile).  After dawn_unet_init_shard
  * the quantile spans the whole clip (n_local * nranks values): the radix-select's four 256-bin histograms and its two tail
  * statistics are all-reduced (NCCL, on `stream`), so every rank applies the bit-identical threshold.  Every rank must call
  * it with the same coefficients; `noise` is this rank's slice of the clip's noise. */
@@ -128,8 +137,9 @@ int dawn_unet_ddim_step(dawn_unet* h, float* x, const float* eps, const float* n
 
 /* The whole sampling loop of one clip (reference ddim_sample :1156-1208: 20 x [UNet forward + DDIM update]) captured
  * once into ONE CUDA graph and replayed per clip with a single launch: no host work between steps.  All addresses are
- * fixed at capture: x (3,F,h,w) start noise in / sample out, eps (3,F,h,w) scratch, noise_all ((nsteps-1) x 3*F*h*w,
- * slice k feeds step k; the last step adds none), t_all (nsteps int64, device), scratch (as dawn_ddim_step).
+ * fixed at capture: x (B,3,F,h,w) start noise in / sample out, eps (B,3,F,h,w) scratch, noise_all ((nsteps-1) x B*3*F*h*w,
+ * slice k feeds step k; the last step adds none), t_all (nsteps int64, device; every clip runs step k at t_all[k]), scratch
+ * (as dawn_ddim_step).
  * coef (host): nsteps x {ca, cb, sqrt_alpha_next, c, sigma}.  Per clip: fill x / noise_all, call
  * dawn_unet_set_clip_invariants (rewrites the same tables), then dawn_unet_sampler_launch(stream).
  * set_num_frames / commit_params / init_shard drop the graph. */
@@ -147,7 +157,8 @@ int dawn_unet_sampler_launch(dawn_unet* h, void* stream);
 int dawn_ddpm_step(float* x, const float* eps, const float* noise, int64_t n, float ca, float cb, float c1, float c2,
                    float sigma, float q, void* scratch, void* stream);
 
-/* The same update for the frames a handle owns.  Unsharded handle: identical to dawn_ddpm_step.  After dawn_unet_init_shard
+/* The same update for the frames a handle owns.  Unsharded handle: B clips back to back, each updated as dawn_ddpm_step would
+ * update it alone.  After dawn_unet_init_shard
  * the quantile spans the whole clip, as in dawn_unet_ddim_step; every rank passes the same coefficients and its slice of
  * the clip's noise. */
 int dawn_unet_ddpm_step(dawn_unet* h, float* x, const float* eps, const float* noise, int64_t n_local, float ca, float cb,
@@ -155,8 +166,8 @@ int dawn_unet_ddpm_step(dawn_unet* h, float* x, const float* eps, const float* n
 
 /* One step of the ancestral loop (reference p_sample_loop :1123-1134) captured as a CUDA graph and replayed once per
  * timestep: forward_x3(x, t = *t_slot) -> eps, the DDPM update with row *t_slot of coef, then *t_slot -= 1.  All
- * addresses are fixed at capture: x (3,F,h,w) in/out, eps (3,F,h,w) scratch, noise (3,F,h,w; refill it on the stream
- * before every replay), t_slot (one int64, device), coef (device, num_timesteps x {ca, cb, c1, c2, sigma}; the slot is
+ * addresses are fixed at capture: x (B,3,F,h,w) in/out, eps (B,3,F,h,w) scratch, noise (B,3,F,h,w; refill it on the stream
+ * before every replay), t_slot (one int64, device, shared by every clip), coef (device, num_timesteps x {ca, cb, c1, c2, sigma}; the slot is
  * clamped to [0, num_timesteps) when the row is read), scratch (as dawn_ddim_step).  Per clip: fill x, set *t_slot =
  * num_timesteps - 1, call dawn_unet_set_clip_invariants, then dawn_unet_ddpm_launch(stream) num_timesteps times.
  * set_num_frames / commit_params / init_shard drop the graph.  It is held beside the dawn_unet_sampler_capture graph:
