@@ -6,6 +6,8 @@
 // With descriptor base_offset = 0 the 128-byte swizzle follows ABSOLUTE shared-memory address bits, so a K-major operand
 // may start at any 128-byte row and use any row-multiple stride between its 8-row groups:
 //     window(dy,dx): start = halo + ((dy+1)*10 + (dx+1))*128 B,  stride between 8-pixel rows (SBO) = 10*128 B.
+// 8x8 images (the deepest level of a 64x64 latent) run in pair mode (tc_conv3_pair_kernel): a tile is two whole frames of one clip, each
+// m64 half one frame with its own 10x10 halo, so only the second half's window offset differs.
 // Everything else follows tc_gemm.cu: FP16x3 split precision, register accumulators drained into an RN fp32 tile in shared
 // memory (every 9, 3 or 1 taps), row-per-thread epilogue with bias + GroupNorm partial statistics.
 //
@@ -37,9 +39,12 @@ using namespace tc;
 
 constexpr int TH = 16, TW = 8;                 // output tile (pixels) -> M = 128 rows, row m = y*8 + x
 constexpr int HH = TH + 2, HW = TW + 2;        // halo tile
-constexpr int HROWS = HH * HW;                 // 180 halo pixels = 180 rows of 128 B
-constexpr int A_HALO = 23 * 1024;              // 180 * 128 = 23040 B, padded to 23 KB (keeps 1024-byte alignment)
 constexpr int NPROD = 256;
+// Pair mode (8 x 8 images): the 128-row tile is two whole frames of one clip, rows 0-63 frame a and rows 64-127 frame b (row
+// 64 * fr + y*8 + x).  The halo stage holds two 10 x 10 halos: frame a from row 0, frame b from row PAIR_ROW_B = 104 rather than
+// 100, so that frame b's TMA destination is 1024-byte aligned as the 128-byte swizzle requires; rows 100-103 are never read.
+constexpr int PAIR_HH = 8 + 2;
+constexpr int PAIR_ROW_B = 104;
 
 // B stages: what fits in 227 KB next to the halo stages and two 128 x 64 fp32 staging tiles (34 KB each).
 // BN = 64: one MMA warpgroup and one epilogue warpgroup; the staging tiles are a double buffer between them, so the epilogue
@@ -49,17 +54,27 @@ constexpr int NPROD = 256;
 // threads allow, and setmaxnreg.inc can only take what other warpgroups of the CTA released.  The producers keep 96, the loader
 // gives 72 back and the MMA and epilogue warpgroups take them (5 x 96 = 480 at launch):
 //   BN =  64: 2 x 96 + 24 + 136 + 128 = 480        BN = 128: 2 x 96 + 24 + 2 x 128 = 472
-template <int BN>
+// Pair mode runs at BN = 64 with three weight stages: its 26 KB halos leave no room for a fourth (or for BN = 128).
+template <int BN, bool PAIR = false>
 struct CCfg {
+  static_assert(!PAIR || BN == 64, "the pair-mode halos fit next to 64-column weight stages only");
   static constexpr int NWG = BN / 64;                          // MMA warpgroups (64 output columns each)
   static constexpr bool SPLIT_EPI = (BN == 64);                // separate epilogue warpgroup
   static constexpr int B_PANEL = BN * 128;                     // one (tap, chunk) weight panel, hi or lo
+  static constexpr int FRAME_ROWS = PAIR ? PAIR_HH * HW : HH * HW;       // halo rows of one frame: 100 (pair) or 180
+  static constexpr int HALO_ROWS = PAIR ? PAIR_ROW_B + FRAME_ROWS : FRAME_ROWS;   // rows spanned in the stage: 204 or 180
+  static constexpr int A_HALO = (HALO_ROWS * 128 + 1023) / 1024 * 1024;  // 26 KB or 23 KB (keeps 1024-byte alignment)
   static constexpr int A_STAGES = 2;
-  static constexpr int B_STAGES = (BN == 64) ? 4 : 2;
+  static constexpr int B_STAGES = PAIR ? 3 : (BN == 64) ? 4 : 2;
   static constexpr int A_BYTES = A_STAGES * 2 * A_HALO;        // hi + lo
   static constexpr int B_BYTES = B_STAGES * 2 * B_PANEL;
   static constexpr int ACC_STAGE = 2 * 128 * kStageLd * 4;
   static constexpr int SMEM_DYN = A_BYTES + B_BYTES + ACC_STAGE + 1024;
+  // 227 KB per block, less under 1 KB of static barriers, GroupNorm and bias scratch:
+  //   BN =  64:       94 208 (A) + 65 536 (B) + 69 632 (staging) + 1 024 (alignment) = 230 400
+  //   BN = 128:       94 208     + 65 536     + 69 632           + 1 024             = 230 400
+  //   BN = 64 pair:  106 496     + 49 152     + 69 632           + 1 024             = 226 304
+  static_assert(SMEM_DYN + 1024 <= 232448, "shared memory");
   static constexpr int EPI_WARP = NPROD / 32 + 4 * NWG;        // first warp of the epilogue warpgroup (SPLIT_EPI)
   static constexpr int LOAD_WARP = EPI_WARP + (SPLIT_EPI ? 4 : 0);
   static constexpr int NTHREADS = 32 * LOAD_WARP + 128;        // the weight loader is a whole warpgroup (one thread works)
@@ -74,13 +89,14 @@ struct CCfg {
 // two dense fp16 planes (hi | lo, written by the producing kernel's epilogue) and ONE thread fetches the halo tile of a 64-channel chunk with
 // two cp.async.bulk.tensor loads (4-D tiled map {C, W, H, F}, box {64, 10, 18, 1}, 128-byte swizzle, out-of-image rows zero-filled by the
 // TMA unit): the smem image is byte-identical to what the producers write (row = hy * 10 + hx of 128 B, absolute-address swizzle).
-template <int BN, bool TMA>
-__global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const GemmParams p, const float* __restrict__ Bimg,
-                                                                          int tiles_y, int tiles_x, int tiles_n,
-                                                                          const __grid_constant__ CUtensorMap tm_hi,
-                                                                          const __grid_constant__ CUtensorMap tm_lo) {
-  using C = CCfg<BN>;
+// In pair mode the thread issues two loads per frame (box {64, 10, 10, 1}), frame b's landing at row PAIR_ROW_B.
+// img_bn: column width of the weight image's n-tiles (tc_tile_n(N)); the pair kernel's 64-column tiles may be halves of them.
+template <int BN, bool TMA, bool PAIR>
+__device__ __forceinline__ void tc_conv3_body(const GemmParams& p, const float* __restrict__ Bimg, int tiles_y, int tiles_x, int tiles_n,
+                                              int img_bn, const CUtensorMap& tm_hi, const CUtensorMap& tm_lo) {
+  using C = CCfg<BN, PAIR>;
   constexpr int B_PANEL = C::B_PANEL, A_STAGES = C::A_STAGES, B_STAGES = C::B_STAGES, NWG = C::NWG;
+  constexpr int A_HALO = C::A_HALO, FRAME_ROWS = C::FRAME_ROWS;
   constexpr bool SPLIT = C::SPLIT_EPI;
   extern __shared__ uint8_t smem_raw[];
   __shared__ uint64_t a_full[A_STAGES], a_free[A_STAGES], b_full[B_STAGES], b_free[B_STAGES];
@@ -108,17 +124,27 @@ __global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const G
   const int F = p.M / (H * W);
   const int NCH = p.Cin / 64;                                  // 64-channel chunks
   const int tiles_sp = tiles_y * tiles_x;
-  const int total_tiles = F * tiles_sp * tiles_n;              // n fastest: CTAs of one patch share its activations in L2
   // Tiles are visited clip by clip (image f * clips + b is the (f, b) frame): a CTA's consecutive tiles then stay in one clip, so the
   // deferred GroupNorm partial sums below are flushed every 8 tiles and not at every change of clip.
   const int fpc = F / p.clips;                                 // frames per clip
-  auto decode = [&](int tile, int& f, int& y0, int& x0, int& nt) {
+  const int ppc = (fpc + 1) / 2;                               // pair mode: tiles per clip; an odd clip ends in a one-frame tile
+  const int total_tiles = (PAIR ? p.clips * ppc : F * tiles_sp) * tiles_n;   // n fastest: CTAs of one patch share its activations in L2
+  // the tile's first image f, its position (y0, x0) and n-tile nt; nf: frames in the tile (pair mode: images f and f + clips)
+  auto decode = [&](int tile, int& f, int& y0, int& x0, int& nt, int& nf) {
     nt = tile % tiles_n;
     const int sp = tile / tiles_n;
-    const int seq = sp / tiles_sp;                             // clip-major image sequence number
-    const int r = sp - seq * tiles_sp;
-    f = p.clips == 1 ? seq : (seq % fpc) * p.clips + seq / fpc;
-    y0 = (r / tiles_x) * TH; x0 = (r % tiles_x) * TW;
+    if constexpr (PAIR) {
+      const int clip = sp / ppc, fa = 2 * (sp - clip * ppc);
+      f = fa * p.clips + clip;
+      nf = fa + 1 < fpc ? 2 : 1;
+      y0 = 0; x0 = 0;
+    } else {
+      const int seq = sp / tiles_sp;                           // clip-major image sequence number
+      const int r = sp - seq * tiles_sp;
+      f = p.clips == 1 ? seq : (seq % fpc) * p.clips + seq / fpc;
+      nf = 1;
+      y0 = (r / tiles_x) * TH; x0 = (r % tiles_x) * TW;
+    }
   };
 
   if (warp < 8) {                                              // keeps the launch register budget
@@ -128,65 +154,89 @@ __global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const G
         const uint64_t mh = reinterpret_cast<uint64_t>(&tm_hi), ml = reinterpret_cast<uint64_t>(&tm_lo);
         uint32_t ait = 0;
         for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-          int f, y0, x0, nt;
-          decode(tile, f, y0, x0, nt);
+          int f, y0, x0, nt, nf;
+          decode(tile, f, y0, x0, nt, nf);
           for (int cc = 0; cc < NCH; ++cc, ++ait) {
             const int s = ait % A_STAGES;
             mbar_wait(&a_free[s], ((ait / A_STAGES) & 1) ^ 1);
-            mbar_arrive_expect_tx(&a_full[s], 2 * HROWS * 128);
-            const uint32_t dst = smem_u32(smemA + s * 2 * A_HALO), bar = smem_u32(&a_full[s]);
+            mbar_arrive_expect_tx(&a_full[s], nf * 2 * FRAME_ROWS * 128);
+            const uint32_t bar = smem_u32(&a_full[s]);
             const int c0 = cc * 64, c1 = x0 - 1, c2 = y0 - 1;
-            asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-                         ::"r"(dst), "l"(mh), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(f) : "memory");
-            asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-                         ::"r"(dst + A_HALO), "l"(ml), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(f) : "memory");
+            for (int fr = 0; fr < nf; ++fr) {                  // a one-frame pair tile leaves rows 64-127 unused (not stored)
+              const uint32_t dst = smem_u32(smemA + s * 2 * A_HALO) + fr * PAIR_ROW_B * 128;
+              const int c3 = f + fr * p.clips;
+              asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
+                           ::"r"(dst), "l"(mh), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
+              asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
+                           ::"r"(dst + A_HALO), "l"(ml), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
+            }
           }
         }
       }
     } else {
       // ============================================================= producers: halo tile of one 64-channel chunk
+      // Logical halo row l = r0 + 32 q (< 180, pair mode < 200) is row hl of frame fr's halo, stored at row fr * PAIR_ROW_B + hl.
+      constexpr int NQ = (C::FRAME_ROWS * (PAIR ? 2 : 1) + 31) / 32;   // 6 row passes, 7 in pair mode
       const int c16 = tid & 7;
-      const int r0 = tid >> 3;                                 // halo rows r0 + 32 q, q = 0..5 (< 180)
+      const int r0 = (tid >> 3) & 31;                          // tid < 256
       uint32_t ait = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        int f, y0, x0, nt;
-        decode(tile, f, y0, x0, nt);
+        int f, y0, x0, nt, nf;
+        decode(tile, f, y0, x0, nt, nf);
         const float* img = p.A + (size_t)f * H * W * p.lda;
+        const float* img_b = PAIR ? img + (size_t)p.clips * H * W * p.lda : img;   // pair mode: frame b
         for (int cc = 0; cc < NCH; ++cc, ++ait) {
           const int s = ait % A_STAGES;
           const uint32_t round = ait / A_STAGES;
-          float4 v[12];
-#pragma unroll
-          for (int q = 0; q < 6; ++q) {
-            const int r = r0 + 32 * q;
+          auto load = [&](int q, float4& a, float4& b) {
+            const int l = r0 + 32 * q;
+            // frame of the row: known from q alone except in the pass that crosses row FRAME_ROWS
+            const int fr = (!PAIR || 32 * q + 31 < FRAME_ROWS) ? 0 : (32 * q >= FRAME_ROWS) ? 1 : (l >= FRAME_ROWS ? 1 : 0);
+            const int r = l - fr * FRAME_ROWS;
             const int hy = r / HW, hx = r - hy * HW;
             const int iy = y0 + hy - 1, ix = x0 + hx - 1;
-            const bool ok = (r < HROWS) && (iy >= 0) && (iy < H) && (ix >= 0) && (ix < W);
+            const bool ok = (r < FRAME_ROWS) && fr < nf && (iy >= 0) && (iy < H) && (ix >= 0) && (ix < W);
             if (ok) {
-              const float4* src = reinterpret_cast<const float4*>(img + (size_t)(iy * W + ix) * p.lda + cc * 64) + 2 * c16;
-              v[2 * q] = __ldg(src);
-              v[2 * q + 1] = __ldg(src + 1);
+              const float* fimg = fr ? img_b : img;
+              const float4* src = reinterpret_cast<const float4*>(fimg + (size_t)(iy * W + ix) * p.lda + cc * 64) + 2 * c16;
+              a = __ldg(src);
+              b = __ldg(src + 1);
             } else {
-              v[2 * q] = make_float4(0.f, 0.f, 0.f, 0.f);
-              v[2 * q + 1] = make_float4(0.f, 0.f, 0.f, 0.f);
+              a = make_float4(0.f, 0.f, 0.f, 0.f);
+              b = make_float4(0.f, 0.f, 0.f, 0.f);
             }
-          }
-          mbar_wait(&a_free[s], (round & 1) ^ 1);
+          };
           uint8_t* a_hi = smemA + s * 2 * A_HALO;
           uint8_t* a_lo = a_hi + A_HALO;
-#pragma unroll
-          for (int q = 0; q < 6; ++q) {
-            const int r = r0 + 32 * q;
-            if (r < HROWS) {
+          auto store = [&](int q, const float4& a, const float4& b) {
+            const int lr = r0 + 32 * q;
+            const int fr = (!PAIR || 32 * q + 31 < FRAME_ROWS) ? 0 : (32 * q >= FRAME_ROWS) ? 1 : (lr >= FRAME_ROWS ? 1 : 0);
+            const int r = lr + fr * (PAIR_ROW_B - FRAME_ROWS);
+            if (lr < FRAME_ROWS * (PAIR ? 2 : 1)) {
               uint32_t h[4], l[4];
-              split_f16x2(v[2 * q].x, v[2 * q].y, h[0], l[0]);
-              split_f16x2(v[2 * q].z, v[2 * q].w, h[1], l[1]);
-              split_f16x2(v[2 * q + 1].x, v[2 * q + 1].y, h[2], l[2]);
-              split_f16x2(v[2 * q + 1].z, v[2 * q + 1].w, h[3], l[3]);
+              split_f16x2(a.x, a.y, h[0], l[0]);
+              split_f16x2(a.z, a.w, h[1], l[1]);
+              split_f16x2(b.x, b.y, h[2], l[2]);
+              split_f16x2(b.z, b.w, h[3], l[3]);
               const uint32_t off = swz(r, c16);                // absolute-row swizzle (halo base is 1024-byte aligned)
               *reinterpret_cast<uint4*>(a_hi + off) = make_uint4(h[0], h[1], h[2], h[3]);
               *reinterpret_cast<uint4*>(a_lo + off) = make_uint4(l[0], l[1], l[2], l[3]);
             }
+          };
+          // six passes are fetched into registers before the wait for the stage; a seventh would spill at 96 registers, so the pair
+          // mode's last pass (rows 192-199) is fetched after it
+          constexpr int NPRE = NQ < 6 ? NQ : 6;
+          float4 v[2 * NPRE];
+#pragma unroll
+          for (int q = 0; q < NPRE; ++q) load(q, v[2 * q], v[2 * q + 1]);
+          mbar_wait(&a_free[s], (round & 1) ^ 1);
+#pragma unroll
+          for (int q = 0; q < NPRE; ++q) store(q, v[2 * q], v[2 * q + 1]);
+#pragma unroll
+          for (int q = NPRE; q < NQ; ++q) {
+            float4 a, b;
+            load(q, a, b);
+            store(q, a, b);
           }
           mbar_arrive_relaxed(&a_full[s]);                     // proxy fence runs on the consumer side (see tc_gemm.cu)
         }
@@ -200,17 +250,26 @@ __global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const G
     if (warp == C::LOAD_WARP && lane == 0) {
       uint32_t bit = 0;
       const int KC = 9 * NCH;                                  // panels per n-tile in the weight image: kc = tap*NCH + cc
+      // pair mode: the kernel's n-tile is 64-column block nt % sub of image n-tile nt / sub, rows [64 (nt % sub), +64) of each panel
+      const int sub = PAIR ? img_bn / BN : 1;
+      const size_t ipanel = (size_t)sub * B_PANEL;             // one image panel, hi or lo
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        int f, y0, x0, nt;
-        decode(tile, f, y0, x0, nt);
-        const uint8_t* src = reinterpret_cast<const uint8_t*>(Bimg) + (size_t)nt * KC * (2 * B_PANEL);
+        int f, y0, x0, nt, nf;
+        decode(tile, f, y0, x0, nt, nf);
+        const uint8_t* src = reinterpret_cast<const uint8_t*>(Bimg) + (size_t)(nt / sub) * KC * (2 * ipanel) + (size_t)(nt % sub) * B_PANEL;
         for (int cc = 0; cc < NCH; ++cc)
           for (int tap = 0; tap < 9; ++tap, ++bit) {
             const int s = bit % B_STAGES;
             const uint32_t round = bit / B_STAGES;
             mbar_wait(&b_free[s], (round & 1) ^ 1);
             mbar_arrive_expect_tx(&b_full[s], 2 * B_PANEL);
-            bulk_copy_g2s(smemB + s * 2 * B_PANEL, src + (size_t)(tap * NCH + cc) * (2 * B_PANEL), 2 * B_PANEL, &b_full[s]);
+            const uint8_t* panel = src + (size_t)(tap * NCH + cc) * (2 * ipanel);
+            if (PAIR) {
+              bulk_copy_g2s(smemB + s * 2 * B_PANEL, panel, B_PANEL, &b_full[s]);
+              bulk_copy_g2s(smemB + s * 2 * B_PANEL + B_PANEL, panel + ipanel, B_PANEL, &b_full[s]);
+            } else {
+              bulk_copy_g2s(smemB + s * 2 * B_PANEL, panel, 2 * B_PANEL, &b_full[s]);
+            }
           }
       }
     }
@@ -224,7 +283,8 @@ __global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const G
   const int etid = ew * 32 + lane;                             // thread in the warpgroup = its tile row in the epilogue
   const int bar_id = 2 + wg;
   constexpr uint32_t SBO_HALO = HW * 128;                      // 10 pixel rows of 128 B between 8-row groups
-  constexpr uint32_t H2 = 8 * HW * 128;                        // output rows 64-127 start 8 halo rows further down
+  // output rows 64-127 start 8 pixel rows of the halo further down, or (pair mode) at frame b's halo
+  constexpr uint32_t H2 = PAIR ? PAIR_ROW_B * 128 : 8 * HW * 128;
   const int dt = (p.drain == 1 || p.drain == 3) ? p.drain : 9; // taps accumulated in registers before a drain
 
   // All MMAs of one tile into `stage`.  The nine taps of a chunk are expanded at compile time for a drain interval DT of 1, 3
@@ -295,7 +355,7 @@ __global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const G
       asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
     }
   };
-  // A tile covers one frame, so one clip (frame % clips): the running sums belong to the clip of the tiles they hold and are flushed
+  // A tile covers one frame, or two of the same clip, so one clip (frame % clips): the running sums belong to the clip of the tiles they hold and are flushed
   // before a tile of another clip is added.
   auto flush_stats = [&](float (&gs)[8], float (&gss)[8], int clip) {
     const int n0f = wg * 64;                                      // tiles_n == 1: this thread's columns never change
@@ -315,8 +375,8 @@ __global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const G
   };
   // epilogue of one tile: thread etid owns tile row etid; its warp's 32 staged rows serve as the store buffer once read back
   auto epilogue_tile = [&](int tile, float* stage, float (&gs)[8], float (&gss)[8], int& pending, int& pclip) {
-    int f, y0, x0, nt;
-    decode(tile, f, y0, x0, nt);
+    int f, y0, x0, nt, nf;
+    decode(tile, f, y0, x0, nt, nf);
     const int clip = p.clips > 1 ? f % p.clips : 0;
     const int n0 = nt * BN + wg * 64;
     const int row_in_tile = etid;
@@ -334,14 +394,17 @@ __global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const G
     __syncwarp();
 #pragma unroll
     for (int i = 0; i < 64; ++i) acc[i] *= p.tc_scale;
-    const int oy = y0 + (row_in_tile >> 3), ox = x0 + (row_in_tile & 7);
-    const bool rv = (oy < H) && (ox < W);
-    size_t opix = (size_t)f * H * W + (size_t)(rv ? oy * W + ox : 0);
+    // pair mode: row 64 fr + y*8 + x of image f + fr * clips; the rows of a one-frame tile's missing frame are not stored or counted
+    const int fr = PAIR ? row_in_tile >> 6 : 0;
+    const int img = f + fr * p.clips;
+    const int oy = y0 + ((row_in_tile >> 3) & (PAIR ? 7 : 15)), ox = x0 + (row_in_tile & 7);
+    const bool rv = (oy < H) && (ox < W) && fr < nf;
+    size_t opix = (size_t)img * H * W + (size_t)(rv ? oy * W + ox : 0);
     int ocol = n0;
     if (p.up2) {
       // transposed conv as one 3x3 conv with 4 x 64 output columns: column block = output parity class (py, px)
       const int cls = n0 >> 6, py = cls >> 1, px = cls & 1;
-      opix = (size_t)f * 4 * H * W + (size_t)(rv ? (2 * oy + py) * 2 * W + 2 * ox + px : 0);
+      opix = (size_t)img * 4 * H * W + (size_t)(rv ? (2 * oy + py) * 2 * W + 2 * ox + px : 0);
       ocol = n0 & 63;
     }
     if (bias_smem) {
@@ -454,10 +517,35 @@ __global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const G
   }
 }
 
+// 16 x 8-pixel tiles of one frame
+template <int BN, bool TMA>
+__global__ void __launch_bounds__(CCfg<BN>::NTHREADS, 1) tc_conv3_kernel(const GemmParams p, const float* __restrict__ Bimg,
+                                                                          int tiles_y, int tiles_x, int tiles_n, int img_bn,
+                                                                          const __grid_constant__ CUtensorMap tm_hi,
+                                                                          const __grid_constant__ CUtensorMap tm_lo) {
+  tc_conv3_body<BN, TMA, false>(p, Bimg, tiles_y, tiles_x, tiles_n, img_bn, tm_hi, tm_lo);
+}
+
+// pair mode: 8 x 8 images, two frames of one clip per tile, 64 output columns
+template <bool TMA>
+__global__ void __launch_bounds__(CCfg<64, true>::NTHREADS, 1) tc_conv3_pair_kernel(const GemmParams p, const float* __restrict__ Bimg,
+                                                                                     int tiles_y, int tiles_x, int tiles_n, int img_bn,
+                                                                                     const __grid_constant__ CUtensorMap tm_hi,
+                                                                                     const __grid_constant__ CUtensorMap tm_lo) {
+  tc_conv3_body<64, TMA, true>(p, Bimg, tiles_y, tiles_x, tiles_n, img_bn, tm_hi, tm_lo);
+}
+
+template <int BN, bool TMA, bool PAIR>
+constexpr auto c3_kernel() {
+  if constexpr (PAIR) return tc_conv3_pair_kernel<TMA>;
+  else return tc_conv3_kernel<BN, TMA>;
+}
+
 // cuTensorMapEncodeTiled through the runtime's driver entry point (no link dependency on libcuda)
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
                                   const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-int halo_tensor_map(const void* plane, int Cin, int W, int H, int F, CUtensorMap* out) {
+// box {64 channels, 10, box_h, 1}: box_h = 18 for a 16 x 8 tile's halo, 10 for one frame of a pair tile
+int halo_tensor_map(const void* plane, int Cin, int W, int H, int F, int box_h, CUtensorMap* out) {
   static EncodeTiledFn fn = nullptr;
   if (!fn) {
     void* ptr = nullptr;
@@ -467,13 +555,13 @@ int halo_tensor_map(const void* plane, int Cin, int W, int H, int F, CUtensorMap
     fn = reinterpret_cast<EncodeTiledFn>(ptr);
   }
   // one map per (plane, geometry): encoding costs microseconds but the activations of a handle live at fixed addresses
-  static std::map<std::tuple<const void*, int, int, int, int>, CUtensorMap> cache;
-  const auto key = std::make_tuple(plane, Cin, W, H, F);
+  static std::map<std::tuple<const void*, int, int, int, int, int>, CUtensorMap> cache;
+  const auto key = std::make_tuple(plane, Cin, W, H, F, box_h);
   auto it = cache.find(key);
   if (it != cache.end()) { *out = it->second; return 0; }
   const cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)F};
   const cuuint64_t strides[3] = {(cuuint64_t)Cin * 2, (cuuint64_t)W * Cin * 2, (cuuint64_t)H * W * Cin * 2};
-  const cuuint32_t box[4] = {64, (cuuint32_t)HW, (cuuint32_t)HH, 1};
+  const cuuint32_t box[4] = {64, (cuuint32_t)HW, (cuuint32_t)box_h, 1};
   const cuuint32_t estr[4] = {1, 1, 1, 1};
   CUtensorMap m;
   const CUresult r = fn(&m, CU_TENSOR_MAP_DATA_TYPE_UINT16, 4, const_cast<void*>(plane), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
@@ -485,45 +573,53 @@ int halo_tensor_map(const void* plane, int Cin, int W, int H, int F, CUtensorMap
   return 0;
 }
 
-template <int BN>
+template <int BN, bool PAIR>
 int launch_c3(const GemmParams& p, const float* Bimg, cudaStream_t st) {
-  using C = CCfg<BN>;
+  using C = CCfg<BN, PAIR>;
   static bool attr_set = false;
   static int num_sms = 0;
   if (!attr_set) {
-    DAWN_CUDA_OK(cudaFuncSetAttribute(tc_conv3_kernel<BN, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_DYN));
-    DAWN_CUDA_OK(cudaFuncSetAttribute(tc_conv3_kernel<BN, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_DYN));
+    DAWN_CUDA_OK(cudaFuncSetAttribute(c3_kernel<BN, false, PAIR>(), cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_DYN));
+    DAWN_CUDA_OK(cudaFuncSetAttribute(c3_kernel<BN, true, PAIR>(), cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_DYN));
     int dev = 0;
     DAWN_CUDA_OK(cudaGetDevice(&dev));
     DAWN_CUDA_OK(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
     attr_set = true;
   }
-  const int tiles_y = p.IH / TH, tiles_x = p.IW / TW, tiles_n = p.N / BN;
+  const int tiles_y = PAIR ? 1 : p.IH / TH, tiles_x = PAIR ? 1 : p.IW / TW, tiles_n = p.N / BN;
   const int F = p.M / (p.IH * p.IW);
-  const int grid = std::min(F * tiles_y * tiles_x * tiles_n, num_sms);
+  const int seqs = PAIR ? p.clips * ((F / p.clips + 1) / 2) : F;   // pair mode: two frames of a clip per tile
+  const int grid = std::min(seqs * tiles_y * tiles_x * tiles_n, num_sms);
+  const int img_bn = tc_tile_n(p.N);
   if (p.A16h != nullptr && p.A16l != nullptr) {
     CUtensorMap mh, ml;
-    if (halo_tensor_map(p.A16h, p.Cin, p.IW, p.IH, F, &mh) != 0 || halo_tensor_map(p.A16l, p.Cin, p.IW, p.IH, F, &ml) != 0) return -2;
-    tc_conv3_kernel<BN, true><<<grid, C::NTHREADS, C::SMEM_DYN, st>>>(p, Bimg, tiles_y, tiles_x, tiles_n, mh, ml);
+    const int box_h = PAIR ? PAIR_HH : HH;
+    if (halo_tensor_map(p.A16h, p.Cin, p.IW, p.IH, F, box_h, &mh) != 0 || halo_tensor_map(p.A16l, p.Cin, p.IW, p.IH, F, box_h, &ml) != 0)
+      return -2;
+    c3_kernel<BN, true, PAIR>()<<<grid, C::NTHREADS, C::SMEM_DYN, st>>>(p, Bimg, tiles_y, tiles_x, tiles_n, img_bn, mh, ml);
   } else {
     CUtensorMap dummy;
     memset(&dummy, 0, sizeof(dummy));
-    tc_conv3_kernel<BN, false><<<grid, C::NTHREADS, C::SMEM_DYN, st>>>(p, Bimg, tiles_y, tiles_x, tiles_n, dummy, dummy);
+    c3_kernel<BN, false, PAIR>()<<<grid, C::NTHREADS, C::SMEM_DYN, st>>>(p, Bimg, tiles_y, tiles_x, tiles_n, img_bn, dummy, dummy);
   }
   DAWN_LAUNCH_OK();
   return 0;
 }
 
+// 8 x 8 images run in pair mode (two frames per tile); other shapes in 16 x 8 tiles
+bool pair_mode(const GemmParams& p) { return p.IH == 8 && p.IW == 8; }
+
 }  // namespace
 
-// 3x3, stride 1, same padding, static weights, spatial size a multiple of the 16x8 tile, 64-channel chunks, EPI_PLAIN without residual
+// 3x3, stride 1, same padding, static weights, spatial size a multiple of the 16x8 tile or exactly 8x8 (pair mode), 64-channel
+// chunks, EPI_PLAIN without residual
 bool tc_conv3_supported(const GemmParams& p, int epi) {
   if (epi != EPI_PLAIN || p.Res != nullptr || p.perm_in || p.perm_out) return false;
   if (p.ntaps != 9 || p.in_stride != 1 || p.out_stride != 1 || p.oy0 != 0 || p.ox0 != 0) return false;
   for (int t = 0; t < 9; ++t)                                  // the kernel's windows are the taps of a same-padded 3x3, in row-major order
     if (p.dy[t] != t / 3 - 1 || p.dx[t] != t % 3 - 1) return false;
   if (p.IH != p.OH || p.IW != p.OW || p.OHs != p.OH || p.OWs != p.OW) return false;
-  if (p.IH % TH != 0 || p.IW % TW != 0) return false;
+  if ((p.IH % TH != 0 || p.IW % TW != 0) && !pair_mode(p)) return false;
   if (p.Cin % 64 != 0 || p.N % 64 != 0 || p.K != 9 * p.Cin) return false;
   if (p.b_batch_stride != 0 || p.rows_per_batch != p.M) return false;
   if ((p.lda & 3) || (p.ldo & 3)) return false;
@@ -534,8 +630,9 @@ bool tc_conv3_supported(const GemmParams& p, int epi) {
 
 int launch_tc_conv3(const GemmParams& p, const float* Bimg, cudaStream_t st) {
   if (!tc_conv3_supported(p, EPI_PLAIN)) { set_last_error("launch_tc_conv3: unsupported geometry"); return -1; }
-  if (tc_tile_n(p.N) == 128) return launch_c3<128>(p, Bimg, st);
-  return launch_c3<64>(p, Bimg, st);
+  if (pair_mode(p)) return launch_c3<64, true>(p, Bimg, st);
+  if (tc_tile_n(p.N) == 128) return launch_c3<128, false>(p, Bimg, st);
+  return launch_c3<64, false>(p, Bimg, st);
 }
 
 }  // namespace dawn
