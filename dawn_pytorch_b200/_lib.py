@@ -45,7 +45,7 @@ class DawnContractionCase(ctypes.Structure):
 
 
 FUSED_TEMPORAL, FUSED_ATTN_TC, FUSED_ATTN_SIMT, FUSED_SLA_CTX, FUSED_SLA_OUT, FUSED_SLA_CTX_UNFUSED, FUSED_CA_WT, \
-    FUSED_CA_RSTD, FUSED_GN_HCOND = range(9)
+    FUSED_CA_RSTD, FUSED_GN_HCOND, FUSED_TEMPORAL_MMA_SYNC = range(10)
 
 
 class DawnFusedCase(ctypes.Structure):

@@ -40,7 +40,8 @@ AttnArgs attn_args(const dawn_fused_case& c) {
 
 int test_fused(const dawn_fused_case& c, Owned& own, cudaStream_t st) {
   switch (c.kernel) {
-    case DAWN_FUSED_TEMPORAL: {
+    case DAWN_FUSED_TEMPORAL:
+    case DAWN_FUSED_TEMPORAL_MMA_SYNC: {
       if (!c.x || !c.res || !c.out || !c.gamma || !c.w_qkv || !c.w_out || !c.rot || !c.bias) return refuse("missing pointer");
       if (c.P < 1 || c.ldx < 64 || c.ldr < 64 || c.ldo < 64 || (c.ldx | c.ldr | c.ldo) & 3) return refuse("bad geometry");
       if (!temporal_fused_supported(c.C, c.F, c.band, c.q_lo, c.q_hi)) return refuse("temporal_fused_supported refuses the geometry");
@@ -57,7 +58,7 @@ int test_fused(const dawn_fused_case& c, Owned& own, cudaStream_t st) {
       a.x = c.x; a.ldx = c.ldx; a.res = c.res; a.ldr = c.ldr; a.out = c.out; a.ldo = c.ldo;
       a.F = c.F; a.P = c.P; a.q_lo = c.q_lo; a.q_hi = c.q_hi;
       a.Wqkv = dq; a.Wout = dwo; a.wsum = wsum; a.rot = c.rot; a.bias = c.bias; a.band = c.band;
-      return launch_temporal_fused(a, st);
+      return launch_temporal_fused(a, st, c.kernel == DAWN_FUSED_TEMPORAL_MMA_SYNC);
     }
     case DAWN_FUSED_ATTN_TC:
     case DAWN_FUSED_ATTN_SIMT: {

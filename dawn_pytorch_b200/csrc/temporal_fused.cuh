@@ -23,8 +23,11 @@ struct TemporalFusedArgs {
   int nbuf;                       // weight stages in shared memory (set by the launcher)
 };
 
+// one of the two kernels takes the shape: temporal_fused_wg_kernel (warpgroup MMAs, F <= 256) or temporal_fused_kernel (mma.sync)
 bool temporal_fused_supported(int C, int F, int band, int q_lo, int q_hi);
-int launch_temporal_fused(const TemporalFusedArgs& a, cudaStream_t st);
+bool temporal_fused_wg_supported(int C, int F, int band, int q_lo, int q_hi);
+// runs temporal_fused_wg_kernel where it takes the shape, else temporal_fused_kernel; mma_sync_only forces the latter (tests)
+int launch_temporal_fused(const TemporalFusedArgs& a, cudaStream_t st, bool mma_sync_only = false);
 void temporal_fused_pack(const float* wqkv, const float* wout, std::vector<uint16_t>& Wq, std::vector<uint16_t>& Wo, float* inv_wscale,
                          float* inv_oscale);
 

@@ -222,7 +222,7 @@ int dawn_test_contraction(const dawn_contraction_case* c, void* stream);
  * when the kernel's own shape predicate refuses the geometry (it never falls back to another kernel), -2 on a CUDA error;
  * synchronises the stream before it returns. */
 enum {
-  DAWN_FUSED_TEMPORAL = 0,         /* temporal_fused_kernel: out = res + to_out(banded attention(rotary(LN-folded q|k|v of x)))
+  DAWN_FUSED_TEMPORAL = 0,         /* temporal_fused_(wg_)kernel: out = res + to_out(banded attention(rotary(LN-folded q|k|v of x)))
                                       over an on-chip sequence of F frames; rows [q_lo, q_hi) of it are written to out / read
                                       from res at row (f - q_lo)*P + pixel */
   DAWN_FUSED_ATTN_TC = 1,          /* attention_tc_kernel: softmax attention core over qkv rows [q | k | v] (256 each) */
@@ -232,7 +232,9 @@ enum {
   DAWN_FUSED_SLA_CTX_UNFUSED = 5,  /* sla_context_kernel: Bf from a qkv buffer (ld 768) */
   DAWN_FUSED_CA_WT = 6,            /* ca_wt_kernel<C>: Wt = rstd * [1, gates] of the three cross-attentions */
   DAWN_FUSED_CA_RSTD = 7,          /* ca_rstd_kernel: Wt from given gates [F*P][24] */
-  DAWN_FUSED_GN_HCOND = 8          /* gn_hcond_kernel: SiLU(FiLM(GN(Y))) + Wt T_f, fp32 rows, or fp16 hi|lo planes if out16h */
+  DAWN_FUSED_GN_HCOND = 8,         /* gn_hcond_kernel: SiLU(FiLM(GN(Y))) + Wt T_f, fp32 rows, or fp16 hi|lo planes if out16h */
+  DAWN_FUSED_TEMPORAL_MMA_SYNC = 9 /* DAWN_FUSED_TEMPORAL on temporal_fused_kernel (mma.sync) also where the warpgroup-MMA
+                                      kernel temporal_fused_wg_kernel would take the shape (F <= 256) */
 };
 typedef struct {
   int kernel;                      /* DAWN_FUSED_* */
