@@ -7,8 +7,8 @@
 //   fp16 hi/lo in shared memory: K row-major [key][d], V transposed [d][key] (B-operand layouts, padded against bank
 //   conflicts).  S = Q K^T per 32-key block -> + bias, band mask -> online softmax (fp32) -> P (accumulator layout
 //   == A-operand layout of the next MMA) -> O = O*corr + P V.
-#include <cuda_fp16.h>
 #include "common.cuh"
+#include "f16x3.cuh"
 #include "kernels.cuh"
 
 namespace dawn {
@@ -20,27 +20,6 @@ constexpr int KROWS = 224;            // rows staged (7 blocks of 32; rows past 
 constexpr int KFULL = 192;            // chunk length in full-attention mode
 constexpr int K_LD = 40;              // halfs per K row (32 + 8 pad): conflict-free B-fragment reads
 constexpr int V_LD = KROWS + 8;       // halfs per V^T row: (V_LD/2) mod 32 == 20 -> conflict-free
-
-__device__ __forceinline__ void mma_f16(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-// (x0, x1) -> fp16 hi pair / lo pair (hi rounded to 11 significant bits in fp32, so its fp16 conversion is exact)
-__device__ __forceinline__ void split2(float x0, float x1, uint32_t& hi, uint32_t& lo) {
-  const float h0 = __uint_as_float((__float_as_uint(x0) + 0x1000u) & 0xFFFFE000u);
-  const float h1 = __uint_as_float((__float_as_uint(x1) + 0x1000u) & 0xFFFFE000u);
-  const __half2 h = __floats2half2_rn(h0, h1);
-  const __half2 l = __floats2half2_rn(x0 - h0, x1 - h1);
-  hi = *reinterpret_cast<const uint32_t*>(&h);
-  lo = *reinterpret_cast<const uint32_t*>(&l);
-}
-__device__ __forceinline__ void split1(float x, __half& hi, __half& lo) {
-  const float h = __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
-  hi = __float2half_rn(h);
-  lo = __float2half_rn(x - h);
-}
 
 constexpr int ATHREADS = 256;
 
@@ -85,7 +64,7 @@ __global__ void __launch_bounds__(ATHREADS) attention_tc_kernel(AttnArgs a) {
         float2 v = make_float2(0.f, 0.f);
         if (row < q1)
           v = *reinterpret_cast<const float2*>(a.qkv + (size_t)(base + (long long)row * estride) * a.ld + head * 32 + col);
-        split2(v.x, v.y, qh[b][ks][r], ql[b][ks][r]);
+        split_f16x2_rn(v.x, v.y, qh[b][ks][r], ql[b][ks][r]);
       }
     }
 #pragma unroll
@@ -126,7 +105,7 @@ __global__ void __launch_bounds__(ATHREADS) attention_tc_kernel(AttnArgs a) {
         const float4 v = vb[u];
         if (c < 8) {
           uint32_t h0, l0, h1, l1;
-          split2(v.x, v.y, h0, l0); split2(v.z, v.w, h1, l1);
+          split_f16x2_rn(v.x, v.y, h0, l0); split_f16x2_rn(v.z, v.w, h1, l1);
           *reinterpret_cast<uint2*>(&sKh[r * K_LD + c * 4]) = make_uint2(h0, h1);
           *reinterpret_cast<uint2*>(&sKl[r * K_LD + c * 4]) = make_uint2(l0, l1);
         } else {
@@ -135,7 +114,7 @@ __global__ void __launch_bounds__(ATHREADS) attention_tc_kernel(AttnArgs a) {
 #pragma unroll
           for (int i = 0; i < 4; ++i) {
             __half hh, ll;
-            split1(vv[i], hh, ll);
+            split_f16_rn(vv[i], hh, ll);
             sVh[(d + i) * V_LD + r] = hh;
             sVl[(d + i) * V_LD + r] = ll;
           }
@@ -163,13 +142,9 @@ __global__ void __launch_bounds__(ATHREADS) attention_tc_kernel(AttnArgs a) {
 #pragma unroll
           for (int ks = 0; ks < 2; ++ks) {
             const int off = krow * K_LD + ks * 16 + 2 * t;
-            const uint32_t bh0 = *reinterpret_cast<const uint32_t*>(&sKh[off]);
-            const uint32_t bh1 = *reinterpret_cast<const uint32_t*>(&sKh[off + 8]);
-            const uint32_t bl0 = *reinterpret_cast<const uint32_t*>(&sKl[off]);
-            const uint32_t bl1 = *reinterpret_cast<const uint32_t*>(&sKl[off + 8]);
-            mma_f16(s[n], ql[b][ks], bh0, bh1);
-            mma_f16(s[n], qh[b][ks], bl0, bl1);
-            mma_f16(s[n], qh[b][ks], bh0, bh1);
+            const uint32_t bk[4] = {*reinterpret_cast<const uint32_t*>(&sKh[off]), *reinterpret_cast<const uint32_t*>(&sKh[off + 8]),
+                                    *reinterpret_cast<const uint32_t*>(&sKl[off]), *reinterpret_cast<const uint32_t*>(&sKl[off + 8])};
+            mma3(s[n], qh[b][ks], ql[b][ks], bk);
           }
         }
         // ---------------- bias, mask, online softmax (rows g and g+8 of the block)
@@ -213,10 +188,10 @@ __global__ void __launch_bounds__(ATHREADS) attention_tc_kernel(AttnArgs a) {
         uint32_t ph[2][4], pl[2][4];
 #pragma unroll
         for (int ks = 0; ks < 2; ++ks) {
-          split2(s[2 * ks][0], s[2 * ks][1], ph[ks][0], pl[ks][0]);
-          split2(s[2 * ks][2], s[2 * ks][3], ph[ks][1], pl[ks][1]);
-          split2(s[2 * ks + 1][0], s[2 * ks + 1][1], ph[ks][2], pl[ks][2]);
-          split2(s[2 * ks + 1][2], s[2 * ks + 1][3], ph[ks][3], pl[ks][3]);
+          split_f16x2_rn(s[2 * ks][0], s[2 * ks][1], ph[ks][0], pl[ks][0]);
+          split_f16x2_rn(s[2 * ks][2], s[2 * ks][3], ph[ks][1], pl[ks][1]);
+          split_f16x2_rn(s[2 * ks + 1][0], s[2 * ks + 1][1], ph[ks][2], pl[ks][2]);
+          split_f16x2_rn(s[2 * ks + 1][2], s[2 * ks + 1][3], ph[ks][3], pl[ks][3]);
         }
 #pragma unroll
         for (int n = 0; n < 4; ++n) {
@@ -225,13 +200,9 @@ __global__ void __launch_bounds__(ATHREADS) attention_tc_kernel(AttnArgs a) {
 #pragma unroll
           for (int ks = 0; ks < 2; ++ks) {
             const int off = drow + kr0 + ks * 16 + 2 * t;
-            const uint32_t bh0 = *reinterpret_cast<const uint32_t*>(&sVh[off]);
-            const uint32_t bh1 = *reinterpret_cast<const uint32_t*>(&sVh[off + 8]);
-            const uint32_t bl0 = *reinterpret_cast<const uint32_t*>(&sVl[off]);
-            const uint32_t bl1 = *reinterpret_cast<const uint32_t*>(&sVl[off + 8]);
-            mma_f16(acc, pl[ks], bh0, bh1);
-            mma_f16(acc, ph[ks], bl0, bl1);
-            mma_f16(acc, ph[ks], bh0, bh1);
+            const uint32_t bv[4] = {*reinterpret_cast<const uint32_t*>(&sVh[off]), *reinterpret_cast<const uint32_t*>(&sVh[off + 8]),
+                                    *reinterpret_cast<const uint32_t*>(&sVl[off]), *reinterpret_cast<const uint32_t*>(&sVl[off + 8])};
+            mma3(acc, ph[ks], pl[ks], bv);
           }
           o[b][n][0] = o[b][n][0] * corr0 + acc[0];
           o[b][n][1] = o[b][n][1] * corr0 + acc[1];

@@ -13,9 +13,9 @@
 #include <cuda_fp16.h>
 #include <algorithm>
 #include <cmath>
-#include <cstring>
 #include <vector>
 #include "common.cuh"
+#include "f16x3.cuh"
 #include "kernels.cuh"
 #include "ca_fused.cuh"
 
@@ -25,35 +25,6 @@ namespace {
 constexpr int NTH = 256;
 constexpr int CHUNK = 128;             // pixels staged per iteration: one 16-pixel group per warp
 constexpr int WT_LD = 36;              // floats per row of a warp's gate / Wt patch (bank-conflict-free column writes)
-
-__device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ void ldsm4(uint32_t (&r)[4], const __half* p) {
-  const uint32_t addr = (uint32_t)__cvta_generic_to_shared(p);
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];\n"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-__device__ __forceinline__ void cp_async_16(void* dst, const void* src) {
-  const uint32_t d = (uint32_t)__cvta_generic_to_shared(dst);
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" :: "r"(d), "l"(src) : "memory");
-}
-__device__ __forceinline__ void split2h(float x0, float x1, uint32_t& hi, uint32_t& lo) {
-  const float h0 = __uint_as_float(__float_as_uint(x0) & 0xFFFFE000u);
-  const float h1 = __uint_as_float(__float_as_uint(x1) & 0xFFFFE000u);
-  const __half2 h = __floats2half2_rn(h0, h1);
-  const __half2 l = __floats2half2_rn(x0 - h0, x1 - h1);
-  hi = *reinterpret_cast<const uint32_t*>(&h);
-  lo = *reinterpret_cast<const uint32_t*>(&l);
-}
-__device__ __forceinline__ float quad_sum(float v) {
-  v += __shfl_xor_sync(0xffffffffu, v, 1);
-  v += __shfl_xor_sync(0xffffffffu, v, 2);
-  return v;
-}
 
 template <int CI>
 __global__ void __launch_bounds__(NTH, (CI == 64) ? 2 : 1) ca_wt_kernel(CaFusedArgs a) {
@@ -81,9 +52,9 @@ __global__ void __launch_bounds__(NTH, (CI == 64) ? 2 : 1) ca_wt_kernel(CaFusedA
     const uint4* src = reinterpret_cast<const uint4*>(a.Wq);      // dense [hi|lo][192][CI] fp16
     for (int i = tid; i < 2 * 192 * CI / 8; i += NTH) {
       const int r = i / (CI / 8), c8 = i - r * (CI / 8);
-      cp_async_16(Wh + r * LD + c8 * 8, src + i);
+      cp_async16(Wh + r * LD + c8 * 8, src + i);
     }
-    asm volatile("cp.async.commit_group;\n" ::: "memory");
+    cp_async_commit();
     for (int i = tid; i < 192; i += NTH) s_kq[i] = a.kq[(size_t)f * 192 + i];
     if (tid < 24) s_nk[tid] = a.nkq[tid];
     for (int i = tid; i < 243; i += NTH) s_G[i] = a.G[(size_t)f * 243 + i];
@@ -109,21 +80,14 @@ __global__ void __launch_bounds__(NTH, (CI == 64) ? 2 : 1) ca_wt_kernel(CaFusedA
     for (int i = 0; i < NPASS; ++i) {
       const int r = i * RPP + tid / LPR;
       const float4 v = xin[i];
-      float s = (v.x + v.y) + (v.z + v.w);
-#pragma unroll
-      for (int o = 1; o < LPR; o <<= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-      const float mu = s * (1.0f / CI);
-      const float d0 = v.x - mu, d1 = v.y - mu, d2 = v.z - mu, d3 = v.w - mu;
-      float ss = (d0 * d0 + d1 * d1) + (d2 * d2 + d3 * d3);
-#pragma unroll
-      for (int o = 1; o < LPR; o <<= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-      const float rs = 1.0f / sqrtf(ss * (1.0f / CI) + 1e-5f);
+      const float2 st = row_ln_stats<LPR, CI>(v);
+      const float mu = st.x, rs = st.y;
       uint32_t h0, l0, h1, l1;
-      split2h(d0 * rs, d1 * rs, h0, l0); split2h(d2 * rs, d3 * rs, h1, l1);
+      split_f16x2_trunc((v.x - mu) * rs, (v.y - mu) * rs, h0, l0); split_f16x2_trunc((v.z - mu) * rs, (v.w - mu) * rs, h1, l1);
       *reinterpret_cast<uint2*>(&Xh[r * LD + lrow * 4]) = make_uint2(h0, h1);
       *reinterpret_cast<uint2*>(&Xl[r * LD + lrow * 4]) = make_uint2(l0, l1);
     }
-    asm volatile("cp.async.wait_group 0;\n" ::: "memory");
+    cp_async_wait<0>();
     __syncthreads();
     if (p0 + CHUNK < px_hi) fetch(p0 + CHUNK);
 
@@ -150,9 +114,7 @@ __global__ void __launch_bounds__(NTH, (CI == 64) ? 2 : 1) ca_wt_kernel(CaFusedA
         for (int n = 0; n < 8; ++n) {
           uint32_t b[4];
           ldsm4(b, ((lm & 2) ? Wl : Wh) + (ca * 64 + n * 8 + lr) * LD + ks * 16 + (lm & 1) * 8);
-          mma16816(q[n], al[ks], b[0], b[1]);
-          mma16816(q[n], ah[ks], b[2], b[3]);
-          mma16816(q[n], ah[ks], b[0], b[1]);
+          mma3(q[n], ah[ks], al[ks], b);
         }
       // per-lane partial sums over its two head dims: |q|^2, q.k, q.k_null for rows g (a) and g+8 (b) of every head
       const float2 nk = *reinterpret_cast<const float2*>(s_nk + ca * 8 + 2 * t);
@@ -271,15 +233,6 @@ int launch_ci(CaFusedArgs a, cudaStream_t st) {
 // a1 = SiLU(FiLM(GroupNorm(y))) + Wt (M x 32) * T_f (32 x co)      (first half of a conditioned ResnetBlock, U:366-380, 454-463)
 // A streaming kernel: Wt rows arrive straight in A-fragment order from global memory, the frame's table T_f sits in shared memory as
 // fp16 hi|lo, the K = 32 product is 6 mma.sync per 8 channels, and the epilogue reads y / writes a1 in 32-byte quad segments.
-// (x0, x1) -> packed fp16 hi pair / lo pair with the round-to-nearest 11-bit split of the wgmma GEMM producers (tc_common.cuh split_f16x2)
-__device__ __forceinline__ void split_rn(float x0, float x1, uint32_t& hi, uint32_t& lo) {
-  const float h0 = __uint_as_float((__float_as_uint(x0) + 0x1000u) & 0xFFFFE000u);
-  const float h1 = __uint_as_float((__float_as_uint(x1) + 0x1000u) & 0xFFFFE000u);
-  const __half2 h = __floats2half2_rn(h0, h1);
-  const __half2 l = __floats2half2_rn(x0 - h0, x1 - h1);
-  hi = *reinterpret_cast<const uint32_t*>(&h);
-  lo = *reinterpret_cast<const uint32_t*>(&l);
-}
 // transpose the 4 x 4 matrix M[lane t of the quad][i] in place: afterwards v[j] = what lane j held in its v[t]
 __device__ __forceinline__ void quad_transpose(uint32_t (&v)[4], int t) {
   {   // exchange 2 x 2 blocks with the lane two away
@@ -314,10 +267,7 @@ __global__ void __launch_bounds__(NTH, 3) gn_hcond_kernel(GnHcondArgs a) {
     const float* T = a.T + (size_t)f * 32 * a.ldbT;
     for (int i = tid; i < 32 * co; i += NTH) {
       const int k = i / co, c = i - k * co;
-      const float v = T[(size_t)k * a.ldbT + c];
-      const float h = __uint_as_float(__float_as_uint(v) & 0xFFFFE000u);
-      Th[c * TLD + k] = __float2half_rn(h);
-      Tl[c * TLD + k] = __float2half_rn(v - h);
+      split_f16_trunc(T[(size_t)k * a.ldbT + c], Th[c * TLD + k], Tl[c * TLD + k]);
     }
     const int clip = a.clips > 1 ? f % a.clips : 0;
     const double* gs = a.gn_stats + 16 * clip;
@@ -345,8 +295,8 @@ __global__ void __launch_bounds__(NTH, 3) gn_hcond_kernel(GnHcondArgs a) {
       const float2 v1 = __ldg(reinterpret_cast<const float2*>(a.Wt + row1 * 32 + ks * 16 + 2 * t));
       const float2 v2 = __ldg(reinterpret_cast<const float2*>(a.Wt + row0 * 32 + ks * 16 + 8 + 2 * t));
       const float2 v3 = __ldg(reinterpret_cast<const float2*>(a.Wt + row1 * 32 + ks * 16 + 8 + 2 * t));
-      split2h(v0.x, v0.y, ah[ks][0], al[ks][0]); split2h(v1.x, v1.y, ah[ks][1], al[ks][1]);
-      split2h(v2.x, v2.y, ah[ks][2], al[ks][2]); split2h(v3.x, v3.y, ah[ks][3], al[ks][3]);
+      split_f16x2_trunc(v0.x, v0.y, ah[ks][0], al[ks][0]); split_f16x2_trunc(v1.x, v1.y, ah[ks][1], al[ks][1]);
+      split_f16x2_trunc(v2.x, v2.y, ah[ks][2], al[ks][2]); split_f16x2_trunc(v3.x, v3.y, ah[ks][3], al[ks][3]);
     }
     const float* y0 = a.Y + row0 * a.ldy;
     const float* y1 = a.Y + row1 * a.ldy;
@@ -367,9 +317,7 @@ __global__ void __launch_bounds__(NTH, 3) gn_hcond_kernel(GnHcondArgs a) {
         for (int ks = 0; ks < 2; ++ks) {
           uint32_t b[4];
           ldsm4(b, ((lm & 2) ? Tl : Th) + (n0 + n * 8 + lr) * TLD + ks * 16 + (lm & 1) * 8);
-          mma16816(acc, al[ks], b[0], b[1]);
-          mma16816(acc, ah[ks], b[2], b[3]);
-          mma16816(acc, ah[ks], b[0], b[1]);
+          mma3(acc, ah[ks], al[ks], b);
         }
         const int c = n0 + n * 8 + 2 * t;
         const float2 al2 = *reinterpret_cast<const float2*>(s_al + c), be2 = *reinterpret_cast<const float2*>(s_be + c);
@@ -379,9 +327,9 @@ __global__ void __launch_bounds__(NTH, 3) gn_hcond_kernel(GnHcondArgs a) {
         if (!SPLIT) {
           *reinterpret_cast<float2*>(o0 + c) = make_float2(r00, r01);
           *reinterpret_cast<float2*>(o1 + c) = make_float2(r10, r11);
-        } else {
-          split_rn(r00, r01, sh[0][n], sl[0][n]);
-          split_rn(r10, r11, sh[1][n], sl[1][n]);
+        } else {                                         // the wgmma GEMM reads these planes in place of its producers' split
+          split_f16x2_rn(r00, r01, sh[0][n], sl[0][n]);
+          split_f16x2_rn(r10, r11, sh[1][n], sl[1][n]);
         }
       }
       if (SPLIT) {
@@ -435,19 +383,11 @@ int launch_ca_fused(const CaFusedArgs& a, int ci, cudaStream_t st) {
 void ca_fused_pack(const float* wq, int ci, std::vector<uint16_t>& W, float* inv_wscale) {
   float mx = 0.f;
   for (size_t i = 0; i < (size_t)ci * 192; ++i) mx = std::max(mx, std::fabs(wq[i]));
-  int e = 0;
-  if (mx > 0.f) std::frexp(mx, &e);
-  const float sc = std::ldexp(1.0f, 11 - e);
+  const float sc = f16_prescale(mx);
   *inv_wscale = 1.0f / sc;
   W.assign((size_t)2 * 192 * ci, 0);
   for (int n = 0; n < 192; ++n)
-    for (int k = 0; k < ci; ++k) {
-      const float v = wq[(size_t)k * 192 + n] * sc;
-      const __half hi = __float2half_rn(v);
-      const __half lo = __float2half_rn(v - __half2float(hi));
-      memcpy(&W[(size_t)n * ci + k], &hi, 2);
-      memcpy(&W[((size_t)192 + n) * ci + k], &lo, 2);
-    }
+    for (int k = 0; k < ci; ++k) split_f16_host(wq[(size_t)k * 192 + n] * sc, W[(size_t)n * ci + k], W[((size_t)192 + n) * ci + k]);
 }
 
 }  // namespace dawn

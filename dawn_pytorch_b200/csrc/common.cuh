@@ -60,15 +60,20 @@ __device__ __forceinline__ float quad_max(float v) {
   return v;
 }
 
-// cp.async 16 B with zero-fill when !pred (src-size = 0); src must still be a valid address.
-__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc, bool pred) {
-  unsigned s = (unsigned)__cvta_generic_to_shared(smem_dst);
-  int sz = pred ? 16 : 0;
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(s), "l"(gsrc), "r"(sz));
+// cp.async 16 B global -> shared
+__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc) {
+  const uint32_t s = (uint32_t)__cvta_generic_to_shared(smem_dst);
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(s), "l"(gsrc) : "memory");
 }
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
+// cp.async 16 B with zero-fill when !pred (src-size = 0); src must still be a valid address.
+__device__ __forceinline__ void cp_async16_zfill(void* smem_dst, const void* gsrc, bool pred) {
+  const uint32_t s = (uint32_t)__cvta_generic_to_shared(smem_dst);
+  const int sz = pred ? 16 : 0;
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(s), "l"(gsrc), "r"(sz) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
 template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N)); }
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N) : "memory"); }
 
 // 3xTF32 split: x ~= hi + lo with hi, lo representable in tf32 (10-bit mantissa), round-to-nearest (ties away),
 // done with full-rate integer ops: cvt.rna.tf32.f32 issues on a slow conversion pipe and was the measured

@@ -83,14 +83,14 @@ __global__ void __launch_bounds__(THREADS, 2) gemm_kernel(const GemmParams p) {
       int iy = a_iy[q] + dy, ix = a_ix[q] + dx;
       bool ok = (a_pix[q] >= 0) && (iy >= 0) && (iy < p.IH) && (ix >= 0) && (ix < p.IW);
       const float* src = ok ? p.A + (size_t)(a_pix[q] + iy * p.IW + ix) * p.lda + c0 + a_c4 : p.A;
-      cp_async16(as + ((tid >> 3) + 32 * q) * A_LD + a_c4, src, ok);
+      cp_async16_zfill(as + ((tid >> 3) + 32 * q) * A_LD + a_c4, src, ok);
     }
     float* bs = Bs + stage * BK * B_LD;
 #pragma unroll
     for (int q = 0; q < 2; ++q) {
       int idx = tid + q * THREADS;          // 0..511 : 32 rows x 16 float4
       int r = idx >> 4, c4 = (idx & 15) * 4;
-      cp_async16(bs + r * B_LD + c4, Bmat + (size_t)(kc * BK + r) * p.ldb + n0 + c4, true);
+      cp_async16_zfill(bs + r * B_LD + c4, Bmat + (size_t)(kc * BK + r) * p.ldb + n0 + c4, true);
     }
   };
 

@@ -1,7 +1,7 @@
 // Non-GEMM kernels of the DAWN denoising UNet: norms, conditioning tables, attention cores, layout.
-#include <cuda_fp16.h>
 #include <algorithm>
 #include "common.cuh"
+#include "f16x3.cuh"
 #include "kernels.cuh"
 
 namespace dawn {
@@ -310,7 +310,7 @@ int launch_ca_rstd(const float* gates, const float* G, int M, int P, float* Wt, 
 }
 
 // =========================================================================== fp16 hi | lo copy of an activation
-// x (M rows, C channels, row stride ld) -> dense hi[M][C], lo[M][C]: the same 11-bit split the wgmma GEMM producers apply on the fly
+// x (M rows, C channels, row stride ld) -> dense hi[M][C], lo[M][C]: the round-to-nearest split the wgmma GEMM producers apply on the fly
 __global__ void split_rows_kernel(const float* __restrict__ x, int ld, int C, long long M, uint2* __restrict__ hi,
                                   uint2* __restrict__ lo) {
   const int c4n = C >> 2;
@@ -319,14 +319,11 @@ __global__ void split_rows_kernel(const float* __restrict__ x, int ld, int C, lo
     const long long row = idx / c4n;
     const int c4 = (int)(idx - row * c4n);
     const float4 v = __ldg(reinterpret_cast<const float4*>(x + (size_t)row * ld) + c4);
-    const float h0 = __uint_as_float((__float_as_uint(v.x) + 0x1000u) & 0xFFFFE000u);
-    const float h1 = __uint_as_float((__float_as_uint(v.y) + 0x1000u) & 0xFFFFE000u);
-    const float h2 = __uint_as_float((__float_as_uint(v.z) + 0x1000u) & 0xFFFFE000u);
-    const float h3 = __uint_as_float((__float_as_uint(v.w) + 0x1000u) & 0xFFFFE000u);
-    const __half2 a = __floats2half2_rn(h0, h1), b = __floats2half2_rn(h2, h3);
-    const __half2 c = __floats2half2_rn(v.x - h0, v.y - h1), d = __floats2half2_rn(v.z - h2, v.w - h3);
-    hi[idx] = make_uint2(*reinterpret_cast<const uint32_t*>(&a), *reinterpret_cast<const uint32_t*>(&b));
-    lo[idx] = make_uint2(*reinterpret_cast<const uint32_t*>(&c), *reinterpret_cast<const uint32_t*>(&d));
+    uint32_t h0, l0, h1, l1;
+    split_f16x2_rn(v.x, v.y, h0, l0);
+    split_f16x2_rn(v.z, v.w, h1, l1);
+    hi[idx] = make_uint2(h0, h1);
+    lo[idx] = make_uint2(l0, l1);
   }
 }
 int launch_split_rows(const float* x, int ld, int C, long long M, void* hi, void* lo, cudaStream_t st) {

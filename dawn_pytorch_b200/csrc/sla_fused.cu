@@ -12,9 +12,9 @@
 #include <cuda_fp16.h>
 #include <algorithm>
 #include <cmath>
-#include <cstring>
 #include <vector>
 #include "common.cuh"
+#include "f16x3.cuh"
 #include "kernels.cuh"
 #include "sla_fused.cuh"
 
@@ -27,42 +27,6 @@ constexpr int CHUNK = 64;              // pixels staged per iteration
 constexpr int NTH = 256;               // 8 warps = 8 heads
 constexpr int PART = 64 + 32 * 32;     // floats per partial: m[32], l[32], ctx[32][32]
 constexpr float LOG2E = 1.4426950408889634f;
-
-__device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ void ldsm4(uint32_t (&r)[4], const __half* p) {
-  const uint32_t addr = (uint32_t)__cvta_generic_to_shared(p);
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];\n"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-__device__ __forceinline__ void cp_async_16(void* dst, const void* src) {
-  const uint32_t d = (uint32_t)__cvta_generic_to_shared(dst);
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" :: "r"(d), "l"(src) : "memory");
-}
-__device__ __forceinline__ float ex2(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;\n" : "=f"(y) : "f"(x));
-  return y;
-}
-// x = hi + lo: hi = leading 11 significant bits (exact in fp16), lo = fp16-rounded remainder
-__device__ __forceinline__ void split2h(float x0, float x1, uint32_t& hi, uint32_t& lo) {
-  const float h0 = __uint_as_float(__float_as_uint(x0) & 0xFFFFE000u);
-  const float h1 = __uint_as_float(__float_as_uint(x1) & 0xFFFFE000u);
-  const __half2 h = __floats2half2_rn(h0, h1);
-  const __half2 l = __floats2half2_rn(x0 - h0, x1 - h1);
-  hi = *reinterpret_cast<const uint32_t*>(&h);
-  lo = *reinterpret_cast<const uint32_t*>(&l);
-}
-// acc += a_lo*b_hi + a_hi*b_lo + a_hi*b_hi,  b = {hi k0-7, hi k8-15, lo k0-7, lo k8-15}
-__device__ __forceinline__ void mma3(float (&acc)[4], const uint32_t (&ah)[4], const uint32_t (&al)[4], const uint32_t (&b)[4]) {
-  mma16816(acc, al, b[0], b[1]);
-  mma16816(acc, ah, b[2], b[3]);
-  mma16816(acc, ah, b[0], b[1]);
-}
 
 __global__ void __launch_bounds__(NTH, 1) sla_ctx_kernel(SlaCtxArgs a) {
   extern __shared__ __align__(16) unsigned char sla_smem[];
@@ -81,9 +45,9 @@ __global__ void __launch_bounds__(NTH, 1) sla_ctx_kernel(SlaCtxArgs a) {
     const uint4* src = reinterpret_cast<const uint4*>(a.Wkv);
     for (int i = tid; i < 2 * 512 * C / 8; i += NTH) {
       const int r = i / (C / 8), c8 = i - r * (C / 8);              // r in [0, 1024): hi rows then lo rows
-      cp_async_16(Wh + r * LD + c8 * 8, src + i);
+      cp_async16(Wh + r * LD + c8 * 8, src + i);
     }
-    asm volatile("cp.async.commit_group;\n" ::: "memory");
+    cp_async_commit();
   }
 
   const int head = warp;
@@ -120,21 +84,14 @@ __global__ void __launch_bounds__(NTH, 1) sla_ctx_kernel(SlaCtxArgs a) {
     for (int i = 0; i < CHUNK / (NTH / 16); ++i) {
       const int r = i * (NTH / 16) + (tid >> 4);
       const float4 v = xin[i];
-      float s = (v.x + v.y) + (v.z + v.w);
-#pragma unroll
-      for (int o = 1; o < 16; o <<= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-      const float mu = s * (1.0f / C);
-      const float d0 = v.x - mu, d1 = v.y - mu, d2 = v.z - mu, d3 = v.w - mu;
-      float ss = (d0 * d0 + d1 * d1) + (d2 * d2 + d3 * d3);
-#pragma unroll
-      for (int o = 1; o < 16; o <<= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-      const float rs = 1.0f / sqrtf(ss * (1.0f / C) + 1e-5f);
+      const float2 st = row_ln_stats<16, C>(v);
+      const float mu = st.x, rs = st.y;
       uint32_t h0, l0, h1, l1;
-      split2h(d0 * rs, d1 * rs, h0, l0); split2h(d2 * rs, d3 * rs, h1, l1);
+      split_f16x2_trunc((v.x - mu) * rs, (v.y - mu) * rs, h0, l0); split_f16x2_trunc((v.z - mu) * rs, (v.w - mu) * rs, h1, l1);
       *reinterpret_cast<uint2*>(&Xh[r * LD + l16 * 4]) = make_uint2(h0, h1);
       *reinterpret_cast<uint2*>(&Xl[r * LD + l16 * 4]) = make_uint2(l0, l1);
     }
-    asm volatile("cp.async.wait_group 0;\n" ::: "memory");
+    cp_async_wait<0>();
     __syncthreads();
     if (p0 + CHUNK < px_hi) fetch(p0 + CHUNK);
 
@@ -193,18 +150,18 @@ __global__ void __launch_bounds__(NTH, 1) sla_ctx_kernel(SlaCtxArgs a) {
 #pragma unroll
         for (int j = 0; j < 4; ++j) { ctx[mi][j][0] *= c0; ctx[mi][j][1] *= c0; ctx[mi][j][2] *= c1; ctx[mi][j][3] *= c1; }
         // accumulator tiles (pixel n-tiles 0, 1) == A fragment (rows d, k = 16 pixels)
-        split2h(kt[mi][0][0], kt[mi][0][1], ph[mi][0], pl[mi][0]);
-        split2h(kt[mi][0][2], kt[mi][0][3], ph[mi][1], pl[mi][1]);
-        split2h(kt[mi][1][0], kt[mi][1][1], ph[mi][2], pl[mi][2]);
-        split2h(kt[mi][1][2], kt[mi][1][3], ph[mi][3], pl[mi][3]);
+        split_f16x2_trunc(kt[mi][0][0], kt[mi][0][1], ph[mi][0], pl[mi][0]);
+        split_f16x2_trunc(kt[mi][0][2], kt[mi][0][3], ph[mi][1], pl[mi][1]);
+        split_f16x2_trunc(kt[mi][1][0], kt[mi][1][1], ph[mi][2], pl[mi][2]);
+        split_f16x2_trunc(kt[mi][1][2], kt[mi][1][3], ph[mi][3], pl[mi][3]);
       }
       // ------------------------------------------------------------ ctx[d][e] += sum_px p[d][px] * v[e][px]
 #pragma unroll
       for (int j = 0; j < 4; ++j) {                     // e tile j = rows 8j..8j+7 of V^T: row tile j>>1, half j&1
         const int vi = j >> 1, hf = (j & 1) * 2;
         uint32_t b[4];                                  // {hi k0-7, hi k8-15, lo k0-7, lo k8-15}, k = pixel
-        split2h(vt[vi][0][hf] * a.inv_wscale, vt[vi][0][hf + 1] * a.inv_wscale, b[0], b[2]);
-        split2h(vt[vi][1][hf] * a.inv_wscale, vt[vi][1][hf + 1] * a.inv_wscale, b[1], b[3]);
+        split_f16x2_trunc(vt[vi][0][hf] * a.inv_wscale, vt[vi][0][hf + 1] * a.inv_wscale, b[0], b[2]);
+        split_f16x2_trunc(vt[vi][1][hf] * a.inv_wscale, vt[vi][1][hf + 1] * a.inv_wscale, b[1], b[3]);
 #pragma unroll
         for (int mi = 0; mi < 2; ++mi) {
           float acc[4] = {0.f, 0.f, 0.f, 0.f};          // RN accumulation across pixel groups outside the tensor core
@@ -298,16 +255,13 @@ __global__ void __launch_bounds__(NTH, 1) sla_out_kernel(SlaOutArgs a) {
     const uint4* src = reinterpret_cast<const uint4*>(a.Wq);
     for (int i = tid; i < 2 * 256 * C / 8; i += NTH) {
       const int r = i / (C / 8), c8 = i - r * (C / 8);              // r in [0, 512): hi rows then lo rows
-      cp_async_16(Wh + r * LD + c8 * 8, src + i);
+      cp_async16(Wh + r * LD + c8 * 8, src + i);
     }
-    asm volatile("cp.async.commit_group;\n" ::: "memory");
+    cp_async_commit();
     const float* Bf = a.Bf + (size_t)f * 256 * a.ldb;
     for (int i = tid; i < 256 * C; i += NTH) {
       const int k = i >> 6, c = i & 63;
-      const float v = Bf[(size_t)k * a.ldb + c];
-      const float h = __uint_as_float(__float_as_uint(v) & 0xFFFFE000u);
-      Bh[c * BLD + k] = __float2half_rn(h);
-      Bl[c * BLD + k] = __float2half_rn(v - h);
+      split_f16_trunc(Bf[(size_t)k * a.ldb + c], Bh[c * BLD + k], Bl[c * BLD + k]);
     }
     if (tid < C) s_bias[tid] = a.bias[tid];
   }
@@ -330,21 +284,14 @@ __global__ void __launch_bounds__(NTH, 1) sla_out_kernel(SlaOutArgs a) {
     for (int i = 0; i < OCH / (NTH / 16); ++i) {
       const int r = i * (NTH / 16) + (tid >> 4);
       const float4 v = xin[i];
-      float s = (v.x + v.y) + (v.z + v.w);
-#pragma unroll
-      for (int o = 1; o < 16; o <<= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-      const float mu = s * (1.0f / C);
-      const float d0 = v.x - mu, d1 = v.y - mu, d2 = v.z - mu, d3 = v.w - mu;
-      float ss = (d0 * d0 + d1 * d1) + (d2 * d2 + d3 * d3);
-#pragma unroll
-      for (int o = 1; o < 16; o <<= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-      const float rs = 1.0f / sqrtf(ss * (1.0f / C) + 1e-5f);
+      const float2 st = row_ln_stats<16, C>(v);
+      const float mu = st.x, rs = st.y;
       uint32_t h0, l0, h1, l1;
-      split2h(d0 * rs, d1 * rs, h0, l0); split2h(d2 * rs, d3 * rs, h1, l1);
+      split_f16x2_trunc((v.x - mu) * rs, (v.y - mu) * rs, h0, l0); split_f16x2_trunc((v.z - mu) * rs, (v.w - mu) * rs, h1, l1);
       *reinterpret_cast<uint2*>(&Xh[r * LD + l16 * 4]) = make_uint2(h0, h1);
       *reinterpret_cast<uint2*>(&Xl[r * LD + l16 * 4]) = make_uint2(l0, l1);
     }
-    asm volatile("cp.async.wait_group 0;\n" ::: "memory");
+    cp_async_wait<0>();
     __syncthreads();
     if (p0 + OCH < px_hi) fetch(p0 + OCH);
 
@@ -399,10 +346,10 @@ __global__ void __launch_bounds__(NTH, 1) sla_out_kernel(SlaOutArgs a) {
       uint32_t ph[2][4], pl[2][4];
 #pragma unroll
       for (int ks = 0; ks < 2; ++ks) {
-        split2h(q[2 * ks][0] * i0, q[2 * ks][1] * i0, ph[ks][0], pl[ks][0]);
-        split2h(q[2 * ks][2] * i1, q[2 * ks][3] * i1, ph[ks][1], pl[ks][1]);
-        split2h(q[2 * ks + 1][0] * i0, q[2 * ks + 1][1] * i0, ph[ks][2], pl[ks][2]);
-        split2h(q[2 * ks + 1][2] * i1, q[2 * ks + 1][3] * i1, ph[ks][3], pl[ks][3]);
+        split_f16x2_trunc(q[2 * ks][0] * i0, q[2 * ks][1] * i0, ph[ks][0], pl[ks][0]);
+        split_f16x2_trunc(q[2 * ks][2] * i1, q[2 * ks][3] * i1, ph[ks][1], pl[ks][1]);
+        split_f16x2_trunc(q[2 * ks + 1][0] * i0, q[2 * ks + 1][1] * i0, ph[ks][2], pl[ks][2]);
+        split_f16x2_trunc(q[2 * ks + 1][2] * i1, q[2 * ks + 1][3] * i1, ph[ks][3], pl[ks][3]);
       }
 #pragma unroll
       for (int n = 0; n < 8; ++n) {
@@ -488,40 +435,26 @@ int launch_sla_out_fused(const SlaOutArgs& a_in, cudaStream_t st) {
 void sla_out_pack(const float* wqkv, std::vector<uint16_t>& W, float* inv_wscale) {
   float mx = 0.f;
   for (size_t i = 0; i < (size_t)256 * C; ++i) mx = std::max(mx, std::fabs(wqkv[i]));
-  int e = 0;
-  if (mx > 0.f) std::frexp(mx, &e);
-  const float sc = std::ldexp(1.0f, 11 - e);
+  const float sc = f16_prescale(mx);
   *inv_wscale = 1.0f / sc;
   W.assign((size_t)2 * 256 * C, 0);
   for (int r = 0; r < 256; ++r)
-    for (int k = 0; k < C; ++k) {
-      const float v = wqkv[(size_t)r * C + k] * sc;
-      const __half hi = __float2half_rn(v);
-      const __half lo = __float2half_rn(v - __half2float(hi));
-      memcpy(&W[(size_t)r * C + k], &hi, 2);
-      memcpy(&W[((size_t)256 + r) * C + k], &lo, 2);
-    }
+    for (int k = 0; k < C; ++k) split_f16_host(wqkv[(size_t)r * C + k] * sc, W[(size_t)r * C + k], W[((size_t)256 + r) * C + k]);
 }
 
 // wkv: rows 256..767 of the gamma-folded to_qkv weight ([768][64]); output [hi|lo][8 heads x (k 32 | v 32)][64] fp16, power-of-two pre-scale
 void sla_fused_pack(const float* wqkv, std::vector<uint16_t>& W, float* inv_wscale) {
   float mx = 0.f;
   for (size_t i = (size_t)256 * C; i < (size_t)768 * C; ++i) mx = std::max(mx, std::fabs(wqkv[i]));
-  int e = 0;
-  if (mx > 0.f) std::frexp(mx, &e);
-  const float sc = std::ldexp(1.0f, 11 - e);
+  const float sc = f16_prescale(mx);
   *inv_wscale = 1.0f / sc;
   W.assign((size_t)2 * 512 * C, 0);
   for (int h = 0; h < 8; ++h)
     for (int part = 0; part < 2; ++part)
       for (int r = 0; r < 32; ++r)
         for (int k = 0; k < C; ++k) {
-          const float v = wqkv[(size_t)(256 + part * 256 + h * 32 + r) * C + k] * sc;
-          const __half hi = __float2half_rn(v);
-          const __half lo = __float2half_rn(v - __half2float(hi));
           const size_t row = (size_t)h * 64 + part * 32 + r;
-          memcpy(&W[row * C + k], &hi, 2);
-          memcpy(&W[((size_t)512 + row) * C + k], &lo, 2);
+          split_f16_host(wqkv[(size_t)(256 + part * 256 + h * 32 + r) * C + k] * sc, W[row * C + k], W[((size_t)512 + row) * C + k]);
         }
 }
 

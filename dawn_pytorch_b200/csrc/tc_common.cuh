@@ -1,7 +1,6 @@
 // Shared device helpers of the wgmma kernels (tc_gemm.cu, tc_conv3.cu, temporal_fused.cu): mbarrier / bulk-copy / wgmma PTX wrappers,
-// shared-memory matrix descriptors, the fp16 hi/lo split and the coalesced row store.
+// shared-memory matrix descriptors and the coalesced row store.
 #pragma once
-#include <cuda_fp16.h>
 #include <type_traits>
 #include "common.cuh"
 
@@ -166,19 +165,6 @@ __device__ __forceinline__ void stage_fragment(float* stage, int r0, const float
 
 // byte offset of 16-byte chunk c (0..7) of row r inside a swizzled panel
 __device__ __forceinline__ uint32_t swz(int r, int c) { return (uint32_t)((r >> 3) * 1024 + (r & 7) * 128 + ((c ^ (r & 7)) << 4)); }
-
-// (x0, x1) -> packed fp16 hi pair and fp16 lo pair.  hi is rounded to 11 significant bits in fp32 with two integer
-// ops (so its fp16 conversion is exact and no f16->f32 unpack is needed: the conversion pipe was the measured
-// producer bottleneck); lo = x - hi is exact in fp32 and rounded once to fp16.  Below fp16's normal range the
-// conversions go subnormal: absolute error <= 2^-25, irrelevant next to O(1) outputs.
-__device__ __forceinline__ void split_f16x2(float x0, float x1, uint32_t& hi, uint32_t& lo) {
-  const float h0 = __uint_as_float((__float_as_uint(x0) + 0x1000u) & 0xFFFFE000u);
-  const float h1 = __uint_as_float((__float_as_uint(x1) + 0x1000u) & 0xFFFFE000u);
-  const __half2 h = __floats2half2_rn(h0, h1);
-  const __half2 l = __floats2half2_rn(x0 - h0, x1 - h1);
-  hi = *reinterpret_cast<const uint32_t*>(&h);
-  lo = *reinterpret_cast<const uint32_t*>(&l);
-}
 
 // Store this warp's 32 rows x 64 columns (row-per-lane registers) to global memory with full-sector transactions:
 // 16 columns at a time go through a per-warp shared-memory buffer so that one store instruction writes 8 rows x 64

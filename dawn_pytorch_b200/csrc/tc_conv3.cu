@@ -28,6 +28,7 @@
 #include <map>
 #include <tuple>
 #include "common.cuh"
+#include "f16x3.cuh"
 #include "gemm.cuh"
 #include "tc_common.cuh"
 #include "tc_gemm.cuh"
@@ -214,10 +215,10 @@ __device__ __forceinline__ void tc_conv3_body(const GemmParams& p, const float* 
             const int r = lr + fr * (PAIR_ROW_B - FRAME_ROWS);
             if (lr < FRAME_ROWS * (PAIR ? 2 : 1)) {
               uint32_t h[4], l[4];
-              split_f16x2(a.x, a.y, h[0], l[0]);
-              split_f16x2(a.z, a.w, h[1], l[1]);
-              split_f16x2(b.x, b.y, h[2], l[2]);
-              split_f16x2(b.z, b.w, h[3], l[3]);
+              split_f16x2_rn(a.x, a.y, h[0], l[0]);
+              split_f16x2_rn(a.z, a.w, h[1], l[1]);
+              split_f16x2_rn(b.x, b.y, h[2], l[2]);
+              split_f16x2_rn(b.z, b.w, h[3], l[3]);
               const uint32_t off = swz(r, c16);                // absolute-row swizzle (halo base is 1024-byte aligned)
               *reinterpret_cast<uint4*>(a_hi + off) = make_uint4(h[0], h[1], h[2], h[3]);
               *reinterpret_cast<uint4*>(a_lo + off) = make_uint4(l[0], l[1], l[2], l[3]);

@@ -19,6 +19,7 @@
 //     MMAs in flight while the next is issued, wait_group 0 comes only before the drain.
 #include <cuda_fp16.h>
 #include "common.cuh"
+#include "f16x3.cuh"
 #include "gemm.cuh"
 #include "tc_common.cuh"
 #include "tc_gemm.cuh"
@@ -160,10 +161,10 @@ __global__ void __launch_bounds__(Cfg<BN>::NTHREADS, 1) tc_gemm_kernel(const Gem
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
         uint32_t h[4], l[4];
-        split_f16x2(v[2 * q].x, v[2 * q].y, h[0], l[0]);
-        split_f16x2(v[2 * q].z, v[2 * q].w, h[1], l[1]);
-        split_f16x2(v[2 * q + 1].x, v[2 * q + 1].y, h[2], l[2]);
-        split_f16x2(v[2 * q + 1].z, v[2 * q + 1].w, h[3], l[3]);
+        split_f16x2_rn(v[2 * q].x, v[2 * q].y, h[0], l[0]);
+        split_f16x2_rn(v[2 * q].z, v[2 * q].w, h[1], l[1]);
+        split_f16x2_rn(v[2 * q + 1].x, v[2 * q + 1].y, h[2], l[2]);
+        split_f16x2_rn(v[2 * q + 1].z, v[2 * q + 1].w, h[3], l[3]);
         const uint32_t off = swz(r0 + 32 * q, c16);
         *reinterpret_cast<uint4*>(a_hi + off) = make_uint4(h[0], h[1], h[2], h[3]);
         *reinterpret_cast<uint4*>(a_lo + off) = make_uint4(l[0], l[1], l[2], l[3]);
@@ -587,23 +588,18 @@ size_t tc_pack_weights(const float* Bkn, int K, int N, int ldb, std::vector<floa
   float mx = 0.f;
   for (int k = 0; k < K; ++k)
     for (int n = 0; n < N; ++n) mx = std::max(mx, std::fabs(Bkn[(size_t)k * ldb + n]));
-  int e = 0;
-  if (mx > 0.f) { std::frexp(mx, &e); }                        // mx = m * 2^e, m in [0.5, 1)
-  const float sc = std::ldexp(1.0f, 11 - e);                   // max |w| * sc in [1024, 2048)
+  const float sc = f16_prescale(mx);
   *scale = sc;
   out.assign(((size_t)NT * KC * 2 * PH + 1) / 2, 0.f);
-  __half* base = reinterpret_cast<__half*>(out.data());
+  uint16_t* base = reinterpret_cast<uint16_t*>(out.data());
   for (int nt = 0; nt < NT; ++nt)
     for (int kc = 0; kc < KC; ++kc) {
-      __half* hi = base + ((size_t)nt * KC + kc) * 2 * PH;
-      __half* lo = hi + PH;
+      uint16_t* hi = base + ((size_t)nt * KC + kc) * 2 * PH;
+      uint16_t* lo = hi + PH;
       for (int n = 0; n < BN; ++n)
         for (int k = 0; k < BKP; ++k) {
-          const float w = Bkn[(size_t)(kc * BKP + k) * ldb + nt * BN + n] * sc;
-          const __half h = __float2half_rn(w);
-          const __half l = __float2half_rn(w - __half2float(h));
           const int off = (n >> 3) * 512 + (n & 7) * 64 + (((k >> 3) ^ (n & 7)) << 3) + (k & 7);   // in fp16 elements
-          hi[off] = h; lo[off] = l;
+          split_f16_host(Bkn[(size_t)(kc * BKP + k) * ldb + nt * BN + n] * sc, hi[off], lo[off]);
         }
     }
   return out.size();

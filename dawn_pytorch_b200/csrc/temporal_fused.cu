@@ -14,10 +14,10 @@
 // operand fragments come from shared memory through ldmatrix.x4 (hi and lo halves of a B fragment in one instruction).
 #include <cuda_fp16.h>
 #include <cmath>
-#include <cstring>
 #include <vector>
 #include <algorithm>
 #include "common.cuh"
+#include "f16x3.cuh"
 #include "kernels.cuh"
 #include "tc_common.cuh"
 #include "temporal_fused.cuh"
@@ -34,50 +34,6 @@ constexpr int NTH = 512;
 constexpr int NWARP = NTH / 32;
 constexpr int W_STAGE = 2 * 96 * W_LD + 2 * 64 * WO_LD;      // halfs per weight stage
 constexpr float LOG2E = 1.4426950408889634f;
-
-__device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-// four 8x8 b16 matrices; lane l supplies the address of row (l & 7) of matrix (l >> 3)
-__device__ __forceinline__ void ldsm4(uint32_t (&r)[4], const __half* p) {
-  const uint32_t addr = (uint32_t)__cvta_generic_to_shared(p);
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];\n"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-__device__ __forceinline__ void ldsm4_trans(uint32_t (&r)[4], const __half* p) {
-  const uint32_t addr = (uint32_t)__cvta_generic_to_shared(p);
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];\n"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-__device__ __forceinline__ void cp_async_16(void* dst, const void* src) {
-  const uint32_t d = (uint32_t)__cvta_generic_to_shared(dst);
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" :: "r"(d), "l"(src) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
-__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;\n" ::: "memory"); }
-__device__ __forceinline__ float ex2(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;\n" : "=f"(y) : "f"(x));
-  return y;
-}
-// x = hi + lo with hi the leading 11 significant bits (truncated, exact in fp16) and lo the fp16-rounded remainder
-__device__ __forceinline__ void split2h(float x0, float x1, uint32_t& hi, uint32_t& lo) {
-  const float h0 = __uint_as_float(__float_as_uint(x0) & 0xFFFFE000u);
-  const float h1 = __uint_as_float(__float_as_uint(x1) & 0xFFFFE000u);
-  const __half2 h = __floats2half2_rn(h0, h1);
-  const __half2 l = __floats2half2_rn(x0 - h0, x1 - h1);
-  hi = *reinterpret_cast<const uint32_t*>(&h);
-  lo = *reinterpret_cast<const uint32_t*>(&l);
-}
-// 3-term split product: acc += a_lo*b_hi + a_hi*b_lo + a_hi*b_hi, b = {hi k0-7, hi k8-15, lo k0-7, lo k8-15}
-__device__ __forceinline__ void mma3(float (&acc)[4], const uint32_t (&ah)[4], const uint32_t (&al)[4], const uint32_t (&b)[4]) {
-  mma16816(acc, al, b[0], b[1]);
-  mma16816(acc, ah, b[2], b[3]);
-  mma16816(acc, ah, b[0], b[1]);
-}
 
 // Banded (+-band, + relative bias) softmax attention of the 16-query tile i0 .. i0+15 of one warp against K_h and V_h in shared
 // memory (FlashAttention-2 style, as attn_tc.cu): scores in the log2 domain, 32-key blocks, each block's P*V added to the output
@@ -152,10 +108,10 @@ __device__ __forceinline__ void banded_attention(const uint32_t (&qh)[2][4], con
 #pragma unroll
     for (int ks = 0; ks < 2; ++ks) {
       uint32_t ph[4], pl[4];                            // P's accumulator tiles (2ks, 2ks+1) == A fragment of k16 step ks
-      split2h(s[2 * ks][0], s[2 * ks][1], ph[0], pl[0]);
-      split2h(s[2 * ks][2], s[2 * ks][3], ph[1], pl[1]);
-      split2h(s[2 * ks + 1][0], s[2 * ks + 1][1], ph[2], pl[2]);
-      split2h(s[2 * ks + 1][2], s[2 * ks + 1][3], ph[3], pl[3]);
+      split_f16x2_trunc(s[2 * ks][0], s[2 * ks][1], ph[0], pl[0]);
+      split_f16x2_trunc(s[2 * ks][2], s[2 * ks][3], ph[1], pl[1]);
+      split_f16x2_trunc(s[2 * ks + 1][0], s[2 * ks + 1][1], ph[2], pl[2]);
+      split_f16x2_trunc(s[2 * ks + 1][2], s[2 * ks + 1][3], ph[3], pl[3]);
 #pragma unroll
       for (int n = 0; n < 4; ++n) {
         uint32_t b[4];
@@ -172,10 +128,10 @@ __device__ __forceinline__ void banded_attention(const uint32_t (&qh)[2][4], con
   const float inv0 = 1.0f / l0, inv1 = 1.0f / l1;
 #pragma unroll
   for (int ks = 0; ks < 2; ++ks) {
-    split2h(o[2 * ks][0] * inv0, o[2 * ks][1] * inv0, oh[ks][0], ol[ks][0]);
-    split2h(o[2 * ks][2] * inv1, o[2 * ks][3] * inv1, oh[ks][1], ol[ks][1]);
-    split2h(o[2 * ks + 1][0] * inv0, o[2 * ks + 1][1] * inv0, oh[ks][2], ol[ks][2]);
-    split2h(o[2 * ks + 1][2] * inv1, o[2 * ks + 1][3] * inv1, oh[ks][3], ol[ks][3]);
+    split_f16x2_trunc(o[2 * ks][0] * inv0, o[2 * ks][1] * inv0, oh[ks][0], ol[ks][0]);
+    split_f16x2_trunc(o[2 * ks][2] * inv1, o[2 * ks][3] * inv1, oh[ks][1], ol[ks][1]);
+    split_f16x2_trunc(o[2 * ks + 1][0] * inv0, o[2 * ks + 1][1] * inv0, oh[ks][2], ol[ks][2]);
+    split_f16x2_trunc(o[2 * ks + 1][2] * inv1, o[2 * ks + 1][3] * inv1, oh[ks][3], ol[ks][3]);
   }
 }
 
@@ -228,18 +184,11 @@ __global__ void __launch_bounds__(NTH, 1) temporal_fused_kernel(TemporalFusedArg
       const int f = f0 + (tid >> 4);
       float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
       if (f < F) v = __ldg(reinterpret_cast<const float4*>(a.x + ((size_t)f * a.P + pix) * a.ldx) + l16);
-      float s = (v.x + v.y) + (v.z + v.w);
-#pragma unroll
-      for (int o = 1; o < 16; o <<= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-      const float mu = s * (1.0f / C);
-      const float d0 = v.x - mu, d1 = v.y - mu, d2 = v.z - mu, d3 = v.w - mu;
-      float ss = (d0 * d0 + d1 * d1) + (d2 * d2 + d3 * d3);
-#pragma unroll
-      for (int o = 1; o < 16; o <<= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
+      const float2 st = row_ln_stats<16, C>(v);
       if (f < Fp) {
-        if (l16 == 0) { s_stat[2 * f] = mu; s_stat[2 * f + 1] = 1.0f / sqrtf(ss * (1.0f / C) + 1e-5f); }
+        if (l16 == 0) { s_stat[2 * f] = st.x; s_stat[2 * f + 1] = st.y; }
         uint32_t h0, l0, h1, l1;
-        split2h(v.x, v.y, h0, l0); split2h(v.z, v.w, h1, l1);
+        split_f16x2_trunc(v.x, v.y, h0, l0); split_f16x2_trunc(v.z, v.w, h1, l1);
         *reinterpret_cast<uint2*>(&Xh[f * X_LD + l16 * 4]) = make_uint2(h0, h1);
         *reinterpret_cast<uint2*>(&Xl[f * X_LD + l16 * 4]) = make_uint2(l0, l1);
       }
@@ -269,13 +218,13 @@ __global__ void __launch_bounds__(NTH, 1) temporal_fused_kernel(TemporalFusedArg
     const uint4* src = reinterpret_cast<const uint4*>(a.Wqkv + (size_t)head * 2 * 96 * C);       // hi then lo, dense [96][64]
     for (int i = tid; i < 2 * 96 * C / 8; i += NTH) {
       const int r = i / (C / 8), c8 = i - r * (C / 8);                                             // r in [0, 192): hi rows then lo rows
-      cp_async_16(dst + r * W_LD + c8 * 8, src + i);
+      cp_async16(dst + r * W_LD + c8 * 8, src + i);
     }
     const uint4* so = reinterpret_cast<const uint4*>(a.Wout + (size_t)head * 2 * 64 * 32);        // hi then lo, dense [64][32]
     __half* od = dst + 2 * 96 * W_LD;
     for (int i = tid; i < 2 * 64 * 32 / 8; i += NTH) {
       const int r = i >> 2, c8 = i & 3;                                                            // r in [0, 128)
-      cp_async_16(od + r * WO_LD + c8 * 8, so + i);
+      cp_async16(od + r * WO_LD + c8 * 8, so + i);
     }
     cp_async_commit();
   };
@@ -320,14 +269,14 @@ __global__ void __launch_bounds__(NTH, 1) temporal_fused_kernel(TemporalFusedArg
   if (nbuf == 2) stage_weights(0, Wst);
   for (int head = 0; head < 8; ++head) {
     if (nbuf == 2) {
-      cp_async_wait_all();
+      cp_async_wait<0>();
       __syncthreads();                                  // this head's weights landed; previous head's K/V and other stage are free
       Wh = Wst + (head & 1) * W_STAGE;
       if (head + 1 < 8) stage_weights(head + 1, Wst + ((head + 1) & 1) * W_STAGE);
     } else {
       __syncthreads();
       stage_weights(head, Wst);
-      cp_async_wait_all();
+      cp_async_wait<0>();
       __syncthreads();
     }
     const __half* Oh = Wh + 2 * 96 * W_LD;              // Wout_h: hi rows [0, 64), lo rows [64, 128)
@@ -341,7 +290,7 @@ __global__ void __launch_bounds__(NTH, 1) temporal_fused_kernel(TemporalFusedArg
 #pragma unroll
       for (int n = 0; n < 4; ++n) {
         uint32_t h0, l0, h1, l1;
-        split2h(acc[n][0], acc[n][1], h0, l0); split2h(acc[n][2], acc[n][3], h1, l1);
+        split_f16x2_trunc(acc[n][0], acc[n][1], h0, l0); split_f16x2_trunc(acc[n][2], acc[n][3], h1, l1);
         *reinterpret_cast<uint32_t*>(&Kh[fr0 * K_LD + n * 8 + 2 * t]) = h0;
         *reinterpret_cast<uint32_t*>(&Kl[fr0 * K_LD + n * 8 + 2 * t]) = l0;
         *reinterpret_cast<uint32_t*>(&Kh[fr1 * K_LD + n * 8 + 2 * t]) = h1;
@@ -351,7 +300,7 @@ __global__ void __launch_bounds__(NTH, 1) temporal_fused_kernel(TemporalFusedArg
 #pragma unroll
       for (int n = 0; n < 4; ++n) {
         uint32_t h0, l0, h1, l1;
-        split2h(acc[n][0], acc[n][1], h0, l0); split2h(acc[n][2], acc[n][3], h1, l1);
+        split_f16x2_trunc(acc[n][0], acc[n][1], h0, l0); split_f16x2_trunc(acc[n][2], acc[n][3], h1, l1);
         *reinterpret_cast<uint32_t*>(&Vh[fr0 * K_LD + n * 8 + 2 * t]) = h0;
         *reinterpret_cast<uint32_t*>(&Vl[fr0 * K_LD + n * 8 + 2 * t]) = l0;
         *reinterpret_cast<uint32_t*>(&Vh[fr1 * K_LD + n * 8 + 2 * t]) = h1;
@@ -369,10 +318,10 @@ __global__ void __launch_bounds__(NTH, 1) temporal_fused_kernel(TemporalFusedArg
         for (int c = 0; c < 4; ++c) acc[n][c] *= LOG2E;   // scores live in the log2 domain: softmax through ex2
 #pragma unroll
       for (int ks = 0; ks < 2; ++ks) {                    // accumulator tiles (2ks, 2ks+1) == A fragment of k16 step ks
-        split2h(acc[2 * ks][0], acc[2 * ks][1], qh[ks][0], ql[ks][0]);
-        split2h(acc[2 * ks][2], acc[2 * ks][3], qh[ks][1], ql[ks][1]);
-        split2h(acc[2 * ks + 1][0], acc[2 * ks + 1][1], qh[ks][2], ql[ks][2]);
-        split2h(acc[2 * ks + 1][2], acc[2 * ks + 1][3], qh[ks][3], ql[ks][3]);
+        split_f16x2_trunc(acc[2 * ks][0], acc[2 * ks][1], qh[ks][0], ql[ks][0]);
+        split_f16x2_trunc(acc[2 * ks][2], acc[2 * ks][3], qh[ks][1], ql[ks][1]);
+        split_f16x2_trunc(acc[2 * ks + 1][0], acc[2 * ks + 1][1], qh[ks][2], ql[ks][2]);
+        split_f16x2_trunc(acc[2 * ks + 1][2], acc[2 * ks + 1][3], qh[ks][3], ql[ks][3]);
       }
     }
     __syncthreads();                                    // K_h, V_h^T of every frame are in shared memory
@@ -447,17 +396,10 @@ __global__ void __launch_bounds__(NTH, 1) temporal_fused_wg_kernel(TemporalFused
       const int f = f0 + (tid >> 4);
       float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
       if (f < F) v = __ldg(reinterpret_cast<const float4*>(a.x + ((size_t)f * a.P + pix) * a.ldx) + l16);
-      float s = (v.x + v.y) + (v.z + v.w);
-#pragma unroll
-      for (int o = 1; o < 16; o <<= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-      const float mu = s * (1.0f / C);
-      const float d0 = v.x - mu, d1 = v.y - mu, d2 = v.z - mu, d3 = v.w - mu;
-      float ss = (d0 * d0 + d1 * d1) + (d2 * d2 + d3 * d3);
-#pragma unroll
-      for (int o = 1; o < 16; o <<= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-      if (l16 == 0) { s_stat[2 * f] = mu; s_stat[2 * f + 1] = f < F ? 1.0f / sqrtf(ss * (1.0f / C) + 1e-5f) : 0.f; }
+      const float2 st = row_ln_stats<16, C>(v);
+      if (l16 == 0) { s_stat[2 * f] = st.x; s_stat[2 * f + 1] = f < F ? st.y : 0.f; }
       uint32_t h0, l0, h1, l1;
-      split2h(v.x, v.y, h0, l0); split2h(v.z, v.w, h1, l1);
+      split_f16x2_trunc(v.x, v.y, h0, l0); split_f16x2_trunc(v.z, v.w, h1, l1);
       const uint32_t off = tc::swz(f, l16 >> 1) + (l16 & 1) * 8;
       *reinterpret_cast<uint2*>(Xh + off) = make_uint2(h0, h1);
       *reinterpret_cast<uint2*>(Xl + off) = make_uint2(l0, l1);
@@ -481,16 +423,16 @@ __global__ void __launch_bounds__(NTH, 1) temporal_fused_wg_kernel(TemporalFused
   // stream one head's weights into a stage: the packed dense images (as temporal_fused_kernel reads them) land in swizzled panels
   auto stage_weights = [&](int head, uint8_t* dst) {
     const uint4* src = reinterpret_cast<const uint4*>(a.Wqkv + (size_t)head * 2 * 96 * C);       // hi then lo, dense [96][64]
-    for (int i = tid; i < 2 * 96 * C / 8; i += NTH) cp_async_16(dst + tc::swz(i >> 3, i & 7), src + i);   // lo panel = rows 96..
+    for (int i = tid; i < 2 * 96 * C / 8; i += NTH) cp_async16(dst + tc::swz(i >> 3, i & 7), src + i);   // lo panel = rows 96..
     const uint4* so = reinterpret_cast<const uint4*>(a.Wout + (size_t)head * 2 * 64 * 32);        // hi then lo, dense [64][32]
     for (int i = tid; i < 2 * 64 * 32 / 8; i += NTH)
-      cp_async_16(dst + 2 * WG_WQ + tc::swz((i >> 2) & 63, (i >> 8) * 4 + (i & 3)), so + i);
+      cp_async16(dst + 2 * WG_WQ + tc::swz((i >> 2) & 63, (i >> 8) * 4 + (i & 3)), so + i);
     cp_async_commit();
   };
 
   stage_weights(0, Wst);
   for (int head = 0; head < 8; ++head) {
-    cp_async_wait_all();
+    cp_async_wait<0>();
     tc::fence_proxy_async();                            // generic-proxy writes (X panels, this head's weights) -> wgmma reads
     __syncthreads();                                    // this head's weights landed; previous head's K/V and other stage are free
     const uint8_t* Ws = Wst + (head & 1) * WG_STAGE;
@@ -540,12 +482,12 @@ __global__ void __launch_bounds__(NTH, 1) temporal_fused_wg_kernel(TemporalFused
 #pragma unroll
         for (int n = 0; n < 4; ++n) {
           uint32_t h0, l0, h1, l1;
-          split2h(d[16 + 4 * n], d[16 + 4 * n + 1], h0, l0); split2h(d[16 + 4 * n + 2], d[16 + 4 * n + 3], h1, l1);
+          split_f16x2_trunc(d[16 + 4 * n], d[16 + 4 * n + 1], h0, l0); split_f16x2_trunc(d[16 + 4 * n + 2], d[16 + 4 * n + 3], h1, l1);
           *reinterpret_cast<uint32_t*>(&Kh[r0 * K_LD + n * 8 + 2 * t]) = h0;
           *reinterpret_cast<uint32_t*>(&Kl[r0 * K_LD + n * 8 + 2 * t]) = l0;
           *reinterpret_cast<uint32_t*>(&Kh[r1 * K_LD + n * 8 + 2 * t]) = h1;
           *reinterpret_cast<uint32_t*>(&Kl[r1 * K_LD + n * 8 + 2 * t]) = l1;
-          split2h(d[32 + 4 * n], d[32 + 4 * n + 1], h0, l0); split2h(d[32 + 4 * n + 2], d[32 + 4 * n + 3], h1, l1);
+          split_f16x2_trunc(d[32 + 4 * n], d[32 + 4 * n + 1], h0, l0); split_f16x2_trunc(d[32 + 4 * n + 2], d[32 + 4 * n + 3], h1, l1);
           *reinterpret_cast<uint32_t*>(&Vh[r0 * K_LD + n * 8 + 2 * t]) = h0;
           *reinterpret_cast<uint32_t*>(&Vl[r0 * K_LD + n * 8 + 2 * t]) = l0;
           *reinterpret_cast<uint32_t*>(&Vh[r1 * K_LD + n * 8 + 2 * t]) = h1;
@@ -557,10 +499,10 @@ __global__ void __launch_bounds__(NTH, 1) temporal_fused_wg_kernel(TemporalFused
         for (int i = 0; i < 16; ++i) d[i] *= LOG2E;     // scores live in the log2 domain: softmax through ex2
 #pragma unroll
         for (int ks = 0; ks < 2; ++ks) {                // accumulator tiles (2ks, 2ks+1) == A fragment of k16 step ks
-          split2h(d[8 * ks], d[8 * ks + 1], qh[ks][0], ql[ks][0]);
-          split2h(d[8 * ks + 2], d[8 * ks + 3], qh[ks][1], ql[ks][1]);
-          split2h(d[8 * ks + 4], d[8 * ks + 5], qh[ks][2], ql[ks][2]);
-          split2h(d[8 * ks + 6], d[8 * ks + 7], qh[ks][3], ql[ks][3]);
+          split_f16x2_trunc(d[8 * ks], d[8 * ks + 1], qh[ks][0], ql[ks][0]);
+          split_f16x2_trunc(d[8 * ks + 2], d[8 * ks + 3], qh[ks][1], ql[ks][1]);
+          split_f16x2_trunc(d[8 * ks + 4], d[8 * ks + 5], qh[ks][2], ql[ks][2]);
+          split_f16x2_trunc(d[8 * ks + 6], d[8 * ks + 7], qh[ks][3], ql[ks][3]);
         }
       }
     }
@@ -645,17 +587,10 @@ void temporal_fused_pack(const float* wqkv, const float* wout, std::vector<uint1
   auto pow2scale = [](const float* p, size_t n) {
     float mx = 0.f;
     for (size_t i = 0; i < n; ++i) mx = std::max(mx, std::fabs(p[i]));
-    int e = 0;
-    if (mx > 0.f) std::frexp(mx, &e);
-    return std::ldexp(1.0f, 11 - e);
+    return f16_prescale(mx);
   };
   const float sq = pow2scale(wqkv, (size_t)768 * 64), so = pow2scale(wout, (size_t)64 * 256);
   *inv_wscale = 1.0f / sq; *inv_oscale = 1.0f / so;
-  auto put = [](uint16_t* hi, uint16_t* lo, float v) {
-    const __half h = __float2half_rn(v);
-    const __half l = __float2half_rn(v - __half2float(h));
-    memcpy(hi, &h, 2); memcpy(lo, &l, 2);
-  };
   Wq.assign((size_t)8 * 2 * 96 * 64, 0);
   Wo.assign((size_t)8 * 2 * 64 * 32, 0);
   for (int h = 0; h < 8; ++h) {
@@ -663,10 +598,10 @@ void temporal_fused_pack(const float* wqkv, const float* wout, std::vector<uint1
     for (int part = 0; part < 3; ++part)
       for (int r = 0; r < 32; ++r)
         for (int k = 0; k < 64; ++k)
-          put(qh + (part * 32 + r) * 64 + k, ql + (part * 32 + r) * 64 + k, wqkv[(size_t)(part * 256 + h * 32 + r) * 64 + k] * sq);
+          split_f16_host(wqkv[(size_t)(part * 256 + h * 32 + r) * 64 + k] * sq, qh[(part * 32 + r) * 64 + k], ql[(part * 32 + r) * 64 + k]);
     uint16_t* oh = Wo.data() + (size_t)h * 2 * 64 * 32; uint16_t* ol = oh + 64 * 32;
     for (int c = 0; c < 64; ++c)
-      for (int d = 0; d < 32; ++d) put(oh + c * 32 + d, ol + c * 32 + d, wout[(size_t)c * 256 + h * 32 + d] * so);
+      for (int d = 0; d < 32; ++d) split_f16_host(wout[(size_t)c * 256 + h * 32 + d] * so, oh[c * 32 + d], ol[c * 32 + d]);
   }
 }
 

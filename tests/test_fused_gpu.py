@@ -10,7 +10,7 @@ values of the same data, so the bound follows the conditioning of each case.
 
 Error model (u = 2^-24):
 
-* Split products.  A round-to-nearest 11-bit hi leaves |x - hi| <= 2^-11 |x|, a truncated hi (split2h) <= 2^-10 |x|; lo is
+* Split products.  A round-to-nearest 11-bit hi leaves |x - hi| <= 2^-11 |x|, a truncated hi (split_f16x2_trunc) <= 2^-10 |x|; lo is
   the fp16 rounding of the rest (2^-11 of it).  With the lo*lo term dropped, one product is off by at most
   3 * 2^-22 |a||b| (both round-to-nearest: attn_tc.cu), 5 * 2^-22 (truncated activation x weight image: projections,
   out-projections) or 8 * 2^-22 (both truncated: the temporal kernel's Q K^T and P V, the SLA context and output products,
