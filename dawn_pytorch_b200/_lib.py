@@ -102,6 +102,10 @@ def _load():
     lib.dawn_unet_ddim_step.argtypes = [vp, fp, fp, fp, ctypes.c_int64] + [ctypes.c_float] * 6 + [vp, vp]
     lib.dawn_unet_sampler_capture.argtypes = [vp, fp, fp, fp, vp, ctypes.POINTER(ctypes.c_float), ctypes.c_int, ctypes.c_float, vp]
     lib.dawn_unet_sampler_launch.argtypes = [vp, vp]
+    lib.dawn_unet_ddim_step_guided.argtypes = [vp, fp, fp, fp, ctypes.c_int64, fp] + [ctypes.c_float] * 6 + [vp, vp]
+    lib.dawn_unet_sampler_capture_guided.argtypes = [vp, fp, fp, fp, vp, fp, ctypes.POINTER(ctypes.c_float), ctypes.c_int,
+                                                     ctypes.c_float, vp]
+    lib.dawn_unet_sampler_launch_guided.argtypes = [vp, vp]
     lib.dawn_ddpm_step.argtypes = [fp, fp, fp, ctypes.c_int64] + [ctypes.c_float] * 6 + [vp, vp]
     lib.dawn_unet_ddpm_step.argtypes = [vp, fp, fp, fp, ctypes.c_int64] + [ctypes.c_float] * 6 + [vp, vp]
     lib.dawn_unet_ddpm_capture.argtypes = [vp, fp, fp, fp, vp, fp, ctypes.c_int, ctypes.c_float, vp]
@@ -134,6 +138,7 @@ EXPORTS = ["dawn_unet_create", "dawn_unet_destroy", "dawn_unet_set_param", "dawn
            "dawn_unet_set_num_frames", "dawn_unet_set_geometry", "dawn_nccl_unique_id", "dawn_unet_init_shard", "dawn_unet_shard_ipc_export", "dawn_unet_shard_ipc_import", "dawn_unet_set_clip_invariants", "dawn_unet_forward",
            "dawn_unet_forward_x3", "dawn_unet_forward_host", "dawn_unet_set_tap", "dawn_unet_tap_shape",
            "dawn_unet_profile_enable", "dawn_unet_profile_read", "dawn_unet_last_launch_count", "dawn_unet_workspace_bytes", "dawn_ddim_step", "dawn_unet_ddim_step", "dawn_unet_sampler_capture", "dawn_unet_sampler_launch",
+           "dawn_unet_ddim_step_guided", "dawn_unet_sampler_capture_guided", "dawn_unet_sampler_launch_guided",
            "dawn_ddpm_step", "dawn_unet_ddpm_step", "dawn_unet_ddpm_capture", "dawn_unet_ddpm_launch",
            "dawn_test_contraction", "dawn_test_fused", "dawn_last_error", "dawn_build_info"]
 

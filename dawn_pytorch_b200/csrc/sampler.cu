@@ -15,11 +15,24 @@
 namespace dawn {
 namespace {
 
-// keys[i] = |ca * x - cb * eps|  (x0 magnitude; non-negative floats order like their bit patterns)
-__global__ void x0_abs_kernel(const float* __restrict__ x, const float* __restrict__ eps, float ca, float cb, long long n,
-                              uint32_t* __restrict__ keys) {
+// classifier-free guidance (reference forward_with_cond_scale U:879-890): null + (cond - null) * s, rounded as its three fp32
+// torch ops (no fused multiply-add)
+__device__ __forceinline__ float guided_eps(float e_cond, float e_null, float s) {
+  return __fadd_rn(e_null, __fmul_rn(__fsub_rn(e_cond, e_null), s));
+}
+
+// eps of a DDIM update: eps[i], or with guidance (eps_n != nullptr) the guided eps of eps[i] and eps_n[i] at scale g, which is
+// formed here and never stored
+__device__ __forceinline__ float update_eps(const float* __restrict__ eps, const float* __restrict__ eps_n, float g, long long i) {
+  return eps_n ? guided_eps(eps[i], eps_n[i], g) : eps[i];
+}
+
+// keys[i] = |ca * x - cb * e|, e = update_eps  (x0 magnitude; non-negative floats order like their bit patterns)
+__global__ void x0_abs_kernel(const float* __restrict__ x, const float* __restrict__ eps, const float* __restrict__ eps_n,
+                              const float* __restrict__ scale, float ca, float cb, long long n, uint32_t* __restrict__ keys) {
+  const float g = eps_n ? *scale : 0.0f;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-    keys[i] = __float_as_uint(fabsf(ca * x[i] - cb * eps[i]));
+    keys[i] = __float_as_uint(fabsf(ca * x[i] - cb * update_eps(eps, eps_n, g, i)));
 }
 
 // one launch instead of a pageable-host memcpy + three memsets (keeps the step capturable in a CUDA graph)
@@ -95,18 +108,23 @@ __global__ void threshold_kernel(const uint32_t* state, const unsigned long long
   *s_out = fmaxf(q, 1.0f);
 }
 
-// img = clamp(x0, -s, s)/s * sqrt(a_next) + c * eps + sigma * noise;  clamp == 0: x0 is used as predicted (clip_denoised=False, U:1183)
-__global__ void ddim_update_kernel(float* __restrict__ x, const float* __restrict__ eps, const float* __restrict__ noise,
+// img = clamp(x0, -s, s)/s * sqrt(a_next) + c * e + sigma * noise, e = update_eps;  clamp == 0: x0 is used as predicted
+// (clip_denoised=False, U:1183).  x_n != nullptr (guidance): the new x also goes to the null slot, so the next forward sees the
+// same x_t in both
+__global__ void ddim_update_kernel(float* __restrict__ x, float* __restrict__ x_n, const float* __restrict__ eps,
+                                   const float* __restrict__ eps_n, const float* __restrict__ scale, const float* __restrict__ noise,
                                    const float* __restrict__ s_ptr, float ca, float cb, float sqrt_an, float c, float sigma,
                                    long long n, int clamp) {
   const float s = s_ptr ? *s_ptr : 1.0f;
+  const float g = eps_n ? *scale : 0.0f;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    const float e = eps[i];
+    const float e = update_eps(eps, eps_n, g, i);
     float x0 = ca * x[i] - cb * e;
     if (clamp) x0 = fminf(fmaxf(x0, -s), s) / s;
     float v = x0 * sqrt_an + c * e;
     if (noise) v += sigma * noise[i];
     x[i] = v;
+    if (x_n) x_n[i] = v;
   }
 }
 
@@ -182,6 +200,24 @@ int clip_threshold(void* scratch, long long n, int64_t n_global, float q, int bl
   return 0;
 }
 
+// the DDIM update behind both entries below; eps_n / scale / x_n are nullptr without guidance
+int ddim_update(float* x, float* x_n, const float* eps, const float* eps_n, const float* scale, const float* noise, int64_t n_local,
+                int64_t n_global, float ca, float cb, float sqrt_an, float c, float sigma, float q, void* scratch, cudaStream_t st,
+                const DdimReduce* red) {
+  const long long n = n_local;
+  const int threads = 256;
+  int blocks = (int)std::min<long long>((n + threads - 1) / threads, 148LL * 8);
+  float* s_ptr = nullptr;
+  if (q > 0.f)
+    DAWN_TRY(clip_threshold(scratch, n, n_global, q, blocks, st, red, &s_ptr, [&](uint32_t* keys) {
+      x0_abs_kernel<<<blocks, threads, 0, st>>>(x, eps, eps_n, scale, ca, cb, n, keys);
+    }));
+  ddim_update_kernel<<<blocks, threads, 0, st>>>(x, x_n, eps, eps_n, scale, noise, s_ptr, ca, cb, sqrt_an, c, sigma, n,
+                                                 q < 0.f ? 0 : 1);
+  DAWN_LAUNCH_OK();
+  return 0;
+}
+
 }  // namespace
 
 // One DDIM update in place on x (n_local floats of this rank's frames of the (3, F, h, w) latent).  The dynamic threshold
@@ -191,17 +227,19 @@ int clip_threshold(void* scratch, long long n, int64_t n_global, float q, int bl
 int ddim_step_impl(float* x, const float* eps, const float* noise, int64_t n_local, int64_t n_global, float ca, float cb,
                    float sqrt_an, float c, float sigma, float q, void* scratch, cudaStream_t st, const DdimReduce* red) {
   if (!x || !eps || !scratch || n_local <= 0 || n_global < n_local) { set_last_error("dawn_ddim_step: bad argument"); return -1; }
-  const long long n = n_local;
-  const int threads = 256;
-  int blocks = (int)std::min<long long>((n + threads - 1) / threads, 148LL * 8);
-  float* s_ptr = nullptr;
-  if (q > 0.f)
-    DAWN_TRY(clip_threshold(scratch, n, n_global, q, blocks, st, red, &s_ptr, [&](uint32_t* keys) {
-      x0_abs_kernel<<<blocks, threads, 0, st>>>(x, eps, ca, cb, n, keys);
-    }));
-  ddim_update_kernel<<<blocks, threads, 0, st>>>(x, eps, noise, s_ptr, ca, cb, sqrt_an, c, sigma, n, q < 0.f ? 0 : 1);
-  DAWN_LAUNCH_OK();
-  return 0;
+  return ddim_update(x, nullptr, eps, nullptr, nullptr, noise, n_local, n_global, ca, cb, sqrt_an, c, sigma, q, scratch, st, red);
+}
+
+// One guided DDIM update of one conditioned / null pair (n values each): the eps of the update is
+// eps_n + (eps_c - eps_n) * *scale, formed inside the key and update kernels; the quantile is over this pair's n values.
+int ddim_guided_step_impl(float* x_c, float* x_n, const float* eps_c, const float* eps_n, const float* noise, int64_t n_clip,
+                          const float* scale, float ca, float cb, float sqrt_an, float c, float sigma, float q, void* scratch,
+                          cudaStream_t st) {
+  if (!x_c || !x_n || !eps_c || !eps_n || !scale || !scratch || n_clip <= 0) {
+    set_last_error("dawn_ddim_step_guided: bad argument");
+    return -1;
+  }
+  return ddim_update(x_c, x_n, eps_c, eps_n, scale, noise, n_clip, n_clip, ca, cb, sqrt_an, c, sigma, q, scratch, st, nullptr);
 }
 
 // One ancestral update in place on x, same threshold and sharding as ddim_step_impl; the step graph passes `tab` and `t_slot`

@@ -17,6 +17,12 @@ struct DdimReduce {
 int ddim_step_impl(float* x, const float* eps, const float* noise, int64_t n_local, int64_t n_global, float ca, float cb,
                    float sqrt_an, float c, float sigma, float q, void* scratch, cudaStream_t st, const DdimReduce* red);
 
+// One classifier-free-guided DDIM update of a conditioned / null pair of one clip each (n_clip floats): the update of
+// ddim_step_impl with eps = eps_n + (eps_c - eps_n) * (*scale) (device float), written to both x_c and x_n.  Unsharded only.
+int ddim_guided_step_impl(float* x_c, float* x_n, const float* eps_c, const float* eps_n, const float* noise, int64_t n_clip,
+                          const float* scale, float ca, float cb, float sqrt_an, float c, float sigma, float q, void* scratch,
+                          cudaStream_t st);
+
 // coefficients of one ancestral (DDPM) step at timestep t; layout of a row of the step graph's device table
 struct DdpmCoef {
   float ca, cb;      // sqrt_recip_alphas_cumprod[t], sqrt_recipm1_alphas_cumprod[t]

@@ -220,6 +220,10 @@ struct dawn_unet {
   // beside samp_exec (neither capture drops the other) and invalidated by the same geometry changes
   cudaGraphExec_t ddpm_exec = nullptr;
   int64_t ddpm_launches = 0;
+  // classifier-free-guided sampling loop (dawn_unet_sampler_capture_guided): its own slot beside samp_exec and ddpm_exec, since
+  // a plain loop over 2 clips and a guided loop over 1 clip run on the same B = 2 geometry
+  cudaGraphExec_t guid_exec = nullptr;
+  int64_t guid_launches = 0;
 
   // per-category kernel timing (CUDA events on the launching stream), see dawn_unet_profile_*
   bool prof_on = false;
@@ -935,6 +939,7 @@ void dawn_unet_destroy(dawn_unet* h) {
   for (cudaEvent_t e : h->prof_ev) cudaEventDestroy(e);
   if (h->samp_exec) cudaGraphExecDestroy(h->samp_exec);
   if (h->ddpm_exec) cudaGraphExecDestroy(h->ddpm_exec);
+  if (h->guid_exec) cudaGraphExecDestroy(h->guid_exec);
   if (h->samp_stream) cudaStreamDestroy(h->samp_stream);
   if (h->sh_comm && g_nccl.ok) g_nccl.CommDestroy(h->sh_comm);
   for (int r = 0; r < kP2pMaxRanks; ++r)
@@ -957,10 +962,14 @@ static void drop_sampler_graph(dawn_unet* h) {
 static void drop_ddpm_graph(dawn_unet* h) {
   if (h->ddpm_exec) { cudaGraphExecDestroy(h->ddpm_exec); h->ddpm_exec = nullptr; }
 }
-// a new geometry, parameter set or sharding invalidates both captured sampler graphs
+static void drop_guided_graph(dawn_unet* h) {
+  if (h->guid_exec) { cudaGraphExecDestroy(h->guid_exec); h->guid_exec = nullptr; }
+}
+// a new geometry, parameter set or sharding invalidates all three captured sampler graphs
 static void drop_graphs(dawn_unet* h) {
   drop_sampler_graph(h);
   drop_ddpm_graph(h);
+  drop_guided_graph(h);
 }
 
 int dawn_unet_commit_params(dawn_unet* h) {
@@ -1420,6 +1429,68 @@ int dawn_unet_sampler_launch(dawn_unet* h, void* stream) {
   DAWN_CHECK(h->have_invariants, "set_clip_invariants must precede sampler_launch");
   DAWN_CUDA_OK(cudaGraphLaunch(h->samp_exec, (cudaStream_t)stream));
   h->launches = h->samp_launches;
+  return 0;
+}
+
+// Classifier-free-guided DDIM update on a handle of B = 2b clips: clips [0, b) are conditioned, clips [b, 2b) their null twins
+// (clip i pairs with clip b + i).  Per pair one exact quantile over its guided x0 and one update written to both slots.
+int dawn_unet_ddim_step_guided(dawn_unet* h, float* x, const float* eps, const float* noise, int64_t n_clip, const float* cond_scale_dev,
+                               float ca, float cb, float sqrt_an, float c, float sigma, float q, void* scratch, void* stream) {
+  DAWN_CHECK(h, "null handle");
+  DAWN_CHECK(h->sh_nranks <= 1, "guided DDIM steps run on an unsharded handle (a frame-sharded handle holds one clip, not a pair)");
+  DAWN_CHECK(h->F > 0 && h->B % 2 == 0, "a guided DDIM step needs an even clip count B = 2b (b conditioned clips, then their null twins)");
+  DAWN_CHECK(x && eps && cond_scale_dev && scratch, "bad argument");
+  DAWN_CHECK(n_clip == (int64_t)(h->cfg.out_grid_dim + h->cfg.out_conf_dim) * h->F * h->H * h->W,
+             "n_clip must be the size of one clip (3 * F * height * width)");
+  const int b = h->B / 2;
+  for (int i = 0; i < b; ++i)
+    DAWN_TRY(ddim_guided_step_impl(x + i * n_clip, x + (b + i) * n_clip, eps + i * n_clip, eps + (b + i) * n_clip,
+                                   noise ? noise + i * n_clip : nullptr, n_clip, cond_scale_dev, ca, cb, sqrt_an, c, sigma, q, scratch,
+                                   (cudaStream_t)stream));
+  return 0;
+}
+
+// The guided sampling loop as one CUDA graph: nsteps x (forward_x3 over the 2b clips + guided update).  Same buffers as
+// dawn_unet_sampler_capture except noise_all, which holds b clips per step, and the device scale read by every update.
+int dawn_unet_sampler_capture_guided(dawn_unet* h, float* x, float* eps, const float* noise_all, const int64_t* t_all,
+                                     const float* cond_scale_dev, const float* coef, int nsteps, float q, void* scratch) {
+  DAWN_CHECK(h && x && eps && t_all && cond_scale_dev && coef && scratch && nsteps >= 1, "bad argument");
+  DAWN_CHECK(noise_all || nsteps == 1, "noise_all is required for more than one step");
+  DAWN_CHECK(h->F > 0 && h->have_invariants, "set_clip_invariants must precede sampler_capture_guided");
+  DAWN_CHECK(h->sh_nranks <= 1 && h->B % 2 == 0, "the guided sampler graph needs an unsharded handle with an even clip count");
+  DAWN_CHECK(!h->prof_on, "disable profiling before capturing the sampler graph");
+  drop_guided_graph(h);
+  if (!h->samp_stream) DAWN_CUDA_OK(cudaStreamCreateWithFlags(&h->samp_stream, cudaStreamNonBlocking));
+  const int64_t nc = (int64_t)(h->cfg.out_grid_dim + h->cfg.out_conf_dim) * h->F * h->H * h->W;
+  const int64_t n_noise = nc * (h->B / 2);
+  cudaStream_t st = h->samp_stream;
+  DAWN_CUDA_OK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+  int rc = 0;
+  int64_t launches = 0;
+  for (int k = 0; k < nsteps && rc == 0; ++k) {
+    rc = forward_x3_impl(h, x, t_all + k, 0, eps, st);               // conditioned and null clips at step k's timestep
+    launches += h->launches;
+    const float* cf = coef + 5 * k;
+    if (rc == 0)
+      rc = dawn_unet_ddim_step_guided(h, x, eps, (k < nsteps - 1) ? noise_all + (size_t)k * n_noise : nullptr, nc, cond_scale_dev,
+                                      cf[0], cf[1], cf[2], cf[3], cf[4], q, scratch, st);
+  }
+  cudaGraph_t graph = nullptr;
+  const cudaError_t e = cudaStreamEndCapture(st, &graph);
+  if (rc != 0) { if (graph) cudaGraphDestroy(graph); return rc; }
+  DAWN_CUDA_OK(e);
+  const cudaError_t ei = cudaGraphInstantiate(&h->guid_exec, graph, 0);
+  cudaGraphDestroy(graph);
+  DAWN_CUDA_OK(ei);
+  h->guid_launches = launches;
+  return 0;
+}
+
+int dawn_unet_sampler_launch_guided(dawn_unet* h, void* stream) {
+  DAWN_CHECK(h && h->guid_exec, "sampler_capture_guided must precede sampler_launch_guided (a geometry change drops the graph)");
+  DAWN_CHECK(h->have_invariants, "set_clip_invariants must precede sampler_launch_guided");
+  DAWN_CUDA_OK(cudaGraphLaunch(h->guid_exec, (cudaStream_t)stream));
+  h->launches = h->guid_launches;
   return 0;
 }
 

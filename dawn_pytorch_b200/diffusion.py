@@ -123,7 +123,10 @@ class GaussianDiffusion(nn.Module):
         noise_fn(step_index, shape) -> tensor lets tests inject the noise the reference draws with torch.randn /
         randn_like (:1166, 1201); step_index -1 is the start image.
         use_graph: replay the whole loop (nsteps x [UNet forward + DDIM update]) as ONE CUDA graph per clip
-        (`dawn_unet_sampler_capture`; captured once per geometry/schedule and cached on the module).
+        (`dawn_unet_sampler_capture`; captured once per geometry/schedule and cached on the module).  With guidance
+        (cond_scale != 1) each step is one pass over the conditioned clips and their all-zero-cond twins plus one fused
+        guided update (`dawn_unet_sampler_capture_guided`); the scale is read on the device, so one capture serves every
+        cond_scale.  Guided graphs need an unsharded UNet.
         Frame-sharded UNet (`unet.init_shard`): `shape`, `cond` and the returned sample hold this rank's frames; the
         dynamic-threshold quantile is selected over the whole clip (all-reduced radix select) and the default noise is
         the rank's slice of ONE clip-wide stream (same `seed` on every rank; drawn on rank 0 and broadcast if None)."""
@@ -140,8 +143,7 @@ class GaussianDiffusion(nn.Module):
         guided = cond_scale != 1 and getattr(unet, "has_cond", True)
         if use_graph:
             if guided:
-                raise NotImplementedError("use_graph captures the cond_scale = 1 loop (DAWN's shipped setting); "
-                                          "classifier-free guidance runs eagerly")
+                return self._ddim_sample_guided_graph(unet, fea, cond, img, pairs, draw, q, st, cond_scale)
             return self._ddim_sample_graph(unet, fea, cond, img, pairs, draw, q, st)
         if self._batched(unet, b, Fr, h, w):
             return self._ddim_sample_batched(unet, fea, cond, img, pairs, draw, q, st, guided, cond_scale)
@@ -260,6 +262,66 @@ class GaussianDiffusion(nn.Module):
                 g["noise"][k].copy_(draw(k, one))
             check(lib.dawn_unet_sampler_launch(unet._handle, st), "dawn_unet_sampler_launch")
             img[sel].copy_(g["x"])
+        return img
+
+    def _ddim_sample_guided_graph(self, unet, fea, cond, img, pairs, draw, q, st, cond_scale):
+        """Classifier-free guidance as one CUDA graph per launch (forward_with_cond_scale U:879-890 inside ddim_sample
+        U:1156-1208): every step is ONE UNet pass over 2m clips, m conditioned clips followed by their twins with all-zero
+        cond (U:920), and one guided update that writes the new x into both halves.  m = b (one launch for the batch) when a
+        pass takes 2b clips, otherwise m = 1 (one launch per clip).  Noise is drawn as the eager sampler draws it.  The
+        scale sits in a device slot, so the cached capture serves every cond_scale."""
+        b, ch, Fr, h, w = img.shape
+        device, n, ns = img.device, ch * Fr * h * w, len(pairs)
+        if getattr(unet, "_shard", None) is not None:
+            raise NotImplementedError("use_graph with cond_scale != 1 runs each clip and its null twin in one pass, and a "
+                                      "frame-sharded UNet runs one clip at a time: sample with use_graph=False")
+        if unet.clips_per_pass(2 * b, Fr, h, w) == 2 * b:
+            m = b
+        elif unet.clips_per_pass(2, Fr, h, w) == 2:
+            m = 1
+        else:
+            raise NotImplementedError(f"use_graph with cond_scale != 1 runs each clip and its null twin in one pass, and two "
+                                      f"clips of {Fr} x {h} x {w} do not fit one pass: sample with use_graph=False")
+        one = (m, ch, Fr, h, w) if m > 1 else (ch, Fr, h, w)
+        fea, cond = fea.contiguous(), cond.contiguous()
+
+        def invariants(sel):                                    # [fea; fea], [cond; 0]
+            f, c = fea[sel], cond[sel]
+            unet.set_clip_invariants(torch.cat([f, f]), torch.cat([c, torch.zeros_like(c)]))
+        key = (Fr, h, w, tuple(pairs), q, device.index, m)
+        g = getattr(self, "_guided_graph", None)
+        unet.update_num_frames(Fr)
+        if g is None or g["key"] != key or g["gen"] != unet.graph_generation():
+            g = dict(key=key, x=torch.empty((2 * m, ch, Fr, h, w), device=device), eps=torch.empty((2 * m, ch, Fr, h, w), device=device),
+                     noise=torch.empty((max(ns - 1, 1), m, ch, Fr, h, w), device=device),
+                     t_all=torch.tensor([p[0] for p in pairs], dtype=torch.long, device=device),
+                     scale=torch.ones(1, device=device), scratch=torch.empty(n + 512, dtype=torch.int32, device=device))
+            coef = (ctypes.c_float * (5 * ns))()
+            for k, (t, t_next) in enumerate(pairs):
+                coef[5 * k:5 * k + 5] = self.ddim_coefficients(t, t_next)
+                assert (t_next > 0) == (k < ns - 1), "only the last DDIM step ends at t = 0 (reference :1201)"
+            invariants(slice(0, m))
+            torch.cuda.synchronize(device)
+            check(lib.dawn_unet_sampler_capture_guided(unet._handle, ctypes.c_void_p(g["x"].data_ptr()), ctypes.c_void_p(g["eps"].data_ptr()),
+                                                       ctypes.c_void_p(g["noise"].data_ptr()), ctypes.c_void_p(g["t_all"].data_ptr()),
+                                                       ctypes.c_void_p(g["scale"].data_ptr()), coef, ns, q,
+                                                       ctypes.c_void_p(g["scratch"].data_ptr())), "dawn_unet_sampler_capture_guided")
+            g["gen"] = unet.graph_generation()
+            self._guided_graph = g
+            self._guided_captures = getattr(self, "_guided_captures", 0) + 1
+        g["scale"].fill_(float(cond_scale))
+        # when the eager and cond_scale = 1 samplers step the b clips together but a pass cannot take 2b clips, the noise is
+        # still drawn as they draw it, (b, ch, F, h, w) per step, and sliced per launch: one seed gives one sample on every path
+        whole = [draw(k, (b, ch, Fr, h, w)) for k in range(ns - 1)] if m < b and self._batched(unet, b, Fr, h, w) else None
+        for i0 in range(0, b, m):
+            sel = slice(i0, i0 + m)
+            invariants(sel)
+            g["x"][:m].copy_(img[sel])
+            g["x"][m:].copy_(img[sel])
+            for k in range(ns - 1):
+                g["noise"][k].view(one).copy_(whole[k][i0] if whole is not None else draw(k, one))
+            check(lib.dawn_unet_sampler_launch_guided(unet._handle, st), "dawn_unet_sampler_launch_guided")
+            img[sel].copy_(g["x"][:m])
         return img
 
     # ------------------------------------------------------------------ ancestral sampling (reference :1087-1134)

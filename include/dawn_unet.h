@@ -60,7 +60,7 @@ int dawn_unet_commit_params(dawn_unet* h);
 int dawn_unet_set_num_frames(dawn_unet* h, int F, int height, int width);
 /* B clips of F frames each in one pass (reference batch dimension, U:892-956); set_num_frames(F, h, w) is set_geometry(1, F, h, w).
  * Sizes the workspace for B*F frames and one GroupNorm statistics / FiLM / init-conv map / cross-attention table slice per clip;
- * drops both captured sampler graphs.  1 <= B <= 16.  B > 1 is refused (-1) on a frame-sharded handle, with debugging taps set,
+ * drops every captured sampler graph.  1 <= B <= 16.  B > 1 is refused (-1) on a frame-sharded handle, with debugging taps set,
  * by init_shard (with more than one rank), forward_host and set_tap. */
 int dawn_unet_set_geometry(dawn_unet* h, int B, int F, int height, int width);
 
@@ -146,6 +146,30 @@ int dawn_unet_ddim_step(dawn_unet* h, float* x, const float* eps, const float* n
 int dawn_unet_sampler_capture(dawn_unet* h, float* x, float* eps, const float* noise_all, const int64_t* t_all,
                               const float* coef, int nsteps, float q, void* scratch);
 int dawn_unet_sampler_launch(dawn_unet* h, void* stream);
+
+/* Classifier-free-guided DDIM update (reference forward_with_cond_scale :879-890 inside ddim_sample :1169-1205) on an
+ * unsharded handle whose geometry holds B = 2b clips: clips 0..b-1 are the conditioned clips, clips b..2b-1 their null twins
+ * (all-zero cond), clip i pairing with clip b+i.  x, eps: device (2b, 3, F, h, w); noise: device (b, 3, F, h, w) or NULL for
+ * the last step; n_clip = 3*F*h*w.  Per pair, with s = *cond_scale_dev (a device float, so one captured graph serves every
+ * scale):
+ *   e = e_null + (e_cond - e_null) * s    (rounded as the reference's three fp32 ops, no fused multiply-add)
+ * then the update of dawn_ddim_step with that e and the pair's own quantile; the combined e is never stored.  The new x is
+ * written to BOTH the conditioned and the null slot.  scratch: n_clip + 512 32-bit words.  Returns -1 on a frame-sharded
+ * handle or an odd B. */
+int dawn_unet_ddim_step_guided(dawn_unet* h, float* x, const float* eps, const float* noise, int64_t n_clip, const float* cond_scale_dev,
+                               float ca, float cb, float sqrt_an, float c, float sigma, float q, void* scratch, void* stream);
+
+/* The guided sampling loop captured as one CUDA graph: nsteps x [forward_x3 over the 2b clips + dawn_unet_ddim_step_guided].
+ * All addresses are fixed at capture: x (2b,3,F,h,w) start noise in both halves / sample out (both halves equal), eps
+ * (2b,3,F,h,w) scratch, noise_all ((nsteps-1) x b*3*F*h*w, slice k feeds step k), t_all (nsteps int64, device),
+ * cond_scale_dev (one float, device; read at every replay), scratch (as dawn_unet_ddim_step_guided), coef (host, as
+ * dawn_unet_sampler_capture).  Per launch: dawn_unet_set_clip_invariants with fea (2b, ...) = [fea; fea] and cond
+ * (2b, F, cond_dim) = [cond; 0], fill both halves of x, noise_all and *cond_scale_dev, then dawn_unet_sampler_launch_guided.
+ * The graph has its own slot: capturing it leaves the dawn_unet_sampler_capture and dawn_unet_ddpm_capture graphs in place,
+ * and capturing either of those leaves it in place.  set_geometry / commit_params / init_shard drop all three. */
+int dawn_unet_sampler_capture_guided(dawn_unet* h, float* x, float* eps, const float* noise_all, const int64_t* t_all,
+                                     const float* cond_scale_dev, const float* coef, int nsteps, float q, void* scratch);
+int dawn_unet_sampler_launch_guided(dawn_unet* h, void* stream);
 
 /* One ancestral (DDPM) update around the UNet (reference GaussianDiffusion.p_sample :1087-1121), in place on x (device,
  * n floats), each operation rounded as the reference's fp32 torch arithmetic (no fused multiply-add):
