@@ -7,7 +7,9 @@
 namespace dawn {
 
 // =========================================================================== row LayerNorm statistics
-// one warp per pixel row; C <= 1024, C % 4 == 0.  biased variance, two-pass from registers (U:186-188, 201-203)
+// one warp per pixel row; C <= 128 * NV (NV float4 per lane), C % 4 == 0.  biased variance, two-pass from registers
+// (U:186-188, 201-203).  NV = 16 serves the 2048-channel inputs of the first up block below a 1024-channel level.
+template <int NV>
 __global__ void rowstats_kernel(const float* __restrict__ x, int ld, int C, int M, float eps,
                                 float* __restrict__ out) {
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -15,10 +17,10 @@ __global__ void rowstats_kernel(const float* __restrict__ x, int ld, int C, int 
   if (row >= M) return;
   const float4* xr = reinterpret_cast<const float4*>(x + (size_t)row * ld);
   const int nvec = C >> 2;
-  float4 v[8];
+  float4 v[NV];
   float s = 0.f;
 #pragma unroll
-  for (int k = 0; k < 8; ++k) {
+  for (int k = 0; k < NV; ++k) {
     const int i = lane + 32 * k;
     v[k] = (i < nvec) ? xr[i] : make_float4(0.f, 0.f, 0.f, 0.f);
     s += (v[k].x + v[k].y) + (v[k].z + v[k].w);
@@ -26,7 +28,7 @@ __global__ void rowstats_kernel(const float* __restrict__ x, int ld, int C, int 
   const float mu = warp_sum(s) / (float)C;
   float ss = 0.f;
 #pragma unroll
-  for (int k = 0; k < 8; ++k) {
+  for (int k = 0; k < NV; ++k) {
     const int i = lane + 32 * k;
     if (i < nvec) {
       const float a = v[k].x - mu, b = v[k].y - mu, c = v[k].z - mu, d = v[k].w - mu;
@@ -41,9 +43,10 @@ __global__ void rowstats_kernel(const float* __restrict__ x, int ld, int C, int 
 }
 
 int launch_rowstats(const float* x, int ld, int C, int M, float eps, float* out, cudaStream_t st) {
-  if (C > 1024 || (C & 3) || (ld & 3)) { set_last_error("rowstats: C must be <= 1024 and a multiple of 4"); return -1; }
+  if (C > 2048 || (C & 3) || (ld & 3)) { set_last_error("rowstats: C must be <= 2048 and a multiple of 4"); return -1; }
   const int wpb = 8;
-  rowstats_kernel<<<(M + wpb - 1) / wpb, wpb * 32, 0, st>>>(x, ld, C, M, eps, out);
+  if (C <= 1024) rowstats_kernel<8><<<(M + wpb - 1) / wpb, wpb * 32, 0, st>>>(x, ld, C, M, eps, out);
+  else rowstats_kernel<16><<<(M + wpb - 1) / wpb, wpb * 32, 0, st>>>(x, ld, C, M, eps, out);
   DAWN_LAUNCH_OK();
   return 0;
 }
@@ -383,8 +386,9 @@ __global__ void film_kernel(const FilmDesc* __restrict__ descs, const float* __r
   if (lane == 0) d.out[(size_t)clip * d.n + j] = acc + d.b[j];
 }
 
-int launch_film(const FilmDesc* descs_dev, int ndesc, int clips, const float* t_silu, int tdim, cudaStream_t st) {
-  dim3 grid(1024 / 8, ndesc, clips);       // n <= 1024 outputs per block descriptor
+// max_n: the largest descriptor n (2 x the widest conditioned block's channels); one warp per output
+int launch_film(const FilmDesc* descs_dev, int ndesc, int max_n, int clips, const float* t_silu, int tdim, cudaStream_t st) {
+  dim3 grid((max_n + 7) / 8, ndesc, clips);
   film_kernel<<<grid, 256, 0, st>>>(descs_dev, t_silu, tdim);
   DAWN_LAUNCH_OK();
   return 0;
@@ -400,32 +404,6 @@ __global__ void rotary_table_kernel(const float* __restrict__ freqs, int F, int 
 }
 int launch_rotary_table(const float* freqs, int F, int pos0, float* out, cudaStream_t st) {
   rotary_table_kernel<<<(F * 16 + 255) / 256, 256, 0, st>>>(freqs, F, pos0, out);
-  DAWN_LAUNCH_OK();
-  return 0;
-}
-
-// T5 bucket of rel = j - i with num_buckets 32, max_distance 32 (U:91-109, 767-768)
-__global__ void relbias_kernel(const float* __restrict__ emb, int w, float* __restrict__ out) {
-  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  const int span = 2 * w + 1;
-  if (idx >= 8 * span) return;
-  const int h = idx / span, rel = idx - h * span - w;
-  int n = -rel;
-  int ret = (n < 0) ? 16 : 0;
-  n = abs(n);
-  int val;
-  if (n < 8) {
-    val = n;
-  } else {
-    // 8 + trunc( log(n/8) / log(32/8) * 8 ), clipped to 15; fp32 like the reference
-    const float v = logf((float)n / 8.0f) / 1.3862943611198906f * 8.0f;
-    val = min(15, 8 + (int)v);
-  }
-  out[idx] = emb[(ret + val) * 8 + h];
-}
-int launch_relbias_table(const float* emb, int w, float* out, cudaStream_t st) {
-  const int n = 8 * (2 * w + 1);
-  relbias_kernel<<<(n + 127) / 128, 128, 0, st>>>(emb, w, out);
   DAWN_LAUNCH_OK();
   return 0;
 }

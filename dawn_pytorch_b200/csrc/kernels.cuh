@@ -45,15 +45,14 @@ int launch_ca_rstd(const float* gates, const float* G, int M, int P, float* Wt /
 
 // ---------------------------------------------------------------- time embedding  U:150-162, 788-794, 366-369
 // one timestep per clip: clip b uses t_dev[b * t_stride] (t_stride 0: one shared timestep) and writes t_silu[b], out[b]
-struct FilmDesc { const float* W; const float* b; float* out; int n; };   // out[clip][n] = W[n][256] silu(t256[clip]) + b
+struct FilmDesc { const float* W; const float* b; float* out; int n; };   // out[clip][n] = W[n][tdim] silu(t[clip]) + b
 int launch_time_mlp(const int64_t* t_dev, int t_stride, int clips, const float* freqs /*[dim/2]*/, int dim, const float* W1, const float* b1,
                     const float* W2, const float* b2, float* t_silu /*[clips][4*dim]*/, cudaStream_t st);
-int launch_film(const FilmDesc* descs_dev, int ndesc, int clips, const float* t_silu, int tdim, cudaStream_t st);
+// max_n >= every descriptor's n: all outputs of every descriptor are written
+int launch_film(const FilmDesc* descs_dev, int ndesc, int max_n, int clips, const float* t_silu, int tdim, cudaStream_t st);
 
 // rotary cos/sin table [F][16][2] from freqs[16], position = pos0 + f
 int launch_rotary_table(const float* freqs, int F, int pos0, float* out, cudaStream_t st);
-// bias[h][rel + w] = E[bucket(rel)][h], rel in [-w, w]             U:77-119
-int launch_relbias_table(const float* emb /*[32][8]*/, int w, float* out /*[8][2w+1]*/, cudaStream_t st);
 
 // ---------------------------------------------------------------- attention cores
 // banded / full softmax attention over strided sequences; qkv rows are [q(256) | k(256) | v(256)], head = 32 dims

@@ -180,7 +180,7 @@ struct dawn_unet {
   std::vector<PackedWeight> down_conv;
   std::vector<UpConv> up_conv;
   float *headW[2] = {nullptr, nullptr}, *headB[2] = {nullptr, nullptr};
-  FilmDesc* film_descs = nullptr; int n_film = 0;
+  FilmDesc* film_descs = nullptr; int n_film = 0, film_max_n = 0;
   CondDesc* cond_descs = nullptr; int n_cond = 0, cond_max_n1 = 0, cond_max_k = 0, cond_max_co = 0;   // batched per-clip prep
 
   // workspace (per set_geometry): B clips of F frames each
@@ -821,7 +821,7 @@ int forward_core(dawn_unet* h, const int64_t* t_dev, int t_stride, float* out, c
     ProfScope ps(c, PC_MISC, 0, 0);
     h->launches += 1;
     DAWN_TRY(launch_time_mlp(t_dev, t_stride, h->B, h->time_freqs, dim, h->tW1, h->tb1, h->tW2, h->tb2, h->TSILU, st));
-    DAWN_TRY(launch_film(h->film_descs, h->n_film, h->B, h->TSILU, h->tdim, st));
+    DAWN_TRY(launch_film(h->film_descs, h->n_film, h->film_max_n, h->B, h->TSILU, h->tdim, st));
   }
 
   const int H0 = h->lH[0], W0 = h->lW[0];
@@ -915,7 +915,7 @@ int dawn_unet_create(const dawn_unet_cfg* cfg, dawn_unet** out) {
   DAWN_TRY(dawn_check_single_device());
   DAWN_CHECK(cfg->attn_heads == 8 && cfg->attn_dim_head == 32, "only attn_heads=8, attn_dim_head=32 are supported");
   DAWN_CHECK(cfg->resnet_groups == 8, "only resnet_groups=8 is supported");
-  DAWN_CHECK(cfg->dim % 64 == 0 && cfg->dim <= 128, "dim must be 64 or 128");
+  DAWN_CHECK(cfg->dim == 64 || cfg->dim == 128, "dim must be 64 or 128");
   DAWN_CHECK(cfg->n_levels >= 2 && cfg->n_levels <= 6, "n_levels out of range");
   DAWN_CHECK(cfg->init_kernel_size == 7 || cfg->init_kernel_size == 5 || cfg->init_kernel_size == 3, "init kernel must be 3, 5 or 7");
   DAWN_CHECK(cfg->win_width >= 1 && cfg->win_width <= 120, "win_width out of range");
@@ -926,7 +926,7 @@ int dawn_unet_create(const dawn_unet_cfg* cfg, dawn_unet** out) {
   for (int i = 0; i < cfg->n_levels; ++i) h->dims.push_back(cfg->dim * cfg->dim_mults[i]);
   for (int i = 0; i < cfg->n_levels; ++i) h->in_out.push_back({h->dims[i], h->dims[i + 1]});
   for (auto& io : h->in_out)
-    if (io.second > 1024 || io.second * 2 > 1024 + 1024) { delete h; set_last_error("channel count too large"); return -1; }
+    if (io.second < 1 || io.second > 1024) { delete h; set_last_error("dim * dim_mults[i] must be in [1, 1024] for every level"); return -1; }
   h->cond_dim = cfg->cond_aud + cfg->cond_pose + cfg->cond_eye;
   h->tdim = 4 * cfg->dim;
   h->cin_pad = round_up(cfg->channels, 32);
@@ -1076,16 +1076,18 @@ int dawn_unet_set_geometry(dawn_unet* h, int B, int F, int height, int width) {
   DAWN_TRY(dev_alloc(own, M0 * 2 * dim, &h->XR, cnt));
   DAWN_TRY(dev_alloc(own, M0 * dim, &h->S0, cnt));
   h->bufA.assign(nlev, nullptr); h->bufB.assign(nlev, nullptr); h->CAT.assign(nlev, nullptr); h->DS.assign(nlev, nullptr);
-  size_t max_mc = 0, max_bf = 0;
+  size_t max_mc = 0, max_bf = 0, max_pc = P0 * dim;                 // max_pc: pixels x channels of the widest temporal layer
   for (int l = 0; l < nlev; ++l) {
     const size_t Ml = (size_t)NF * h->lH[l] * h->lW[l];
     const int ci = h->in_out[l].first, co = h->in_out[l].second;
-    DAWN_TRY(dev_alloc(own, Ml * co, &h->bufA[l], cnt));
-    DAWN_TRY(dev_alloc(own, Ml * co, &h->bufB[l], cnt));
+    const int cw = std::max(ci, co);                                   // down blocks run at co channels, up blocks at ci
+    DAWN_TRY(dev_alloc(own, Ml * cw, &h->bufA[l], cnt));
+    DAWN_TRY(dev_alloc(own, Ml * cw, &h->bufB[l], cnt));
     DAWN_TRY(dev_alloc(own, Ml * 2 * co, &h->CAT[l], cnt));
     if (l > 0) DAWN_TRY(dev_alloc(own, Ml * ci, &h->DS[l], cnt));
-    max_mc = std::max(max_mc, Ml * co);
-    max_bf = std::max(max_bf, (size_t)NF * 256 * round_up(co, 64));
+    max_mc = std::max(max_mc, Ml * cw);
+    max_bf = std::max(max_bf, (size_t)NF * 256 * round_up(cw, 64));
+    max_pc = std::max(max_pc, (size_t)h->lH[l] * h->lW[l] * cw);
   }
   max_mc = std::max(max_mc, M0 * dim);
   DAWN_TRY(dev_alloc(own, max_mc, &h->Y, cnt));
@@ -1094,7 +1096,7 @@ int dawn_unet_set_geometry(dawn_unet* h, int B, int F, int height, int width) {
   DAWN_TRY(dev_alloc(own, Mext * 768, &h->QKV, cnt));
   DAWN_TRY(dev_alloc(own, Mext * 256, &h->O, cnt));
   DAWN_TRY(dev_alloc(own, Mext * 2, &h->ROWSTATS, cnt));
-  DAWN_TRY(dev_alloc(own, Mext * dim, &h->XE, cnt));
+  DAWN_TRY(dev_alloc(own, (size_t)(NF + 2 * h->cfg.win_width) * max_pc, &h->XE, cnt));
   DAWN_TRY(dev_alloc(own, M0 * 24, &h->GATES, cnt));
   DAWN_TRY(dev_alloc(own, M0 * 32, &h->WT, cnt));
   DAWN_TRY(dev_alloc(own, max_bf, &h->BF, cnt));
@@ -1127,6 +1129,8 @@ int dawn_unet_set_geometry(dawn_unet* h, int B, int F, int height, int width) {
     float* d; DAWN_TRY(dev_alloc(own, descs.size() * sizeof(FilmDesc) / sizeof(float) + 4, &d, cnt));
     DAWN_CUDA_OK(cudaMemcpy(d, descs.data(), descs.size() * sizeof(FilmDesc), cudaMemcpyHostToDevice));
     h->film_descs = (FilmDesc*)d; h->n_film = (int)descs.size();
+    h->film_max_n = 0;
+    for (const auto& fd : descs) h->film_max_n = std::max(h->film_max_n, fd.n);
   }
   {
     // descriptors of the per-clip conditioning pipeline: one per (conditioned block, cross-attention), own scratch each
