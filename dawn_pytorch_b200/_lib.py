@@ -60,6 +60,19 @@ class DawnFusedCase(ctypes.Structure):
                 ("gn_stats", _p), ("gn_count", ctypes.c_double), ("cpg", _i), ("gn_w", _p), ("gn_b", _p), ("film", _p)]
 
 
+LFG_MOTION_PACK, LFG_WARP_BLEND, LFG_AFFINE_RELU, LFG_RESIDUAL_BN_RELU, LFG_RELU_AVGPOOL2, LFG_CHW_TO_HWC, LFG_HWC_TO_CHW, \
+    LFG_FINAL_CONV = range(8)
+
+
+class DawnLfgKernelCase(ctypes.Structure):
+    """include/dawn_lfg.h: dawn_lfg_kernel_case (pointers are device addresses)"""
+    _i, _p = ctypes.c_int, ctypes.c_void_p
+    _fields_ = [("kernel", _i), ("F", _i), ("H", _i), ("W", _i), ("h", _i), ("w", _i), ("C", _i), ("Cpad", _i),
+                ("layout", _i), ("blend", _i), ("ldx", _i), ("ldp", _i), ("ldo", _i), ("M", ctypes.c_longlong),
+                ("x", _p), ("y", _p), ("flow", _p), ("occ", _p), ("motion", _p), ("prev", _p), ("scale", _p), ("shift", _p),
+                ("weight", _p), ("bias", _p), ("source", _p), ("out", _p), ("out2", _p)]
+
+
 class DawnError(RuntimeError):
     pass
 
@@ -127,6 +140,7 @@ def _load():
     lib.dawn_lfg_last_launch_count.restype = ctypes.c_int64
     lib.dawn_lfg_workspace_bytes.argtypes = [vp]
     lib.dawn_lfg_workspace_bytes.restype = ctypes.c_int64
+    lib.dawn_lfg_test_kernel.argtypes = [ctypes.POINTER(DawnLfgKernelCase), vp]
     lib.dawn_last_error.restype = cp
     lib.dawn_build_info.restype = cp
     return lib
@@ -145,7 +159,7 @@ EXPORTS = ["dawn_unet_create", "dawn_unet_destroy", "dawn_unet_set_param", "dawn
 
 LFG_EXPORTS = ["dawn_lfg_create", "dawn_lfg_destroy", "dawn_lfg_set_param", "dawn_lfg_commit_params", "dawn_lfg_set_geometry",
                "dawn_lfg_set_source", "dawn_lfg_get_fea", "dawn_lfg_decode", "dawn_lfg_decode_sample", "dawn_lfg_read_tap",
-               "dawn_lfg_last_launch_count", "dawn_lfg_workspace_bytes"]
+               "dawn_lfg_last_launch_count", "dawn_lfg_workspace_bytes", "dawn_lfg_test_kernel"]
 MISC_EXPORTS = ["dawn_conv3x3_s2_relu"]
 
 PROF_CATS = ["conv3x3", "conv_other", "qkv_proj", "out_proj", "ca_gate", "gn_hcond", "attn_core", "sla_context",

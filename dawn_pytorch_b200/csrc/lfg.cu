@@ -198,10 +198,18 @@ int dawn_lfg_create(const dawn_lfg_cfg* cfg, dawn_lfg** out) {
   DAWN_CHECK(cfg->block_expansion % 64 == 0 && cfg->block_expansion <= 128, "lfg: block_expansion must be 64 or 128");
   DAWN_CHECK(cfg->num_down_blocks >= 1 && cfg->num_down_blocks <= 4, "lfg: num_down_blocks out of range");
   DAWN_CHECK(cfg->num_bottleneck_blocks >= 0 && cfg->num_bottleneck_blocks <= 32, "lfg: num_bottleneck_blocks out of range");
+  // the last up block yields min(max_features, block_expansion) channels and the final conv takes block_expansion (generator.py:59)
+  DAWN_CHECK(cfg->max_features >= cfg->block_expansion, "lfg: max_features must be at least block_expansion");
+  std::vector<int> C;
+  for (int i = 0; i <= cfg->num_down_blocks; ++i) {
+    C.push_back(std::min(cfg->max_features, cfg->block_expansion << i));                                        // generator.py:40-50
+    DAWN_CHECK(C.back() % 32 == 0, "lfg: every level width min(max_features, block_expansion * 2^i) must be a multiple of 32, got " +
+                                       std::to_string(C.back()));                                               // launch_gemm's n-tiles
+  }
   dawn_lfg* h = new dawn_lfg();
   h->cfg = *cfg;
   h->n = cfg->num_down_blocks;
-  for (int i = 0; i <= h->n; ++i) h->C.push_back(std::min(cfg->max_features, cfg->block_expansion << i));     // generator.py:40-50
+  h->C = C;
   *out = h;
   return 0;
 }
@@ -258,13 +266,9 @@ int dawn_lfg_commit_params(dawn_lfg* h) {
     const HostParam *w, *b;
     DAWN_TRY(h->raw.need("final.weight", {3, h->C[0], 7, 7}, &w));
     DAWN_TRY(h->raw.need("final.bias", {3}, &b));
-    std::vector<float> wp((size_t)49 * h->C[0] * 4, 0.f), bp(4, 0.f);
-    for (int o = 0; o < 3; ++o) {
-      bp[o] = b->data[o];
-      for (int c = 0; c < h->C[0]; ++c)
-        for (int t = 0; t < 49; ++t) wp[((size_t)t * h->C[0] + c) * 4 + o] = w->data[((size_t)o * h->C[0] + c) * 49 + t];
-    }
-    DAWN_TRY(dev_upload(h->owned, wp, &h->final_w));
+    std::vector<float> bp(4, 0.f);
+    for (int o = 0; o < 3; ++o) bp[o] = b->data[o];
+    DAWN_TRY(dev_upload(h->owned, lfg_final_pack(w->data.data(), h->C[0]), &h->final_w));
     DAWN_TRY(dev_upload(h->owned, bp, &h->final_b));
   }
   h->committed = true;

@@ -323,6 +323,13 @@ int launch_conv3x3_s2_relu(const float* x, int Ci, int H, int W, const float* wg
   DAWN_LAUNCH_OK();
   return 0;
 }
+std::vector<float> lfg_final_pack(const float* weight, int Cin) {
+  std::vector<float> wp((size_t)FK * FK * Cin * 4, 0.f);
+  for (int o = 0; o < 3; ++o)
+    for (int c = 0; c < Cin; ++c)
+      for (int t = 0; t < FK * FK; ++t) wp[((size_t)t * Cin + c) * 4 + o] = weight[((size_t)o * Cin + c) * FK * FK + t];
+  return wp;
+}
 int launch_lfg_final(const float* x, int ldx, int Cin, int F, int H, int W, const float* wpack, const float* bias3,
                      const float* source, const float4* motion, int h, int w, int blend, float* prediction, float* deformed,
                      cudaStream_t st) {

@@ -2,6 +2,7 @@
 // All activations are channels-last fp32 (frames, H, W, C); the per-clip source features are one frame (H, W, C).
 #pragma once
 #include <cuda_runtime.h>
+#include <vector>
 
 namespace dawn {
 
@@ -34,7 +35,9 @@ int launch_conv3x3_s2_relu(const float* x, int Ci, int H, int W, const float* wg
 // final 7x7 conv (Cin -> 3) + sigmoid + the last apply_optical with the source image (generator.py:163-167):
 //   prediction[f] = grid_sample(source, flow_f^) * occ_f^ + sigmoid(conv(x_f)) * (1 - occ_f^)     written as (F, 3, H, W)
 //   deformed[f]   = grid_sample(source, flow_f^)                                                  (optional, generator.py:152)
-// x: (F, H, W, Cin) channels-last; wpack: [49][Cin][4] (3 outputs + pad); source: (3, H, W) planar.
+// x: (F, H, W, Cin) channels-last; wpack: [49][Cin][4] (3 outputs + pad), lfg_final_pack of the (3, Cin, 7, 7) Conv2d weight;
+// source: (3, H, W) planar.
+std::vector<float> lfg_final_pack(const float* weight, int Cin);
 int launch_lfg_final(const float* x, int ldx, int Cin, int F, int H, int W, const float* wpack, const float* bias3,
                      const float* source, const float4* motion, int h, int w, int blend, float* prediction, float* deformed,
                      cudaStream_t st);

@@ -66,6 +66,31 @@ int dawn_conv3x3_s2_relu(const float* x, int Ci, int H, int W, const float* weig
 int64_t dawn_lfg_last_launch_count(dawn_lfg* h);
 int64_t dawn_lfg_workspace_bytes(dawn_lfg* h);
 
+/* Per-kernel tests: one decoder kernel on caller-owned device buffers, then a stream synchronise.  Channels-last tensors are
+ * (rows, ld) fp32 with the channels first in each row; motion is (F, h, w, 4) = (grid_x, grid_y, occlusion, unused).
+ *   MOTION_PACK       flow, occ (layout 0) or flow = sample (layout 1), F, h, w            -> out = motion
+ *   WARP_BLEND        x = skip (H, W, C), motion, F, h, w, prev / ldp (may be NULL)       -> out (F, H, W, ldo)
+ *   AFFINE_RELU       x (M, ldx), scale / shift (C, both NULL: plain ReLU), C, M           -> out (M, ldo); out may be x
+ *   RESIDUAL_BN_RELU  y, x (M, C), scale / shift, C, M                                    -> out = y + x, out2 (or NULL)
+ *   RELU_AVGPOOL2     x (H, W, C)                                                         -> out (H/2, W/2, C)
+ *   CHW_TO_HWC        x (C, H, W), Cpad                                                   -> out (H, W, Cpad)
+ *   HWC_TO_CHW        x (M, ldx), C, M                                                    -> out (C, M)
+ *   FINAL_CONV        x (F, H, W, ldx), C = Cin, weight (3, Cin, 7, 7), bias (3), source (3, H, W), motion, h, w,
+ *                     blend                                                               -> out = prediction, out2 = deformed
+ *                                                                                            (F, 3, H, W; out2 may be NULL)
+ * Returns -1 with a message for a missing pointer or a geometry the kernel does not take. */
+enum { DAWN_LFG_MOTION_PACK, DAWN_LFG_WARP_BLEND, DAWN_LFG_AFFINE_RELU, DAWN_LFG_RESIDUAL_BN_RELU, DAWN_LFG_RELU_AVGPOOL2,
+       DAWN_LFG_CHW_TO_HWC, DAWN_LFG_HWC_TO_CHW, DAWN_LFG_FINAL_CONV };
+typedef struct {
+  int kernel;
+  int F, H, W, h, w, C, Cpad, layout, blend;
+  int ldx, ldp, ldo;
+  long long M;
+  const float *x, *y, *flow, *occ, *motion, *prev, *scale, *shift, *weight, *bias, *source;
+  float *out, *out2;
+} dawn_lfg_kernel_case;
+int dawn_lfg_test_kernel(const dawn_lfg_kernel_case* c, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -129,9 +129,16 @@ def lfg_synth_value(name: str, shape) -> np.ndarray:
     raise ValueError(f"no synthetic LFG rule for {name} {shape}")
 
 
-def lfg_synth_state_dict(schema):
+def lfg_synth_state_dict(schema, residual_gain=1.0):
+    """residual_gain scales every ResBlock's second conv (weight and bias): with the He-uniform rule each block grows the
+    bottleneck activations by about 1.4x, so a long stack needs a smaller residual branch to stay O(1), as a trained one does."""
     import torch
-    return {n: torch.from_numpy(np.ascontiguousarray(lfg_synth_value(n, s))) for n, s in schema}
+    sd = {n: torch.from_numpy(np.ascontiguousarray(lfg_synth_value(n, s))) for n, s in schema}
+    if residual_gain != 1.0:
+        for n in sd:
+            if n.startswith('bottleneck.') and '.conv2.' in n:
+                sd[n] = sd[n] * np.float32(residual_gain)
+    return sd
 
 
 def lfg_synth_inputs(tag: str, F: int, H: int, W: int, h: int, w: int):
