@@ -3,4 +3,5 @@ Python module interface (DynamicNfUnet3D / DynamicNfGaussianDiffusion)."""
 from .unet import DynamicNfUnet3D, Unet3D  # noqa: F401
 from .diffusion import DynamicNfGaussianDiffusion, GaussianDiffusion  # noqa: F401
 from .lfg import Generator as LfgGenerator  # noqa: F401
+from .lfg import BGMotionPredictor, FlowAE, MotionGenerator, RegionPredictor  # noqa: F401
 from .flow_diffusion import Face_loc_Encoder, FlowDiffusion  # noqa: F401

@@ -73,6 +73,31 @@ class DawnLfgKernelCase(ctypes.Structure):
                 ("weight", _p), ("bias", _p), ("source", _p), ("out", _p), ("out2", _p)]
 
 
+class DawnLfgMotionCfg(ctypes.Structure):
+    """include/dawn_lfg.h: dawn_lfg_motion_cfg"""
+    _i, _f = ctypes.c_int, ctypes.c_float
+    _fields_ = [("num_regions", _i), ("num_channels", _i), ("estimate_affine", _i), ("pca_based", _i), ("fast_svd", _i),
+                ("rp_block_expansion", _i), ("rp_max_features", _i), ("rp_num_blocks", _i), ("rp_temperature", _f),
+                ("rp_scale_factor", _f), ("bg_block_expansion", _i), ("bg_max_features", _i), ("bg_num_blocks", _i),
+                ("bg_type", _i), ("pw_block_expansion", _i), ("pw_max_features", _i), ("pw_num_blocks", _i),
+                ("pw_scale_factor", _f), ("use_covar_heatmap", _i), ("use_deformed_source", _i),
+                ("estimate_occlusion_map", _i), ("revert_axis_swap", _i)]
+
+
+LFG_BG_ZERO, LFG_BG_AFFINE = 0, 1
+LFGM_AA_DOWN, LFGM_REGION_MOMENTS, LFGM_FLOW_INPUT, LFGM_FLOW_COMBINE, LFGM_BG_HEAD = range(5)
+
+
+class DawnLfgMotionKernelCase(ctypes.Structure):
+    """include/dawn_lfg.h: dawn_lfg_motion_kernel_case (pointers are device addresses)"""
+    _i, _p = ctypes.c_int, ctypes.c_void_p
+    _fields_ = [("kernel", _i), ("N", _i), ("H", _i), ("W", _i), ("h", _i), ("w", _i), ("R", _i), ("ld", _i), ("off", _i),
+                ("cw", _i), ("ldl", _i), ("revert", _i), ("temperature", ctypes.c_float),
+                ("x", _p), ("weight", _p), ("logits", _p), ("motion", _p), ("source", _p), ("bg", _p), ("fc_w", _p), ("fc_b", _p),
+                ("src_shift", _p), ("src_covar", _p), ("src_affine", _p), ("drv_shift", _p), ("drv_covar", _p), ("drv_affine", _p),
+                ("out", _p), ("out2", _p), ("out3", _p)]
+
+
 class DawnError(RuntimeError):
     pass
 
@@ -141,6 +166,21 @@ def _load():
     lib.dawn_lfg_workspace_bytes.argtypes = [vp]
     lib.dawn_lfg_workspace_bytes.restype = ctypes.c_int64
     lib.dawn_lfg_test_kernel.argtypes = [ctypes.POINTER(DawnLfgKernelCase), vp]
+    lib.dawn_lfg_motion_create.argtypes = [ctypes.POINTER(DawnLfgMotionCfg), ctypes.POINTER(vp)]
+    lib.dawn_lfg_motion_destroy.argtypes = [vp]
+    lib.dawn_lfg_motion_destroy.restype = None
+    lib.dawn_lfg_motion_set_param.argtypes = [vp, cp, fp, i64p, ctypes.c_int]
+    lib.dawn_lfg_motion_commit_params.argtypes = [vp]
+    lib.dawn_lfg_motion_set_geometry.argtypes = [vp] + [ctypes.c_int] * 3
+    lib.dawn_lfg_motion_regions.argtypes = [vp, fp, ctypes.c_int, fp, fp, fp, vp]
+    lib.dawn_lfg_motion_bg.argtypes = [vp, fp, ctypes.c_int, fp, ctypes.c_int, fp, vp]
+    lib.dawn_lfg_motion_flow.argtypes = [vp, fp, ctypes.c_int] + [fp] * 9 + [vp]
+    lib.dawn_lfg_motion_read_tap.argtypes = [vp, cp, fp, ip, ip, ip, ip, vp]
+    lib.dawn_lfg_motion_last_launch_count.argtypes = [vp]
+    lib.dawn_lfg_motion_last_launch_count.restype = ctypes.c_int64
+    lib.dawn_lfg_motion_workspace_bytes.argtypes = [vp]
+    lib.dawn_lfg_motion_workspace_bytes.restype = ctypes.c_int64
+    lib.dawn_lfg_motion_test_kernel.argtypes = [ctypes.POINTER(DawnLfgMotionKernelCase), vp]
     lib.dawn_last_error.restype = cp
     lib.dawn_build_info.restype = cp
     return lib
@@ -160,6 +200,11 @@ EXPORTS = ["dawn_unet_create", "dawn_unet_destroy", "dawn_unet_set_param", "dawn
 LFG_EXPORTS = ["dawn_lfg_create", "dawn_lfg_destroy", "dawn_lfg_set_param", "dawn_lfg_commit_params", "dawn_lfg_set_geometry",
                "dawn_lfg_set_source", "dawn_lfg_get_fea", "dawn_lfg_decode", "dawn_lfg_decode_sample", "dawn_lfg_read_tap",
                "dawn_lfg_last_launch_count", "dawn_lfg_workspace_bytes", "dawn_lfg_test_kernel"]
+LFG_MOTION_EXPORTS = ["dawn_lfg_motion_create", "dawn_lfg_motion_destroy", "dawn_lfg_motion_set_param",
+                      "dawn_lfg_motion_commit_params", "dawn_lfg_motion_set_geometry", "dawn_lfg_motion_regions", "dawn_lfg_motion_bg",
+                      "dawn_lfg_motion_flow", "dawn_lfg_motion_read_tap", "dawn_lfg_motion_last_launch_count",
+                      "dawn_lfg_motion_workspace_bytes", "dawn_lfg_motion_test_kernel"]
+LFG_EXPORTS += LFG_MOTION_EXPORTS                       # both handles are declared in include/dawn_lfg.h
 MISC_EXPORTS = ["dawn_conv3x3_s2_relu"]
 
 PROF_CATS = ["conv3x3", "conv_other", "qkv_proj", "out_proj", "ca_gate", "gn_hcond", "attn_core", "sla_context",

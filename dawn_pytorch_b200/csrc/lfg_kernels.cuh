@@ -6,6 +6,26 @@
 
 namespace dawn {
 
+// F.grid_sample(mode='bilinear', padding_mode='zeros', align_corners=False): corner indices, weights and validity (shared with
+// the motion estimator's sparse-motion sampling, lfg_motion_kernels.cu)
+struct Corners { int x0, y0; float wnw, wne, wsw, wse; bool vnw, vne, vsw, vse; };
+__device__ __forceinline__ Corners grid_corners(float gx, float gy, int H, int W) {
+  const float ix = ((gx + 1.f) * (float)W - 1.f) * 0.5f;
+  const float iy = ((gy + 1.f) * (float)H - 1.f) * 0.5f;
+  const float fx = floorf(ix), fy = floorf(iy);
+  Corners c;
+  // float -> int conversion saturates; far-away samples are simply invalid
+  c.x0 = (int)fminf(fmaxf(fx, -2.f), (float)W + 1.f);
+  c.y0 = (int)fminf(fmaxf(fy, -2.f), (float)H + 1.f);
+  const float ex = (fx + 1.f) - ix, ey = (fy + 1.f) - iy;        // (ix_se - ix), (iy_se - iy)
+  const float dx = ix - fx, dy = iy - fy;
+  c.wnw = ex * ey; c.wne = dx * ey; c.wsw = ex * dy; c.wse = dx * dy;
+  const bool inx0 = (fx >= 0.f) && (fx <= (float)(W - 1)), inx1 = (fx + 1.f >= 0.f) && (fx + 1.f <= (float)(W - 1));
+  const bool iny0 = (fy >= 0.f) && (fy <= (float)(H - 1)), iny1 = (fy + 1.f >= 0.f) && (fy + 1.f <= (float)(H - 1));
+  c.vnw = inx0 && iny0; c.vne = inx1 && iny0; c.vsw = inx0 && iny1; c.vse = inx1 && iny1;
+  return c;
+}
+
 // motion[f][y][x] = (grid_x, grid_y, occlusion, 0).
 // layout 0: flow (F, h, w, 2) + occ (F, 1, h, w)                              (forward_with_flow's arguments, generator.py:138)
 // layout 1: sample (3, F, h, w) = [grid_x, grid_y, conf]; occlusion = (conf + 1) / 2   (sample_one_video, FD:366-369)

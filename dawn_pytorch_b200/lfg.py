@@ -212,3 +212,408 @@ class Generator(nn.Module):
 
     def workspace_bytes(self):
         return int(lib.dawn_lfg_workspace_bytes(self._handle)) if self._handle is not None else 0
+
+
+# ====================================================================================================================================
+# Motion estimator of the LFG autoencoder: RegionPredictor, BGMotionPredictor, the Generator's PixelwiseFlowPredictor, and FlowAE
+# (LFG/modules/region_predictor.py, bg_motion_predictor.py, pixelwise_flow_predictor.py, flow_autoenc.py) behind the
+# dawn_lfg_motion handle of include/dawn_lfg.h.  Same constructor keywords and state_dict keys as the reference modules; the
+# sub-modules only hold parameters.  The 2x2 SVD of the region covariances runs on the host, as in the reference
+# (region_predictor.py:16-25): one device-to-host copy per RegionPredictor call.
+MOTION_CHUNK = 50                    # frames per stage call: bounds the workspace (the full-resolution background encoder) and
+                                     # keeps every activation index below 2^31
+
+
+def _encoder(be, cin, mx, nb):                               # Encoder (util.py:153-169)
+    m = _Holder()
+    m.down_blocks = nn.ModuleList([_conv_bn(cin if i == 0 else min(mx, be * 2 ** i), min(mx, be * 2 ** (i + 1)), 3)
+                                   for i in range(nb)])
+    return m
+
+
+def _hourglass(be, cin, mx, nb):                             # Hourglass (util.py:172-215)
+    m = _Holder()
+    m.encoder = _encoder(be, cin, mx, nb)
+    m.decoder = _Holder()
+    m.decoder.up_blocks = nn.ModuleList([_conv_bn((1 if i == nb - 1 else 2) * min(mx, be * 2 ** (i + 1)), min(mx, be * 2 ** i), 3)
+                                         for i in reversed(range(nb))])
+    m.out_filters = be + cin
+    return m
+
+
+def _anti_alias(channels, scale):
+    """AntiAliasInterpolation2d (util.py:217-251): the Gaussian `weight` buffer, built as the reference builds it."""
+    m = _Holder()
+    sigma = (1 / scale - 1) / 2
+    ks = 2 * round(sigma * 4) + 1
+    g = torch.exp(-(torch.arange(ks, dtype=torch.float32) - (ks - 1) / 2) ** 2 / (2 * sigma ** 2))
+    k = g.view(-1, 1) * g.view(1, -1)
+    m.register_buffer('weight', (k / torch.sum(k)).view(1, 1, ks, ks).repeat(channels, 1, 1, 1))
+    return m
+
+
+def _motion_cfg(**kw):
+    c = _lib.DawnLfgMotionCfg(num_regions=10, num_channels=3, estimate_affine=1, pca_based=1, fast_svd=0,
+                              rp_block_expansion=32, rp_max_features=1024, rp_num_blocks=5, rp_temperature=0.1, rp_scale_factor=0.25,
+                              bg_block_expansion=32, bg_max_features=1024, bg_num_blocks=5, bg_type=_lib.LFG_BG_AFFINE,
+                              pw_block_expansion=64, pw_max_features=1024, pw_num_blocks=5, pw_scale_factor=0.25,
+                              use_covar_heatmap=1, use_deformed_source=1, estimate_occlusion_map=1, revert_axis_swap=1)
+    for k, v in kw.items():
+        setattr(c, k, v)
+    return c
+
+
+class _MotionHandle:
+    """One dawn_lfg_motion handle holding one module's part of the motion estimator (its parameters under `prefix`)."""
+
+    def __init__(self, cfg, prefix):
+        self.cfg, self.prefix = cfg, prefix
+        self.handle, self.device_index, self.dirty, self.geom = None, None, True, None
+
+    def validate(self):
+        """dawn_lfg_motion_create refuses what the library cannot run; it needs no GPU."""
+        hd = ctypes.c_void_p()
+        check(lib.dawn_lfg_motion_create(ctypes.byref(self.cfg), ctypes.byref(hd)), "dawn_lfg_motion_create")
+        lib.dawn_lfg_motion_destroy(hd)
+
+    def destroy(self):
+        if self.handle is not None:
+            lib.dawn_lfg_motion_destroy(self.handle)
+        self.handle, self.geom = None, None
+
+    def ensure(self, module, device, n, H, W):
+        if device.type != "cuda":
+            raise _lib.DawnError("the LFG motion estimator runs on CUDA (sm_90a) only; there is no CPU path")
+        idx = device.index if device.index is not None else torch.cuda.current_device()
+        if self.handle is not None and self.device_index != idx:
+            self.destroy()
+            self.dirty = True
+        with torch.cuda.device(idx):
+            if self.handle is None:
+                hd = ctypes.c_void_p()
+                check(lib.dawn_lfg_motion_create(ctypes.byref(self.cfg), ctypes.byref(hd)), "dawn_lfg_motion_create")
+                self.handle, self.device_index = hd, idx
+            if self.dirty:
+                for name, t in module.state_dict().items():
+                    # a MotionGenerator's state_dict also holds the decoder, which its Generator handle uploads
+                    if name.endswith("num_batches_tracked") or (self.prefix == Generator.IGNORED_PREFIX and not name.startswith(self.prefix)):
+                        continue
+                    full = name if name.startswith(self.prefix) else self.prefix + name
+                    t = t.detach().to(device="cpu", dtype=torch.float32).contiguous()
+                    shape = (ctypes.c_int64 * max(t.dim(), 1))(*t.shape)
+                    check(lib.dawn_lfg_motion_set_param(self.handle, full.encode(), ctypes.c_void_p(t.data_ptr()), shape, t.dim()),
+                          f"dawn_lfg_motion_set_param({full})")
+                check(lib.dawn_lfg_motion_commit_params(self.handle), "dawn_lfg_motion_commit_params")
+                self.dirty, self.geom = False, None
+            frames = min(n, MOTION_CHUNK)
+            if self.geom is None or self.geom[1:] != (H, W) or self.geom[0] < frames:
+                check(lib.dawn_lfg_motion_set_geometry(self.handle, frames, H, W), "dawn_lfg_motion_set_geometry")
+                self.geom = (frames, H, W)
+        return self.geom[0]
+
+    def read_tap(self, name):
+        C, n, Hl, Wl = ctypes.c_int(), ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
+        args = (ctypes.byref(C), ctypes.byref(n), ctypes.byref(Hl), ctypes.byref(Wl))
+        check(lib.dawn_lfg_motion_read_tap(self.handle, name.encode(), None, *args, None), "dawn_lfg_motion_read_tap")
+        t = torch.empty((C.value, n.value, Hl.value, Wl.value), device=torch.device("cuda", self.device_index))
+        with torch.cuda.device(self.device_index):
+            check(lib.dawn_lfg_motion_read_tap(self.handle, name.encode(), ctypes.c_void_p(t.data_ptr()), *args,
+                                               ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)), "dawn_lfg_motion_read_tap")
+        return t.permute(1, 0, 2, 3).contiguous()
+
+
+class _MotionModule(nn.Module):
+    def _init_handle(self, cfg, prefix):
+        self._motion = _MotionHandle(cfg, prefix)
+        self._motion.validate()
+        self.register_load_state_dict_post_hook(lambda module, incompatible: module.mark_dirty())
+        self.eval()
+
+    def mark_dirty(self):
+        self._motion.dirty = True
+
+    def _apply(self, fn, *a, **k):
+        if "_motion" in self.__dict__:
+            self._motion.dirty = True
+        return super()._apply(fn, *a, **k)
+
+    def train(self, mode=True):
+        if mode:
+            raise NotImplementedError("the LFG motion estimator is inference-only (eval-mode BatchNorm)")
+        return super().train(False)
+
+    def __del__(self):
+        m = self.__dict__.get("_motion")
+        if m is not None:
+            try:
+                m.destroy()
+            except Exception:
+                pass
+
+    def read_tap(self, name):
+        """(n, C, Hl, Wl) copy of the last call's 'region_predictor' / 'bg_encoder' / 'flow_hourglass' output (last chunk)."""
+        return self._motion.read_tap(name)
+
+    def last_launch_count(self):
+        return int(lib.dawn_lfg_motion_last_launch_count(self._motion.handle)) if self._motion.handle is not None else 0
+
+
+def _ptr(t):
+    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
+
+
+class RegionPredictor(_MotionModule):
+    """region_predictor.py:28-117 with DAWN's region_predictor_params (pca_based, host SVD)."""
+
+    def __init__(self, block_expansion, num_regions, num_channels, max_features, num_blocks, temperature, estimate_affine=False,
+                 scale_factor=1, pca_based=False, fast_svd=False, pad=3):
+        super().__init__()
+        self.predictor = _hourglass(block_expansion, num_channels, max_features, num_blocks)
+        self.regions = nn.Conv2d(self.predictor.out_filters, num_regions, kernel_size=(7, 7), padding=pad)
+        self.jacobian = None
+        self.temperature, self.scale_factor, self.pca_based, self.fast_svd = temperature, scale_factor, pca_based, fast_svd
+        if scale_factor != 1:
+            self.down = _anti_alias(num_channels, scale_factor)
+        if pad != 3:
+            raise _lib.DawnError("RegionPredictor: only pad 3 (the 7x7 regions conv's same padding) is supported")
+        self._init_handle(_motion_cfg(num_regions=num_regions, num_channels=num_channels, estimate_affine=int(bool(estimate_affine)),
+                                      pca_based=int(bool(pca_based)), fast_svd=int(bool(fast_svd)), rp_block_expansion=block_expansion,
+                                      rp_max_features=max_features, rp_num_blocks=num_blocks, rp_temperature=temperature,
+                                      rp_scale_factor=scale_factor), "region_predictor.")
+
+    @torch.no_grad()
+    def forward(self, x):
+        n, _, H, W = x.shape
+        dev = x.device
+        chunk = self._motion.ensure(self, dev, n, H, W)
+        R = self.regions.out_channels
+        x = x.contiguous().float()
+        shift = torch.empty((n, R, 2), device=dev)
+        covar = torch.empty((n, R, 2, 2), device=dev)
+        heat = torch.empty((n, R, H // 4, W // 4), device=dev)
+        with torch.cuda.device(dev):
+            st = Generator._stream()
+            for a in range(0, n, chunk):
+                b = min(n, a + chunk)
+                check(lib.dawn_lfg_motion_regions(self._motion.handle, _ptr(x[a:b]), b - a, _ptr(shift[a:b]), _ptr(covar[a:b]),
+                                                  _ptr(heat[a:b]), st), "dawn_lfg_motion_regions")
+        u, s, _ = torch.svd(covar.view(-1, 2, 2).cpu())                   # region_predictor.py:16-25, as the reference does
+        u, s = u.to(dev), s.to(dev)
+        d = torch.diag_embed(s ** 0.5)
+        affine = torch.matmul(u, d).view(n, R, 2, 2)
+        return {"shift": shift, "covar": covar, "heatmap": heat, "affine": affine, "u": u, "d": d}
+
+
+class BGMotionPredictor(_MotionModule):
+    """bg_motion_predictor.py:15-57 with bg_type 'affine' (DAWN's) or 'zero'."""
+
+    def __init__(self, block_expansion, num_channels, max_features, num_blocks, bg_type='zero'):
+        super().__init__()
+        if bg_type not in ('zero', 'affine'):
+            raise _lib.DawnError(f"dawn_lfg_motion_create failed: lfg_motion: bg_type must be 'affine' or 'zero', got {bg_type!r}")
+        self.bg_type = bg_type
+        if bg_type != 'zero':
+            self.encoder = _encoder(block_expansion, num_channels * 2, max_features, num_blocks)
+            self.fc = nn.Linear(min(max_features, block_expansion * 2 ** num_blocks), 6)
+        self._init_handle(_motion_cfg(num_channels=num_channels, bg_block_expansion=block_expansion, bg_max_features=max_features,
+                                      bg_num_blocks=num_blocks,
+                                      bg_type=_lib.LFG_BG_AFFINE if bg_type == 'affine' else _lib.LFG_BG_ZERO), "bg_predictor.")
+
+    @torch.no_grad()
+    def forward(self, source_image, driving_image):
+        n, _, H, W = driving_image.shape
+        dev = driving_image.device
+        if source_image.device != dev:
+            raise _lib.DawnError("source and driving images must be on the same device")
+        chunk = self._motion.ensure(self, dev, n, H, W)
+        src = source_image.contiguous().float()
+        drv = driving_image.contiguous().float()
+        shared = src.shape[0] == 1 and n > 1
+        out = torch.empty((n, 3, 3), device=dev)
+        with torch.cuda.device(dev):
+            st = Generator._stream()
+            for a in range(0, n, chunk):
+                b = min(n, a + chunk)
+                s = src if shared else src[a:b]
+                check(lib.dawn_lfg_motion_bg(self._motion.handle, _ptr(s), s.shape[0], _ptr(drv[a:b]), b - a, _ptr(out[a:b]), st),
+                      "dawn_lfg_motion_bg")
+        return out
+
+
+class _FlowPredictor(_Holder):
+    """pixelwise_flow_predictor.py:16-46: parameters only; the computation is MotionGenerator.forward."""
+
+    def __init__(self, block_expansion, num_blocks, max_features, num_regions, num_channels, estimate_occlusion_map=False,
+                 scale_factor=1, region_var=0.01, use_covar_heatmap=False, use_deformed_source=True, revert_axis_swap=False):
+        super().__init__()
+        self.hourglass = _hourglass(block_expansion, (num_regions + 1) * (num_channels * use_deformed_source + 1), max_features,
+                                    num_blocks)
+        self.mask = nn.Conv2d(self.hourglass.out_filters, num_regions + 1, kernel_size=(7, 7), padding=(3, 3))
+        self.occlusion = nn.Conv2d(self.hourglass.out_filters, 1, kernel_size=(7, 7), padding=(3, 3)) if estimate_occlusion_map else None
+        if scale_factor != 1:
+            self.down = _anti_alias(num_channels, scale_factor)
+        self.cfg_kw = dict(pw_block_expansion=block_expansion, pw_num_blocks=num_blocks, pw_max_features=max_features,
+                           num_regions=num_regions, num_channels=num_channels, estimate_occlusion_map=int(bool(estimate_occlusion_map)),
+                           pw_scale_factor=scale_factor, use_covar_heatmap=int(bool(use_covar_heatmap)),
+                           use_deformed_source=int(bool(use_deformed_source)), revert_axis_swap=int(bool(revert_axis_swap)))
+
+
+class MotionGenerator(Generator):
+    """The reference Generator with its pixelwise flow predictor (generator.py:20-130): the state_dict holds all of the
+    checkpoint's `generator` entry, and forward(source_image, driving_region_params, source_region_params, bg_params) runs the flow
+    predictor on the device, then the decoder of Generator (one decode per distinct source image)."""
+
+    def __init__(self, num_channels, num_regions, block_expansion, max_features, num_down_blocks, num_bottleneck_blocks,
+                 pixelwise_flow_predictor_params=None, skips=False, revert_axis_swap=True):
+        if pixelwise_flow_predictor_params is None:
+            raise _lib.DawnError("MotionGenerator needs pixelwise_flow_predictor_params; use Generator for the decoder alone")
+        pw = _FlowPredictor(num_regions=num_regions, num_channels=num_channels, revert_axis_swap=revert_axis_swap,
+                            **pixelwise_flow_predictor_params)
+        Generator.__init__(self, num_channels, num_regions, block_expansion, max_features, num_down_blocks, num_bottleneck_blocks,
+                           None, skips, revert_axis_swap)
+        self._modules = {"pixelwise_flow_predictor": pw, **self._modules}    # registered first, as generator.py:29-34 does
+        self.num_regions = num_regions
+        self._motion = _MotionHandle(_motion_cfg(**pw.cfg_kw), Generator.IGNORED_PREFIX)
+        self._motion.validate()
+
+    # keeps pixelwise_flow_predictor.* (the parent class drops them)
+    @classmethod
+    def _drop_training_only_keys(cls, state_dict, prefix, *args):
+        return None
+
+    def mark_dirty(self):
+        self._dirty = True
+        if "_motion" in self.__dict__:
+            self._motion.dirty = True
+
+    def _apply(self, fn, *a, **k):
+        if "_motion" in self.__dict__:
+            self._motion.dirty = True
+        return super()._apply(fn, *a, **k)
+
+    def __del__(self):
+        m = self.__dict__.get("_motion")
+        if m is not None:
+            try:
+                m.destroy()
+            except Exception:
+                pass
+        super().__del__()
+
+    @torch.no_grad()
+    def flow(self, source_image, driving_region_params, source_region_params, bg_params=None):
+        """pixelwise_flow_predictor.py:111-137 for n frames of one source image (1 or n, 3, H, W) -> optical_flow, occlusion_map."""
+        drv, srcp = driving_region_params, source_region_params
+        n = drv["shift"].shape[0]
+        H, W = source_image.shape[-2:]
+        dev = source_image.device
+        chunk = self._motion.ensure(self, dev, n, H, W)
+        R = self.num_regions
+        src = source_image.reshape(-1, 3, H, W)[0].contiguous().float()
+
+        def per_frame(t, shape):
+            t = t.float()
+            return (t.expand(n, *shape) if t.shape[0] == 1 else t).contiguous()
+
+        ss, sc, sa = per_frame(srcp["shift"], (R, 2)), per_frame(srcp["covar"], (R, 2, 2)), per_frame(srcp["affine"], (R, 2, 2))
+        ds, dc, da = per_frame(drv["shift"], (R, 2)), per_frame(drv["covar"], (R, 2, 2)), per_frame(drv["affine"], (R, 2, 2))
+        bg = per_frame(bg_params, (3, 3)) if bg_params is not None else None
+        flow = torch.empty((n, H // 4, W // 4, 2), device=dev)
+        occ = torch.empty((n, 1, H // 4, W // 4), device=dev)
+        with torch.cuda.device(dev):
+            st = self._stream()
+            for a in range(0, n, chunk):
+                b = min(n, a + chunk)
+                check(lib.dawn_lfg_motion_flow(self._motion.handle, _ptr(src), b - a, _ptr(ss[a:b]), _ptr(sc[a:b]), _ptr(sa[a:b]),
+                                               _ptr(ds[a:b]), _ptr(dc[a:b]), _ptr(da[a:b]), _ptr(bg[a:b]) if bg is not None else None,
+                                               _ptr(flow[a:b]), _ptr(occ[a:b]), st), "dawn_lfg_motion_flow")
+        return {"optical_flow": flow, "occlusion_map": occ}
+
+    @torch.no_grad()
+    def forward(self, source_image, driving_region_params, source_region_params, bg_params=None):
+        """generator.py:92-130: prediction, deformed, optical_flow, occlusion_map and bottle_neck_feat for a batch of frames.
+        Frames that share one source image are decoded together."""
+        if source_image.device.type != "cuda":
+            raise _lib.DawnError("the LFG motion estimator runs on CUDA (sm_90a) only; there is no CPU path")
+        n = source_image.shape[0]
+        groups = []                                                     # runs of frames with the same source image
+        for i in range(n):
+            if groups and torch.equal(source_image[i], source_image[groups[-1][0]]):
+                groups[-1].append(i)
+            else:
+                groups.append([i])
+        outs = []
+        for g in groups:
+            a, b = g[0], g[-1] + 1
+            sel = lambda p: {k: v[a:b] for k, v in p.items()}            # noqa: E731
+            m = self.flow(source_image[a:a + 1], sel(driving_region_params), sel(source_region_params),
+                          bg_params[a:b] if bg_params is not None else None)
+            o = self.forward_with_flow(source_image[a:a + 1], m["optical_flow"], m["occlusion_map"])
+            fea = self.compute_fea(source_image[a:a + 1])
+            outs.append({"prediction": o["prediction"], "deformed": o["deformed"], "optical_flow": m["optical_flow"],
+                         "occlusion_map": m["occlusion_map"], "bottle_neck_feat": fea.expand(b - a, -1, -1, -1)})
+        out = {k: torch.cat([o[k] for o in outs]) for k in outs[0]}
+        out["bottle_neck_feat"] = out["bottle_neck_feat"].contiguous()
+        return out
+
+    def read_tap(self, name):
+        """'flow_hourglass' reads the flow predictor; every other name the decoder (Generator.read_tap)."""
+        return self._motion.read_tap(name) if name == "flow_hourglass" else super().read_tap(name)
+
+
+class FlowAE(nn.Module):
+    """flow_autoenc.py:15-51: region predictor, background predictor and generator of one LFG checkpoint; forward() reconstructs
+    dri_img from ref_img into self.generated.  CUDA tensors only."""
+
+    def __init__(self, is_train=False, config_pth=None):
+        super().__init__()
+        if is_train:
+            raise NotImplementedError("FlowAE training is out of scope: this is the inference path")
+        mp = _default_model_params()
+        if config_pth is not None:
+            import yaml
+            with open(config_pth) as f:
+                mp = yaml.safe_load(f)['model_params']
+        self.generator = MotionGenerator(num_regions=mp['num_regions'], num_channels=mp['num_channels'],
+                                         revert_axis_swap=mp['revert_axis_swap'], **mp['generator_params'])
+        self.region_predictor = RegionPredictor(num_regions=mp['num_regions'], num_channels=mp['num_channels'],
+                                                estimate_affine=mp['estimate_affine'], **mp['region_predictor_params'])
+        self.bg_predictor = BGMotionPredictor(num_channels=mp['num_channels'], **mp['bg_predictor_params'])
+        self.is_train = is_train
+        self.ref_img = self.dri_img = self.generated = None
+        self.eval()
+
+    def train(self, mode=True):
+        if mode:
+            raise NotImplementedError("FlowAE here is inference-only")
+        return super().train(False)
+
+    def set_train_input(self, ref_img, dri_img):
+        self.ref_img, self.dri_img = ref_img, dri_img
+
+    @torch.no_grad()
+    def forward(self):
+        for t in (self.ref_img, self.dri_img):
+            if t.device.type != "cuda":
+                raise _lib.DawnError("FlowAE runs on CUDA (sm_90a) only; there is no CPU path")
+        source_region_params = self.region_predictor(self.ref_img)
+        self.driving_region_params = self.region_predictor(self.dri_img)
+        bg_params = self.bg_predictor(self.ref_img, self.dri_img)
+        self.generated = self.generator(self.ref_img, source_region_params=source_region_params,
+                                        driving_region_params=self.driving_region_params, bg_params=bg_params)
+        self.generated.update({'source_region_params': source_region_params, 'driving_region_params': self.driving_region_params})
+
+
+def _default_model_params():
+    """model_params of config/hdtf256.yaml (== hdtf128.yaml)."""
+    return {
+        'num_regions': 10, 'num_channels': 3, 'estimate_affine': True, 'revert_axis_swap': True,
+        'bg_predictor_params': {'block_expansion': 32, 'max_features': 1024, 'num_blocks': 5, 'bg_type': 'affine'},
+        'region_predictor_params': {'temperature': 0.1, 'block_expansion': 32, 'max_features': 1024, 'scale_factor': 0.25,
+                                    'num_blocks': 5, 'pca_based': True, 'fast_svd': False},
+        'generator_params': {'block_expansion': 64, 'max_features': 512, 'num_down_blocks': 2, 'num_bottleneck_blocks': 6,
+                             'skips': True,
+                             'pixelwise_flow_predictor_params': {'block_expansion': 64, 'max_features': 1024, 'num_blocks': 5,
+                                                                 'scale_factor': 0.25, 'use_deformed_source': True,
+                                                                 'use_covar_heatmap': True, 'estimate_occlusion_map': True}},
+    }

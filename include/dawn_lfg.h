@@ -91,6 +91,81 @@ typedef struct {
 } dawn_lfg_kernel_case;
 int dawn_lfg_test_kernel(const dawn_lfg_kernel_case* c, void* stream);
 
+/* ================================================================================================================================
+ * dawn_lfg_motion — the motion estimator of the LFG autoencoder: RegionPredictor (LFG/modules/region_predictor.py),
+ * BGMotionPredictor (bg_motion_predictor.py) and the Generator's PixelwiseFlowPredictor (pixelwise_flow_predictor.py), which
+ * FlowAE (flow_autoenc.py) runs before the decoder above.  Same conventions as dawn_lfg: one handle per GPU, not thread-safe,
+ * stream-ordered, no host synchronisation inside the three stage entries, fp32 device tensors, 0 / -1 / -2 returns.
+ * The 2x2 SVD of the region covariances (region_predictor.py:16-25) is not here: the reference runs it on the host.
+ */
+typedef struct dawn_lfg_motion dawn_lfg_motion;
+
+enum { DAWN_LFG_BG_ZERO = 0, DAWN_LFG_BG_AFFINE = 1 };
+
+/* model_params of config/hdtf128.yaml / hdtf256.yaml; create accepts exactly DAWN's shipped values (in the comments), except
+ * bg_type (zero or affine) and revert_axis_swap (either) */
+typedef struct {
+  int num_regions, num_channels;                                 /* 10, 3 */
+  int estimate_affine, pca_based, fast_svd;                      /* 1, 1, 0 */
+  int rp_block_expansion, rp_max_features, rp_num_blocks;        /* 32, 1024, 5 */
+  float rp_temperature, rp_scale_factor;                         /* 0.1, 0.25 */
+  int bg_block_expansion, bg_max_features, bg_num_blocks;        /* 32, 1024, 5 */
+  int bg_type;                                                   /* DAWN_LFG_BG_AFFINE or DAWN_LFG_BG_ZERO */
+  int pw_block_expansion, pw_max_features, pw_num_blocks;        /* 64, 1024, 5 */
+  float pw_scale_factor;                                         /* 0.25 */
+  int use_covar_heatmap, use_deformed_source, estimate_occlusion_map;   /* 1, 1, 1 */
+  int revert_axis_swap;                                          /* 0 or 1 */
+} dawn_lfg_motion_cfg;
+
+int dawn_lfg_motion_create(const dawn_lfg_motion_cfg* cfg, dawn_lfg_motion** out);
+void dawn_lfg_motion_destroy(dawn_lfg_motion* h);
+/* reference state_dict keys: region_predictor.* / bg_predictor.* entries as those modules name them, prefixed "region_predictor."
+ * and "bg_predictor.", and the generator's "pixelwise_flow_predictor.*" (including each down.weight Gaussian buffer);
+ * *.num_batches_tracked is accepted and ignored */
+int dawn_lfg_motion_set_param(dawn_lfg_motion* h, const char* name, const float* host, const int64_t* shape, int ndim);
+/* fold the eval-mode BatchNorms into the convolutions that precede them, repack and upload */
+int dawn_lfg_motion_commit_params(dawn_lfg_motion* h);
+/* at most `frames` frames per stage call; H, W multiples of 128 */
+int dawn_lfg_motion_set_geometry(dawn_lfg_motion* h, int frames, int H, int W);
+
+/* RegionPredictor.forward up to the SVD (region_predictor.py:77-104): images (n, 3, H, W) -> shift (n, R, 2), covar (n, R, 2, 2),
+ * heatmap (n, R, H/4, W/4) or NULL */
+int dawn_lfg_motion_regions(dawn_lfg_motion* h, const float* images, int n, float* shift, float* covar, float* heatmap, void* stream);
+/* BGMotionPredictor.forward: source (n_source = 1 or n, 3, H, W), driving (n, 3, H, W) -> bg (n, 3, 3) */
+int dawn_lfg_motion_bg(dawn_lfg_motion* h, const float* source, int n_source, const float* driving, int n, float* bg, void* stream);
+/* PixelwiseFlowPredictor.forward for n frames of one source image (3, H, W): region parameters (n, R, 2) / (n, R, 2, 2) of the
+ * source and of the driving frames, bg (n, 3, 3) or NULL -> flow (n, H/4, W/4, 2) and occlusion (n, 1, H/4, W/4), the layout
+ * dawn_lfg_decode takes */
+int dawn_lfg_motion_flow(dawn_lfg_motion* h, const float* source, int n, const float* src_shift, const float* src_covar,
+                         const float* src_affine, const float* drv_shift, const float* drv_covar, const float* drv_affine,
+                         const float* bg, float* flow, float* occlusion, void* stream);
+/* sub-module parity: the last call's "region_predictor" (Hourglass output, 35 channels), "bg_encoder" (last Encoder level) or
+ * "flow_hourglass" (108 channels) as (C, n, Hl, Wl); *n is the frame count of that call.  dst may be NULL to query the shape. */
+int dawn_lfg_motion_read_tap(dawn_lfg_motion* h, const char* name, float* dst, int* C, int* n, int* Hl, int* Wl, void* stream);
+int64_t dawn_lfg_motion_last_launch_count(dawn_lfg_motion* h);
+int64_t dawn_lfg_motion_workspace_bytes(dawn_lfg_motion* h);
+
+/* Per-kernel tests: one motion-estimator kernel on caller-owned device buffers, then a stream synchronise.
+ *   AA_DOWN         x = images (N, 3, H, W), weight (3, 13, 13)      -> out (N, H/4, W/4, ld): channels [off, off + cw), 3 real
+ *   REGION_MOMENTS  logits (N, h, w, ldl) first R columns, temperature -> out = shift (N, R, 2), out2 = covar (N, R, 2, 2),
+ *                                                                         out3 = heatmap (N, R, h, w) or NULL
+ *   FLOW_INPUT      source (h, w, 4) channels-last, src_/drv_ shift / covar / affine (N, R, ...), bg (N, 3, 3) or NULL, revert
+ *                                                                      -> out (N, h, w, ld) channels [off, off + cw), 4 (R + 1) real;
+ *                                                                         out2 = motion (N, h, w, 2 (R + 1))
+ *   FLOW_COMBINE    logits (N, h, w, ldl) R + 2 columns, motion (N, h, w, 2 (R + 1)) -> out = flow (N, h, w, 2), out2 = occ (N, 1, h, w)
+ *   BG_HEAD         x (N, P = h w, ld) C = cw channels, fc_w (6, C) / fc_b (6) or both NULL -> out (N, 3, 3) */
+enum { DAWN_LFG_MOTION_AA_DOWN, DAWN_LFG_MOTION_REGION_MOMENTS, DAWN_LFG_MOTION_FLOW_INPUT, DAWN_LFG_MOTION_FLOW_COMBINE,
+       DAWN_LFG_MOTION_BG_HEAD };
+typedef struct {
+  int kernel;
+  int N, H, W, h, w, R, ld, off, cw, ldl, revert;
+  float temperature;
+  const float *x, *weight, *logits, *motion, *source, *bg, *fc_w, *fc_b;
+  const float *src_shift, *src_covar, *src_affine, *drv_shift, *drv_covar, *drv_affine;
+  float *out, *out2, *out3;
+} dawn_lfg_motion_kernel_case;
+int dawn_lfg_motion_test_kernel(const dawn_lfg_motion_kernel_case* c, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
