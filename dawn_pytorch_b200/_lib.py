@@ -60,6 +60,34 @@ class DawnFusedCase(ctypes.Structure):
                 ("gn_stats", _p), ("gn_count", ctypes.c_double), ("cpg", _i), ("gn_w", _p), ("gn_b", _p), ("film", _p)]
 
 
+KERNEL_ROWSTATS, KERNEL_GN_APPLY, KERNEL_COND_TABLES, KERNEL_TIME_MLP, KERNEL_FILM, KERNEL_ROTARY, KERNEL_SPLIT_ROWS, \
+    KERNEL_NCF_TO_NHWC, KERNEL_FRAME_INVARIANCE, KERNEL_FEA_SHIFT, KERNEL_MAP_REDUCE, KERNEL_INIT_CONV_X3, KERNEL_HEADS_OUT = range(13)
+KERNEL_MAX_DESC = 16
+
+
+class DawnKernelDesc(ctypes.Structure):
+    """include/dawn_unet.h: dawn_kernel_desc (pointers are device addresses)"""
+    _i, _p = ctypes.c_int, ctypes.c_void_p
+    _fields_ = [("off", _i), ("K", _i), ("co", _i), ("ldbT", _i), ("ca", _i),
+                ("mW", _p), ("mB", _p), ("Wkv", _p), ("nkv", _p), ("qs", _p), ("ks", _p), ("Wout", _p), ("gout", _p),
+                ("ctx", _p), ("kv", _p), ("kq", _p), ("nkq", _p), ("T", _p), ("G", _p),
+                ("W", _p), ("b", _p), ("out", _p), ("n", _i)]
+
+
+class DawnKernelCase(ctypes.Structure):
+    """include/dawn_unet.h: dawn_kernel_case (pointers are device addresses)"""
+    _i, _p, _ll = ctypes.c_int, ctypes.c_void_p, ctypes.c_longlong
+    _fields_ = [("kernel", _i), ("M", _i), ("C", _i), ("ld", _i), ("ldy", _i), ("ldr", _i), ("ldo", _i),
+                ("F", _i), ("H", _i), ("W", _i), ("P", _i), ("clips", _i),
+                ("Cpad", _i), ("c0", _i), ("k", _i), ("skip_if", _i), ("cpg", _i), ("t_stride", _i), ("pos0", _i), ("dim", _i),
+                ("ng", _i), ("nc", _i), ("cond_ld", _i), ("ndesc", _i),
+                ("n", _ll), ("cstride", _ll), ("clip_stride", _ll), ("count", ctypes.c_double), ("eps", ctypes.c_float),
+                ("x", _p), ("y", _p), ("res", _p), ("w", _p), ("b", _p), ("w2", _p), ("b2", _p),
+                ("map", _p), ("freqs", _p), ("stats", _p), ("t", _p), ("skip_flag", _p),
+                ("out", _p), ("out_hi", _p), ("out_lo", _p), ("flag", _p),
+                ("desc", DawnKernelDesc * KERNEL_MAX_DESC)]
+
+
 LFG_MOTION_PACK, LFG_WARP_BLEND, LFG_AFFINE_RELU, LFG_RESIDUAL_BN_RELU, LFG_RELU_AVGPOOL2, LFG_CHW_TO_HWC, LFG_HWC_TO_CHW, \
     LFG_FINAL_CONV = range(8)
 
@@ -132,6 +160,7 @@ def _load():
     lib.dawn_unet_workspace_bytes.restype = ctypes.c_int64
     lib.dawn_test_contraction.argtypes = [ctypes.POINTER(DawnContractionCase), vp]
     lib.dawn_test_fused.argtypes = [ctypes.POINTER(DawnFusedCase), vp]
+    lib.dawn_test_kernel.argtypes = [ctypes.POINTER(DawnKernelCase), vp]
     lib.dawn_nccl_unique_id.argtypes = [ctypes.c_char_p]
     lib.dawn_unet_init_shard.argtypes = [vp, ctypes.c_char_p, ctypes.c_int, ctypes.c_int, ctypes.c_int]
     lib.dawn_unet_shard_ipc_export.argtypes = [vp, ctypes.c_char_p]
@@ -194,7 +223,7 @@ EXPORTS = ["dawn_unet_create", "dawn_unet_destroy", "dawn_unet_set_param", "dawn
            "dawn_unet_profile_enable", "dawn_unet_profile_read", "dawn_unet_last_launch_count", "dawn_unet_workspace_bytes", "dawn_ddim_step", "dawn_unet_ddim_step", "dawn_unet_sampler_capture", "dawn_unet_sampler_launch",
            "dawn_unet_ddim_step_guided", "dawn_unet_sampler_capture_guided", "dawn_unet_sampler_launch_guided",
            "dawn_ddpm_step", "dawn_unet_ddpm_step", "dawn_unet_ddpm_capture", "dawn_unet_ddpm_launch",
-           "dawn_test_contraction", "dawn_test_fused", "dawn_last_error", "dawn_build_info"]
+           "dawn_test_contraction", "dawn_test_fused", "dawn_test_kernel", "dawn_last_error", "dawn_build_info"]
 
 
 LFG_EXPORTS = ["dawn_lfg_create", "dawn_lfg_destroy", "dawn_lfg_set_param", "dawn_lfg_commit_params", "dawn_lfg_set_geometry",

@@ -27,12 +27,16 @@ __device__ __forceinline__ float update_eps(const float* __restrict__ eps, const
   return eps_n ? guided_eps(eps[i], eps_n[i], g) : eps[i];
 }
 
-// keys[i] = |ca * x - cb * e|, e = update_eps  (x0 magnitude; non-negative floats order like their bit patterns)
+// x0 = ca * x - cb * e rounded like the reference's two products and one difference (U:1072-1076).  A fused multiply-add
+// would keep ca * x unrounded: near t = 999 both products are ~3e4 times x and cancel, so that moved the sample by 1e-5.
+__device__ __forceinline__ float ddim_x0(float ca, float x, float cb, float e) { return __fsub_rn(__fmul_rn(ca, x), __fmul_rn(cb, e)); }
+
+// keys[i] = |x0|, e = update_eps  (x0 magnitude; non-negative floats order like their bit patterns)
 __global__ void x0_abs_kernel(const float* __restrict__ x, const float* __restrict__ eps, const float* __restrict__ eps_n,
                               const float* __restrict__ scale, float ca, float cb, long long n, uint32_t* __restrict__ keys) {
   const float g = eps_n ? *scale : 0.0f;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-    keys[i] = __float_as_uint(fabsf(ca * x[i] - cb * update_eps(eps, eps_n, g, i)));
+    keys[i] = __float_as_uint(fabsf(ddim_x0(ca, x[i], cb, update_eps(eps, eps_n, g, i))));
 }
 
 // one launch instead of a pageable-host memcpy + three memsets (keeps the step capturable in a CUDA graph)
@@ -119,7 +123,7 @@ __global__ void ddim_update_kernel(float* __restrict__ x, float* __restrict__ x_
   const float g = eps_n ? *scale : 0.0f;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const float e = update_eps(eps, eps_n, g, i);
-    float x0 = ca * x[i] - cb * e;
+    float x0 = ddim_x0(ca, x[i], cb, e);
     if (clamp) x0 = fminf(fmaxf(x0, -s), s) / s;
     float v = x0 * sqrt_an + c * e;
     if (noise) v += sigma * noise[i];

@@ -283,6 +283,55 @@ typedef struct {
 } dawn_fused_case;
 int dawn_test_fused(const dawn_fused_case* c, void* stream);
 
+/* One per-clip or per-step glue kernel of the UNet (csrc/kernels.cu), through the launcher the network calls, on caller-owned
+ * buffers, for per-kernel tests against a high-precision reference.  The COND_TABLES and FILM descriptor arrays are built
+ * on the device from `desc`.  Returns -1 and launches nothing when the geometry is refused, -2 on a CUDA error; synchronises
+ * the stream before it returns.  Fields a kernel does not name are ignored. */
+enum {
+  DAWN_KERNEL_ROWSTATS = 0,        /* out[m] = (mean, 1/sqrt(biased var + eps)) of x row m (C channels, stride ld), m < M */
+  DAWN_KERNEL_GN_APPLY = 1,        /* out = SiLU(GN(y) w + b) (+ res) from stats [clips][8][2] (fp64 sum, sum of squares over count
+                                      values), cpg channels per group; row r is in clip (r / P) % clips */
+  DAWN_KERNEL_COND_TABLES = 2,     /* desc[0..ndesc): ctx = Linear(SiLU(x[:, off:off+K])) (x = cond, row stride cond_ld), kv = ctx Wkv^T,
+                                      then kq, nkq, G, T of slot ca; F table frames of `clips` clips */
+  DAWN_KERNEL_TIME_MLP = 3,        /* out[clip] = SiLU(Linear2(GELU(Linear1(sinusoidal(t[clip * t_stride]))))), freqs [dim/2] */
+  DAWN_KERNEL_FILM = 4,            /* desc[d].out[clip][j] = desc[d].W[j] . x[clip] + desc[d].b[j], x = t_silu [clips][C] */
+  DAWN_KERNEL_ROTARY = 5,          /* out[f][i] = (cos, sin)((pos0 + f) freqs[i]), f < F, i < 16 */
+  DAWN_KERNEL_SPLIT_ROWS = 6,      /* out_hi / out_lo = fp16 hi | lo planes [M][C] of x (row stride ld) */
+  DAWN_KERNEL_NCF_TO_NHWC = 7,     /* x (clips, C, F, P) -> out (F * clips, P, Cpad) at channel c0, other channels zero */
+  DAWN_KERNEL_FRAME_INVARIANCE = 8,/* flag[b] = channels [c0, C) of clip b of x (clips, C, F, P) differ between frames; flag[clips] counts */
+  DAWN_KERNEL_FEA_SHIFT = 9,       /* k row-shifted channels-last copies (Cpad, at channel c0) of one (C, H, W) frame per clip */
+  DAWN_KERNEL_MAP_REDUCE = 10,     /* out[i] = b[i % C] + sum_{s < k} x[s * n + i], i < n */
+  DAWN_KERNEL_INIT_CONV_X3 = 11,   /* out[f * clips + b][p][0, C) (row stride ldo) = map[b][p] + k x k conv of x (clip b at
+                                      x + b * clip_stride, (3, F, H, W)) with w [k * k * 3][C] */
+  DAWN_KERNEL_HEADS_OUT = 12       /* out[b][j][f][p] = 1x1 heads of x (j < ng: w, b) and y (j >= ng: w2, b2), C channels, P = H*W */
+};
+#define DAWN_KERNEL_MAX_DESC 16
+typedef struct {
+  int off, K, co, ldbT, ca;        /* COND_TABLES: cond columns [off, off + K), block width co (MLP width 2 co), T row stride, slot */
+  const float* mW; const float* mB;/* [2 co][K], [2 co] */
+  const float* Wkv;                /* [128][2 co] */
+  const float* nkv; const float* qs; const float* ks;   /* [2][8], [8], [8] */
+  const float* Wout; const float* gout;                 /* [co][64], [co] */
+  float* ctx; float* kv;           /* [F][2 co], [F][128] (table order) */
+  float* kq; float* nkq; float* T; float* G;            /* [F][3][64], [3][8], [F][32][ldbT], [F][3][81] */
+  const float* W; const float* b; float* out; int n;    /* FILM: [n][C], [n], [clips][n] */
+} dawn_kernel_desc;
+typedef struct {
+  int kernel;                      /* DAWN_KERNEL_* */
+  int M, C, ld, ldy, ldr, ldo;
+  int F, H, W, P, clips;
+  int Cpad, c0, k, skip_if, cpg, t_stride, pos0, dim, ng, nc, cond_ld, ndesc;
+  long long n, cstride, clip_stride;
+  double count; float eps;
+  /* device pointers owned by the caller */
+  const float* x; const float* y; const float* res;
+  const float* w; const float* b; const float* w2; const float* b2;
+  const float* map; const float* freqs; const double* stats; const int64_t* t; const int* skip_flag;
+  float* out; void* out_hi; void* out_lo; int* flag;
+  dawn_kernel_desc desc[DAWN_KERNEL_MAX_DESC];
+} dawn_kernel_case;
+int dawn_test_kernel(const dawn_kernel_case* c, void* stream);
+
 const char* dawn_last_error(void);
 const char* dawn_build_info(void);
 

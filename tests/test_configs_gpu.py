@@ -6,7 +6,11 @@ These configurations reach paths DAWN's own never runs: FiLM tables of 1024-chan
 (init_conv_x3_kernel: 3x3 / 5x5 kernels, 128 output channels), level-0 temporal attention on the general path (128 channels),
 1x1 images at the deepest level, equal-width levels, the SIMT banded attention kernel for windows over 40 frames, and other
 input / conditioning / output widths."""
+import json
+import os
 import re
+import subprocess
+import sys
 
 import pytest
 import torch
@@ -114,7 +118,12 @@ def kernel_names(tag):
 @pytest.mark.parametrize("tag,kernel", [("dim128", "init_conv_x3_kernel"), ("w120", "attention_kernel")])
 def test_config_runs_the_path_it_is_for(tag, kernel):
     """dim128 runs the general hoisted init-conv kernel (not the 7x7 / 64-channel tiled one); w120's 120-frame window runs the
-    SIMT banded attention kernel (the tensor-core one takes windows up to 40, the fused temporal one up to 64)."""
-    names = kernel_names(tag)
+    SIMT banded attention kernel (the tensor-core one takes windows up to 40, the fused temporal one up to 64).  The profile is
+    taken in a new Python process: torch.profiler records no device events once a process is a few minutes old."""
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    code = f"import json; from tests import test_configs_gpu as T; print(json.dumps(sorted(T.kernel_names({tag!r}))))"
+    r = subprocess.run([sys.executable, "-s", "-B", "-c", code], cwd=root, capture_output=True, text=True, timeout=600)
+    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
+    names = json.loads(r.stdout.strip().splitlines()[-1])
     pat = re.compile(r"(?<!\w)" + kernel + r"(?!\w)")
     assert any(pat.search(n) for n in names), sorted(names)

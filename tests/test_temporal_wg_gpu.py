@@ -6,8 +6,12 @@ forces the mma.sync kernel for the same case.  Each case checks the warpgroup ke
 tests/test_fused_gpu.py (elementwise bound of tests/fused_ref.py, norm-wise tau scaled by the rows' largest |mean| / std), checks
 that the two kernels agree within tau of each other, and keeps the sentinels around the output, in its row padding and in the
 rows an output indexed by the on-chip frame instead of f - q_lo would reach.  Which kernel ran is read from the profiler's
-kernel names: F 256 runs the warpgroup kernel, F 257 the mma.sync one."""
+kernel names: F 256 runs the warpgroup kernel, F 257 the mma.sync one.  That check runs in a new process, where the profiler
+still records device events."""
 import math
+import os
+import subprocess
+import sys
 
 import pytest
 import torch
@@ -91,7 +95,7 @@ def kernels_run(kernel, F, P, band, q_lo, q_hi):
     return out, names
 
 
-def test_dispatch_by_sequence_length():
+def dispatch_check():
     """F 256 runs the warpgroup kernel; F 257 (frames [8, 248) of it produce output: 16 query tiles) is refused by its predicate
     and runs the mma.sync kernel, bit for bit as when forced"""
     L = TF._lib()
@@ -101,3 +105,12 @@ def test_dispatch_by_sequence_length():
     assert names and not any("temporal_fused_wg_kernel" in n for n in names), names
     forced, _ = kernels_run(L.FUSED_TEMPORAL_MMA_SYNC, 257, 8, 40, 8, 248)
     assert torch.equal(out, forced)
+
+
+def test_dispatch_by_sequence_length():
+    """dispatch_check in a new Python process: torch.profiler records no device events once a process is a few minutes old, so
+    in a long pytest run the kernel names would come back empty whichever kernel ran"""
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    r = subprocess.run([sys.executable, "-s", "-B", "-c", "from tests import test_temporal_wg_gpu as T; T.dispatch_check()"],
+                       cwd=root, capture_output=True, text=True, timeout=600)
+    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
