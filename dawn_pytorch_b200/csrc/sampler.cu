@@ -6,12 +6,6 @@
 #include "sampler.cuh"
 #include "../../include/dawn_unet.h"
 
-#define DAWN_TRY(expr)         \
-  do {                         \
-    int _rc = (expr);          \
-    if (_rc != 0) return _rc;  \
-  } while (0)
-
 namespace dawn {
 namespace {
 
@@ -169,13 +163,16 @@ __global__ void ddpm_update_kernel(float* __restrict__ x, const float* __restric
 // the step graph's last node: the next replay runs timestep t - 1
 __global__ void ddpm_advance_kernel(int64_t* t_slot) { *t_slot -= 1; }
 
+// launch shape of the grid-stride key, statistics and update kernels: kThreads per block, at most 148 x 8 blocks
+constexpr int kThreads = 256;
+int update_blocks(long long n) { return (int)std::min<long long>((n + kThreads - 1) / kThreads, 148LL * 8); }
+
 // s = max(1, q-quantile of the n_global keys) by exact radix select, written to scratch word 263 (*s_ptr points there).
 // write_keys(keys) enqueues the kernel that fills this rank's n keys at scratch word 512 once the select state is reset.
 // scratch layout (32-bit words): [0,4) select state | [4,260) histogram | [260,262) count_le (u64) | 262 min_gt | 263 s | [512, 512+n) keys
 template <class WriteKeys>
 int clip_threshold(void* scratch, long long n, int64_t n_global, float q, int blocks, cudaStream_t st, const DdimReduce* red,
                    float** s_ptr, WriteKeys write_keys) {
-  const int threads = 256;
   uint32_t* base = (uint32_t*)scratch;
   uint32_t* state = base;
   unsigned int* hist = base + 4;
@@ -194,7 +191,7 @@ int clip_threshold(void* scratch, long long n, int64_t n_global, float q, int bl
     if (red) DAWN_TRY(red->sum_u32(red->ctx, hist, 256, st));
     radix_pick_kernel<<<1, 32, 0, st>>>(state, shift, hist);
   }
-  next_stat_kernel<<<blocks, threads, 0, st>>>(keys, n, state, count_le, min_gt);
+  next_stat_kernel<<<blocks, kThreads, 0, st>>>(keys, n, state, count_le, min_gt);
   if (red) {
     DAWN_TRY(red->sum_u64(red->ctx, count_le, 1, st));
     DAWN_TRY(red->min_u32(red->ctx, min_gt, 1, st));
@@ -209,15 +206,14 @@ int ddim_update(float* x, float* x_n, const float* eps, const float* eps_n, cons
                 int64_t n_global, float ca, float cb, float sqrt_an, float c, float sigma, float q, void* scratch, cudaStream_t st,
                 const DdimReduce* red) {
   const long long n = n_local;
-  const int threads = 256;
-  int blocks = (int)std::min<long long>((n + threads - 1) / threads, 148LL * 8);
+  const int blocks = update_blocks(n);
   float* s_ptr = nullptr;
   if (q > 0.f)
     DAWN_TRY(clip_threshold(scratch, n, n_global, q, blocks, st, red, &s_ptr, [&](uint32_t* keys) {
-      x0_abs_kernel<<<blocks, threads, 0, st>>>(x, eps, eps_n, scale, ca, cb, n, keys);
+      x0_abs_kernel<<<blocks, kThreads, 0, st>>>(x, eps, eps_n, scale, ca, cb, n, keys);
     }));
-  ddim_update_kernel<<<blocks, threads, 0, st>>>(x, x_n, eps, eps_n, scale, noise, s_ptr, ca, cb, sqrt_an, c, sigma, n,
-                                                 q < 0.f ? 0 : 1);
+  ddim_update_kernel<<<blocks, kThreads, 0, st>>>(x, x_n, eps, eps_n, scale, noise, s_ptr, ca, cb, sqrt_an, c, sigma, n,
+                                                  q < 0.f ? 0 : 1);
   DAWN_LAUNCH_OK();
   return 0;
 }
@@ -256,14 +252,13 @@ int ddpm_step_impl(float* x, const float* eps, const float* noise, int64_t n_loc
     return -1;
   }
   const long long n = n_local;
-  const int threads = 256;
-  int blocks = (int)std::min<long long>((n + threads - 1) / threads, 148LL * 8);
+  const int blocks = update_blocks(n);
   float* s_ptr = nullptr;
   if (q > 0.f)
     DAWN_TRY(clip_threshold(scratch, n, n_global, q, blocks, st, red, &s_ptr, [&](uint32_t* keys) {
-      ddpm_x0_abs_kernel<<<blocks, threads, 0, st>>>(x, eps, c, tab, t_slot, num_t, n, keys);
+      ddpm_x0_abs_kernel<<<blocks, kThreads, 0, st>>>(x, eps, c, tab, t_slot, num_t, n, keys);
     }));
-  ddpm_update_kernel<<<blocks, threads, 0, st>>>(x, eps, noise, s_ptr, c, tab, t_slot, num_t, n, q < 0.f ? 0 : 1);
+  ddpm_update_kernel<<<blocks, kThreads, 0, st>>>(x, eps, noise, s_ptr, c, tab, t_slot, num_t, n, q < 0.f ? 0 : 1);
   DAWN_LAUNCH_OK();
   return 0;
 }

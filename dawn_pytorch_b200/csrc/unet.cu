@@ -154,6 +154,12 @@ __global__ void gn_p2p_allreduce_kernel(double* __restrict__ stats, P2pPeers pee
   }
 }
 
+// A captured sampler graph and the UNet kernel launches one replay makes (what dawn_unet_last_launch_count reports after it)
+struct SamplerGraph {
+  cudaGraphExec_t exec = nullptr;
+  int64_t launches = 0;
+};
+
 struct dawn_unet {
   dawn_unet_cfg cfg{};
   int nlev = 0;
@@ -212,18 +218,12 @@ struct dawn_unet {
   std::map<std::string, float*> taps;
   int64_t launches = 0;
 
-  // whole-clip sampling loop captured as one CUDA graph (dawn_unet_sampler_capture); invalidated by any geometry change
-  cudaGraphExec_t samp_exec = nullptr;
+  // captured sampler graphs, one slot each so that no capture drops another (a plain loop over 2 clips and a guided loop over
+  // 1 clip run on the same B = 2 geometry); any geometry, parameter or sharding change drops all three (drop_graphs):
+  SamplerGraph ddim_graph;                     // whole DDIM loop (dawn_unet_sampler_capture)
+  SamplerGraph guided_graph;                   // whole classifier-free-guided DDIM loop (dawn_unet_sampler_capture_guided)
+  SamplerGraph ddpm_graph;                     // one ancestral step, replayed T times (dawn_unet_ddpm_capture)
   cudaStream_t samp_stream = nullptr;          // capture origin (the legacy default stream cannot be captured)
-  int64_t samp_launches = 0;
-  // one ancestral step (forward_x3 + DDPM update + timestep advance) captured for T replays (dawn_unet_ddpm_capture); held
-  // beside samp_exec (neither capture drops the other) and invalidated by the same geometry changes
-  cudaGraphExec_t ddpm_exec = nullptr;
-  int64_t ddpm_launches = 0;
-  // classifier-free-guided sampling loop (dawn_unet_sampler_capture_guided): its own slot beside samp_exec and ddpm_exec, since
-  // a plain loop over 2 clips and a guided loop over 1 clip run on the same B = 2 geometry
-  cudaGraphExec_t guid_exec = nullptr;
-  int64_t guid_launches = 0;
 
   // per-category kernel timing (CUDA events on the launching stream), see dawn_unet_profile_*
   bool prof_on = false;
@@ -934,12 +934,20 @@ int dawn_unet_create(const dawn_unet_cfg* cfg, dawn_unet** out) {
   return 0;
 }
 
+static void drop_graph(SamplerGraph& g) {
+  if (g.exec) { cudaGraphExecDestroy(g.exec); g.exec = nullptr; }
+}
+// a new geometry, parameter set or sharding invalidates all three captured sampler graphs
+static void drop_graphs(dawn_unet* h) {
+  drop_graph(h->ddim_graph);
+  drop_graph(h->ddpm_graph);
+  drop_graph(h->guided_graph);
+}
+
 void dawn_unet_destroy(dawn_unet* h) {
   if (!h) return;
   for (cudaEvent_t e : h->prof_ev) cudaEventDestroy(e);
-  if (h->samp_exec) cudaGraphExecDestroy(h->samp_exec);
-  if (h->ddpm_exec) cudaGraphExecDestroy(h->ddpm_exec);
-  if (h->guid_exec) cudaGraphExecDestroy(h->guid_exec);
+  drop_graphs(h);
   if (h->samp_stream) cudaStreamDestroy(h->samp_stream);
   if (h->sh_comm && g_nccl.ok) g_nccl.CommDestroy(h->sh_comm);
   for (int r = 0; r < kP2pMaxRanks; ++r)
@@ -954,22 +962,6 @@ int dawn_unet_set_param(dawn_unet* h, const char* name, const float* host, const
   h->raw.set(name, host, shape, ndim);
   h->committed = false;
   return 0;
-}
-
-static void drop_sampler_graph(dawn_unet* h) {
-  if (h->samp_exec) { cudaGraphExecDestroy(h->samp_exec); h->samp_exec = nullptr; }
-}
-static void drop_ddpm_graph(dawn_unet* h) {
-  if (h->ddpm_exec) { cudaGraphExecDestroy(h->ddpm_exec); h->ddpm_exec = nullptr; }
-}
-static void drop_guided_graph(dawn_unet* h) {
-  if (h->guid_exec) { cudaGraphExecDestroy(h->guid_exec); h->guid_exec = nullptr; }
-}
-// a new geometry, parameter set or sharding invalidates all three captured sampler graphs
-static void drop_graphs(dawn_unet* h) {
-  drop_sampler_graph(h);
-  drop_ddpm_graph(h);
-  drop_guided_graph(h);
 }
 
 int dawn_unet_commit_params(dawn_unet* h) {
@@ -1362,9 +1354,8 @@ int dawn_unet_shard_ipc_import(dawn_unet* h, const char* handles) {
   return 0;
 }
 
-// DDIM update of this handle's frames (see sampler.cu).  Unsharded: identical to dawn_ddim_step.  Frame-sharded: the
-// clip-wide quantile (U:1186-1190) is selected over ALL ranks' values by all-reducing the radix-select's histograms
-// (4 x 256 u32) and its two tail statistics — 6 tiny collectives per step instead of gathering x0 (4.9 MB per rank).
+// Frame-sharded handles select the clip-wide quantile (U:1186-1190) over ALL ranks' values by all-reducing the radix-select's
+// histograms (4 x 256 u32) and its two tail statistics — 6 tiny collectives per step instead of gathering x0 (4.9 MB per rank).
 static int red_sum_u32(void* ctx, unsigned int* b, size_t n, cudaStream_t st) {
   DAWN_NCCL_OK(g_nccl.AllReduce(b, b, n, kNcclUint32, kNcclSum, (ncclComm_t)ctx, st)); return 0;
 }
@@ -1374,21 +1365,70 @@ static int red_sum_u64(void* ctx, unsigned long long* b, size_t n, cudaStream_t 
 static int red_min_u32(void* ctx, unsigned int* b, size_t n, cudaStream_t st) {
   DAWN_NCCL_OK(g_nccl.AllReduce(b, b, n, kNcclUint32, kNcclMin, (ncclComm_t)ctx, st)); return 0;
 }
-int dawn_unet_ddim_step(dawn_unet* h, float* x, const float* eps, const float* noise, int64_t n_local, float ca, float cb,
-                        float sqrt_an, float c, float sigma, float q, void* scratch, void* stream) {
-  DAWN_CHECK(h, "null handle");
+
+}  // extern "C"
+
+// One sampler update of this handle's frames (see sampler.cu) through step(offset, n_local, n_global, red), which updates the
+// n_local values at offset.  Unsharded: B clips back to back, each clip's quantile its own (U:1184-1193), so one call per clip
+// on the same scratch.  Frame-sharded: one call whose quantile is selected over the n_global values of all ranks through red.
+template <class Step>
+static int update_clips(dawn_unet* h, int64_t n_local, Step step) {
   if (h->sh_nranks <= 1 || !h->sh_comm) {
-    // B clips back to back: each clip's quantile is its own (U:1184-1193), so one select per clip on the same scratch
     DAWN_CHECK(n_local % h->B == 0, "n must be a multiple of the clip count");
     const int64_t nc = n_local / h->B;
-    for (int b = 0; b < h->B; ++b)
-      DAWN_TRY(ddim_step_impl(x + b * nc, eps + b * nc, noise ? noise + b * nc : nullptr, nc, nc, ca, cb, sqrt_an, c, sigma, q, scratch,
-                              (cudaStream_t)stream, nullptr));
+    for (int b = 0; b < h->B; ++b) DAWN_TRY(step(b * nc, nc, nc, nullptr));
     return 0;
   }
   DdimReduce red{(void*)h->sh_comm, red_sum_u32, red_sum_u64, red_min_u32};
-  return ddim_step_impl(x, eps, noise, n_local, n_local * h->sh_nranks, ca, cb, sqrt_an, c, sigma, q, scratch,
-                        (cudaStream_t)stream, &red);
+  return step(0, n_local, n_local * h->sh_nranks, &red);
+}
+
+// values of one clip's output (3, F, h, w)
+static int64_t clip_values(const dawn_unet* h) {
+  return (int64_t)(h->cfg.out_grid_dim + h->cfg.out_conf_dim) * h->F * h->H * h->W;
+}
+
+// Captures one sampler graph into slot g: body(stream) enqueues the graph's work on the handle's capture stream and returns the
+// UNet kernel launches one replay makes, or an error code (< 0).  `entry` and `graph` name the capture in its refusals.
+template <class Body>
+static int capture_graph(dawn_unet* h, SamplerGraph& g, const char* entry, const char* graph, Body body) {
+  DAWN_CHECK(h->F > 0 && h->have_invariants, std::string("set_clip_invariants must precede ") + entry);
+  DAWN_CHECK(!h->prof_on, std::string("disable profiling before capturing ") + graph);
+  drop_graph(g);
+  if (!h->samp_stream) DAWN_CUDA_OK(cudaStreamCreateWithFlags(&h->samp_stream, cudaStreamNonBlocking));
+  DAWN_CUDA_OK(cudaStreamBeginCapture(h->samp_stream, cudaStreamCaptureModeThreadLocal));
+  const int64_t launches = body(h->samp_stream);
+  cudaGraph_t captured = nullptr;
+  const cudaError_t e = cudaStreamEndCapture(h->samp_stream, &captured);
+  if (launches < 0) { if (captured) cudaGraphDestroy(captured); return (int)launches; }
+  DAWN_CUDA_OK(e);
+  const cudaError_t ei = cudaGraphInstantiate(&g.exec, captured, 0);
+  cudaGraphDestroy(captured);
+  DAWN_CUDA_OK(ei);
+  g.launches = launches;
+  return 0;
+}
+
+// Replays the graph in slot `slot`, captured by `entry`, as the `launch` entry.
+static int launch_graph(dawn_unet* h, SamplerGraph dawn_unet::*slot, const char* entry, const char* launch, void* stream) {
+  DAWN_CHECK(h && (h->*slot).exec, std::string(entry) + " must precede " + launch + " (a geometry change drops the graph)");
+  DAWN_CHECK(h->have_invariants, std::string("set_clip_invariants must precede ") + launch);
+  const SamplerGraph& g = h->*slot;
+  DAWN_CUDA_OK(cudaGraphLaunch(g.exec, (cudaStream_t)stream));
+  h->launches = g.launches;
+  return 0;
+}
+
+extern "C" {
+
+// DDIM update of this handle's frames.  Unsharded: identical to dawn_ddim_step.
+int dawn_unet_ddim_step(dawn_unet* h, float* x, const float* eps, const float* noise, int64_t n_local, float ca, float cb,
+                        float sqrt_an, float c, float sigma, float q, void* scratch, void* stream) {
+  DAWN_CHECK(h, "null handle");
+  return update_clips(h, n_local, [&](int64_t o, int64_t n, int64_t n_global, const DdimReduce* red) {
+    return ddim_step_impl(x + o, eps + o, noise ? noise + o : nullptr, n, n_global, ca, cb, sqrt_an, c, sigma, q, scratch,
+                          (cudaStream_t)stream, red);
+  });
 }
 
 // The whole sampling loop of one clip as ONE CUDA graph (SURVEY 8f N2): nsteps x (forward_x3 + DDIM update), no host work
@@ -1400,40 +1440,22 @@ int dawn_unet_sampler_capture(dawn_unet* h, float* x, float* eps, const float* n
                               const float* coef, int nsteps, float q, void* scratch) {
   DAWN_CHECK(h && x && eps && t_all && coef && scratch && nsteps >= 1, "bad argument");
   DAWN_CHECK(noise_all || nsteps == 1, "noise_all is required for more than one step");
-  DAWN_CHECK(h->F > 0 && h->have_invariants, "set_clip_invariants must precede sampler_capture");
-  DAWN_CHECK(!h->prof_on, "disable profiling before capturing the sampler graph");
-  drop_sampler_graph(h);
-  if (!h->samp_stream) DAWN_CUDA_OK(cudaStreamCreateWithFlags(&h->samp_stream, cudaStreamNonBlocking));
-  const int64_t n = (int64_t)(h->cfg.out_grid_dim + h->cfg.out_conf_dim) * h->B * h->F * h->H * h->W;
-  cudaStream_t st = h->samp_stream;
-  DAWN_CUDA_OK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-  int rc = 0;
-  int64_t launches = 0;
-  for (int k = 0; k < nsteps && rc == 0; ++k) {
-    rc = forward_x3_impl(h, x, t_all + k, 0, eps, st);               // every clip at step k's timestep
-    launches += h->launches;
-    const float* cf = coef + 5 * k;
-    if (rc == 0)
-      rc = dawn_unet_ddim_step(h, x, eps, (k < nsteps - 1) ? noise_all + (size_t)k * n : nullptr, n, cf[0], cf[1], cf[2], cf[3], cf[4],
-                               q, scratch, st);
-  }
-  cudaGraph_t graph = nullptr;
-  const cudaError_t e = cudaStreamEndCapture(st, &graph);
-  if (rc != 0) { if (graph) cudaGraphDestroy(graph); return rc; }
-  DAWN_CUDA_OK(e);
-  const cudaError_t ei = cudaGraphInstantiate(&h->samp_exec, graph, 0);
-  cudaGraphDestroy(graph);
-  DAWN_CUDA_OK(ei);
-  h->samp_launches = launches;
-  return 0;
+  return capture_graph(h, h->ddim_graph, "sampler_capture", "the sampler graph", [&](cudaStream_t st) -> int64_t {
+    const int64_t n = clip_values(h) * h->B;
+    int64_t launches = 0;
+    for (int k = 0; k < nsteps; ++k) {
+      DAWN_TRY(forward_x3_impl(h, x, t_all + k, 0, eps, st));          // every clip at step k's timestep
+      launches += h->launches;
+      const float* cf = coef + 5 * k;
+      DAWN_TRY(dawn_unet_ddim_step(h, x, eps, (k < nsteps - 1) ? noise_all + (size_t)k * n : nullptr, n, cf[0], cf[1], cf[2], cf[3],
+                                   cf[4], q, scratch, st));
+    }
+    return launches;
+  });
 }
 
 int dawn_unet_sampler_launch(dawn_unet* h, void* stream) {
-  DAWN_CHECK(h && h->samp_exec, "sampler_capture must precede sampler_launch (a geometry change drops the graph)");
-  DAWN_CHECK(h->have_invariants, "set_clip_invariants must precede sampler_launch");
-  DAWN_CUDA_OK(cudaGraphLaunch(h->samp_exec, (cudaStream_t)stream));
-  h->launches = h->samp_launches;
-  return 0;
+  return launch_graph(h, &dawn_unet::ddim_graph, "sampler_capture", "sampler_launch", stream);
 }
 
 // Classifier-free-guided DDIM update on a handle of B = 2b clips: clips [0, b) are conditioned, clips [b, 2b) their null twins
@@ -1444,8 +1466,7 @@ int dawn_unet_ddim_step_guided(dawn_unet* h, float* x, const float* eps, const f
   DAWN_CHECK(h->sh_nranks <= 1, "guided DDIM steps run on an unsharded handle (a frame-sharded handle holds one clip, not a pair)");
   DAWN_CHECK(h->F > 0 && h->B % 2 == 0, "a guided DDIM step needs an even clip count B = 2b (b conditioned clips, then their null twins)");
   DAWN_CHECK(x && eps && cond_scale_dev && scratch, "bad argument");
-  DAWN_CHECK(n_clip == (int64_t)(h->cfg.out_grid_dim + h->cfg.out_conf_dim) * h->F * h->H * h->W,
-             "n_clip must be the size of one clip (3 * F * height * width)");
+  DAWN_CHECK(n_clip == clip_values(h), "n_clip must be the size of one clip (3 * F * height * width)");
   const int b = h->B / 2;
   for (int i = 0; i < b; ++i)
     DAWN_TRY(ddim_guided_step_impl(x + i * n_clip, x + (b + i) * n_clip, eps + i * n_clip, eps + (b + i) * n_clip,
@@ -1460,58 +1481,33 @@ int dawn_unet_sampler_capture_guided(dawn_unet* h, float* x, float* eps, const f
                                      const float* cond_scale_dev, const float* coef, int nsteps, float q, void* scratch) {
   DAWN_CHECK(h && x && eps && t_all && cond_scale_dev && coef && scratch && nsteps >= 1, "bad argument");
   DAWN_CHECK(noise_all || nsteps == 1, "noise_all is required for more than one step");
-  DAWN_CHECK(h->F > 0 && h->have_invariants, "set_clip_invariants must precede sampler_capture_guided");
-  DAWN_CHECK(h->sh_nranks <= 1 && h->B % 2 == 0, "the guided sampler graph needs an unsharded handle with an even clip count");
-  DAWN_CHECK(!h->prof_on, "disable profiling before capturing the sampler graph");
-  drop_guided_graph(h);
-  if (!h->samp_stream) DAWN_CUDA_OK(cudaStreamCreateWithFlags(&h->samp_stream, cudaStreamNonBlocking));
-  const int64_t nc = (int64_t)(h->cfg.out_grid_dim + h->cfg.out_conf_dim) * h->F * h->H * h->W;
-  const int64_t n_noise = nc * (h->B / 2);
-  cudaStream_t st = h->samp_stream;
-  DAWN_CUDA_OK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-  int rc = 0;
-  int64_t launches = 0;
-  for (int k = 0; k < nsteps && rc == 0; ++k) {
-    rc = forward_x3_impl(h, x, t_all + k, 0, eps, st);               // conditioned and null clips at step k's timestep
-    launches += h->launches;
-    const float* cf = coef + 5 * k;
-    if (rc == 0)
-      rc = dawn_unet_ddim_step_guided(h, x, eps, (k < nsteps - 1) ? noise_all + (size_t)k * n_noise : nullptr, nc, cond_scale_dev,
-                                      cf[0], cf[1], cf[2], cf[3], cf[4], q, scratch, st);
-  }
-  cudaGraph_t graph = nullptr;
-  const cudaError_t e = cudaStreamEndCapture(st, &graph);
-  if (rc != 0) { if (graph) cudaGraphDestroy(graph); return rc; }
-  DAWN_CUDA_OK(e);
-  const cudaError_t ei = cudaGraphInstantiate(&h->guid_exec, graph, 0);
-  cudaGraphDestroy(graph);
-  DAWN_CUDA_OK(ei);
-  h->guid_launches = launches;
-  return 0;
+  return capture_graph(h, h->guided_graph, "sampler_capture_guided", "the sampler graph", [&](cudaStream_t st) -> int64_t {
+    // checked here, before anything is enqueued, so that a missing set_clip_invariants is reported first
+    DAWN_CHECK(h->sh_nranks <= 1 && h->B % 2 == 0, "the guided sampler graph needs an unsharded handle with an even clip count");
+    const int64_t nc = clip_values(h), n_noise = nc * (h->B / 2);
+    int64_t launches = 0;
+    for (int k = 0; k < nsteps; ++k) {
+      DAWN_TRY(forward_x3_impl(h, x, t_all + k, 0, eps, st));          // conditioned and null clips at step k's timestep
+      launches += h->launches;
+      const float* cf = coef + 5 * k;
+      DAWN_TRY(dawn_unet_ddim_step_guided(h, x, eps, (k < nsteps - 1) ? noise_all + (size_t)k * n_noise : nullptr, nc, cond_scale_dev,
+                                          cf[0], cf[1], cf[2], cf[3], cf[4], q, scratch, st));
+    }
+    return launches;
+  });
 }
 
 int dawn_unet_sampler_launch_guided(dawn_unet* h, void* stream) {
-  DAWN_CHECK(h && h->guid_exec, "sampler_capture_guided must precede sampler_launch_guided (a geometry change drops the graph)");
-  DAWN_CHECK(h->have_invariants, "set_clip_invariants must precede sampler_launch_guided");
-  DAWN_CUDA_OK(cudaGraphLaunch(h->guid_exec, (cudaStream_t)stream));
-  h->launches = h->guid_launches;
-  return 0;
+  return launch_graph(h, &dawn_unet::guided_graph, "sampler_capture_guided", "sampler_launch_guided", stream);
 }
 
-// Ancestral update of this handle's frames (see sampler.cu); frame-sharded handles select the quantile over the whole clip
-// exactly as dawn_unet_ddim_step does.
+// Ancestral update of this handle's frames, sharded as dawn_unet_ddim_step: the by-value coefficients c, or with tab the row of
+// the device table at *t_slot (the step graph).
 static int ddpm_step_handle(dawn_unet* h, float* x, const float* eps, const float* noise, int64_t n_local, DdpmCoef c,
                             const DdpmCoef* tab, const int64_t* t_slot, int num_t, float q, void* scratch, cudaStream_t st) {
-  if (h->sh_nranks <= 1 || !h->sh_comm) {
-    DAWN_CHECK(n_local % h->B == 0, "n must be a multiple of the clip count");
-    const int64_t nc = n_local / h->B;
-    for (int b = 0; b < h->B; ++b)       // one select per clip: each clip's quantile is its own
-      DAWN_TRY(ddpm_step_impl(x + b * nc, eps + b * nc, noise ? noise + b * nc : nullptr, nc, nc, c, tab, t_slot, num_t, q, scratch, st,
-                              nullptr));
-    return 0;
-  }
-  DdimReduce red{(void*)h->sh_comm, red_sum_u32, red_sum_u64, red_min_u32};
-  return ddpm_step_impl(x, eps, noise, n_local, n_local * h->sh_nranks, c, tab, t_slot, num_t, q, scratch, st, &red);
+  return update_clips(h, n_local, [&](int64_t o, int64_t n, int64_t n_global, const DdimReduce* red) {
+    return ddpm_step_impl(x + o, eps + o, noise ? noise + o : nullptr, n, n_global, c, tab, t_slot, num_t, q, scratch, st, red);
+  });
 }
 
 int dawn_unet_ddpm_step(dawn_unet* h, float* x, const float* eps, const float* noise, int64_t n_local, float ca, float cb,
@@ -1528,36 +1524,18 @@ int dawn_unet_ddpm_capture(dawn_unet* h, float* x, float* eps, const float* nois
                            int num_timesteps, float q, void* scratch) {
   static_assert(sizeof(DdpmCoef) == 5 * sizeof(float), "a coefficient table row is 5 floats");
   DAWN_CHECK(h && x && eps && noise && t_slot && coef && scratch && num_timesteps >= 1, "bad argument");
-  DAWN_CHECK(h->F > 0 && h->have_invariants, "set_clip_invariants must precede ddpm_capture");
-  DAWN_CHECK(!h->prof_on, "disable profiling before capturing the ancestral step graph");
-  drop_ddpm_graph(h);
-  if (!h->samp_stream) DAWN_CUDA_OK(cudaStreamCreateWithFlags(&h->samp_stream, cudaStreamNonBlocking));
-  const int64_t n = (int64_t)(h->cfg.out_grid_dim + h->cfg.out_conf_dim) * h->B * h->F * h->H * h->W;
-  cudaStream_t st = h->samp_stream;
-  DAWN_CUDA_OK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-  int rc = forward_x3_impl(h, x, t_slot, 0, eps, st);                // the one time slot applies to every clip
-  const int64_t launches = h->launches;
-  if (rc == 0)
-    rc = ddpm_step_handle(h, x, eps, noise, n, DdpmCoef{}, reinterpret_cast<const DdpmCoef*>(coef), t_slot, num_timesteps, q,
-                          scratch, st);
-  if (rc == 0) rc = ddpm_advance_slot(t_slot, st);
-  cudaGraph_t graph = nullptr;
-  const cudaError_t e = cudaStreamEndCapture(st, &graph);
-  if (rc != 0) { if (graph) cudaGraphDestroy(graph); return rc; }
-  DAWN_CUDA_OK(e);
-  const cudaError_t ei = cudaGraphInstantiate(&h->ddpm_exec, graph, 0);
-  cudaGraphDestroy(graph);
-  DAWN_CUDA_OK(ei);
-  h->ddpm_launches = launches;
-  return 0;
+  return capture_graph(h, h->ddpm_graph, "ddpm_capture", "the ancestral step graph", [&](cudaStream_t st) -> int64_t {
+    DAWN_TRY(forward_x3_impl(h, x, t_slot, 0, eps, st));              // the one time slot applies to every clip
+    const int64_t launches = h->launches;
+    DAWN_TRY(ddpm_step_handle(h, x, eps, noise, clip_values(h) * h->B, DdpmCoef{}, reinterpret_cast<const DdpmCoef*>(coef), t_slot,
+                              num_timesteps, q, scratch, st));
+    DAWN_TRY(ddpm_advance_slot(t_slot, st));
+    return launches;
+  });
 }
 
 int dawn_unet_ddpm_launch(dawn_unet* h, void* stream) {
-  DAWN_CHECK(h && h->ddpm_exec, "ddpm_capture must precede ddpm_launch (a geometry change drops the graph)");
-  DAWN_CHECK(h->have_invariants, "set_clip_invariants must precede ddpm_launch");
-  DAWN_CUDA_OK(cudaGraphLaunch(h->ddpm_exec, (cudaStream_t)stream));
-  h->launches = h->ddpm_launches;
-  return 0;
+  return launch_graph(h, &dawn_unet::ddpm_graph, "ddpm_capture", "ddpm_launch", stream);
 }
 
 int64_t dawn_unet_last_launch_count(dawn_unet* h) { return h ? h->launches : 0; }

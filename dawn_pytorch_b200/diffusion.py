@@ -11,12 +11,23 @@ once per clip (`set_clip_invariants`), each step is `forward_x3` + one fused upd
 synchronisation.
 """
 import ctypes
+import math
 
 import torch
 import torch.nn.functional as F
 from torch import nn
 
 from ._lib import check, lib
+
+
+def _ptr(t):
+    return ctypes.c_void_p(t.data_ptr())
+
+
+def _update_scratch(n, device):
+    """int32 scratch of one clip's update (n values): the 512-word header of the clip-wide threshold's radix select, then the n
+    keys; the layout is set out beside `clip_threshold` in csrc/sampler.cu."""
+    return torch.empty(n + 512, dtype=torch.int32, device=device)
 
 
 def _cosine_beta_schedule(timesteps, s=0.008):
@@ -131,12 +142,10 @@ class GaussianDiffusion(nn.Module):
         dynamic-threshold quantile is selected over the whole clip (all-reduced radix select) and the default noise is
         the rank's slice of ONE clip-wide stream (same `seed` on every rank; drawn on rank 0 and broadcast if None)."""
         device = self.betas.device
-        b, ch, Fr, h, w = shape
         unet = self.denoise_fn
         pairs = self.ddim_schedule() if pairs is None else pairs
         draw = noise_fn if noise_fn is not None else self._default_noise(unet, device, seed)
         img = draw(-1, shape).to(device).contiguous()
-        n = ch * Fr * h * w
         q = self._clip_q(clip_denoised)
         self._check_sample_shape("ddim_sample", fea, shape, cond)
         st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
@@ -145,66 +154,45 @@ class GaussianDiffusion(nn.Module):
             if guided:
                 return self._ddim_sample_guided_graph(unet, fea, cond, img, pairs, draw, q, st, cond_scale)
             return self._ddim_sample_graph(unet, fea, cond, img, pairs, draw, q, st)
-        if self._batched(unet, b, Fr, h, w):
-            return self._ddim_sample_batched(unet, fea, cond, img, pairs, draw, q, st, guided, cond_scale)
-        scratch = torch.empty(n + 512, dtype=torch.int32, device=device)
-        eps = torch.empty((ch, Fr, h, w), device=device)
+        steps = [(t, self.ddim_coefficients(t, t_next)) for t, t_next in pairs]
+        return self._sample_eager("dawn_unet_ddim_step", fea, cond, img, steps, cond_scale, q,
+                                  lambda k, sel, one: draw(k, one).to(device).contiguous() if pairs[k][1] > 0 else None)
+
+    def _sample_eager(self, entry, fea, cond, img, steps, cond_scale, q, noise):
+        """Runs `steps`, a list of (t, coefficients of the native update `entry`), in place on img (b, 3, F, h, w): all b clips
+        together when `_batched` (one forward and one update per step), otherwise one clip after the other.  noise(k, sel, shape)
+        is step k's noise for img[sel] of that shape, or None when the step adds none (U:1201)."""
+        unet = self.denoise_fn
+        b, ch, Fr, h, w = img.shape
+        batched = self._batched(unet, b, Fr, h, w)
+        one = tuple(img.shape) if batched else (ch, Fr, h, w)
+        guided = cond_scale != 1 and getattr(unet, "has_cond", True)
+        eps = torch.empty(one, device=img.device)
         eps_null = torch.empty_like(eps) if guided else None
-        for i in range(b):
+        scratch = _update_scratch(ch * Fr * h * w, img.device)
+        st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+        for i in range(1 if batched else b):
+            sel = slice(None) if batched else i
+            x = img[sel]
             unet.update_num_frames(Fr)
             if not guided:
-                unet.set_clip_invariants(fea[i], cond[i])
-            x = img[i]
-            for k, (t, t_next) in enumerate(pairs):
-                t_dev = torch.full((1,), t, device=device, dtype=torch.long)
+                unet.set_clip_invariants(fea[sel], cond[sel])
+            for k, (t, coef) in enumerate(steps):
+                t_dev = torch.full((b if batched else 1,), t, device=img.device, dtype=torch.long)
                 if guided:
-                    # classifier-free guidance (reference forward_with_cond_scale U:879-890 inside ddim_sample U:1176-1180):
-                    # eps = eps_null + (eps_cond - eps_null) * cond_scale, the null condition being all zeros (learn_null_cond=False,
-                    # U:920).  Two hoisted forwards per step, each after rebuilding the per-clip conditioning tables (~0.5 ms).
-                    unet.set_clip_invariants(fea[i], cond[i])
+                    # classifier-free guidance (reference forward_with_cond_scale U:879-890): null + (cond - null) * cond_scale in
+                    # its three fp32 ops, the null condition being all zeros (learn_null_cond=False, U:920).  Two hoisted forwards
+                    # per step, each after rebuilding the per-clip conditioning tables.
+                    unet.set_clip_invariants(fea[sel], cond[sel])
                     unet.forward_x3(x, t_dev, eps)
-                    unet.set_clip_invariants(fea[i], torch.zeros_like(cond[i]))
+                    unet.set_clip_invariants(fea[sel], torch.zeros_like(cond[sel]))
                     unet.forward_x3(x, t_dev, eps_null)
-                    torch.add(eps_null, eps - eps_null, alpha=float(cond_scale), out=eps)
+                    eps.sub_(eps_null).mul_(float(cond_scale)).add_(eps_null)
                 else:
                     unet.forward_x3(x, t_dev, eps)
-                ca, cb, san, c, sigma = self.ddim_coefficients(t, t_next)
-                noise = draw(k, (ch, Fr, h, w)).to(device).contiguous() if t_next > 0 else None
-                check(lib.dawn_unet_ddim_step(unet._handle, ctypes.c_void_p(x.data_ptr()), ctypes.c_void_p(eps.data_ptr()),
-                                              ctypes.c_void_p(noise.data_ptr()) if noise is not None else None, n,
-                                              ca, cb, san, c, sigma, q,
-                                              ctypes.c_void_p(scratch.data_ptr()), st), "dawn_unet_ddim_step")
-        return img
-
-    def _ddim_sample_batched(self, unet, fea, cond, img, pairs, draw, q, st, guided, cond_scale):
-        """All b clips of an unsharded UNet step together (reference ddim_sample over the batch, U:1156-1208): one forward and
-        one update per step, each clip with its own timestep embedding slot and its own dynamic-threshold quantile.  Noise is
-        drawn as the reference draws it, noise_fn(k, (b, ch, F, h, w)) per step."""
-        b, ch, Fr, h, w = img.shape
-        device, n = img.device, ch * Fr * h * w
-        unet.update_num_frames(Fr)
-        scratch = torch.empty(n + 512, dtype=torch.int32, device=device)
-        eps = torch.empty_like(img)
-        eps_null = torch.empty_like(img) if guided else None
-        fea, cond = fea.contiguous(), cond.contiguous()
-        null = torch.zeros_like(cond) if guided else None
-        if not guided:
-            unet.set_clip_invariants(fea, cond)
-        for k, (t, t_next) in enumerate(pairs):
-            t_dev = torch.full((b,), t, device=device, dtype=torch.long)
-            if guided:                                   # cond, then all-zero null cond, per step (U:879-890, 920)
-                unet.set_clip_invariants(fea, cond)
-                unet.forward_x3(img, t_dev, eps)
-                unet.set_clip_invariants(fea, null)
-                unet.forward_x3(img, t_dev, eps_null)
-                torch.add(eps_null, eps - eps_null, alpha=float(cond_scale), out=eps)
-            else:
-                unet.forward_x3(img, t_dev, eps)
-            ca, cb, san, c, sigma = self.ddim_coefficients(t, t_next)
-            noise = draw(k, (b, ch, Fr, h, w)).to(device).contiguous() if t_next > 0 else None
-            check(lib.dawn_unet_ddim_step(unet._handle, ctypes.c_void_p(img.data_ptr()), ctypes.c_void_p(eps.data_ptr()),
-                                          ctypes.c_void_p(noise.data_ptr()) if noise is not None else None, b * n,
-                                          ca, cb, san, c, sigma, q, ctypes.c_void_p(scratch.data_ptr()), st), "dawn_unet_ddim_step")
+                z = noise(k, sel, one)
+                check(getattr(lib, entry)(unet._handle, _ptr(x), _ptr(eps), _ptr(z) if z is not None else None, x.numel(), *coef, q,
+                                          _ptr(scratch), st), entry)
         return img
 
     @staticmethod
@@ -229,31 +217,49 @@ class GaussianDiffusion(nn.Module):
             return full[..., rank * Fl:(rank + 1) * Fl, :, :].contiguous()
         return draw
 
+    def _captured_graph(self, attr, entry, key, unet, invariants, x_shape, noise_shape, ts, args, count, q):
+        """The sampler graph cached under `attr`, reused while its key and the UNet's graph generation hold.  Otherwise its
+        buffers are allocated (x and eps of x_shape, noise of noise_shape, the timesteps ts on the device, the scratch),
+        invariants() sets the invariants of the first launch's clips and `entry` captures it.  Every capture entry takes
+        (handle, x, eps, noise, t, *args, count, q, scratch); args() builds the entry's own arguments, kept in the dict by
+        name.  Returns (the dict, whether it was captured now)."""
+        unet.update_num_frames(x_shape[-3])
+        g = getattr(self, attr, None)
+        if g is not None and g["key"] == key and g["gen"] == unet.graph_generation():
+            return g, False
+        device = self.betas.device
+        extra = args()
+        g = dict(key=key, x=torch.empty(x_shape, device=device), eps=torch.empty(x_shape, device=device),
+                 noise=torch.empty(noise_shape, device=device), t=torch.tensor(ts, dtype=torch.long, device=device),
+                 scratch=_update_scratch(math.prod(x_shape[-4:]), device), **extra)
+        invariants()
+        torch.cuda.synchronize(device)
+        ins = [_ptr(g[k]) for k in ("x", "eps", "noise", "t")] + [_ptr(v) if torch.is_tensor(v) else v for v in extra.values()]
+        check(getattr(lib, entry)(unet._handle, *ins, count, q, _ptr(g["scratch"])), entry)
+        g["gen"] = unet.graph_generation()
+        setattr(self, attr, g)
+        return g, True
+
+    def _ddim_coef_array(self, pairs):
+        """Host fp32 array {ca, cb, sqrt_alpha_next, c, sigma} per step, as the DDIM graph captures take it."""
+        ns = len(pairs)
+        coef = (ctypes.c_float * (5 * ns))()
+        for k, (t, t_next) in enumerate(pairs):
+            coef[5 * k:5 * k + 5] = self.ddim_coefficients(t, t_next)
+            assert (t_next > 0) == (k < ns - 1), "only the last DDIM step ends at t = 0 (reference :1201)"
+        return coef
+
     def _ddim_sample_graph(self, unet, fea, cond, img, pairs, draw, q, st):
         b, ch, Fr, h, w = img.shape
-        device, n, ns = img.device, ch * Fr * h * w, len(pairs)
+        ns = len(pairs)
         # one graph launch runs the whole batch (leading clip dimension) or one clip
         batched = self._batched(unet, b, Fr, h, w)
         one = (b, ch, Fr, h, w) if batched else (ch, Fr, h, w)
-        key = (Fr, h, w, tuple(pairs), q, device.index, one)
-        g = getattr(self, "_graph", None)
-        unet.update_num_frames(Fr)
-        if g is None or g["key"] != key or g["gen"] != unet.graph_generation():
-            g = dict(key=key, x=torch.empty(one, device=device), eps=torch.empty(one, device=device),
-                     noise=torch.empty((max(ns - 1, 1),) + one, device=device),
-                     t_all=torch.tensor([p[0] for p in pairs], dtype=torch.long, device=device),
-                     scratch=torch.empty(n + 512, dtype=torch.int32, device=device))
-            coef = (ctypes.c_float * (5 * ns))()
-            for k, (t, t_next) in enumerate(pairs):
-                coef[5 * k:5 * k + 5] = self.ddim_coefficients(t, t_next)
-                assert (t_next > 0) == (k < ns - 1), "only the last DDIM step ends at t = 0 (reference :1201)"
-            unet.set_clip_invariants(*((fea, cond) if batched else (fea[0], cond[0])))
-            torch.cuda.synchronize(device)
-            check(lib.dawn_unet_sampler_capture(unet._handle, ctypes.c_void_p(g["x"].data_ptr()), ctypes.c_void_p(g["eps"].data_ptr()),
-                                                ctypes.c_void_p(g["noise"].data_ptr()), ctypes.c_void_p(g["t_all"].data_ptr()),
-                                                coef, ns, q, ctypes.c_void_p(g["scratch"].data_ptr())), "dawn_unet_sampler_capture")
-            g["gen"] = unet.graph_generation()
-            self._graph = g
+        g, _ = self._captured_graph(
+            "_graph", "dawn_unet_sampler_capture", (Fr, h, w, tuple(pairs), q, img.device.index, one), unet,
+            lambda: unet.set_clip_invariants(*((fea, cond) if batched else (fea[0], cond[0]))), x_shape=one,
+            noise_shape=(max(ns - 1, 1),) + one, ts=[p[0] for p in pairs], args=lambda: dict(coef=self._ddim_coef_array(pairs)),
+            count=ns, q=q)
         for i in range(1 if batched else b):
             sel = slice(None) if batched else i
             unet.set_clip_invariants(fea[sel], cond[sel])
@@ -271,7 +277,7 @@ class GaussianDiffusion(nn.Module):
         pass takes 2b clips, otherwise m = 1 (one launch per clip).  Noise is drawn as the eager sampler draws it.  The
         scale sits in a device slot, so the cached capture serves every cond_scale."""
         b, ch, Fr, h, w = img.shape
-        device, n, ns = img.device, ch * Fr * h * w, len(pairs)
+        device, ns = img.device, len(pairs)
         if getattr(unet, "_shard", None) is not None:
             raise NotImplementedError("use_graph with cond_scale != 1 runs each clip and its null twin in one pass, and a "
                                       "frame-sharded UNet runs one clip at a time: sample with use_graph=False")
@@ -288,26 +294,12 @@ class GaussianDiffusion(nn.Module):
         def invariants(sel):                                    # [fea; fea], [cond; 0]
             f, c = fea[sel], cond[sel]
             unet.set_clip_invariants(torch.cat([f, f]), torch.cat([c, torch.zeros_like(c)]))
-        key = (Fr, h, w, tuple(pairs), q, device.index, m)
-        g = getattr(self, "_guided_graph", None)
-        unet.update_num_frames(Fr)
-        if g is None or g["key"] != key or g["gen"] != unet.graph_generation():
-            g = dict(key=key, x=torch.empty((2 * m, ch, Fr, h, w), device=device), eps=torch.empty((2 * m, ch, Fr, h, w), device=device),
-                     noise=torch.empty((max(ns - 1, 1), m, ch, Fr, h, w), device=device),
-                     t_all=torch.tensor([p[0] for p in pairs], dtype=torch.long, device=device),
-                     scale=torch.ones(1, device=device), scratch=torch.empty(n + 512, dtype=torch.int32, device=device))
-            coef = (ctypes.c_float * (5 * ns))()
-            for k, (t, t_next) in enumerate(pairs):
-                coef[5 * k:5 * k + 5] = self.ddim_coefficients(t, t_next)
-                assert (t_next > 0) == (k < ns - 1), "only the last DDIM step ends at t = 0 (reference :1201)"
-            invariants(slice(0, m))
-            torch.cuda.synchronize(device)
-            check(lib.dawn_unet_sampler_capture_guided(unet._handle, ctypes.c_void_p(g["x"].data_ptr()), ctypes.c_void_p(g["eps"].data_ptr()),
-                                                       ctypes.c_void_p(g["noise"].data_ptr()), ctypes.c_void_p(g["t_all"].data_ptr()),
-                                                       ctypes.c_void_p(g["scale"].data_ptr()), coef, ns, q,
-                                                       ctypes.c_void_p(g["scratch"].data_ptr())), "dawn_unet_sampler_capture_guided")
-            g["gen"] = unet.graph_generation()
-            self._guided_graph = g
+        g, captured = self._captured_graph(
+            "_guided_graph", "dawn_unet_sampler_capture_guided", (Fr, h, w, tuple(pairs), q, device.index, m), unet,
+            lambda: invariants(slice(0, m)), x_shape=(2 * m, ch, Fr, h, w), noise_shape=(max(ns - 1, 1), m, ch, Fr, h, w),
+            ts=[p[0] for p in pairs], args=lambda: dict(scale=torch.ones(1, device=device), coef=self._ddim_coef_array(pairs)),
+            count=ns, q=q)
+        if captured:
             self._guided_captures = getattr(self, "_guided_captures", 0) + 1
         g["scale"].fill_(float(cond_scale))
         # when the eager and cond_scale = 1 samplers step the b clips together but a pass cannot take 2b clips, the noise is
@@ -348,25 +340,6 @@ class GaussianDiffusion(nn.Module):
         """(ca, cb, c1, c2, sigma) of the ancestral update at timestep t, as Python floats (see ddpm_table)."""
         return tuple(float(v) for v in self.ddpm_table()[t])
 
-    def _ddpm_step(self, unet, fea_i, cond_i, x, t, cond_scale, guided, eps, eps_null, noise, q, scratch, st):
-        """One ancestral step in place on x (3, F, h, w), this handle's frames of one clip, or on x (b, 3, F, h, w), a batch
-        run in one pass (U:1087-1121).  Without guidance the caller has set the clip invariants of (fea_i, cond_i)."""
-        t_dev = torch.full((x.shape[0] if x.dim() == 5 else 1,), t, device=x.device, dtype=torch.long)
-        if guided:
-            # forward_with_cond_scale (U:879-890): null + (cond - null) * cond_scale, the null condition being all zeros
-            # (learn_null_cond=False, U:920); two hoisted forwards, each after rebuilding the per-clip conditioning tables
-            unet.set_clip_invariants(fea_i, cond_i)
-            unet.forward_x3(x, t_dev, eps)
-            unet.set_clip_invariants(fea_i, torch.zeros_like(cond_i))
-            unet.forward_x3(x, t_dev, eps_null)
-            eps.sub_(eps_null).mul_(float(cond_scale)).add_(eps_null)
-        else:
-            unet.forward_x3(x, t_dev, eps)
-        ca, cb, c1, c2, sigma = self.ddpm_coefficients(t)
-        check(lib.dawn_unet_ddpm_step(unet._handle, ctypes.c_void_p(x.data_ptr()), ctypes.c_void_p(eps.data_ptr()),
-                                      ctypes.c_void_p(noise.data_ptr()) if noise is not None else None, x.numel(),
-                                      ca, cb, c1, c2, sigma, q, ctypes.c_void_p(scratch.data_ptr()), st), "dawn_unet_ddpm_step")
-
     @torch.no_grad()
     def p_sample(self, x, t, fea, cond=None, cond_scale=1., clip_denoised=True, noise=None):
         """reference p_sample (U:1112-1121): one ancestral step of x (b, 3, F, h, w) at timestep t (an int, or the reference's
@@ -381,29 +354,15 @@ class GaussianDiffusion(nn.Module):
         if not 0 <= t < self.num_timesteps:
             raise ValueError(f"p_sample: t = {t} is outside [0, {self.num_timesteps})")
         device = self.betas.device
-        b, ch, Fr, h, w = x.shape
         self._check_sample_shape("p_sample", fea, tuple(x.shape), cond)
-        unet = self.denoise_fn
         if noise is None:
-            noise = self._default_noise(unet, device, None)(0, tuple(x.shape))
+            noise = self._default_noise(self.denoise_fn, device, None)(0, tuple(x.shape))
         if tuple(noise.shape) != tuple(x.shape):
             raise ValueError(f"p_sample: noise {tuple(noise.shape)} does not match x {tuple(x.shape)}")
         img = x.to(device=device, dtype=torch.float32).contiguous().clone()
         noise = noise.to(device=device, dtype=torch.float32).contiguous()
-        guided = cond_scale != 1 and getattr(unet, "has_cond", True)
-        st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-        scratch = torch.empty(ch * Fr * h * w + 512, dtype=torch.int32, device=device)
-        batched = self._batched(unet, b, Fr, h, w)
-        eps = torch.empty(tuple(img.shape) if batched else (ch, Fr, h, w), device=device)
-        eps_null = torch.empty_like(eps) if guided else None
-        q = self._clip_q(clip_denoised)
-        for i in range(1 if batched else b):
-            sel = slice(None) if batched else i
-            unet.update_num_frames(Fr)
-            if not guided:
-                unet.set_clip_invariants(fea[sel], cond[sel])
-            self._ddpm_step(unet, fea[sel], cond[sel], img[sel], t, cond_scale, guided, eps, eps_null, noise[sel], q, scratch, st)
-        return img
+        return self._sample_eager("dawn_unet_ddpm_step", fea, cond, img, [(t, self.ddpm_coefficients(t))], cond_scale,
+                                  self._clip_q(clip_denoised), lambda k, sel, one: noise[sel])
 
     @torch.no_grad()
     def p_sample_loop(self, fea, shape, cond=None, cond_scale=1., clip_denoised=True, noise_fn=None, use_graph=False, seed=None):
@@ -418,55 +377,30 @@ class GaussianDiffusion(nn.Module):
         each replay.  Frame-sharded UNet: as ddim_sample (clip-wide quantile; default noise = this rank's slice of one
         clip-wide seeded stream)."""
         device = self.betas.device
-        b, ch, Fr, h, w = shape
         unet = self.denoise_fn
         self._check_sample_shape("p_sample_loop", fea, shape, cond)
         draw = noise_fn if noise_fn is not None else self._default_noise(unet, device, seed)
         img = draw(-1, shape).to(device).contiguous()
         q = self._clip_q(clip_denoised)
         st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-        guided = cond_scale != 1 and getattr(unet, "has_cond", True)
         if use_graph:
-            if guided:
+            if cond_scale != 1 and getattr(unet, "has_cond", True):
                 raise NotImplementedError("use_graph captures the cond_scale = 1 step (DAWN's shipped setting); "
                                           "classifier-free guidance runs eagerly")
             return self._p_sample_loop_graph(unet, fea, cond, img, draw, q, st)
-        scratch = torch.empty(ch * Fr * h * w + 512, dtype=torch.int32, device=device)
-        batched = self._batched(unet, b, Fr, h, w)
-        one = tuple(shape) if batched else (ch, Fr, h, w)
-        eps = torch.empty(one, device=device)
-        eps_null = torch.empty_like(eps) if guided else None
-        T = self.num_timesteps
-        for i in range(1 if batched else b):
-            sel = slice(None) if batched else i
-            unet.update_num_frames(Fr)
-            if not guided:
-                unet.set_clip_invariants(fea[sel], cond[sel])
-            for k in range(T):
-                noise = draw(k, one).to(device).contiguous()
-                self._ddpm_step(unet, fea[sel], cond[sel], img[sel], T - 1 - k, cond_scale, guided, eps, eps_null, noise, q, scratch, st)
-        return img
+        steps = [(t, self.ddpm_coefficients(t)) for t in reversed(range(self.num_timesteps))]
+        return self._sample_eager("dawn_unet_ddpm_step", fea, cond, img, steps, cond_scale, q,
+                                  lambda k, sel, one: draw(k, one).to(device).contiguous())
 
     def _p_sample_loop_graph(self, unet, fea, cond, img, draw, q, st):
         b, ch, Fr, h, w = img.shape
-        device, n, T = img.device, ch * Fr * h * w, self.num_timesteps
+        device, T = img.device, self.num_timesteps
         batched = self._batched(unet, b, Fr, h, w)
         one = (b, ch, Fr, h, w) if batched else (ch, Fr, h, w)
-        key = (Fr, h, w, T, q, device.index, one)
-        g = getattr(self, "_ddpm_graph", None)
-        unet.update_num_frames(Fr)
-        if g is None or g["key"] != key or g["gen"] != unet.graph_generation():
-            g = dict(key=key, x=torch.empty(one, device=device), eps=torch.empty(one, device=device),
-                     noise=torch.empty(one, device=device), t=torch.empty(1, dtype=torch.long, device=device),
-                     coef=torch.empty((T, 5), device=device), scratch=torch.empty(n + 512, dtype=torch.int32, device=device))
-            unet.set_clip_invariants(*((fea, cond) if batched else (fea[0], cond[0])))
-            torch.cuda.synchronize(device)
-            check(lib.dawn_unet_ddpm_capture(unet._handle, ctypes.c_void_p(g["x"].data_ptr()), ctypes.c_void_p(g["eps"].data_ptr()),
-                                             ctypes.c_void_p(g["noise"].data_ptr()), ctypes.c_void_p(g["t"].data_ptr()),
-                                             ctypes.c_void_p(g["coef"].data_ptr()), T, q, ctypes.c_void_p(g["scratch"].data_ptr())),
-                  "dawn_unet_ddpm_capture")
-            g["gen"] = unet.graph_generation()
-            self._ddpm_graph = g
+        g, _ = self._captured_graph(
+            "_ddpm_graph", "dawn_unet_ddpm_capture", (Fr, h, w, T, q, device.index, one), unet,
+            lambda: unet.set_clip_invariants(*((fea, cond) if batched else (fea[0], cond[0]))), x_shape=one, noise_shape=one,
+            ts=[T - 1], args=lambda: dict(coef=torch.empty((T, 5), device=device)), count=T, q=q)
         g["coef"].copy_(self.ddpm_table())          # the schedule buffers may have been reloaded since the capture
         for i in range(1 if batched else b):
             sel = slice(None) if batched else i
