@@ -12,7 +12,8 @@ class DawnUnetCfg(ctypes.Structure):
                 ("channels", ctypes.c_int), ("cond_aud", ctypes.c_int), ("cond_pose", ctypes.c_int),
                 ("cond_eye", ctypes.c_int), ("out_grid_dim", ctypes.c_int), ("out_conf_dim", ctypes.c_int),
                 ("attn_heads", ctypes.c_int), ("attn_dim_head", ctypes.c_int), ("resnet_groups", ctypes.c_int),
-                ("init_kernel_size", ctypes.c_int), ("win_width", ctypes.c_int)]
+                ("init_kernel_size", ctypes.c_int), ("win_width", ctypes.c_int),
+                ("upconv", ctypes.c_int), ("pad_mode", ctypes.c_int), ("no_sla", ctypes.c_int)]
 
 
 class DawnLfgCfg(ctypes.Structure):

@@ -215,19 +215,23 @@ int pack_up(std::vector<void*>& owner, int ci, int co, const int (&off)[2][2], c
   return 0;
 }
 
-int run_up(const GemmParams& in, const UpConv& u, float* out, int ldo, const std::function<int(const GemmParams&)>& run) {
-  GemmParams p = in;
-  set_weights(p, u.all); set_square_taps(p, 3, 1);
-  p.up2 = 1; p.Out = out; p.ldo = ldo;
-  if (path_ok(p, EPI_PLAIN, DAWN_PATH_TC_CONV3, 0)) return run(p);
+int run_up(const GemmParams& in, const UpConv& u, float* out, int ldo, const std::function<int(const GemmParams&)>& run, int border) {
+  if (!border) {
+    GemmParams p = in;
+    set_weights(p, u.all); set_square_taps(p, 3, 1);
+    p.up2 = 1; p.Out = out; p.ldo = ldo;
+    if (path_ok(p, EPI_PLAIN, DAWN_PATH_TC_CONV3, 0)) return run(p);
+  }
   for (int py = 0; py < 2; ++py)
     for (int px = 0; px < 2; ++px) {
       GemmParams q = in;
       set_weights(q, u.cls[py * 2 + px]);
       q.ntaps = 4;
       for (int ty = 0; ty < 2; ++ty)
-        for (int tx = 0; tx < 2; ++tx) { q.dy[ty * 2 + tx] = (signed char)u.off[py][ty]; q.dx[ty * 2 + tx] = (signed char)u.off[px][tx]; }
-      q.OH = 2 * in.IH; q.OW = 2 * in.IW; q.out_stride = 2; q.oy0 = py; q.ox0 = px;
+        for (int tx = 0; tx < 2; ++tx) {
+          q.dy[ty * 2 + tx] = (signed char)(u.off[py][ty] + border); q.dx[ty * 2 + tx] = (signed char)(u.off[px][tx] + border);
+        }
+      q.OH = 2 * in.OHs; q.OW = 2 * in.OWs; q.out_stride = 2; q.oy0 = py; q.ox0 = px;
       q.Out = out; q.ldo = ldo;
       DAWN_TRY(run(q));
     }

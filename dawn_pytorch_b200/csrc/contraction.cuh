@@ -73,10 +73,17 @@ struct UpConv {
   int off[2][2];
 };
 using UpWeight = std::function<float(int py, int px, int ty, int tx, int c, int n)>;   // weight of class tap (ty, tx), c -> n
+// Nearest x2 followed by a 3x3 conv (padding 1) on the low-resolution grid: parity p's tap t reads offset kUpOff[p][t] and its
+// weight is the sum of the kernel indices k with up_in_set(p, t, k), i.e. p = 0: {-1 <- k0, 0 <- k1 + k2}, p = 1: {0 <- k0 + k1,
+// +1 <- k2}.  Zero padding is the same on both grids (upsampled index -1 / 2H <-> low-resolution index -1 / H).
+constexpr int kUpOff[2][2] = {{-1, 0}, {0, 1}};
+inline bool up_in_set(int parity, int tap, int k) { return parity == 0 ? (tap == 0 ? k == 0 : k >= 1) : (tap == 0 ? k <= 1 : k == 2); }
 int pack_up(std::vector<void*>& owner, int ci, int co, const int (&off)[2][2], const std::vector<float>& bias, const UpWeight& weight,
             UpConv* u);
 // in: base_params of the low-resolution input; out: (frames, 2H, 2W) rows of stride ldo.  run launches one contraction: once with
-// the up2 halo conv when that path takes it, otherwise once per parity class.
-int run_up(const GemmParams& in, const UpConv& u, float* out, int ldo, const std::function<int(const GemmParams&)>& run);
+// the up2 halo conv when that path takes it, otherwise once per parity class.  border = 1: `in` reads a grid that carries a
+// one-pixel border (IH = OHs + 2, IW = OWs + 2); the classes then run as valid 2x2 convs over it, so no tap leaves the grid.
+int run_up(const GemmParams& in, const UpConv& u, float* out, int ldo, const std::function<int(const GemmParams&)>& run,
+           int border = 0);
 
 }  // namespace dawn

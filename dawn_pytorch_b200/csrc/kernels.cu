@@ -337,6 +337,33 @@ int launch_split_rows(const float* x, int ld, int C, long long M, void* hi, void
   return 0;
 }
 
+// =========================================================================== one-pixel border of the upconv input
+// x (frames, H, W, C) rows of stride ld -> dense out (frames, H + 2, W + 2, C): the interior is x, border row / column -1 and H / W
+// read x at the clamped (wrap = 0) or wrapped (wrap = 1) index
+__global__ void pad_border_kernel(const float* __restrict__ x, int ld, int C, int frames, int H, int W, int wrap,
+                                  float4* __restrict__ out) {
+  const int c4n = C >> 2, PW = W + 2, PH = H + 2;
+  const long long total = (long long)frames * PH * PW * c4n;
+  for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
+    long long r = idx / c4n;
+    const int c4 = (int)(idx - r * c4n);
+    const int px = (int)(r % PW) - 1; r /= PW;
+    const int py = (int)(r % PH) - 1;
+    const long long f = r / PH;
+    const int sy = wrap ? (py + H) % H : min(max(py, 0), H - 1);
+    const int sx = wrap ? (px + W) % W : min(max(px, 0), W - 1);
+    out[idx] = __ldg(reinterpret_cast<const float4*>(x + ((size_t)(f * H + sy) * W + sx) * ld) + c4);
+  }
+}
+int launch_pad_border(const float* x, int ld, int C, int frames, int H, int W, int wrap, float* out, cudaStream_t st) {
+  DAWN_CHECK(C % 4 == 0 && ld % 4 == 0, "launch_pad_border: channels and row stride must be multiples of 4");
+  const long long total = (long long)frames * (H + 2) * (W + 2) * (C >> 2);
+  const int blocks = (int)std::min<long long>((total + 255) / 256, 148LL * 16);
+  pad_border_kernel<<<blocks, 256, 0, st>>>(x, ld, C, frames, H, W, wrap, reinterpret_cast<float4*>(out));
+  DAWN_LAUNCH_OK();
+  return 0;
+}
+
 // =========================================================================== time embedding
 __global__ void time_mlp_kernel(const int64_t* __restrict__ t, const float* __restrict__ freqs, int dim,
                                 const float* __restrict__ W1, const float* __restrict__ b1,

@@ -81,6 +81,10 @@ int launch_split_rows(const float* x, int ld, int C, long long M, void* hi, void
 int launch_sla_context(const float* qkv, int ld, int F, int P, const float* WoutT /*[256][C]*/, int C,
                        float* Bf, int ldb, cudaStream_t st);
 
+// x (frames, H, W, C) rows of stride ld -> dense (frames, H + 2, W + 2, C) with a one-pixel border at the clamped (wrap = 0) or
+// wrapped (wrap = 1) index: the upconv's reflect / replicate / circular padding seen on the low-resolution grid (unet.cu)
+int launch_pad_border(const float* x, int ld, int C, int frames, int H, int W, int wrap, float* out, cudaStream_t st);
+
 // ---------------------------------------------------------------- layout / heads / init conv
 // x (clips, C, F, H*W) channel-major -> (F * clips, H*W, Cpad) channels-last (frame f of clip b at f * clips + b), zero padding
 // channels [C, Cpad).  skip_flag (device int, optional): the kernel returns at once when *skip_flag == skip_if (device-side path

@@ -84,12 +84,8 @@ int pack_conv(dawn_lfg* h, const std::string& conv, const std::string& bn_after,
 }
 // UpBlock2d (util.py:106-111): F.interpolate(scale_factor=2) [nearest] -> conv3x3 -> BN -> ReLU.  On the LOW-resolution grid the
 // output pixel (2y+py, 2x+px) sees rows {y-1 (ky=0), y (ky=1,2)} for py=0 and {y (ky=0,1), y+1 (ky=2)} for py=1 (same for columns):
-// each output-parity class is a 2x2 conv whose taps are sums of the 3x3 kernel's taps — 2.25x fewer MACs and the upsampled
-// tensor never exists.  Zero padding is the same on both grids (upsampled index -1 / 2H <-> low-res index -1 / H).
-const int kUpOff[2][2] = {{-1, 0}, {0, 1}};                     // [parity][tap] -> low-res offset
-inline bool up_in_set(int parity, int tap, int k) {             // does kernel index k feed (parity, tap)?
-  return parity == 0 ? (tap == 0 ? k == 0 : k >= 1) : (tap == 0 ? k <= 1 : k == 2);
-}
+// each output-parity class is a 2x2 conv whose taps are sums of the 3x3 kernel's taps (kUpOff, up_in_set: contraction.cuh) — 2.25x
+// fewer MACs and the upsampled tensor never exists.
 int pack_up(dawn_lfg* h, const std::string& name, int co, int ci, UpConv* u) {
   const HostParam *w, *b;
   DAWN_TRY(h->raw.need(name + ".conv.weight", {co, ci, 3, 3}, &w));

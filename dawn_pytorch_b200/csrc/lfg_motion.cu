@@ -102,8 +102,6 @@ int pack_convs(dawn_lfg_motion* h, const std::vector<std::pair<std::string, int>
 }
 
 // UpBlock2d (util.py:106-111): nearest x2 -> conv3x3 -> BN as four parity-class 2x2 convs on the low-resolution grid (lfg.cu)
-const int kUpOff[2][2] = {{-1, 0}, {0, 1}};
-inline bool up_in_set(int parity, int tap, int k) { return parity == 0 ? (tap == 0 ? k == 0 : k >= 1) : (tap == 0 ? k <= 1 : k == 2); }
 int pack_up(dawn_lfg_motion* h, const std::string& name, int co, int ci, UpConv* u) {
   const HostParam *w, *b;
   DAWN_TRY(h->raw.need(name + ".conv.weight", {co, ci, 3, 3}, &w));

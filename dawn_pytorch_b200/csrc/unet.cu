@@ -199,6 +199,7 @@ struct dawn_unet {
   std::vector<float*> bufA, bufB, CAT, DS;
   float *Y = nullptr, *A1 = nullptr, *QKV = nullptr, *O = nullptr, *ROWSTATS = nullptr, *GATES = nullptr, *WT = nullptr;
   float *BF = nullptr, *HF = nullptr, *HO = nullptr, *ROT = nullptr, *TSILU = nullptr;
+  float* UPPAD = nullptr;                      // upconv input with its one-pixel border (reflect, replicate, circular only)
   double* STATS = nullptr; int n_stats = 0;
   int64_t* T_HOSTSIDE = nullptr;               // device int64 for forward_host
   float *H_XT = nullptr, *H_FEA = nullptr, *H_COND = nullptr, *H_OUT = nullptr;   // device staging for forward_host
@@ -385,6 +386,21 @@ int pack_up(dawn_unet* h, const std::string& name, int C, UpConv* u) {
   }, u);
 }
 
+// Upsample(use_deconv=False) (U:168-172): nearest x2, then Conv3d (1,3,3) weight (co=C, ci=C, 1, 3, 3) at "<name>.1": the same
+// four parity classes, each tap the sum of the 3x3 taps it covers (kUpOff, up_in_set), summed in fp64 and rounded once
+int pack_upconv(dawn_unet* h, const std::string& name, int C, UpConv* u) {
+  const HostParam *w, *b;
+  DAWN_TRY(h->raw.need(name + ".1.weight", {C, C, 1, 3, 3}, &w));
+  DAWN_TRY(h->raw.need(name + ".1.bias", {C}, &b));
+  return dawn::pack_up(h->owned, C, C, kUpOff, b->data, [&](int py, int px, int ty, int tx, int c, int n) {
+    double acc = 0.0;
+    for (int ky = 0; ky < 3; ++ky)
+      for (int kx = 0; kx < 3; ++kx)
+        if (up_in_set(py, ty, ky) && up_in_set(px, tx, kx)) acc += (double)w->data[(((size_t)n * C + c) * 3 + ky) * 3 + kx];
+    return (float)acc;
+  }, u);
+}
+
 // ------------------------------------------------------------------------------------------ GEMM wrappers
 void base_params(GemmParams& p, const Act& in, int F) { dawn::base_params(p, in.p, in.ld, in.C, F, in.H, in.W); }
 
@@ -392,7 +408,7 @@ void base_params(GemmParams& p, const Act& in, int F) { dawn::base_params(p, in.
 // profile categories (dawn_unet_profile_read)
 enum ProfCat : int {
   PC_CONV3 = 0,      // 3x3 conv implicit GEMM (+GroupNorm statistics)
-  PC_CONV_OTHER,     // init 7x7, 4x4 down / transposed up, 1x1 residual convs
+  PC_CONV_OTHER,     // init 7x7, 4x4 down / transposed or nearest x2 up (+ its border pass), 1x1 residual convs
   PC_QKV,            // LayerNorm-folded qkv projections (temporal / spatial-linear / mid attention)
   PC_OUTPROJ,        // attention output projections (+ residual)
   PC_CA_GATE,        // cross-attention q projection + 2-key softmax gate
@@ -748,9 +764,27 @@ int downsample(Ctx& c, const PackedWeight& w, const Act& x, const Act& out, cons
   return tap(c, name, out);
 }
 
-int upsample(Ctx& c, const UpConv& u, const Act& x, const Act& out, const std::string& name) {   // U:165-167
-  GemmParams p; base_params(p, x, c.h->F * c.h->B);
-  DAWN_TRY(run_up(p, u, out.p, out.ld, [&](const GemmParams& q) { return c.gemm(q, EPI_PLAIN, PC_CONV_OTHER); }));
+int upsample(Ctx& c, const UpConv& u, const Act& x, const Act& out, const std::string& name) {   // U:165-172
+  dawn_unet* h = c.h;
+  const int NF = h->F * h->B;
+  auto run = [&](const GemmParams& q) { return c.gemm(q, EPI_PLAIN, PC_CONV_OTHER); };
+  GemmParams p;
+  if (h->cfg.pad_mode == 0) {                        // ConvTranspose, or zero padding: taps off the grid read zeros on both grids
+    base_params(p, x, NF);
+    DAWN_TRY(run_up(p, u, out.p, out.ld, run));
+    return tap(c, name, out);
+  }
+  // A one-pixel reflect or replicate pad of the upsampled grid reads low-resolution index clamp(i) at i = -1 and H, a circular
+  // pad reads i mod H (DESIGN.md section 2).  One pass writes that border around the input; the classes then run as valid convs.
+  {
+    const double px = (double)NF * x.C;
+    ProfScope ps(c, PC_CONV_OTHER, 0, 4.0 * px * ((double)x.H * x.W + (x.H + 2.0) * (x.W + 2)));
+    DAWN_TRY(launch_pad_border(x.p, x.ld, x.C, NF, x.H, x.W, h->cfg.pad_mode == 3, h->UPPAD, c.st));
+  }
+  base_params(p, h->UPPAD, x.C, x.C, NF, x.H + 2, x.W + 2);
+  p.OHs = x.H; p.OWs = x.W; p.OH = x.H; p.OW = x.W; p.P = x.H * x.W;
+  p.M = NF * x.H * x.W; p.rows_per_batch = p.M;
+  DAWN_TRY(run_up(p, u, out.p, out.ld, run, 1));
   return tap(c, name, out);
 }
 
@@ -838,7 +872,7 @@ int forward_core(dawn_unet* h, const int64_t* t_dev, int t_stride, float* out, c
     const std::string pre = "downs." + std::to_string(L);
     DAWN_TRY(resblock(c, h->rb[h->rb_index[pre + ".0"]], x, a));
     DAWN_TRY(resblock(c, h->rb[h->rb_index[pre + ".1"]], a, b));
-    DAWN_TRY(sla(c, h->down_sla[L], b, pre + ".2"));
+    if (!h->cfg.no_sla) DAWN_TRY(sla(c, h->down_sla[L], b, pre + ".2"));
     DAWN_TRY(temporal_attn(c, h->down_ta[L], b, skip, pre + ".3"));
     if (L < nlev - 1) {
       Act d{h->DS[L + 1], co, co, h->lH[L + 1], h->lW[L + 1]};
@@ -865,7 +899,7 @@ int forward_core(dawn_unet* h, const int64_t* t_dev, int t_stride, float* out, c
     const std::string pre = "ups." + std::to_string(K);
     DAWN_TRY(resblock(c, h->rb[h->rb_index[pre + ".0"]], cat, a));
     DAWN_TRY(resblock(c, h->rb[h->rb_index[pre + ".1"]], a, b));
-    DAWN_TRY(sla(c, h->up_sla[K], b, pre + ".2"));
+    if (!h->cfg.no_sla) DAWN_TRY(sla(c, h->up_sla[K], b, pre + ".2"));
     if (K < nlev - 1) {
       DAWN_TRY(temporal_attn(c, h->up_ta[K], b, b, pre + ".3"));
       const int cn = h->in_out[l - 1].second;        // == ci
@@ -919,6 +953,10 @@ int dawn_unet_create(const dawn_unet_cfg* cfg, dawn_unet** out) {
   DAWN_CHECK(cfg->n_levels >= 2 && cfg->n_levels <= 6, "n_levels out of range");
   DAWN_CHECK(cfg->init_kernel_size == 7 || cfg->init_kernel_size == 5 || cfg->init_kernel_size == 3, "init kernel must be 3, 5 or 7");
   DAWN_CHECK(cfg->win_width >= 1 && cfg->win_width <= 120, "win_width out of range");
+  DAWN_CHECK(cfg->upconv == 0 || cfg->upconv == 1, "upconv must be 0 (ConvTranspose3d) or 1 (nearest x2 + 3x3 conv)");
+  DAWN_CHECK(cfg->pad_mode >= 0 && cfg->pad_mode <= 3, "pad_mode must be 0 (zeros), 1 (reflect), 2 (replicate) or 3 (circular)");
+  DAWN_CHECK(cfg->pad_mode == 0 || cfg->upconv == 1, "pad_mode applies to the upconv variant only (upconv = 1)");
+  DAWN_CHECK(cfg->no_sla == 0 || cfg->no_sla == 1, "no_sla must be 0 or 1");
   dawn_unet* h = new dawn_unet();
   h->cfg = *cfg;
   h->nlev = cfg->n_levels;
@@ -997,7 +1035,7 @@ int dawn_unet_commit_params(dawn_unet* h) {
     const std::string pre = "downs." + std::to_string(L);
     DAWN_TRY(pack_resblock(h, pre + ".0", ci, co, true, &stat_counter));
     DAWN_TRY(pack_resblock(h, pre + ".1", co, co, true, &stat_counter));
-    SlaW s; DAWN_TRY(pack_sla(h, pre + ".2.fn", co, &s)); h->down_sla.push_back(s);
+    if (!cfg.no_sla) { SlaW s; DAWN_TRY(pack_sla(h, pre + ".2.fn", co, &s)); h->down_sla.push_back(s); }
     AttnW a; DAWN_TRY(pack_attn(h, pre + ".3.fn.norm", pre + ".3.fn.fn.fn", co, &a)); h->down_ta.push_back(a);
     if (L < nlev - 1) {
       PackedWeight d; DAWN_TRY(pack_conv(h, pre + ".4", co, co, 4, 4, co, true, &d)); h->down_conv.push_back(d);
@@ -1014,10 +1052,10 @@ int dawn_unet_commit_params(dawn_unet* h) {
     const std::string pre = "ups." + std::to_string(K);
     DAWN_TRY(pack_resblock(h, pre + ".0", 2 * co, ci, true, &stat_counter));
     DAWN_TRY(pack_resblock(h, pre + ".1", ci, ci, true, &stat_counter));
-    SlaW s; DAWN_TRY(pack_sla(h, pre + ".2.fn", ci, &s)); h->up_sla.push_back(s);
+    if (!cfg.no_sla) { SlaW s; DAWN_TRY(pack_sla(h, pre + ".2.fn", ci, &s)); h->up_sla.push_back(s); }
     AttnW a; DAWN_TRY(pack_attn(h, pre + ".3.fn.norm", pre + ".3.fn.fn.fn", ci, &a)); h->up_ta.push_back(a);
     if (K < nlev - 1) {
-      UpConv u; DAWN_TRY(pack_up(h, pre + ".4", ci, &u)); h->up_conv.push_back(u);
+      UpConv u; DAWN_TRY(cfg.upconv ? pack_upconv(h, pre + ".4", ci, &u) : pack_up(h, pre + ".4", ci, &u)); h->up_conv.push_back(u);
     }
   }
   // heads: ResnetBlock_ca_mul without time/cond MLPs (their cross-attention parameters exist but never run, U:862, 875)
@@ -1080,6 +1118,11 @@ int dawn_unet_set_geometry(dawn_unet* h, int B, int F, int height, int width) {
     max_mc = std::max(max_mc, Ml * cw);
     max_bf = std::max(max_bf, (size_t)NF * 256 * round_up(cw, 64));
     max_pc = std::max(max_pc, (size_t)h->lH[l] * h->lW[l] * cw);
+  }
+  if (h->cfg.pad_mode != 0) {                                         // bordered inputs of the up path's upconvs (levels >= 1)
+    size_t n = 0;
+    for (int l = 1; l < nlev; ++l) n = std::max(n, (size_t)NF * (h->lH[l] + 2) * (h->lW[l] + 2) * h->in_out[l].first);
+    DAWN_TRY(dev_alloc(own, n, &h->UPPAD, cnt));
   }
   max_mc = std::max(max_mc, M0 * dim);
   DAWN_TRY(dev_alloc(own, max_mc, &h->Y, cnt));
@@ -1259,6 +1302,8 @@ int dawn_unet_tap_shape(dawn_unet* h, const char* name, int* C, int* hl, int* wl
   if (n == "init_conv" || n == "init_temporal_attn" || n == "final_conv.0" || n == "occlusion_map.0") return set(dim, 0);
   if (n.rfind("mid_", 0) == 0) return set(h->dims.back(), nlev - 1);
   int L = -1, j = -1;
+  if ((sscanf(name, "downs.%d.%d", &L, &j) == 2 || sscanf(name, "ups.%d.%d", &L, &j) == 2) && j == 2)
+    DAWN_CHECK(!h->cfg.no_sla, "no such tap: the network has no spatial linear attention");
   if (sscanf(name, "downs.%d.%d", &L, &j) == 2 && L >= 0 && L < nlev) {
     if (j == 4) { DAWN_CHECK(L < nlev - 1, "no such tap"); return set(h->in_out[L].second, L + 1); }
     return set(h->in_out[L].second, L);

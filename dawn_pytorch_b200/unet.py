@@ -17,6 +17,7 @@ from torch import nn
 from . import _lib
 from ._lib import DawnUnetCfg, check, lib
 
+PADDING_MODES = ("zeros", "reflect", "replicate", "circular")   # nn.Conv3d's, in the order of dawn_unet_cfg.pad_mode
 MAX_CLIPS = 16                  # clips per native pass the library accepts (kMaxClips, csrc/common.cuh)
 # Largest batched pass, in frames x latent pixels over all its clips: bounds the workspace of a pass (~9 KiB per pixel-frame,
 # ~19 GiB at the cap: two 200-frame 64x64 clips, ten 200-frame 32x32 clips).  Per-clip times: DESIGN.md section 5.
@@ -151,9 +152,11 @@ class Unet3D(nn.Module):
         super().__init__()
         if init_dim is not None and init_dim != dim:
             raise NotImplementedError("init_dim != dim is not supported by the CUDA library")
-        if not use_sparse_linear_attn or not use_deconv or padding_mode != "zeros" or use_final_activation or learn_null_cond:
-            raise NotImplementedError("only the configuration DAWN ships is supported: use_sparse_linear_attn=True, "
-                                      "use_deconv=True, padding_mode='zeros', use_final_activation=False, learn_null_cond=False")
+        if learn_null_cond:
+            # the reference draws a fresh random null embedding inside every forward (U:917-918): nothing to load or match
+            raise NotImplementedError("learn_null_cond=True is not supported")
+        if padding_mode not in PADDING_MODES:
+            raise ValueError(f"padding_mode must be one of {PADDING_MODES}, but got padding_mode='{padding_mode}'")
         self.null_cond_mask = None
         self.null_cond_emb = None
         self.channels = channels
@@ -189,6 +192,14 @@ class Unet3D(nn.Module):
         def cond_block(a, b):
             return _resnet_block(a, b, resnet_groups, time_dim, cond_aud, cond_pose, cond_eye)
 
+        def sla(d):                                                         # U:832-833, 854-855
+            return _prenorm_residual(d, _spatial_linear_attention(d, attn_heads)) if use_sparse_linear_attn else nn.Identity()
+
+        def upsample(d):                                                    # U:165-172: nn.Upsample holds no parameters
+            if use_deconv:
+                return nn.ConvTranspose3d(d, d, (1, 4, 4), (1, 2, 2), (0, 1, 1))
+            return nn.Sequential(_Holder(), nn.Conv3d(d, d, (1, 3, 3), (1, 1, 1), (0, 1, 1), padding_mode=padding_mode))
+
         self.downs = nn.ModuleList([])
         self.ups = nn.ModuleList([])
         n_res = len(in_out)
@@ -196,7 +207,7 @@ class Unet3D(nn.Module):
             last = ind >= n_res - 1
             self.downs.append(nn.ModuleList([
                 cond_block(di, do), cond_block(do, do),
-                _prenorm_residual(do, _spatial_linear_attention(do, attn_heads)),
+                sla(do),
                 _prenorm_residual(do, temporal(do)),
                 nn.Conv3d(do, do, (1, 4, 4), (1, 2, 2), (0, 1, 1)) if not last else nn.Identity()]))
         mid = dims[-1]
@@ -208,11 +219,13 @@ class Unet3D(nn.Module):
             last = ind >= n_res - 1
             self.ups.append(nn.ModuleList([
                 cond_block(do * 2, di), cond_block(di, di),
-                _prenorm_residual(di, _spatial_linear_attention(di, attn_heads)),
+                sla(di),
                 _prenorm_residual(di, temporal(di)),
-                nn.ConvTranspose3d(di, di, (1, 4, 4), (1, 2, 2), (0, 1, 1)) if not last else nn.Identity()]))
+                upsample(di) if not last else nn.Identity()]))
         self.final_conv = nn.Sequential(_resnet_block(dim * 2, dim, resnet_groups), nn.Conv3d(dim, out_grid_dim, 1))
-        self.final_activation = nn.Identity()
+        # use_final_activation=True creates nn.Tanh() (U:867-871) but forward never applies it (U:956 returns the two heads as they
+        # are): the flag is accepted and changes nothing
+        self.final_activation = nn.Tanh() if use_final_activation else nn.Identity()
         self.occlusion_map = nn.Sequential(_resnet_block(dim * 2, dim, resnet_groups), nn.Conv3d(dim, out_conf_dim, 1))
 
         cfg = DawnUnetCfg()
@@ -223,6 +236,9 @@ class Unet3D(nn.Module):
         cfg.out_grid_dim, cfg.out_conf_dim = out_grid_dim, out_conf_dim
         cfg.attn_heads, cfg.attn_dim_head, cfg.resnet_groups = attn_heads, attn_dim_head, resnet_groups
         cfg.init_kernel_size, cfg.win_width = init_kernel_size, win_width
+        cfg.upconv = 0 if use_deconv else 1
+        cfg.pad_mode = 0 if use_deconv else PADDING_MODES.index(padding_mode)
+        cfg.no_sla = 0 if use_sparse_linear_attn else 1
         self._cfg = cfg
         self._handle = None
         self._dirty = True

@@ -40,6 +40,10 @@ typedef struct {
   int resnet_groups;    /* 8  (only 8 supported) */
   int init_kernel_size; /* 7 */
   int win_width;        /* 40: temporal attention attends |i-j| <= win_width (reference :117) */
+  /* Fields below are zero for DAWN's own network. */
+  int upconv;           /* 0: up path ConvTranspose3d (1,4,4)/(1,2,2) (use_deconv=True); 1: nearest x2 + Conv3d (1,3,3) (U:165-172) */
+  int pad_mode;         /* upconv only, the Conv3d's padding_mode on H and W: 0 zeros, 1 reflect, 2 replicate, 3 circular */
+  int no_sla;           /* 1: no spatial linear attention in the down and up blocks (use_sparse_linear_attn=False, U:833, 855) */
 } dawn_unet_cfg;
 
 /* replaces Unet3D.__init__ / DynamicNfUnet3D.__init__ (reference :728-877, 959-963) */
