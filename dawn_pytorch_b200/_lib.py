@@ -62,7 +62,8 @@ class DawnFusedCase(ctypes.Structure):
 
 
 KERNEL_ROWSTATS, KERNEL_GN_APPLY, KERNEL_COND_TABLES, KERNEL_TIME_MLP, KERNEL_FILM, KERNEL_ROTARY, KERNEL_SPLIT_ROWS, \
-    KERNEL_NCF_TO_NHWC, KERNEL_FRAME_INVARIANCE, KERNEL_FEA_SHIFT, KERNEL_MAP_REDUCE, KERNEL_INIT_CONV_X3, KERNEL_HEADS_OUT = range(13)
+    KERNEL_NCF_TO_NHWC, KERNEL_FRAME_INVARIANCE, KERNEL_FEA_SHIFT, KERNEL_MAP_REDUCE, KERNEL_INIT_CONV_X3, KERNEL_HEADS_OUT, \
+    KERNEL_DDIM_STEP, KERNEL_DDPM_STEP = range(15)
 KERNEL_MAX_DESC = 16
 
 
@@ -86,7 +87,9 @@ class DawnKernelCase(ctypes.Structure):
                 ("x", _p), ("y", _p), ("res", _p), ("w", _p), ("b", _p), ("w2", _p), ("b2", _p),
                 ("map", _p), ("freqs", _p), ("stats", _p), ("t", _p), ("skip_flag", _p),
                 ("out", _p), ("out_hi", _p), ("out_lo", _p), ("flag", _p),
-                ("desc", DawnKernelDesc * KERNEL_MAX_DESC)]
+                ("desc", DawnKernelDesc * KERNEL_MAX_DESC),
+                ("xs", _p), ("e", _p), ("noise", _p), ("scratch", _p), ("tab", _p), ("t_slot", _p), ("num_t", _i),
+                ("replicas", _i), ("coef", ctypes.c_float * 5), ("q", ctypes.c_float)]
 
 
 LFG_MOTION_PACK, LFG_WARP_BLEND, LFG_AFFINE_RELU, LFG_RESIDUAL_BN_RELU, LFG_RELU_AVGPOOL2, LFG_CHW_TO_HWC, LFG_HWC_TO_CHW, \

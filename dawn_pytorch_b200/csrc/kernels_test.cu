@@ -1,6 +1,6 @@
-// dawn_test_kernel (include/dawn_unet.h): one per-clip or per-step glue kernel of the UNet through the launcher unet.cu calls, on
-// caller-owned buffers, for per-kernel tests against a high-precision reference.  Every geometry is checked here, before any CUDA
-// call, so a refused case launches nothing.
+// dawn_test_kernel (include/dawn_unet.h): one per-clip or per-step glue kernel of the UNet through the launcher unet.cu calls, or
+// one sampler update through the step functions of sampler.cu, on caller-owned buffers, for per-kernel tests against a
+// high-precision reference.  Every geometry is checked here, before any CUDA call, so a refused case launches nothing.
 #include <algorithm>
 #include <string>
 #include <vector>
@@ -9,6 +9,7 @@
 #include "common.cuh"
 #include "contraction.cuh"
 #include "kernels.cuh"
+#include "sampler.cuh"
 
 namespace dawn {
 namespace {
@@ -79,6 +80,40 @@ int film(const dawn_kernel_case& c, Owned& own, cudaStream_t st) {
   return launch_film(dd, c.ndesc, max_n, c.clips, c.x, c.C, st);
 }
 
+// The cross-rank reductions of W ranks that all hold the caller's keys: every sum is W times the own value and every min the
+// own value, so one GPU runs the frame-sharded select and its result is known from the local keys alone.
+template <class T>
+__global__ void times_kernel(T* b, size_t n, T w) {
+  for (size_t i = threadIdx.x; i < n; i += blockDim.x) b[i] *= w;
+}
+int replica_sum_u32(void* ctx, unsigned int* b, size_t n, cudaStream_t st) {
+  times_kernel<<<1, 256, 0, st>>>(b, n, (unsigned int)*static_cast<const int*>(ctx));
+  DAWN_LAUNCH_OK();
+  return 0;
+}
+int replica_sum_u64(void* ctx, unsigned long long* b, size_t n, cudaStream_t st) {
+  times_kernel<<<1, 256, 0, st>>>(b, n, (unsigned long long)*static_cast<const int*>(ctx));
+  DAWN_LAUNCH_OK();
+  return 0;
+}
+int replica_min_u32(void*, unsigned int*, size_t, cudaStream_t) { return 0; }
+
+int sampler_step(const dawn_kernel_case& c, cudaStream_t st) {
+  const DdpmCoef* tab = c.kernel == DAWN_KERNEL_DDPM_STEP ? reinterpret_cast<const DdpmCoef*>(c.tab) : nullptr;
+  if (!c.xs || !c.e || !c.scratch || (tab && !c.t_slot)) return refuse("missing pointer");
+  // every digit bin and count_le of W replicas stays below 2^32 when W n does
+  if (c.n < 1 || c.replicas < 0 || (long long)c.replicas * c.n >= (1LL << 32) || (tab && c.num_t < 1)) return refuse("bad geometry");
+  int w = c.replicas;
+  const DdimReduce rep{&w, replica_sum_u32, replica_sum_u64, replica_min_u32};
+  const DdimReduce* red = w > 0 ? &rep : nullptr;
+  const int64_t n_global = c.n * (w > 0 ? w : 1);
+  const float* k = c.coef;
+  if (c.kernel == DAWN_KERNEL_DDIM_STEP)
+    return ddim_step_impl(c.xs, c.e, c.noise, c.n, n_global, k[0], k[1], k[2], k[3], k[4], c.q, c.scratch, st, red);
+  return ddpm_step_impl(c.xs, c.e, c.noise, c.n, n_global, DdpmCoef{k[0], k[1], k[2], k[3], k[4]}, tab, c.t_slot, c.num_t, c.q,
+                        c.scratch, st, red);
+}
+
 int test_kernel(const dawn_kernel_case& c, Owned& own, cudaStream_t st) {
   switch (c.kernel) {
     case DAWN_KERNEL_ROWSTATS:
@@ -144,6 +179,9 @@ int test_kernel(const dawn_kernel_case& c, Owned& own, cudaStream_t st) {
           c.nc < 0 || c.ng + c.nc < 1)
         return refuse("bad geometry");
       return launch_heads_out(c.x, c.y, c.C, c.M, c.P, c.clips, c.w, c.b, c.ng, c.w2, c.b2, c.nc, c.out, st);
+    case DAWN_KERNEL_DDIM_STEP:
+    case DAWN_KERNEL_DDPM_STEP:
+      return sampler_step(c, st);
   }
   return refuse("unknown kernel");
 }

@@ -33,13 +33,19 @@ __global__ void x0_abs_kernel(const float* __restrict__ x, const float* __restri
     keys[i] = __float_as_uint(fabsf(ddim_x0(ca, x[i], cb, update_eps(eps, eps_n, g, i))));
 }
 
-// one launch instead of a pageable-host memcpy + three memsets (keeps the step capturable in a CUDA graph)
+// clamp(x0, -s, s) / s as torch evaluates it (U:1107, 1196): a NaN x0 stays NaN, where fmaxf / fminf would return a bound,
+// and a NaN s makes the quotient NaN
+__device__ __forceinline__ float clip_x0(float x0, float s) {
+  return __fdiv_rn(isnan(x0) ? x0 : fminf(fmaxf(x0, -s), s), s);
+}
+
+// one launch instead of a pageable-host memcpy + four memsets (keeps the step capturable in a CUDA graph)
 __global__ void select_init_kernel(uint32_t* state, unsigned int* hist, unsigned long long* count_le, unsigned int* min_gt,
-                                   unsigned long long lo) {
+                                   unsigned int* any_nan, unsigned long long lo) {
   hist[threadIdx.x] = 0;
   if (threadIdx.x == 0) {
     state[0] = 0u; state[1] = 0u; state[2] = (uint32_t)(lo & 0xFFFFFFFFull); state[3] = (uint32_t)(lo >> 32);
-    *count_le = 0ull; *min_gt = 0xFFFFFFFFu;
+    *count_le = 0ull; *min_gt = 0xFFFFFFFFu; *any_nan = 0u;
   }
 }
 
@@ -75,40 +81,49 @@ __global__ void radix_pick_kernel(uint32_t* state, int shift, unsigned int* hist
   for (int i = 0; i < 256; ++i) hist[i] = 0;
 }
 
-// after the 4 digit passes state[0] is the key of order statistic `lo`.  next[0] = #keys <= it, next[1] = min key above it
+// after the 4 digit passes state[0] is the key of order statistic `lo`: count_le = #keys <= it, min_gt = min key above it,
+// any_nan != 0 when a key is NaN (a bit pattern above +inf's)
 __global__ void next_stat_kernel(const uint32_t* __restrict__ keys, long long n, const uint32_t* __restrict__ state,
-                                 unsigned long long* __restrict__ count_le, unsigned int* __restrict__ min_gt) {
+                                 unsigned long long* __restrict__ count_le, unsigned int* __restrict__ min_gt,
+                                 unsigned int* __restrict__ any_nan) {
   const uint32_t v = state[0];
   unsigned long long c = 0;
   unsigned int m = 0xFFFFFFFFu;
+  bool nan = false;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const uint32_t k = keys[i];
     if (k <= v) ++c; else m = min(m, k);
+    nan |= k > 0x7F800000u;
   }
   for (int o = 16; o > 0; o >>= 1) {
     c += __shfl_xor_sync(0xffffffffu, c, o);
     m = min(m, __shfl_xor_sync(0xffffffffu, m, o));
   }
+  nan = __any_sync(0xffffffffu, nan);
   if ((threadIdx.x & 31) == 0) {
     atomicAdd(count_le, c);
     atomicMin(min_gt, m);
+    if (nan) atomicOr(any_nan, 1u);
   }
 }
 
-// s = max(1, lerp(v[lo], v[hi], w)) exactly as torch.quantile + clamp_(min=1)  (U:1186-1193)
+// s = max(1, lerp(v[lo], v[hi], w)) exactly as torch.quantile + clamp_(min=1)  (U:1186-1193).  Both give NaN when a key is NaN
+// (torch.quantile moves every rank onto the NaN the sort put last) or when the lerp does (inf - inf), and clamp_ keeps it.
 __global__ void threshold_kernel(const uint32_t* state, const unsigned long long* count_le, const unsigned int* min_gt,
-                                 long long lo, long long hi, float w, float* s_out) {
+                                 const unsigned int* any_nan, long long lo, long long hi, float w, float* s_out) {
   const float vlo = __uint_as_float(state[0]);
   float vhi = vlo;
   if (hi > lo && *count_le < (unsigned long long)(lo + 2)) vhi = __uint_as_float(*min_gt);
   const float d = vhi - vlo;
   const float q = (w < 0.5f) ? (vlo + w * d) : (vhi - d * (1.0f - w));     // at::lerp
-  *s_out = fmaxf(q, 1.0f);
+  *s_out = (*any_nan || isnan(q)) ? __uint_as_float(0x7FC00000u) : fmaxf(q, 1.0f);
 }
 
-// img = clamp(x0, -s, s)/s * sqrt(a_next) + c * e + sigma * noise, e = update_eps;  clamp == 0: x0 is used as predicted
-// (clip_denoised=False, U:1183).  x_n != nullptr (guidance): the new x also goes to the null slot, so the next forward sees the
-// same x_t in both
+// img = clamp(x0, -s, s)/s * sqrt(a_next) + c * e + sigma * noise, e = update_eps, each product and sum rounded as the
+// reference's fp32 ops (U:1203-1205; fused multiply-adds moved about one element in four by an ulp).  noise == nullptr is the
+// last step, where the reference adds sigma * 0. (U:1201): that add turns a -0 sum into +0.  clamp == 0: x0 is used as
+// predicted (clip_denoised=False, U:1183).  x_n != nullptr (guidance): the new x also goes to the null slot, so the next
+// forward sees the same x_t in both
 __global__ void ddim_update_kernel(float* __restrict__ x, float* __restrict__ x_n, const float* __restrict__ eps,
                                    const float* __restrict__ eps_n, const float* __restrict__ scale, const float* __restrict__ noise,
                                    const float* __restrict__ s_ptr, float ca, float cb, float sqrt_an, float c, float sigma,
@@ -118,9 +133,9 @@ __global__ void ddim_update_kernel(float* __restrict__ x, float* __restrict__ x_
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const float e = update_eps(eps, eps_n, g, i);
     float x0 = ddim_x0(ca, x[i], cb, e);
-    if (clamp) x0 = fminf(fmaxf(x0, -s), s) / s;
-    float v = x0 * sqrt_an + c * e;
-    if (noise) v += sigma * noise[i];
+    if (clamp) x0 = clip_x0(x0, s);
+    float v = __fadd_rn(__fmul_rn(x0, sqrt_an), __fmul_rn(c, e));
+    v = __fadd_rn(v, __fmul_rn(sigma, noise ? noise[i] : 0.0f));
     x[i] = v;
     if (x_n) x_n[i] = v;
   }
@@ -153,7 +168,7 @@ __global__ void ddpm_update_kernel(float* __restrict__ x, const float* __restric
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const float xi = x[i];
     float x0 = __fsub_rn(__fmul_rn(k.ca, xi), __fmul_rn(k.cb, eps[i]));
-    if (clamp) x0 = __fdiv_rn(fminf(fmaxf(x0, -s), s), s);
+    if (clamp) x0 = clip_x0(x0, s);
     float v = __fadd_rn(__fmul_rn(k.c1, x0), __fmul_rn(k.c2, xi));
     if (noise) v = __fadd_rn(v, __fmul_rn(k.sigma, noise[i]));
     x[i] = v;
@@ -169,7 +184,8 @@ int update_blocks(long long n) { return (int)std::min<long long>((n + kThreads -
 
 // s = max(1, q-quantile of the n_global keys) by exact radix select, written to scratch word 263 (*s_ptr points there).
 // write_keys(keys) enqueues the kernel that fills this rank's n keys at scratch word 512 once the select state is reset.
-// scratch layout (32-bit words): [0,4) select state | [4,260) histogram | [260,262) count_le (u64) | 262 min_gt | 263 s | [512, 512+n) keys
+// scratch layout (32-bit words): [0,4) select state | [4,260) histogram | [260,262) count_le (u64) | 262 min_gt | 263 s |
+// 264 any_nan | [512, 512+n) keys
 template <class WriteKeys>
 int clip_threshold(void* scratch, long long n, int64_t n_global, float q, int blocks, cudaStream_t st, const DdimReduce* red,
                    float** s_ptr, WriteKeys write_keys) {
@@ -179,24 +195,26 @@ int clip_threshold(void* scratch, long long n, int64_t n_global, float q, int bl
   unsigned long long* count_le = (unsigned long long*)(base + 260);
   unsigned int* min_gt = base + 262;
   float* s_out = (float*)(base + 263);
+  unsigned int* any_nan = base + 264;
   uint32_t* keys = base + 512;
   // torch.quantile: ranks = q * (n - 1) evaluated in fp32 (ATen quantile_compute), lerp between floor and ceil
   const float rank_f = q * (float)(n_global - 1);
   const long long lo = (long long)floorf(rank_f), hi = (long long)ceilf(rank_f);
   const float w = rank_f - floorf(rank_f);
-  select_init_kernel<<<1, 256, 0, st>>>(state, hist, count_le, min_gt, (unsigned long long)lo);
+  select_init_kernel<<<1, 256, 0, st>>>(state, hist, count_le, min_gt, any_nan, (unsigned long long)lo);
   write_keys(keys);
   for (int shift = 24; shift >= 0; shift -= 8) {
     radix_hist_kernel<<<blocks, 256, 0, st>>>(keys, n, state, shift, hist);
     if (red) DAWN_TRY(red->sum_u32(red->ctx, hist, 256, st));
     radix_pick_kernel<<<1, 32, 0, st>>>(state, shift, hist);
   }
-  next_stat_kernel<<<blocks, kThreads, 0, st>>>(keys, n, state, count_le, min_gt);
+  next_stat_kernel<<<blocks, kThreads, 0, st>>>(keys, n, state, count_le, min_gt, any_nan);
   if (red) {
     DAWN_TRY(red->sum_u64(red->ctx, count_le, 1, st));
     DAWN_TRY(red->min_u32(red->ctx, min_gt, 1, st));
+    DAWN_TRY(red->sum_u32(red->ctx, any_nan, 1, st));
   }
-  threshold_kernel<<<1, 1, 0, st>>>(state, count_le, min_gt, lo, hi, w, s_out);
+  threshold_kernel<<<1, 1, 0, st>>>(state, count_le, min_gt, any_nan, lo, hi, w, s_out);
   *s_ptr = s_out;
   return 0;
 }

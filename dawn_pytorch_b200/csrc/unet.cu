@@ -1400,7 +1400,8 @@ int dawn_unet_shard_ipc_import(dawn_unet* h, const char* handles) {
 }
 
 // Frame-sharded handles select the clip-wide quantile (U:1186-1190) over ALL ranks' values by all-reducing the radix-select's
-// histograms (4 x 256 u32) and its two tail statistics — 6 tiny collectives per step instead of gathering x0 (4.9 MB per rank).
+// histograms (4 x 256 u32), its two tail statistics and its any-NaN flag — 7 tiny collectives per step instead of gathering x0
+// (4.9 MB per rank).
 static int red_sum_u32(void* ctx, unsigned int* b, size_t n, cudaStream_t st) {
   DAWN_NCCL_OK(g_nccl.AllReduce(b, b, n, kNcclUint32, kNcclSum, (ncclComm_t)ctx, st)); return 0;
 }

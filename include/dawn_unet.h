@@ -126,15 +126,17 @@ int64_t dawn_unet_workspace_bytes(dawn_unet* h);
 /* One DDIM update around the UNet (reference GaussianDiffusion.ddim_sample :1169-1205), in place on x (device, n floats):
  *   x0 = ca*x - cb*eps;  s = max(1, quantile_q(|x0|)) over all n values (torch.quantile semantics) if q > 0, else 1;
  *   q < 0: x0 is neither clamped nor divided (the reference's clip_denoised=False, U:1183);
- *   x = clamp(x0,-s,s)/s * sqrt_an + c*eps + sigma*noise      (noise = NULL for the last step)
+ *   x = clamp(x0,-s,s)/s * sqrt_an + c*eps + sigma*noise      (noise = NULL for the last step: sigma*0 is added, as there)
+ * every operation rounded as the reference's fp32 torch op, so the result is bit-identical to it.  As torch.quantile and clamp,
+ * s is NaN when an |x0| is NaN or the quantile's lerp is inf - inf, and a NaN x0 or s gives a NaN element.
  * scratch: device buffer of n + 512 32-bit words.  No host synchronisation. */
 int dawn_ddim_step(float* x, const float* eps, const float* noise, int64_t n, float ca, float cb, float sqrt_an, float c,
                    float sigma, float q, void* scratch, void* stream);
 
 /* The same update for the frames a handle owns.  Unsharded handle: x, eps, noise hold the B clips back to back (n = B * per-clip
  * size) and each clip is updated as dawn_ddim_step would update it alone (its own quantile).  After dawn_unet_init_shard
- * the quantile spans the whole clip (n_local * nranks values): the radix-select's four 256-bin histograms and its two tail
- * statistics are all-reduced (NCCL, on `stream`), so every rank applies the bit-identical threshold.  Every rank must call
+ * the quantile spans the whole clip (n_local * nranks values): the radix-select's four 256-bin histograms, its two tail
+ * statistics and its NaN flag are all-reduced (NCCL, on `stream`), so every rank applies the bit-identical threshold.  Every rank must call
  * it with the same coefficients; `noise` is this rank's slice of the clip's noise. */
 int dawn_unet_ddim_step(dawn_unet* h, float* x, const float* eps, const float* noise, int64_t n_local, float ca, float cb,
                         float sqrt_an, float c, float sigma, float q, void* scratch, void* stream);
@@ -307,7 +309,11 @@ enum {
   DAWN_KERNEL_MAP_REDUCE = 10,     /* out[i] = b[i % C] + sum_{s < k} x[s * n + i], i < n */
   DAWN_KERNEL_INIT_CONV_X3 = 11,   /* out[f * clips + b][p][0, C) (row stride ldo) = map[b][p] + k x k conv of x (clip b at
                                       x + b * clip_stride, (3, F, H, W)) with w [k * k * 3][C] */
-  DAWN_KERNEL_HEADS_OUT = 12       /* out[b][j][f][p] = 1x1 heads of x (j < ng: w, b) and y (j >= ng: w2, b2), C channels, P = H*W */
+  DAWN_KERNEL_HEADS_OUT = 12,      /* out[b][j][f][p] = 1x1 heads of x (j < ng: w, b) and y (j >= ng: w2, b2), C channels, P = H*W */
+  DAWN_KERNEL_DDIM_STEP = 13,      /* the DDIM update of dawn_ddim_step on xs (n values, in place) with eps e, noise (may be NULL),
+                                      coef {ca, cb, sqrt_alpha_next, c, sigma}, q and scratch (n + 512 words); see `replicas` */
+  DAWN_KERNEL_DDPM_STEP = 14       /* the ancestral update of dawn_ddpm_step, coef {ca, cb, c1, c2, sigma}; with tab (num_t rows of
+                                      those five) the coefficients are row clamp(*t_slot, 0, num_t - 1), read on the device */
 };
 #define DAWN_KERNEL_MAX_DESC 16
 typedef struct {
@@ -333,6 +339,13 @@ typedef struct {
   const float* map; const float* freqs; const double* stats; const int64_t* t; const int* skip_flag;
   float* out; void* out_hi; void* out_lo; int* flag;
   dawn_kernel_desc desc[DAWN_KERNEL_MAX_DESC];
+  /* DDIM_STEP / DDPM_STEP.  replicas W >= 1 runs the frame-sharded select as one of W ranks that each hold these n values:
+   * n_global = W n, and the cross-rank reductions are replaced by sum = W x own value, min = own value (needs W n < 2^32, the
+   * range of a histogram count).  replicas = 0: the unsharded select. */
+  float* xs; const float* e; const float* noise; void* scratch;
+  const float* tab; const int64_t* t_slot; int num_t;
+  int replicas;
+  float coef[5]; float q;
 } dawn_kernel_case;
 int dawn_test_kernel(const dawn_kernel_case* c, void* stream);
 
