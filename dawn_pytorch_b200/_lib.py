@@ -3,6 +3,8 @@ missing or fails to load, importing this module raises."""
 import ctypes
 import os
 
+import torch
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libdawn_unet.so")
 
@@ -248,3 +250,20 @@ PROF_NCAT = 20
 def check(rc, what):
     if rc != 0:
         raise DawnError(f"{what} failed (rc={rc}): {lib.dawn_last_error().decode()}")
+
+
+def stream():
+    """The current torch CUDA stream, as the library's `void* stream` argument."""
+    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+def ptr(t):
+    """Device address of tensor t; None -> NULL."""
+    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
+
+
+def put_param(set_param, handle, name, t):
+    """Hands tensor t to a handle's `*_set_param` entry under `name`, as fp32 host values in t's shape."""
+    t = t.detach().to(device="cpu", dtype=torch.float32).contiguous()
+    shape = (ctypes.c_int64 * max(t.dim(), 1))(*t.shape)
+    check(set_param(handle, name.encode(), ctypes.c_void_p(t.data_ptr()), shape, t.dim()), f"{set_param.__name__}({name})")

@@ -5,6 +5,9 @@
 #include <cstdio>
 #include <string>
 
+// unet.cu: -1 when this process already launched on another CUDA device (the library runs one GPU per process)
+extern "C" int dawn_check_single_device(void);
+
 namespace dawn {
 
 // ---------------------------------------------------------------- error plumbing (no exceptions across the C-ABI)

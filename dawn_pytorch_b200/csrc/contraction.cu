@@ -1,6 +1,7 @@
 // Host side of every contraction (contraction.cuh), and dawn_test_contraction (include/dawn_unet.h), which runs one
 // contraction through the same weight upload and path launcher as the networks.
 #include <algorithm>
+#include <cmath>
 #include <cstring>
 
 #include "common.cuh"
@@ -117,6 +118,50 @@ void fold_ca_q(const float* const to_q[3], const float* const gain[3], int ci, s
   }
 }
 
+int bn_affine(const HostParams& raw, const std::string& prefix, int c, std::vector<double>& s, std::vector<double>& t) {
+  const HostParam *g, *b, *rm, *rv;
+  DAWN_TRY(raw.need(prefix + ".weight", {c}, &g));
+  DAWN_TRY(raw.need(prefix + ".bias", {c}, &b));
+  DAWN_TRY(raw.need(prefix + ".running_mean", {c}, &rm));
+  DAWN_TRY(raw.need(prefix + ".running_var", {c}, &rv));
+  s.resize(c); t.resize(c);
+  for (int i = 0; i < c; ++i) {
+    s[i] = (double)g->data[i] / std::sqrt((double)rv->data[i] + 1e-5);
+    t[i] = (double)b->data[i] - (double)rm->data[i] * s[i];
+  }
+  return 0;
+}
+
+void pack_conv_taps(const float* w, int co, int ci, int taps, int ci_pad, int ldb, int n0, const double* scale, std::vector<float>& m) {
+  for (int n = 0; n < co; ++n) {
+    const double sn = scale ? scale[n] : 1.0;            // (float)((double)w * 1.0) == w: no scale is an exact copy
+    for (int c = 0; c < ci; ++c)
+      for (int tp = 0; tp < taps; ++tp)
+        m[((size_t)tp * ci_pad + c) * ldb + n0 + n] = (float)((double)w[((size_t)n * ci + c) * taps + tp] * sn);
+  }
+}
+
+int pack_lfg_conv(const HostParams& raw, std::vector<void*>& owner, const std::vector<std::pair<std::string, int>>& convs,
+                  const std::string& bn_after, int ci, int k, int ci_pad, PackedWeight* out) {
+  int N = 0;
+  for (auto& c : convs) N += c.second;
+  const int ldb = round_up(N, 64), K = k * k * ci_pad;
+  std::vector<float> m((size_t)K * ldb, 0.f), bias(N);
+  int n0 = 0;
+  for (auto& cv : convs) {
+    const int co = cv.second;
+    const HostParam *w, *b;
+    DAWN_TRY(raw.need(cv.first + ".weight", {co, ci, k, k}, &w));
+    DAWN_TRY(raw.need(cv.first + ".bias", {co}, &b));
+    std::vector<double> s(co, 1.0), t(co, 0.0);
+    if (!bn_after.empty()) DAWN_TRY(bn_affine(raw, bn_after, co, s, t));
+    for (int n = 0; n < co; ++n) bias[n0 + n] = (float)((double)b->data[n] * s[n] + t[n]);
+    pack_conv_taps(w->data.data(), co, ci, k * k, ci_pad, ldb, n0, s.data(), m);
+    n0 += co;
+  }
+  return upload_weight(owner, m, K, N, ldb, bias, out);
+}
+
 // ------------------------------------------------------------------------------------------ GemmParams
 void base_params(GemmParams& p, const float* A, int lda, int Cin, int frames, int H, int W) {
   memset(&p, 0, sizeof(p));
@@ -213,6 +258,29 @@ int pack_up(std::vector<void*>& owner, int ci, int co, const int (&off)[2][2], c
     DAWN_TRY(upload_weight(owner, m, 9 * ci, N4, N4, b4, &u->all));
   }
   return 0;
+}
+
+int pack_up_nearest(std::vector<void*>& owner, const float* w, int ci, int co, const double* scale, const std::vector<float>& bias,
+                    UpConv* u) {
+  return pack_up(owner, ci, co, kUpOff, bias, [&](int py, int px, int ty, int tx, int c, int n) {
+    double acc = 0.0;
+    for (int ky = 0; ky < 3; ++ky)
+      for (int kx = 0; kx < 3; ++kx)
+        if (up_in_set(py, ty, ky) && up_in_set(px, tx, kx)) acc += (double)w[(((size_t)n * ci + c) * 3 + ky) * 3 + kx];
+    return (float)(scale ? acc * scale[n] : acc);
+  }, u);
+}
+
+int pack_lfg_up(const HostParams& raw, std::vector<void*>& owner, const std::string& name, int co, int ci, UpConv* u) {
+  // on the low-resolution grid each output-parity class is a 2x2 conv: 2.25x fewer MACs, and the upsampled tensor never exists
+  const HostParam *w, *b;
+  DAWN_TRY(raw.need(name + ".conv.weight", {co, ci, 3, 3}, &w));
+  DAWN_TRY(raw.need(name + ".conv.bias", {co}, &b));
+  std::vector<double> s, t;
+  DAWN_TRY(bn_affine(raw, name + ".norm", co, s, t));
+  std::vector<float> bias(co);
+  for (int n = 0; n < co; ++n) bias[n] = (float)((double)b->data[n] * s[n] + t[n]);
+  return pack_up_nearest(owner, w->data.data(), ci, co, s.data(), bias, u);
 }
 
 int run_up(const GemmParams& in, const UpConv& u, float* out, int ldo, const std::function<int(const GemmParams&)>& run, int border) {

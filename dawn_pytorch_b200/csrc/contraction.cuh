@@ -1,11 +1,13 @@
-// Host side of every contraction of the UNet and the LFG decoder (contraction.cu): the host-parameter store and device
-// allocations, packed weight matrices with their wgmma images, GemmParams builders, the choice among the kernel paths
-// (DAWN_PATH_* in include/dawn_unet.h) and their launch, and the 2x upsampling conv.
+// Host side of every contraction of the UNet and the LFG networks (contraction.cu): the host-parameter store and device
+// allocations, packed weight matrices with their wgmma images, the linear, BatchNorm and conv weight folds, GemmParams builders,
+// the choice among the kernel paths (DAWN_PATH_* in include/dawn_unet.h) and their launch, and the 2x upsampling conv with the
+// nearest-upsample fold.
 #pragma once
 #include <cstdint>
 #include <functional>
 #include <string>
 #include <unordered_map>
+#include <utility>
 #include <vector>
 
 #include "../../include/dawn_unet.h"
@@ -50,6 +52,16 @@ std::vector<float> row_sums(const std::vector<float>& w, int N, int K);
 // the three cross-attentions' to_q [64][ci] with their LayerNorm_img gains folded, as one k-major [ci][192] matrix and its wsum
 void fold_ca_q(const float* const to_q[3], const float* const gain[3], int ci, std::vector<float>& wq, std::vector<float>& wsum);
 
+// eval-mode BatchNorm `prefix` (weight, bias, running_mean, running_var; c channels) as y = x s + t with eps 1e-5, in fp64
+// (LFG sync_batchnorm/batchnorm.py:50-53: F.batch_norm with the running statistics)
+int bn_affine(const HostParams& raw, const std::string& prefix, int c, std::vector<double>& s, std::vector<double>& t);
+// conv weight w (co, ci, taps) -> m[(tap ci_pad + c) ldb + n0 + n] = w[n][c][tap] * scale[n], rounded once (scale null: a copy)
+void pack_conv_taps(const float* w, int co, int ci, int taps, int ci_pad, int ldb, int n0, const double* scale, std::vector<float>& m);
+// The LFG networks' Conv2d weights (co_j, ci, k, k) and biases of `convs` (state_dict prefix, co_j), side by side in the output
+// columns, with the BatchNorm `bn_after` (none when empty) folded in: W' = W s, b' = b s + t.  Input channels ci..ci_pad stay zero.
+int pack_lfg_conv(const HostParams& raw, std::vector<void*>& owner, const std::vector<std::pair<std::string, int>>& convs,
+                  const std::string& bn_after, int ci, int k, int ci_pad, PackedWeight* out);
+
 // ---------------------------------------------------------------- GemmParams
 // 1x1 contraction of (frames, H, W, Cin) rows of stride lda onto the same grid
 void base_params(GemmParams& p, const float* A, int lda, int Cin, int frames, int H, int W);
@@ -80,6 +92,12 @@ constexpr int kUpOff[2][2] = {{-1, 0}, {0, 1}};
 inline bool up_in_set(int parity, int tap, int k) { return parity == 0 ? (tap == 0 ? k == 0 : k >= 1) : (tap == 0 ? k <= 1 : k == 2); }
 int pack_up(std::vector<void*>& owner, int ci, int co, const int (&off)[2][2], const std::vector<float>& bias, const UpWeight& weight,
             UpConv* u);
+// nearest x2 -> 3x3 conv with weight w (co, ci, 3, 3) [times scale[n]] as the parity classes above: each class tap is the sum of
+// the 3x3 taps it covers, summed in fp64 and rounded once (scale null: no scale)
+int pack_up_nearest(std::vector<void*>& owner, const float* w, int ci, int co, const double* scale, const std::vector<float>& bias,
+                    UpConv* u);
+// the LFG networks' UpBlock2d `name` (util.py:106-111): nearest x2 -> conv3x3 (name.conv) -> BatchNorm (name.norm) folded
+int pack_lfg_up(const HostParams& raw, std::vector<void*>& owner, const std::string& name, int co, int ci, UpConv* u);
 // in: base_params of the low-resolution input; out: (frames, 2H, 2W) rows of stride ldo.  run launches one contraction: once with
 // the up2 halo conv when that path takes it, otherwise once per parity class.  border = 1: `in` reads a grid that carries a
 // one-pixel border (IH = OHs + 2, IW = OWs + 2); the classes then run as valid 2x2 convs over it, so no tap leaves the grid.

@@ -5,7 +5,6 @@
 // UNet (tc_conv3.cu / tc_gemm.cu, FP16x3 split precision, fp32 accumulation); eval-mode BatchNorms are folded into the conv
 // that precedes them (conv -> BN) or applied as a per-channel affine in the elementwise pass (BN -> ReLU -> conv).
 #include <algorithm>
-#include <cmath>
 #include <string>
 #include <vector>
 
@@ -50,58 +49,6 @@ struct dawn_lfg {
 };
 
 namespace {
-
-// eval-mode BatchNorm as y = x * s + t   (LFG/sync_batchnorm/batchnorm.py:50-53: F.batch_norm with running statistics, eps 1e-5)
-int bn_affine(dawn_lfg* h, const std::string& p, int c, std::vector<double>& s, std::vector<double>& t) {
-  const HostParam *g, *b, *rm, *rv;
-  DAWN_TRY(h->raw.need(p + ".weight", {c}, &g));
-  DAWN_TRY(h->raw.need(p + ".bias", {c}, &b));
-  DAWN_TRY(h->raw.need(p + ".running_mean", {c}, &rm));
-  DAWN_TRY(h->raw.need(p + ".running_var", {c}, &rv));
-  s.resize(c); t.resize(c);
-  for (int i = 0; i < c; ++i) {
-    s[i] = (double)g->data[i] / std::sqrt((double)rv->data[i] + 1e-5);
-    t[i] = (double)b->data[i] - (double)rm->data[i] * s[i];
-  }
-  return 0;
-}
-// Conv2d weight (co, ci, k, k) [+ a following BatchNorm folded: W' = W * s[co], b' = b * s + t] -> [(ky*k + kx)*ci_pad + c][ldb]
-int pack_conv(dawn_lfg* h, const std::string& conv, const std::string& bn_after, int co, int ci, int k, int ci_pad, PackedWeight* out) {
-  const HostParam *w, *b;
-  DAWN_TRY(h->raw.need(conv + ".weight", {co, ci, k, k}, &w));
-  DAWN_TRY(h->raw.need(conv + ".bias", {co}, &b));
-  std::vector<double> s(co, 1.0), t(co, 0.0);
-  if (!bn_after.empty()) DAWN_TRY(bn_affine(h, bn_after, co, s, t));
-  const int ldb = round_up(co, 64), K = k * k * ci_pad;
-  std::vector<float> m((size_t)K * ldb, 0.f), bias(co);
-  for (int n = 0; n < co; ++n) {
-    bias[n] = (float)((double)b->data[n] * s[n] + t[n]);
-    for (int c = 0; c < ci; ++c)
-      for (int tp = 0; tp < k * k; ++tp)
-        m[((size_t)tp * ci_pad + c) * ldb + n] = (float)((double)w->data[((size_t)n * ci + c) * k * k + tp] * s[n]);
-  }
-  return upload_weight(h->owned, m, K, co, ldb, bias, out);
-}
-// UpBlock2d (util.py:106-111): F.interpolate(scale_factor=2) [nearest] -> conv3x3 -> BN -> ReLU.  On the LOW-resolution grid the
-// output pixel (2y+py, 2x+px) sees rows {y-1 (ky=0), y (ky=1,2)} for py=0 and {y (ky=0,1), y+1 (ky=2)} for py=1 (same for columns):
-// each output-parity class is a 2x2 conv whose taps are sums of the 3x3 kernel's taps (kUpOff, up_in_set: contraction.cuh) — 2.25x
-// fewer MACs and the upsampled tensor never exists.
-int pack_up(dawn_lfg* h, const std::string& name, int co, int ci, UpConv* u) {
-  const HostParam *w, *b;
-  DAWN_TRY(h->raw.need(name + ".conv.weight", {co, ci, 3, 3}, &w));
-  DAWN_TRY(h->raw.need(name + ".conv.bias", {co}, &b));
-  std::vector<double> s, t;
-  DAWN_TRY(bn_affine(h, name + ".norm", co, s, t));
-  std::vector<float> bias(co);
-  for (int n = 0; n < co; ++n) bias[n] = (float)((double)b->data[n] * s[n] + t[n]);
-  return dawn::pack_up(h->owned, ci, co, kUpOff, bias, [&](int py, int px, int ty, int tx, int c, int n) {
-    double acc = 0.0;
-    for (int ky = 0; ky < 3; ++ky)
-      for (int kx = 0; kx < 3; ++kx)
-        if (up_in_set(py, ty, ky) && up_in_set(px, tx, kx)) acc += (double)w->data[(((size_t)n * ci + c) * 3 + ky) * 3 + kx];
-    return (float)(acc * s[n]);
-  }, u);
-}
 
 // ------------------------------------------------------------------------------------------ contraction dispatch
 int run_conv(dawn_lfg* h, const GemmParams& p, cudaStream_t st) {
@@ -185,8 +132,6 @@ int decode_core(dawn_lfg* h, float* prediction, float* deformed, cudaStream_t st
 
 extern "C" {
 
-int dawn_check_single_device(void);          // unet.cu: one GPU per process
-
 int dawn_lfg_create(const dawn_lfg_cfg* cfg, dawn_lfg** out) {
   DAWN_CHECK(cfg && out, "null argument");
   DAWN_TRY(dawn_check_single_device());
@@ -233,29 +178,31 @@ int dawn_lfg_commit_params(dawn_lfg* h) {
   free_all(h->owned);
   h->down.clear(); h->res.clear(); h->up.clear();
   const int n = h->n;
-  DAWN_TRY(pack_conv(h, "first.conv", "first.norm", h->C[0], h->cfg.num_channels, 7, 32, &h->first));           // generator.py:36
+  const HostParams& raw = h->raw;
+  auto& own = h->owned;
+  DAWN_TRY(pack_lfg_conv(raw, own, {{"first.conv", h->C[0]}}, "first.norm", h->cfg.num_channels, 7, 32, &h->first));    // generator.py:36
   for (int i = 0; i < n; ++i) {
     PackedWeight d;
     const std::string p = "down_blocks." + std::to_string(i);
-    DAWN_TRY(pack_conv(h, p + ".conv", p + ".norm", h->C[i + 1], h->C[i], 3, h->C[i], &d));                       // generator.py:38-44
+    DAWN_TRY(pack_lfg_conv(raw, own, {{p + ".conv", h->C[i + 1]}}, p + ".norm", h->C[i], 3, h->C[i], &d));                 // :38-44
     h->down.push_back(d);
   }
   const int Cb = h->C[n];
   for (int r = 0; r < h->cfg.num_bottleneck_blocks; ++r) {
     ResPack rp;
     const std::string p = "bottleneck.r" + std::to_string(r);
-    DAWN_TRY(pack_conv(h, p + ".conv1", p + ".norm2", Cb, Cb, 3, Cb, &rp.c1));      // util.py:88-89: conv1 -> norm2 folded
-    DAWN_TRY(pack_conv(h, p + ".conv2", "", Cb, Cb, 3, Cb, &rp.c2));
+    DAWN_TRY(pack_lfg_conv(raw, own, {{p + ".conv1", Cb}}, p + ".norm2", Cb, 3, Cb, &rp.c1));   // util.py:88-89: conv1 -> norm2 folded
+    DAWN_TRY(pack_lfg_conv(raw, own, {{p + ".conv2", Cb}}, "", Cb, 3, Cb, &rp.c2));
     std::vector<double> s, t;
-    DAWN_TRY(bn_affine(h, p + ".norm1", Cb, s, t));
+    DAWN_TRY(bn_affine(raw, p + ".norm1", Cb, s, t));
     std::vector<float> sf(s.begin(), s.end()), tf(t.begin(), t.end());
-    DAWN_TRY(dev_upload(h->owned, sf, &rp.s1));
-    DAWN_TRY(dev_upload(h->owned, tf, &rp.t1));
+    DAWN_TRY(dev_upload(own, sf, &rp.s1));
+    DAWN_TRY(dev_upload(own, tf, &rp.t1));
     h->res.push_back(rp);
   }
   for (int i = 0; i < n; ++i) {
     UpConv u;
-    DAWN_TRY(pack_up(h, "up_blocks." + std::to_string(i), h->C[n - i - 1], h->C[n - i], &u));                     // generator.py:46-52
+    DAWN_TRY(pack_lfg_up(raw, own, "up_blocks." + std::to_string(i), h->C[n - i - 1], h->C[n - i], &u));            // generator.py:46-52
     h->up.push_back(u);
   }
   {
@@ -325,7 +272,7 @@ int dawn_lfg_set_source(dawn_lfg* h, const float* source, void* stream) {
   for (int i = 0; i < n; ++i) {
     DAWN_TRY(conv_same(h, h->down[i], 3, h->SKIP[i], h->C[i], 1, h->lH[i], h->lW[i], h->TMP, st));
     h->launches++;
-    DAWN_TRY(launch_lfg_relu_avgpool2(h->TMP, h->lH[i], h->lW[i], h->C[i + 1], h->SKIP[i + 1], st));
+    DAWN_TRY(launch_lfg_relu_avgpool2(h->TMP, h->lH[i], h->lW[i], h->C[i + 1], h->SKIP[i + 1], h->C[i + 1], st));
   }
   h->have_source = true;
   return 0;

@@ -118,11 +118,11 @@ __global__ void __launch_bounds__(256) residual_bn_relu_kernel(const float* __re
   }
 }
 
-__global__ void relu_avgpool2_kernel(const float* __restrict__ x, int H, int W, int C, float* __restrict__ out) {
-  const int cg = C >> 2, Ho = H >> 1, Wo = W >> 1;
-  const long long total = (long long)Ho * Wo * cg;
+// one thread = one output pixel x 4 channels; rows = frames * H with H even, so a 2x2 window never spans two frames
+__global__ void relu_avgpool2_kernel(const float* __restrict__ x, int rows, int W, int C, float* __restrict__ out, int ldo) {
+  const int cg = C >> 2, Ho = rows >> 1, Wo = W >> 1;
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= total) return;
+  if (idx >= (long long)Ho * Wo * cg) return;
   const int c4 = (int)(idx % cg) * 4;
   const long long pix = idx / cg;
   const int xo = (int)(pix % Wo), yo = (int)(pix / Wo);
@@ -134,7 +134,7 @@ __global__ void relu_avgpool2_kernel(const float* __restrict__ x, int H, int W, 
       const float4 v = *reinterpret_cast<const float4*>(x + ((size_t)(2 * yo + dy) * W + 2 * xo + dx) * C + c4);
       acc.x += fmaxf(v.x, 0.f); acc.y += fmaxf(v.y, 0.f); acc.z += fmaxf(v.z, 0.f); acc.w += fmaxf(v.w, 0.f);
     }
-  *reinterpret_cast<float4*>(out + (size_t)pix * C + c4) = make_float4(acc.x * 0.25f, acc.y * 0.25f, acc.z * 0.25f, acc.w * 0.25f);
+  *reinterpret_cast<float4*>(out + (size_t)pix * ldo + c4) = make_float4(acc.x * 0.25f, acc.y * 0.25f, acc.z * 0.25f, acc.w * 0.25f);
 }
 
 __global__ void chw_to_hwc_kernel(const float* __restrict__ x, int C, int HW, int Cpad, float* __restrict__ out) {
@@ -280,9 +280,9 @@ int launch_lfg_residual_bn_relu(const float* y, const float* x, int C, long long
   DAWN_LAUNCH_OK();
   return 0;
 }
-int launch_lfg_relu_avgpool2(const float* x, int H, int W, int C, float* out, cudaStream_t st) {
-  const long long n = (long long)(H >> 1) * (W >> 1) * (C >> 2);
-  relu_avgpool2_kernel<<<(int)((n + 255) / 256), 256, 0, st>>>(x, H, W, C, out);
+int launch_lfg_relu_avgpool2(const float* x, int rows, int W, int C, float* out, int ldo, cudaStream_t st) {
+  const long long n = (long long)(rows >> 1) * (W >> 1) * (C >> 2);
+  relu_avgpool2_kernel<<<(int)((n + 255) / 256), 256, 0, st>>>(x, rows, W, C, out, ldo);
   DAWN_LAUNCH_OK();
   return 0;
 }

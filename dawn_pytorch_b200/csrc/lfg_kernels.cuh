@@ -43,8 +43,9 @@ int launch_lfg_affine_relu(const float* x, int ldx, const float* scale, const fl
 // xnew = y + x (ResBlock2d's `out += x`, util.py:92) and, when z != null, z = relu(xnew * scale + shift) for the next block
 int launch_lfg_residual_bn_relu(const float* y, const float* x, int C, long long M, float* xnew, const float* scale,
                                 const float* shift, float* z, cudaStream_t st);
-// 2x2 average pooling (util.py:124, 131) with ReLU applied to the inputs first: out = avgpool(relu(x)); one frame
-int launch_lfg_relu_avgpool2(const float* x, int H, int W, int C, float* out, cudaStream_t st);
+// DownBlock2d's ReLU + 2x2 average pooling (util.py:124, 129-131): out = avgpool(relu(x)) over `rows` = frames * H rows (H even)
+// of x (rows, W, C), into rows of stride ldo (e.g. the skip half of an Hourglass concatenation)
+int launch_lfg_relu_avgpool2(const float* x, int rows, int W, int C, float* out, int ldo, cudaStream_t st);
 // (C, H, W) -> (H, W, Cpad) channels-last, zero padded; and back: (M, C) rows -> (C, M)
 int launch_lfg_chw_to_hwc(const float* x, int C, int HW, int Cpad, float* out, cudaStream_t st);
 int launch_lfg_hwc_to_chw(const float* x, int ld, int C, long long M, float* out, cudaStream_t st);

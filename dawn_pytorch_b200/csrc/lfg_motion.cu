@@ -5,7 +5,6 @@
 // [up-block output | encoder skip] with the concatenation formed through the row stride; level 0 holds [up | input | zeros]
 // so that the input conv and the 7x7 output conv both read 32- / 64-channel aligned rows.
 #include <algorithm>
-#include <cmath>
 #include <string>
 #include <vector>
 
@@ -60,65 +59,6 @@ namespace {
 
 constexpr int kLdLogits = 16;
 
-int bn_affine(dawn_lfg_motion* h, const std::string& p, int c, std::vector<double>& s, std::vector<double>& t) {
-  const HostParam *g, *b, *rm, *rv;
-  DAWN_TRY(h->raw.need(p + ".weight", {c}, &g));
-  DAWN_TRY(h->raw.need(p + ".bias", {c}, &b));
-  DAWN_TRY(h->raw.need(p + ".running_mean", {c}, &rm));
-  DAWN_TRY(h->raw.need(p + ".running_var", {c}, &rv));
-  s.resize(c); t.resize(c);
-  for (int i = 0; i < c; ++i) {                   // LFG/sync_batchnorm/batchnorm.py:50-53 in eval mode, eps 1e-5
-    s[i] = (double)g->data[i] / std::sqrt((double)rv->data[i] + 1e-5);
-    t[i] = (double)b->data[i] - (double)rm->data[i] * s[i];
-  }
-  return 0;
-}
-
-// Conv2d weights (co_j, ci, k, k) of one or more convs side by side in the output columns, [+ BatchNorm folded]
-// -> [(ky k + kx) ci_pad + c][ldb]; input channels ci..ci_pad stay zero
-int pack_convs(dawn_lfg_motion* h, const std::vector<std::pair<std::string, int>>& convs, const std::string& bn_after, int ci, int k,
-               int ci_pad, PackedWeight* out) {
-  int N = 0;
-  for (auto& c : convs) N += c.second;
-  const int ldb = round_up(N, 64), K = k * k * ci_pad;
-  std::vector<float> m((size_t)K * ldb, 0.f), bias(N);
-  int n0 = 0;
-  for (auto& cv : convs) {
-    const int co = cv.second;
-    const HostParam *w, *b;
-    DAWN_TRY(h->raw.need(cv.first + ".weight", {co, ci, k, k}, &w));
-    DAWN_TRY(h->raw.need(cv.first + ".bias", {co}, &b));
-    std::vector<double> s(co, 1.0), t(co, 0.0);
-    if (!bn_after.empty()) DAWN_TRY(bn_affine(h, bn_after, co, s, t));
-    for (int n = 0; n < co; ++n) {
-      bias[n0 + n] = (float)((double)b->data[n] * s[n] + t[n]);
-      for (int c = 0; c < ci; ++c)
-        for (int tp = 0; tp < k * k; ++tp)
-          m[((size_t)tp * ci_pad + c) * ldb + n0 + n] = (float)((double)w->data[((size_t)n * ci + c) * k * k + tp] * s[n]);
-    }
-    n0 += co;
-  }
-  return upload_weight(h->owned, m, K, N, ldb, bias, out);
-}
-
-// UpBlock2d (util.py:106-111): nearest x2 -> conv3x3 -> BN as four parity-class 2x2 convs on the low-resolution grid (lfg.cu)
-int pack_up(dawn_lfg_motion* h, const std::string& name, int co, int ci, UpConv* u) {
-  const HostParam *w, *b;
-  DAWN_TRY(h->raw.need(name + ".conv.weight", {co, ci, 3, 3}, &w));
-  DAWN_TRY(h->raw.need(name + ".conv.bias", {co}, &b));
-  std::vector<double> s, t;
-  DAWN_TRY(bn_affine(h, name + ".norm", co, s, t));
-  std::vector<float> bias(co);
-  for (int n = 0; n < co; ++n) bias[n] = (float)((double)b->data[n] * s[n] + t[n]);
-  return dawn::pack_up(h->owned, ci, co, kUpOff, bias, [&](int py, int px, int ty, int tx, int c, int n) {
-    double acc = 0.0;
-    for (int ky = 0; ky < 3; ++ky)
-      for (int kx = 0; kx < 3; ++kx)
-        if (up_in_set(py, ty, ky) && up_in_set(px, tx, kx)) acc += (double)w->data[(((size_t)n * ci + c) * 3 + ky) * 3 + kx];
-    return (float)(acc * s[n]);
-  }, u);
-}
-
 void init_net(Net& net, const std::string& prefix, bool decoder, int nb, int be, int mx, int cin, int cpad) {
   net = Net();
   net.prefix = prefix; net.decoder = decoder; net.nb = nb; net.be = be; net.mx = mx; net.cin = cin; net.cpad = cpad;
@@ -131,7 +71,8 @@ int pack_net(dawn_lfg_motion* h, Net& net) {
   for (int i = 0; i < net.nb; ++i) {
     const std::string p = net.prefix + ".encoder.down_blocks." + std::to_string(i);
     PackedWeight d;
-    DAWN_TRY(pack_convs(h, {{p + ".conv", net.Ce[i + 1]}}, p + ".norm", net.Ce[i], 3, i == 0 ? net.cpad : net.Ce[i], &d));
+    DAWN_TRY(pack_lfg_conv(h->raw, h->owned, {{p + ".conv", net.Ce[i + 1]}}, p + ".norm", net.Ce[i], 3, i == 0 ? net.cpad : net.Ce[i],
+                           &d));
     net.down.push_back(d);
   }
   if (!net.decoder) return 0;
@@ -139,7 +80,7 @@ int pack_net(dawn_lfg_motion* h, Net& net) {
     const int i = net.nb - 1 - j;
     const int ci = (i == net.nb - 1 ? 1 : 2) * net.width(i + 1), co = net.width(i);
     UpConv u;
-    DAWN_TRY(pack_up(h, net.prefix + ".decoder.up_blocks." + std::to_string(j), co, ci, &u));
+    DAWN_TRY(pack_lfg_up(h->raw, h->owned, net.prefix + ".decoder.up_blocks." + std::to_string(j), co, ci, &u));
     net.up.push_back(u);
     net.upco.push_back(co);
   }
@@ -190,7 +131,7 @@ int run_net(dawn_lfg_motion* h, Net& net, int n, cudaStream_t st) {
     const float* in = (i == 0) ? (net.decoder ? net.L[0] + net.width(0) : net.L[0]) : net.enc_ptr(i);
     DAWN_TRY(conv_same(h, net.down[i], 3, in, net.ld[i], i == 0 ? net.cpad : net.Ce[i], n, Hi, Wi, h->TMP, co, st));
     h->launches++;
-    DAWN_TRY(launch_lfgm_relu_avgpool2(h->TMP, n * Hi, Wi, co, net.enc_ptr(i + 1), net.ld[i + 1], st));
+    DAWN_TRY(launch_lfg_relu_avgpool2(h->TMP, n * Hi, Wi, co, net.enc_ptr(i + 1), net.ld[i + 1], st));
   }
   if (net.decoder) {
     for (int j = 0; j < net.nb; ++j) {                                              // UpBlock2d, then cat([out, skip]) in place
@@ -218,8 +159,6 @@ int check_n(dawn_lfg_motion* h, int n, bool part, const char* what) {
 }  // namespace
 
 extern "C" {
-
-int dawn_check_single_device(void);          // unet.cu: one GPU per process
 
 int dawn_lfg_motion_create(const dawn_lfg_motion_cfg* cfg, dawn_lfg_motion** out) {
   DAWN_CHECK(cfg && out, "null argument");
@@ -284,16 +223,16 @@ int dawn_lfg_motion_commit_params(dawn_lfg_motion* h) {
   const int R = h->cfg.num_regions;
   if (h->have_rp) {
     DAWN_TRY(pack_net(h, h->rp));
-    DAWN_TRY(pack_convs(h, {{"region_predictor.regions", R}}, "", h->rp.be + h->rp.cin, 7, round_up(h->rp.be + h->rp.cpad, 64),
-                        &h->regions));                                                       // region_predictor.py:39-40
+    DAWN_TRY(pack_lfg_conv(h->raw, h->owned, {{"region_predictor.regions", R}}, "", h->rp.be + h->rp.cin, 7,
+                           round_up(h->rp.be + h->rp.cpad, 64), &h->regions));                 // region_predictor.py:39-40
     const HostParam* g;
     DAWN_TRY(h->raw.need("region_predictor.down.weight", {3, 1, kAAK, kAAK}, &g));
     DAWN_TRY(dev_upload(h->owned, g->data, &h->rp_aa));
   }
   if (h->have_pw) {
     DAWN_TRY(pack_net(h, h->pw));
-    DAWN_TRY(pack_convs(h, {{"pixelwise_flow_predictor.mask", R + 1}, {"pixelwise_flow_predictor.occlusion", 1}}, "",
-                        h->pw.be + h->pw.cin, 7, round_up(h->pw.be + h->pw.cpad, 64), &h->mask_occ));   // pixelwise_flow_predictor.py:32-37
+    DAWN_TRY(pack_lfg_conv(h->raw, h->owned, {{"pixelwise_flow_predictor.mask", R + 1}, {"pixelwise_flow_predictor.occlusion", 1}}, "",
+                           h->pw.be + h->pw.cin, 7, round_up(h->pw.be + h->pw.cpad, 64), &h->mask_occ));   // pixelwise_flow_predictor.py:32-37
     const HostParam* g;
     DAWN_TRY(h->raw.need("pixelwise_flow_predictor.down.weight", {3, 1, kAAK, kAAK}, &g));
     DAWN_TRY(dev_upload(h->owned, g->data, &h->pw_aa));
@@ -405,51 +344,5 @@ int dawn_lfg_motion_read_tap(dawn_lfg_motion* h, const char* name, float* dst, i
 
 int64_t dawn_lfg_motion_last_launch_count(dawn_lfg_motion* h) { return h ? h->launches : 0; }
 int64_t dawn_lfg_motion_workspace_bytes(dawn_lfg_motion* h) { return h ? h->ws_bytes : 0; }
-
-// ------------------------------------------------------------------------------------------ per-kernel tests
-int dawn_lfg_motion_test_kernel(const dawn_lfg_motion_kernel_case* c, void* stream) {
-  DAWN_CHECK(c, "dawn_lfg_motion_test_kernel: null case");
-  const cudaStream_t st = (cudaStream_t)stream;
-  const bool geo = c->N >= 1 && c->N <= 65535;
-  int rc = -1;
-  switch (c->kernel) {
-    case DAWN_LFG_MOTION_AA_DOWN:
-      DAWN_CHECK(c->x && c->weight && c->out, "dawn_lfg_motion_test_kernel: missing pointer");
-      DAWN_CHECK(geo && c->H >= 4 && c->W >= 4 && c->H % 4 == 0 && c->W % 4 == 0 && c->cw >= 3 && c->off >= 0 && c->off + c->cw <= c->ld,
-                 "dawn_lfg_motion_test_kernel: bad geometry");
-      rc = launch_lfgm_aa_down(c->x, c->N, c->H, c->W, c->weight, c->out, c->ld, c->off, c->cw, st);
-      break;
-    case DAWN_LFG_MOTION_REGION_MOMENTS:
-      DAWN_CHECK(c->logits && c->out && c->out2, "dawn_lfg_motion_test_kernel: missing pointer");
-      DAWN_CHECK(geo && c->h >= 2 && c->w >= 2 && c->R >= 1 && c->ldl >= c->R && c->temperature > 0.f, "dawn_lfg_motion_test_kernel: bad geometry");
-      rc = launch_lfgm_region_moments(c->logits, c->ldl, c->N, c->h, c->w, c->R, c->temperature, c->out, c->out2, c->out3, st);
-      break;
-    case DAWN_LFG_MOTION_FLOW_INPUT:
-      DAWN_CHECK(c->source && c->src_shift && c->src_covar && c->src_affine && c->drv_shift && c->drv_covar && c->drv_affine && c->out &&
-                 c->out2, "dawn_lfg_motion_test_kernel: missing pointer");
-      DAWN_CHECK(geo && c->h >= 2 && c->w >= 2 && c->R >= 1 && c->R <= kMotionMaxRegions && c->off >= 0 && c->cw >= 4 * (c->R + 1) &&
-                 c->off + c->cw <= c->ld, "dawn_lfg_motion_test_kernel: bad geometry");
-      rc = launch_lfgm_flow_input(c->source, c->N, c->h, c->w, c->R, c->src_shift, c->src_covar, c->src_affine, c->drv_shift, c->drv_covar,
-                                  c->drv_affine, c->bg, c->revert, c->out, c->ld, c->off, c->cw, c->out2, st);
-      break;
-    case DAWN_LFG_MOTION_FLOW_COMBINE:
-      DAWN_CHECK(c->logits && c->motion && c->out && c->out2, "dawn_lfg_motion_test_kernel: missing pointer");
-      DAWN_CHECK(geo && c->h >= 1 && c->w >= 1 && c->R >= 1 && c->R <= kMotionMaxRegions && c->ldl >= c->R + 2,
-                 "dawn_lfg_motion_test_kernel: bad geometry");
-      rc = launch_lfgm_flow_combine(c->logits, c->ldl, c->motion, c->N, c->h, c->w, c->R, c->out, c->out2, st);
-      break;
-    case DAWN_LFG_MOTION_BG_HEAD:
-      DAWN_CHECK(c->out && (c->fc_w == nullptr) == (c->fc_b == nullptr) && (c->x || !c->fc_w), "dawn_lfg_motion_test_kernel: missing pointer");
-      DAWN_CHECK(geo && (!c->fc_w || (c->cw >= 1 && c->cw <= 8192 && c->ld >= c->cw && c->h * c->w >= 1)),
-                 "dawn_lfg_motion_test_kernel: bad geometry");
-      rc = launch_lfgm_bg_head(c->x, c->ld, c->cw, c->N, c->h * c->w, c->fc_w, c->fc_b, c->out, st);
-      break;
-    default:
-      DAWN_CHECK(false, "dawn_lfg_motion_test_kernel: unknown kernel");
-  }
-  if (rc != 0) return rc;
-  DAWN_CUDA_OK(cudaStreamSynchronize(st));
-  return 0;
-}
 
 }  // extern "C"

@@ -1,6 +1,6 @@
 // Non-GEMM kernels of the LFG motion estimator: the anti-aliased 1/4 downsample, the region softmax and moments, the flow
-// predictor's input assembly and output combine, the background head, and two layout passes.  The convolutions run on the shared
-// contraction kernels (lfg_motion.cu).  Reference: LFG/modules/region_predictor.py, bg_motion_predictor.py,
+// predictor's input assembly and output combine, the background head and its input packing.  The convolutions run on the shared
+// contraction kernels and the pooling on the decoder's (lfg_motion.cu).  Reference: LFG/modules/region_predictor.py, bg_motion_predictor.py,
 // pixelwise_flow_predictor.py, util.py:22-67 (region2gaussian, make_coordinate_grid), :217-275 (AntiAliasInterpolation2d).
 #include <algorithm>
 #include <cmath>
@@ -238,7 +238,7 @@ __global__ void __launch_bounds__(256) bg_head_kernel(const float* __restrict__ 
   if (threadIdx.x < 3) o[6 + threadIdx.x] = (float)(threadIdx.x == 2);
 }
 
-// --------------------------------------------------------------------------------------------- layout passes
+// --------------------------------------------------------------------------------------------- layout pass
 __global__ void pack_pair_kernel(const float* __restrict__ source, int n_source, const float* __restrict__ driving, int HW, long long total,
                                  float* __restrict__ out) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -250,24 +250,6 @@ __global__ void pack_pair_kernel(const float* __restrict__ source, int n_source,
   if (c < 3) v = source[((size_t)(n_source == 1 ? 0 : n) * 3 + c) * HW + p];
   else if (c < 6) v = driving[((size_t)n * 3 + c - 3) * HW + p];
   out[idx] = v;
-}
-
-__global__ void relu_avgpool2_kernel(const float* __restrict__ x, int rows, int W, int C, float* __restrict__ out, int ldo) {
-  const int cg = C >> 2, Ho = rows >> 1, Wo = W >> 1;
-  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= (long long)Ho * Wo * cg) return;
-  const int c4 = (int)(idx % cg) * 4;
-  const long long pix = idx / cg;
-  const int xo = (int)(pix % Wo), yo = (int)(pix / Wo);
-  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-  for (int dy = 0; dy < 2; ++dy)
-#pragma unroll
-    for (int dx = 0; dx < 2; ++dx) {
-      const float4 v = *reinterpret_cast<const float4*>(x + ((size_t)(2 * yo + dy) * W + 2 * xo + dx) * C + c4);
-      acc.x += fmaxf(v.x, 0.f); acc.y += fmaxf(v.y, 0.f); acc.z += fmaxf(v.z, 0.f); acc.w += fmaxf(v.w, 0.f);
-    }
-  *reinterpret_cast<float4*>(out + (size_t)pix * ldo + c4) = make_float4(acc.x * 0.25f, acc.y * 0.25f, acc.z * 0.25f, acc.w * 0.25f);
 }
 
 }  // namespace
@@ -309,12 +291,6 @@ int launch_lfgm_bg_head(const float* x, int ld, int C, int N, int P, const float
 int launch_lfgm_pack_pair(const float* source, int n_source, const float* driving, int N, int HW, float* out, cudaStream_t st) {
   const long long total = (long long)N * HW * 32;
   pack_pair_kernel<<<(int)((total + 255) / 256), 256, 0, st>>>(source, n_source, driving, HW, total, out);
-  DAWN_LAUNCH_OK();
-  return 0;
-}
-int launch_lfgm_relu_avgpool2(const float* x, int rows, int W, int C, float* out, int ldo, cudaStream_t st) {
-  const long long n = (long long)(rows >> 1) * (W >> 1) * (C >> 2);
-  relu_avgpool2_kernel<<<(int)((n + 255) / 256), 256, 0, st>>>(x, rows, W, C, out, ldo);
   DAWN_LAUNCH_OK();
   return 0;
 }

@@ -33,8 +33,5 @@ int launch_lfgm_bg_head(const float* x, int ld, int C, int N, int P, const float
 
 // BGMotionPredictor's input cat([source, driving]) (N, 6, H, W) as (N, H, W, 32) zero padded; n_source 1 shares one source
 int launch_lfgm_pack_pair(const float* source, int n_source, const float* driving, int N, int HW, float* out, cudaStream_t st);
-// DownBlock2d's ReLU + 2x2 average pooling (util.py:129-131) over `rows` = frames * H rows of x (rows, W, C) into a row stride
-// ldo (the skip half of an Hourglass concatenation)
-int launch_lfgm_relu_avgpool2(const float* x, int rows, int W, int C, float* out, int ldo, cudaStream_t st);
 
 }  // namespace dawn

@@ -248,10 +248,7 @@ int pack_conv(dawn_unet* h, const std::string& prefix, int co, int ci, int kh, i
   const int ldb = round_up(co, 64);
   const int K = kh * kw * ci_pad;
   std::vector<float> m((size_t)K * ldb, 0.f);
-  for (int n = 0; n < co; ++n)
-    for (int c = 0; c < ci; ++c)
-      for (int t = 0; t < kh * kw; ++t)
-        m[((size_t)t * ci_pad + c) * ldb + n] = w->data[((size_t)n * ci + c) * kh * kw + t];
+  pack_conv_taps(w->data.data(), co, ci, kh * kw, ci_pad, ldb, 0, nullptr, m);
   return upload_weight(h->owned, m, K, co, ldb, b ? b->data : std::vector<float>{}, out);
 }
 
@@ -387,18 +384,12 @@ int pack_up(dawn_unet* h, const std::string& name, int C, UpConv* u) {
 }
 
 // Upsample(use_deconv=False) (U:168-172): nearest x2, then Conv3d (1,3,3) weight (co=C, ci=C, 1, 3, 3) at "<name>.1": the same
-// four parity classes, each tap the sum of the 3x3 taps it covers (kUpOff, up_in_set), summed in fp64 and rounded once
+// four parity classes (pack_up_nearest)
 int pack_upconv(dawn_unet* h, const std::string& name, int C, UpConv* u) {
   const HostParam *w, *b;
   DAWN_TRY(h->raw.need(name + ".1.weight", {C, C, 1, 3, 3}, &w));
   DAWN_TRY(h->raw.need(name + ".1.bias", {C}, &b));
-  return dawn::pack_up(h->owned, C, C, kUpOff, b->data, [&](int py, int px, int ty, int tx, int c, int n) {
-    double acc = 0.0;
-    for (int ky = 0; ky < 3; ++ky)
-      for (int kx = 0; kx < 3; ++kx)
-        if (up_in_set(py, ty, ky) && up_in_set(px, tx, kx)) acc += (double)w->data[(((size_t)n * C + c) * 3 + ky) * 3 + kx];
-    return (float)acc;
-  }, u);
+  return pack_up_nearest(h->owned, w->data.data(), C, C, nullptr, b->data, u);
 }
 
 // ------------------------------------------------------------------------------------------ GEMM wrappers

@@ -17,11 +17,7 @@ import torch
 import torch.nn.functional as F
 from torch import nn
 
-from ._lib import check, lib
-
-
-def _ptr(t):
-    return ctypes.c_void_p(t.data_ptr())
+from ._lib import check, lib, ptr, stream
 
 
 def _update_scratch(n, device):
@@ -148,7 +144,7 @@ class GaussianDiffusion(nn.Module):
         img = draw(-1, shape).to(device).contiguous()
         q = self._clip_q(clip_denoised)
         self._check_sample_shape("ddim_sample", fea, shape, cond)
-        st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+        st = stream()
         guided = cond_scale != 1 and getattr(unet, "has_cond", True)
         if use_graph:
             if guided:
@@ -170,7 +166,7 @@ class GaussianDiffusion(nn.Module):
         eps = torch.empty(one, device=img.device)
         eps_null = torch.empty_like(eps) if guided else None
         scratch = _update_scratch(ch * Fr * h * w, img.device)
-        st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+        st = stream()
         for i in range(1 if batched else b):
             sel = slice(None) if batched else i
             x = img[sel]
@@ -191,8 +187,7 @@ class GaussianDiffusion(nn.Module):
                 else:
                     unet.forward_x3(x, t_dev, eps)
                 z = noise(k, sel, one)
-                check(getattr(lib, entry)(unet._handle, _ptr(x), _ptr(eps), _ptr(z) if z is not None else None, x.numel(), *coef, q,
-                                          _ptr(scratch), st), entry)
+                check(getattr(lib, entry)(unet._handle, ptr(x), ptr(eps), ptr(z), x.numel(), *coef, q, ptr(scratch), st), entry)
         return img
 
     @staticmethod
@@ -234,8 +229,8 @@ class GaussianDiffusion(nn.Module):
                  scratch=_update_scratch(math.prod(x_shape[-4:]), device), **extra)
         invariants()
         torch.cuda.synchronize(device)
-        ins = [_ptr(g[k]) for k in ("x", "eps", "noise", "t")] + [_ptr(v) if torch.is_tensor(v) else v for v in extra.values()]
-        check(getattr(lib, entry)(unet._handle, *ins, count, q, _ptr(g["scratch"])), entry)
+        ins = [ptr(g[k]) for k in ("x", "eps", "noise", "t")] + [ptr(v) if torch.is_tensor(v) else v for v in extra.values()]
+        check(getattr(lib, entry)(unet._handle, *ins, count, q, ptr(g["scratch"])), entry)
         g["gen"] = unet.graph_generation()
         setattr(self, attr, g)
         return g, True
@@ -382,7 +377,7 @@ class GaussianDiffusion(nn.Module):
         draw = noise_fn if noise_fn is not None else self._default_noise(unet, device, seed)
         img = draw(-1, shape).to(device).contiguous()
         q = self._clip_q(clip_denoised)
-        st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+        st = stream()
         if use_graph:
             if cond_scale != 1 and getattr(unet, "has_cond", True):
                 raise NotImplementedError("use_graph captures the cond_scale = 1 step (DAWN's shipped setting); "

@@ -15,7 +15,7 @@ import torch
 from torch import nn
 
 from . import _lib
-from ._lib import DawnLfgCfg, check, lib
+from ._lib import DawnLfgCfg, check, lib, ptr, stream
 
 
 class _Holder(nn.Module):
@@ -39,8 +39,96 @@ def _res_block(c):                                          # ResBlock2d (util.p
     return m
 
 
-class Generator(nn.Module):
+class _Handle:
+    """One native handle of include/dawn_lfg.h (entry points `<api>_*`, api "dawn_lfg" or "dawn_lfg_motion") that holds a
+    module's parameters.  It is created on the device of the module's inputs and created again after a device change, and the
+    module's state_dict is uploaded and committed whenever `dirty`.  param_name(key) is the library's name of a state_dict
+    entry, or None for an entry the handle does not take.  `geom` is the geometry its user set last; create and commit void it."""
+
+    def __init__(self, api, cfg, what, param_name=lambda key: key):
+        self.api, self.cfg, self.what, self.param_name = api, cfg, what, param_name
+        self.handle, self.device_index, self.dirty, self.geom = None, None, True, None
+
+    def _entry(self, name):
+        return getattr(lib, f"{self.api}_{name}")
+
+    def _create(self):
+        hd = ctypes.c_void_p()
+        check(self._entry("create")(ctypes.byref(self.cfg), ctypes.byref(hd)), f"{self.api}_create")
+        return hd
+
+    def validate(self):
+        """Create refuses what the library cannot run; it needs no GPU."""
+        self._entry("destroy")(self._create())
+
+    def destroy(self):
+        if self.handle is not None:
+            self._entry("destroy")(self.handle)
+        self.handle, self.geom = None, None
+
+    def ensure(self, module, device):
+        """Readies the handle for a call on `device` with the parameters of `module`; returns the device index."""
+        if device.type != "cuda":
+            raise _lib.DawnError(f"{self.what} runs on CUDA (sm_90a) only; there is no CPU path")
+        idx = device.index if device.index is not None else torch.cuda.current_device()
+        if self.handle is not None and self.device_index != idx:
+            self.destroy()
+            self.dirty = True
+        with torch.cuda.device(idx):
+            if self.handle is None:
+                self.handle, self.device_index = self._create(), idx
+            if self.dirty:
+                for key, t in module.state_dict().items():
+                    name = None if key.endswith("num_batches_tracked") else self.param_name(key)
+                    if name is not None:
+                        _lib.put_param(self._entry("set_param"), self.handle, name, t)
+                check(self._entry("commit_params")(self.handle), f"{self.api}_commit_params")
+                self.dirty, self.geom = False, None
+        return idx
+
+    def last_launch_count(self):
+        return int(self._entry("last_launch_count")(self.handle)) if self.handle is not None else 0
+
+
+class _LfgModule(nn.Module):
+    """Base of the LFG modules, whose parameters feed the native handles in `_handles`: load_state_dict and .to() / .cuda()
+    mark every handle dirty, and the handles die with the module.  Inference only: train(True) raises `TRAIN_REFUSAL`."""
+    TRAIN_REFUSAL = ""
+
+    def _hold(self, *handles):
+        self._handles = list(handles)
+        self.register_load_state_dict_post_hook(lambda module, incompatible: module.mark_dirty())
+        self.eval()
+
+    def mark_dirty(self):
+        for h in self._handles:
+            h.dirty = True
+
+    def _apply(self, fn, *a, **k):
+        for h in self.__dict__.get("_handles", ()):
+            h.dirty = True
+        return super()._apply(fn, *a, **k)
+
+    def train(self, mode=True):
+        if mode:
+            raise NotImplementedError(self.TRAIN_REFUSAL)
+        return super().train(False)
+
+    def __del__(self):
+        for h in self.__dict__.get("_handles", ()):
+            try:
+                h.destroy()
+            except Exception:
+                pass
+
+    def last_launch_count(self):
+        """Kernels the last call of the module's first handle enqueued."""
+        return self._handles[0].last_launch_count()
+
+
+class Generator(_LfgModule):
     IGNORED_PREFIX = "pixelwise_flow_predictor."
+    TRAIN_REFUSAL = "this LFG decoder is inference-only (eval-mode BatchNorm, FD:121)"
 
     def __init__(self, num_channels, num_regions, block_expansion, max_features, num_down_blocks, num_bottleneck_blocks,
                  pixelwise_flow_predictor_params=None, skips=False, revert_axis_swap=True):
@@ -63,11 +151,14 @@ class Generator(nn.Module):
         cfg = DawnLfgCfg()
         cfg.num_channels, cfg.block_expansion, cfg.max_features = num_channels, block_expansion, max_features
         cfg.num_down_blocks, cfg.num_bottleneck_blocks, cfg.skips = num_down_blocks, num_bottleneck_blocks, int(bool(skips))
-        self._cfg = cfg
-        self._handle, self._dirty, self._geom, self._device_index, self._src_key = None, True, None, None, None
+        self._lfg = _Handle("dawn_lfg", cfg, "the LFG decoder")
         self._register_load_state_dict_pre_hook(self._drop_training_only_keys)
-        self.register_load_state_dict_post_hook(lambda module, incompatible: module.mark_dirty())
-        self.eval()
+        self._hold(self._lfg)
+
+    @property
+    def _cfg(self):
+        """the dawn_lfg_cfg the decoder's handle is created with"""
+        return self._lfg.cfg
 
     # the reference checkpoint's `generator` entry also holds the training-time flow predictor (generator.py:29-34)
     @classmethod
@@ -75,56 +166,12 @@ class Generator(nn.Module):
         for k in [k for k in state_dict if k.startswith(prefix + cls.IGNORED_PREFIX)]:
             del state_dict[k]
 
-    def mark_dirty(self):
-        self._dirty = True
-
-    def _apply(self, fn, *a, **k):
-        self._dirty = True
-        return super()._apply(fn, *a, **k)
-
-    def train(self, mode=True):
-        if mode:
-            raise NotImplementedError("this LFG decoder is inference-only (eval-mode BatchNorm, FD:121)")
-        return super().train(False)
-
-    def __del__(self):
-        h = self.__dict__.get("_handle")
-        self.__dict__["_handle"] = None
-        if h is not None:
-            try:
-                lib.dawn_lfg_destroy(h)
-            except Exception:
-                pass
-
-    @staticmethod
-    def _stream():
-        return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-
     def _ensure(self, device, frames, H, W, fh, fw):
-        if device.type != "cuda":
-            raise _lib.DawnError("the LFG decoder runs on CUDA (sm_90a) only; there is no CPU path")
-        idx = device.index if device.index is not None else torch.cuda.current_device()
-        if self._handle is not None and self._device_index != idx:
-            lib.dawn_lfg_destroy(self._handle)
-            self._handle, self._dirty, self._geom = None, True, None
-        with torch.cuda.device(idx):
-            if self._handle is None:
-                hd = ctypes.c_void_p()
-                check(lib.dawn_lfg_create(ctypes.byref(self._cfg), ctypes.byref(hd)), "dawn_lfg_create")
-                self._handle, self._device_index = hd, idx
-            if self._dirty:
-                for name, t in self.state_dict().items():
-                    if name.endswith("num_batches_tracked"):
-                        continue
-                    t = t.detach().to(device="cpu", dtype=torch.float32).contiguous()
-                    shape = (ctypes.c_int64 * max(t.dim(), 1))(*t.shape)
-                    check(lib.dawn_lfg_set_param(self._handle, name.encode(), ctypes.c_void_p(t.data_ptr()), shape, t.dim()),
-                          f"dawn_lfg_set_param({name})")
-                check(lib.dawn_lfg_commit_params(self._handle), "dawn_lfg_commit_params")
-                self._dirty, self._geom, self._src_key = False, None, None
-            if self._geom != (frames, H, W, fh, fw):
-                check(lib.dawn_lfg_set_geometry(self._handle, frames, H, W, fh, fw), "dawn_lfg_set_geometry")
-                self._geom, self._src_key = (frames, H, W, fh, fw), None
+        idx = self._lfg.ensure(self, device)
+        if self._lfg.geom != (frames, H, W, fh, fw):
+            with torch.cuda.device(idx):
+                check(lib.dawn_lfg_set_geometry(self._lfg.handle, frames, H, W, fh, fw), "dawn_lfg_set_geometry")
+            self._lfg.geom = (frames, H, W, fh, fw)
 
     def _set_source(self, source_image):
         src = source_image.reshape(-1, *source_image.shape[-3:])
@@ -132,7 +179,7 @@ class Generator(nn.Module):
             raise ValueError("one source image per call (the reference decodes with batch 1, FD:375-383)")
         src = src[0].contiguous().float()
         with torch.cuda.device(src.device):
-            check(lib.dawn_lfg_set_source(self._handle, ctypes.c_void_p(src.data_ptr()), self._stream()), "dawn_lfg_set_source")
+            check(lib.dawn_lfg_set_source(self._lfg.handle, ptr(src), stream()), "dawn_lfg_set_source")
         return src
 
     # ------------------------------------------------------------------ reference API
@@ -142,13 +189,13 @@ class Generator(nn.Module):
         b, _, H, W = source_image.shape
         d = 2 ** self.num_down_blocks
         out = torch.empty((b, self.bottleneck_channels, H // d, W // d), device=source_image.device, dtype=torch.float32)
-        g = self._geom
+        g = self._lfg.geom
         fh, fw, frames = (g[3], g[4], g[0]) if g is not None and g[1:3] == (H, W) else (H // d, W // d, 1)
         self._ensure(source_image.device, frames, H, W, fh, fw)
         for i in range(b):
             self._set_source(source_image[i:i + 1])
             with torch.cuda.device(source_image.device):
-                check(lib.dawn_lfg_get_fea(self._handle, ctypes.c_void_p(out[i].data_ptr()), self._stream()), "dawn_lfg_get_fea")
+                check(lib.dawn_lfg_get_fea(self._lfg.handle, ptr(out[i]), stream()), "dawn_lfg_get_fea")
         return out
 
     @torch.no_grad()
@@ -166,10 +213,7 @@ class Generator(nn.Module):
         pred = torch.empty((F_, 3, H, W), device=dev, dtype=torch.float32)
         deformed = torch.empty_like(pred) if need_deformed else None
         with torch.cuda.device(dev):
-            check(lib.dawn_lfg_decode(self._handle, ctypes.c_void_p(flow.data_ptr()), ctypes.c_void_p(occ.data_ptr()),
-                                      ctypes.c_void_p(pred.data_ptr()),
-                                      ctypes.c_void_p(deformed.data_ptr()) if deformed is not None else None, self._stream()),
-                  "dawn_lfg_decode")
+            check(lib.dawn_lfg_decode(self._lfg.handle, ptr(flow), ptr(occ), ptr(pred), ptr(deformed), stream()), "dawn_lfg_decode")
         return {"prediction": pred, "deformed": deformed}
 
     @torch.no_grad()
@@ -185,9 +229,7 @@ class Generator(nn.Module):
         pred = torch.empty((F_, 3, H, W), device=dev, dtype=torch.float32)
         deformed = torch.empty_like(pred) if need_deformed else None
         with torch.cuda.device(dev):
-            check(lib.dawn_lfg_decode_sample(self._handle, ctypes.c_void_p(s.data_ptr()), ctypes.c_void_p(pred.data_ptr()),
-                                             ctypes.c_void_p(deformed.data_ptr()) if deformed is not None else None, self._stream()),
-                  "dawn_lfg_decode_sample")
+            check(lib.dawn_lfg_decode_sample(self._lfg.handle, ptr(s), ptr(pred), ptr(deformed), stream()), "dawn_lfg_decode_sample")
         return (pred, deformed) if need_deformed else pred
 
     def forward(self, *a, **k):
@@ -198,20 +240,17 @@ class Generator(nn.Module):
     def read_tap(self, name):
         """(frames, C, Hl, Wl) copy of an internal activation of the last decode: 'bottleneck', 'up0', 'up1'."""
         C, Hl, Wl = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
-        check(lib.dawn_lfg_read_tap(self._handle, name.encode(), None, ctypes.byref(C), ctypes.byref(Hl), ctypes.byref(Wl), None),
+        h = self._lfg
+        check(lib.dawn_lfg_read_tap(h.handle, name.encode(), None, ctypes.byref(C), ctypes.byref(Hl), ctypes.byref(Wl), None),
               "dawn_lfg_read_tap")
-        frames = self._geom[0]
-        t = torch.empty((C.value, frames, Hl.value, Wl.value), device=torch.device("cuda", self._device_index))
-        with torch.cuda.device(self._device_index):
-            check(lib.dawn_lfg_read_tap(self._handle, name.encode(), ctypes.c_void_p(t.data_ptr()), ctypes.byref(C), ctypes.byref(Hl),
-                                        ctypes.byref(Wl), self._stream()), "dawn_lfg_read_tap")
+        t = torch.empty((C.value, h.geom[0], Hl.value, Wl.value), device=torch.device("cuda", h.device_index))
+        with torch.cuda.device(h.device_index):
+            check(lib.dawn_lfg_read_tap(h.handle, name.encode(), ptr(t), ctypes.byref(C), ctypes.byref(Hl), ctypes.byref(Wl), stream()),
+                  "dawn_lfg_read_tap")
         return t.permute(1, 0, 2, 3).contiguous()
 
-    def last_launch_count(self):
-        return int(lib.dawn_lfg_last_launch_count(self._handle)) if self._handle is not None else 0
-
     def workspace_bytes(self):
-        return int(lib.dawn_lfg_workspace_bytes(self._handle)) if self._handle is not None else 0
+        return int(lib.dawn_lfg_workspace_bytes(self._lfg.handle)) if self._lfg.handle is not None else 0
 
 
 # ====================================================================================================================================
@@ -263,107 +302,41 @@ def _motion_cfg(**kw):
     return c
 
 
-class _MotionHandle:
-    """One dawn_lfg_motion handle holding one module's part of the motion estimator (its parameters under `prefix`)."""
+def _motion_handle(cfg, param_name):
+    h = _Handle("dawn_lfg_motion", cfg, "the LFG motion estimator", param_name)
+    h.validate()
+    return h
 
-    def __init__(self, cfg, prefix):
-        self.cfg, self.prefix = cfg, prefix
-        self.handle, self.device_index, self.dirty, self.geom = None, None, True, None
 
-    def validate(self):
-        """dawn_lfg_motion_create refuses what the library cannot run; it needs no GPU."""
-        hd = ctypes.c_void_p()
-        check(lib.dawn_lfg_motion_create(ctypes.byref(self.cfg), ctypes.byref(hd)), "dawn_lfg_motion_create")
-        lib.dawn_lfg_motion_destroy(hd)
-
-    def destroy(self):
-        if self.handle is not None:
-            lib.dawn_lfg_motion_destroy(self.handle)
-        self.handle, self.geom = None, None
-
-    def ensure(self, module, device, n, H, W):
-        if device.type != "cuda":
-            raise _lib.DawnError("the LFG motion estimator runs on CUDA (sm_90a) only; there is no CPU path")
-        idx = device.index if device.index is not None else torch.cuda.current_device()
-        if self.handle is not None and self.device_index != idx:
-            self.destroy()
-            self.dirty = True
+def _motion_geometry(h, module, device, n, H, W):
+    """Readies the motion handle h of `module` for n frames of (H, W) images; returns the frames per stage call.  The
+    workspace only grows: fewer frames of the same size reuse it."""
+    idx = h.ensure(module, device)
+    frames = min(n, MOTION_CHUNK)
+    if h.geom is None or h.geom[1:] != (H, W) or h.geom[0] < frames:
         with torch.cuda.device(idx):
-            if self.handle is None:
-                hd = ctypes.c_void_p()
-                check(lib.dawn_lfg_motion_create(ctypes.byref(self.cfg), ctypes.byref(hd)), "dawn_lfg_motion_create")
-                self.handle, self.device_index = hd, idx
-            if self.dirty:
-                for name, t in module.state_dict().items():
-                    # a MotionGenerator's state_dict also holds the decoder, which its Generator handle uploads
-                    if name.endswith("num_batches_tracked") or (self.prefix == Generator.IGNORED_PREFIX and not name.startswith(self.prefix)):
-                        continue
-                    full = name if name.startswith(self.prefix) else self.prefix + name
-                    t = t.detach().to(device="cpu", dtype=torch.float32).contiguous()
-                    shape = (ctypes.c_int64 * max(t.dim(), 1))(*t.shape)
-                    check(lib.dawn_lfg_motion_set_param(self.handle, full.encode(), ctypes.c_void_p(t.data_ptr()), shape, t.dim()),
-                          f"dawn_lfg_motion_set_param({full})")
-                check(lib.dawn_lfg_motion_commit_params(self.handle), "dawn_lfg_motion_commit_params")
-                self.dirty, self.geom = False, None
-            frames = min(n, MOTION_CHUNK)
-            if self.geom is None or self.geom[1:] != (H, W) or self.geom[0] < frames:
-                check(lib.dawn_lfg_motion_set_geometry(self.handle, frames, H, W), "dawn_lfg_motion_set_geometry")
-                self.geom = (frames, H, W)
-        return self.geom[0]
-
-    def read_tap(self, name):
-        C, n, Hl, Wl = ctypes.c_int(), ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
-        args = (ctypes.byref(C), ctypes.byref(n), ctypes.byref(Hl), ctypes.byref(Wl))
-        check(lib.dawn_lfg_motion_read_tap(self.handle, name.encode(), None, *args, None), "dawn_lfg_motion_read_tap")
-        t = torch.empty((C.value, n.value, Hl.value, Wl.value), device=torch.device("cuda", self.device_index))
-        with torch.cuda.device(self.device_index):
-            check(lib.dawn_lfg_motion_read_tap(self.handle, name.encode(), ctypes.c_void_p(t.data_ptr()), *args,
-                                               ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)), "dawn_lfg_motion_read_tap")
-        return t.permute(1, 0, 2, 3).contiguous()
+            check(lib.dawn_lfg_motion_set_geometry(h.handle, frames, H, W), "dawn_lfg_motion_set_geometry")
+        h.geom = (frames, H, W)
+    return h.geom[0]
 
 
-class _MotionModule(nn.Module):
-    def _init_handle(self, cfg, prefix):
-        self._motion = _MotionHandle(cfg, prefix)
-        self._motion.validate()
-        self.register_load_state_dict_post_hook(lambda module, incompatible: module.mark_dirty())
-        self.eval()
-
-    def mark_dirty(self):
-        self._motion.dirty = True
-
-    def _apply(self, fn, *a, **k):
-        if "_motion" in self.__dict__:
-            self._motion.dirty = True
-        return super()._apply(fn, *a, **k)
-
-    def train(self, mode=True):
-        if mode:
-            raise NotImplementedError("the LFG motion estimator is inference-only (eval-mode BatchNorm)")
-        return super().train(False)
-
-    def __del__(self):
-        m = self.__dict__.get("_motion")
-        if m is not None:
-            try:
-                m.destroy()
-            except Exception:
-                pass
-
-    def read_tap(self, name):
-        """(n, C, Hl, Wl) copy of the last call's 'region_predictor' / 'bg_encoder' / 'flow_hourglass' output (last chunk)."""
-        return self._motion.read_tap(name)
-
-    def last_launch_count(self):
-        return int(lib.dawn_lfg_motion_last_launch_count(self._motion.handle)) if self._motion.handle is not None else 0
+def _motion_read_tap(h, name):
+    """(n, C, Hl, Wl) copy of the last call's 'region_predictor' / 'bg_encoder' / 'flow_hourglass' output (last chunk)."""
+    C, n, Hl, Wl = ctypes.c_int(), ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
+    args = (ctypes.byref(C), ctypes.byref(n), ctypes.byref(Hl), ctypes.byref(Wl))
+    check(lib.dawn_lfg_motion_read_tap(h.handle, name.encode(), None, *args, None), "dawn_lfg_motion_read_tap")
+    t = torch.empty((C.value, n.value, Hl.value, Wl.value), device=torch.device("cuda", h.device_index))
+    with torch.cuda.device(h.device_index):
+        check(lib.dawn_lfg_motion_read_tap(h.handle, name.encode(), ptr(t), *args, stream()), "dawn_lfg_motion_read_tap")
+    return t.permute(1, 0, 2, 3).contiguous()
 
 
-def _ptr(t):
-    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
+_MOTION_TRAIN_REFUSAL = "the LFG motion estimator is inference-only (eval-mode BatchNorm)"
 
 
-class RegionPredictor(_MotionModule):
+class RegionPredictor(_LfgModule):
     """region_predictor.py:28-117 with DAWN's region_predictor_params (pca_based, host SVD)."""
+    TRAIN_REFUSAL = _MOTION_TRAIN_REFUSAL
 
     def __init__(self, block_expansion, num_regions, num_channels, max_features, num_blocks, temperature, estimate_affine=False,
                  scale_factor=1, pca_based=False, fast_svd=False, pad=3):
@@ -376,36 +349,42 @@ class RegionPredictor(_MotionModule):
             self.down = _anti_alias(num_channels, scale_factor)
         if pad != 3:
             raise _lib.DawnError("RegionPredictor: only pad 3 (the 7x7 regions conv's same padding) is supported")
-        self._init_handle(_motion_cfg(num_regions=num_regions, num_channels=num_channels, estimate_affine=int(bool(estimate_affine)),
-                                      pca_based=int(bool(pca_based)), fast_svd=int(bool(fast_svd)), rp_block_expansion=block_expansion,
-                                      rp_max_features=max_features, rp_num_blocks=num_blocks, rp_temperature=temperature,
-                                      rp_scale_factor=scale_factor), "region_predictor.")
+        self._motion = _motion_handle(_motion_cfg(num_regions=num_regions, num_channels=num_channels,
+                                                  estimate_affine=int(bool(estimate_affine)), pca_based=int(bool(pca_based)),
+                                                  fast_svd=int(bool(fast_svd)), rp_block_expansion=block_expansion,
+                                                  rp_max_features=max_features, rp_num_blocks=num_blocks, rp_temperature=temperature,
+                                                  rp_scale_factor=scale_factor), lambda key: "region_predictor." + key)
+        self._hold(self._motion)
 
     @torch.no_grad()
     def forward(self, x):
         n, _, H, W = x.shape
         dev = x.device
-        chunk = self._motion.ensure(self, dev, n, H, W)
+        chunk = _motion_geometry(self._motion, self, dev, n, H, W)
         R = self.regions.out_channels
         x = x.contiguous().float()
         shift = torch.empty((n, R, 2), device=dev)
         covar = torch.empty((n, R, 2, 2), device=dev)
         heat = torch.empty((n, R, H // 4, W // 4), device=dev)
         with torch.cuda.device(dev):
-            st = Generator._stream()
+            st = stream()
             for a in range(0, n, chunk):
                 b = min(n, a + chunk)
-                check(lib.dawn_lfg_motion_regions(self._motion.handle, _ptr(x[a:b]), b - a, _ptr(shift[a:b]), _ptr(covar[a:b]),
-                                                  _ptr(heat[a:b]), st), "dawn_lfg_motion_regions")
+                check(lib.dawn_lfg_motion_regions(self._motion.handle, ptr(x[a:b]), b - a, ptr(shift[a:b]), ptr(covar[a:b]),
+                                                  ptr(heat[a:b]), st), "dawn_lfg_motion_regions")
         u, s, _ = torch.svd(covar.view(-1, 2, 2).cpu())                   # region_predictor.py:16-25, as the reference does
         u, s = u.to(dev), s.to(dev)
         d = torch.diag_embed(s ** 0.5)
         affine = torch.matmul(u, d).view(n, R, 2, 2)
         return {"shift": shift, "covar": covar, "heatmap": heat, "affine": affine, "u": u, "d": d}
 
+    def read_tap(self, name):
+        return _motion_read_tap(self._motion, name)
 
-class BGMotionPredictor(_MotionModule):
+
+class BGMotionPredictor(_LfgModule):
     """bg_motion_predictor.py:15-57 with bg_type 'affine' (DAWN's) or 'zero'."""
+    TRAIN_REFUSAL = _MOTION_TRAIN_REFUSAL
 
     def __init__(self, block_expansion, num_channels, max_features, num_blocks, bg_type='zero'):
         super().__init__()
@@ -415,9 +394,11 @@ class BGMotionPredictor(_MotionModule):
         if bg_type != 'zero':
             self.encoder = _encoder(block_expansion, num_channels * 2, max_features, num_blocks)
             self.fc = nn.Linear(min(max_features, block_expansion * 2 ** num_blocks), 6)
-        self._init_handle(_motion_cfg(num_channels=num_channels, bg_block_expansion=block_expansion, bg_max_features=max_features,
-                                      bg_num_blocks=num_blocks,
-                                      bg_type=_lib.LFG_BG_AFFINE if bg_type == 'affine' else _lib.LFG_BG_ZERO), "bg_predictor.")
+        self._motion = _motion_handle(_motion_cfg(num_channels=num_channels, bg_block_expansion=block_expansion,
+                                                  bg_max_features=max_features, bg_num_blocks=num_blocks,
+                                                  bg_type=_lib.LFG_BG_AFFINE if bg_type == 'affine' else _lib.LFG_BG_ZERO),
+                                      lambda key: "bg_predictor." + key)
+        self._hold(self._motion)
 
     @torch.no_grad()
     def forward(self, source_image, driving_image):
@@ -425,19 +406,22 @@ class BGMotionPredictor(_MotionModule):
         dev = driving_image.device
         if source_image.device != dev:
             raise _lib.DawnError("source and driving images must be on the same device")
-        chunk = self._motion.ensure(self, dev, n, H, W)
+        chunk = _motion_geometry(self._motion, self, dev, n, H, W)
         src = source_image.contiguous().float()
         drv = driving_image.contiguous().float()
         shared = src.shape[0] == 1 and n > 1
         out = torch.empty((n, 3, 3), device=dev)
         with torch.cuda.device(dev):
-            st = Generator._stream()
+            st = stream()
             for a in range(0, n, chunk):
                 b = min(n, a + chunk)
                 s = src if shared else src[a:b]
-                check(lib.dawn_lfg_motion_bg(self._motion.handle, _ptr(s), s.shape[0], _ptr(drv[a:b]), b - a, _ptr(out[a:b]), st),
+                check(lib.dawn_lfg_motion_bg(self._motion.handle, ptr(s), s.shape[0], ptr(drv[a:b]), b - a, ptr(out[a:b]), st),
                       "dawn_lfg_motion_bg")
         return out
+
+    def read_tap(self, name):
+        return _motion_read_tap(self._motion, name)
 
 
 class _FlowPredictor(_Holder):
@@ -473,32 +457,13 @@ class MotionGenerator(Generator):
                            None, skips, revert_axis_swap)
         self._modules = {"pixelwise_flow_predictor": pw, **self._modules}    # registered first, as generator.py:29-34 does
         self.num_regions = num_regions
-        self._motion = _MotionHandle(_motion_cfg(**pw.cfg_kw), Generator.IGNORED_PREFIX)
-        self._motion.validate()
+        self._motion = _motion_handle(_motion_cfg(**pw.cfg_kw), lambda key: key if key.startswith(Generator.IGNORED_PREFIX) else None)
+        self._handles.append(self._motion)
 
     # keeps pixelwise_flow_predictor.* (the parent class drops them)
     @classmethod
     def _drop_training_only_keys(cls, state_dict, prefix, *args):
         return None
-
-    def mark_dirty(self):
-        self._dirty = True
-        if "_motion" in self.__dict__:
-            self._motion.dirty = True
-
-    def _apply(self, fn, *a, **k):
-        if "_motion" in self.__dict__:
-            self._motion.dirty = True
-        return super()._apply(fn, *a, **k)
-
-    def __del__(self):
-        m = self.__dict__.get("_motion")
-        if m is not None:
-            try:
-                m.destroy()
-            except Exception:
-                pass
-        super().__del__()
 
     @torch.no_grad()
     def flow(self, source_image, driving_region_params, source_region_params, bg_params=None):
@@ -507,7 +472,7 @@ class MotionGenerator(Generator):
         n = drv["shift"].shape[0]
         H, W = source_image.shape[-2:]
         dev = source_image.device
-        chunk = self._motion.ensure(self, dev, n, H, W)
+        chunk = _motion_geometry(self._motion, self, dev, n, H, W)
         R = self.num_regions
         src = source_image.reshape(-1, 3, H, W)[0].contiguous().float()
 
@@ -521,12 +486,12 @@ class MotionGenerator(Generator):
         flow = torch.empty((n, H // 4, W // 4, 2), device=dev)
         occ = torch.empty((n, 1, H // 4, W // 4), device=dev)
         with torch.cuda.device(dev):
-            st = self._stream()
+            st = stream()
             for a in range(0, n, chunk):
                 b = min(n, a + chunk)
-                check(lib.dawn_lfg_motion_flow(self._motion.handle, _ptr(src), b - a, _ptr(ss[a:b]), _ptr(sc[a:b]), _ptr(sa[a:b]),
-                                               _ptr(ds[a:b]), _ptr(dc[a:b]), _ptr(da[a:b]), _ptr(bg[a:b]) if bg is not None else None,
-                                               _ptr(flow[a:b]), _ptr(occ[a:b]), st), "dawn_lfg_motion_flow")
+                check(lib.dawn_lfg_motion_flow(self._motion.handle, ptr(src), b - a, ptr(ss[a:b]), ptr(sc[a:b]), ptr(sa[a:b]),
+                                               ptr(ds[a:b]), ptr(dc[a:b]), ptr(da[a:b]), ptr(bg[a:b]) if bg is not None else None,
+                                               ptr(flow[a:b]), ptr(occ[a:b]), st), "dawn_lfg_motion_flow")
         return {"optical_flow": flow, "occlusion_map": occ}
 
     @torch.no_grad()
@@ -558,7 +523,7 @@ class MotionGenerator(Generator):
 
     def read_tap(self, name):
         """'flow_hourglass' reads the flow predictor; every other name the decoder (Generator.read_tap)."""
-        return self._motion.read_tap(name) if name == "flow_hourglass" else super().read_tap(name)
+        return _motion_read_tap(self._motion, name) if name == "flow_hourglass" else super().read_tap(name)
 
 
 class FlowAE(nn.Module):

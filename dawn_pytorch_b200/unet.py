@@ -15,7 +15,7 @@ import torch
 from torch import nn
 
 from . import _lib
-from ._lib import DawnUnetCfg, check, lib
+from ._lib import DawnUnetCfg, check, lib, ptr, stream
 
 PADDING_MODES = ("zeros", "reflect", "replicate", "circular")   # nn.Conv3d's, in the order of dawn_unet_cfg.pad_mode
 MAX_CLIPS = 16                  # clips per native pass the library accepts (kMaxClips, csrc/common.cuh)
@@ -304,10 +304,7 @@ class Unet3D(nn.Module):
     def sync_parameters(self):
         """Repack the module's parameters into kernel layouts (once per parameter change)."""
         def put(name, t):
-            t = t.detach().to(device="cpu", dtype=torch.float32).contiguous()
-            shape = (ctypes.c_int64 * max(t.dim(), 1))(*t.shape)
-            check(lib.dawn_unet_set_param(self._handle, name.encode(), ctypes.c_void_p(t.data_ptr()), shape, t.dim()),
-                  f"dawn_unet_set_param({name})")
+            _lib.put_param(lib.dawn_unet_set_param, self._handle, name, t)
         for name, t in self.state_dict().items():
             put(name, t)
         put("aux.time_freqs", _time_freqs(self.dim))
@@ -322,10 +319,6 @@ class Unet3D(nn.Module):
         self._shard = None
         if self._geom is not None:
             self._geom = self._geom  # commit re-sized the per-clip tables for the current geometry
-
-    @staticmethod
-    def _stream():
-        return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
     # ------------------------------------------------------------------ reference API
     def forward_with_cond_scale(self, *args, cond_scale=2., **kwargs):      # reference :879-890
@@ -364,7 +357,7 @@ class Unet3D(nn.Module):
             cond = torch.where(self.null_cond_mask[..., None], torch.zeros((), device=device), cond)
         cond = cond.contiguous()
         out = torch.empty((b, self.out_dim, F, h, w), device=device, dtype=torch.float32)
-        st = self._stream()
+        st = stream()
         with torch.cuda.device(device):
             # passes of n clips; a short last pass is filled up with copies of its last clip (their output is dropped), so the
             # handle keeps one geometry
@@ -375,8 +368,7 @@ class Unet3D(nn.Module):
                     pad = lambda a: torch.cat([a, a[-1:].expand((n - (i1 - i0),) + a.shape[1:])]).contiguous()   # noqa: E731
                     xs, ts, cs = pad(xs), pad(ts), pad(cs)
                     os_ = torch.empty((n,) + out.shape[1:], device=device, dtype=torch.float32)
-                check(lib.dawn_unet_forward(self._handle, ctypes.c_void_p(xs.data_ptr()), ctypes.c_void_p(ts.data_ptr()),
-                                            ctypes.c_void_p(cs.data_ptr()), ctypes.c_void_p(os_.data_ptr()), st),
+                check(lib.dawn_unet_forward(self._handle, ptr(xs), ptr(ts), ptr(cs), ptr(os_), st),
                       "dawn_unet_forward")
                 if os_.data_ptr() != out[i0:i1].data_ptr():
                     out[i0:i1].copy_(os_[:i1 - i0])
@@ -405,8 +397,7 @@ class Unet3D(nn.Module):
         self._cond = cond.contiguous().float()
         self._inv_batched = batched
         with torch.cuda.device(fea.device):
-            check(lib.dawn_unet_set_clip_invariants(self._handle, ctypes.c_void_p(self._fea.data_ptr()),
-                                                    ctypes.c_void_p(self._cond.data_ptr()), self._stream()),
+            check(lib.dawn_unet_set_clip_invariants(self._handle, ptr(self._fea), ptr(self._cond), stream()),
                   "dawn_unet_set_clip_invariants")
 
     def init_shard(self, F_local, h, w, device):
@@ -471,8 +462,7 @@ class Unet3D(nn.Module):
             raise ValueError(f"forward_x3: out must be contiguous float32 {oshape} on {x_t.device}")
         x_t = x_t.contiguous()
         with torch.cuda.device(x_t.device):
-            check(lib.dawn_unet_forward_x3(self._handle, ctypes.c_void_p(x_t.data_ptr()), ctypes.c_void_p(time.data_ptr()),
-                                           ctypes.c_void_p(out.data_ptr()), self._stream()), "dawn_unet_forward_x3")
+            check(lib.dawn_unet_forward_x3(self._handle, ptr(x_t), ptr(time), ptr(out), stream()), "dawn_unet_forward_x3")
         return out
 
     def forward_host(self, x_t, fea, cond, t, out=None):
@@ -481,8 +471,7 @@ class Unet3D(nn.Module):
         self._ensure(torch.device("cuda", torch.cuda.current_device()), F, h, w)      # one clip
         if out is None:
             out = torch.empty((self.out_dim, F, h, w), dtype=torch.float32, pin_memory=True)
-        check(lib.dawn_unet_forward_host(self._handle, ctypes.c_void_p(x_t.data_ptr()), ctypes.c_void_p(fea.data_ptr()),
-                                         ctypes.c_void_p(cond.data_ptr()), int(t), ctypes.c_void_p(out.data_ptr())),
+        check(lib.dawn_unet_forward_host(self._handle, ptr(x_t), ptr(fea), ptr(cond), int(t), ptr(out)),
               "dawn_unet_forward_host")
         return out
 
@@ -495,7 +484,7 @@ class Unet3D(nn.Module):
             check(lib.dawn_unet_tap_shape(self._handle, n.encode(), ctypes.byref(C), ctypes.byref(hl), ctypes.byref(wl)),
                   f"dawn_unet_tap_shape({n})")
             t = torch.zeros((1, C.value, F, hl.value, wl.value), device=device, dtype=torch.float32)
-            check(lib.dawn_unet_set_tap(self._handle, n.encode(), ctypes.c_void_p(t.data_ptr())), "dawn_unet_set_tap")
+            check(lib.dawn_unet_set_tap(self._handle, n.encode(), ptr(t)), "dawn_unet_set_tap")
             bufs[n] = t
         self._tap_bufs = bufs
         return bufs

@@ -72,7 +72,7 @@ int64_t dawn_lfg_workspace_bytes(dawn_lfg* h);
  *   WARP_BLEND        x = skip (H, W, C), motion, F, h, w, prev / ldp (may be NULL)       -> out (F, H, W, ldo)
  *   AFFINE_RELU       x (M, ldx), scale / shift (C, both NULL: plain ReLU), C, M           -> out (M, ldo); out may be x
  *   RESIDUAL_BN_RELU  y, x (M, C), scale / shift, C, M                                    -> out = y + x, out2 (or NULL)
- *   RELU_AVGPOOL2     x (H, W, C)                                                         -> out (H/2, W/2, C)
+ *   RELU_AVGPOOL2     x (H, W, C), H = rows (frames x an even height), ldo (0: C)        -> out (H/2, W/2, ldo)
  *   CHW_TO_HWC        x (C, H, W), Cpad                                                   -> out (H, W, Cpad)
  *   HWC_TO_CHW        x (M, ldx), C, M                                                    -> out (C, M)
  *   FINAL_CONV        x (F, H, W, ldx), C = Cin, weight (3, Cin, 7, 7), bias (3), source (3, H, W), motion, h, w,

@@ -1,19 +1,19 @@
 """CPU: the algebraic rewrites the CUDA paths rely on, checked with plain torch ops (host-side logic, no GPU):
  * nearest-2x upsample + 3x3 conv == four output-parity 2x2 convs over the low-resolution grid with summed taps
-   (the summed taps in csrc/lfg.cu::pack_up, the class convs in csrc/contraction.cu::pack_up / run_up,
+   (the summed taps in csrc/contraction.cu::pack_up_nearest, the class convs in csrc/contraction.cu::pack_up / run_up,
    reference UpBlock2d LFG/modules/util.py:106-111);
  * a k x k conv == the sum of k row-convolutions (1 x k) over vertically shifted copies of the input
    (csrc/unet.cu::init_map, the per-clip part of the 7x7 init conv, reference U:776-777);
  * the init conv is linear in its input channels: conv(cat[x_t, fea]) == conv3(x_t) + map(fea)  (SURVEY a2, U:1167, 1177);
- * eval-mode BatchNorm after a conv folds into the conv's weights and bias (csrc/lfg.cu::pack_conv).
+ * eval-mode BatchNorm after a conv folds into the conv's weights and bias (csrc/contraction.cu::pack_lfg_conv).
 """
 import torch
 import torch.nn.functional as F
 
-K_UP_OFF = [[-1, 0], [0, 1]]                       # csrc/lfg.cu: kUpOff[parity][tap] -> low-resolution offset
+K_UP_OFF = [[-1, 0], [0, 1]]                       # csrc/contraction.cuh: kUpOff[parity][tap] -> low-resolution offset
 
 
-def up_in_set(parity, tap, k):                      # csrc/lfg.cu: up_in_set
+def up_in_set(parity, tap, k):                      # csrc/contraction.cuh: up_in_set
     return (k == 0 if tap == 0 else k >= 1) if parity == 0 else (k <= 1 if tap == 0 else k == 2)
 
 

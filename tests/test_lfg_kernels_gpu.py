@@ -43,7 +43,8 @@ Coverage: kernel x variant -> test.
                     resized motion, saturated sigmoid                                        test_final_conv
   affine_relu       scale or not, in place, strided                                          test_affine_relu
   residual_bn_relu  with and without z                                                       test_residual_bn_relu
-  relu_avgpool2, chw_to_hwc (padding), hwc_to_chw (strided rows)                             test_relu_avgpool2, test_layouts
+  relu_avgpool2     one frame, strided output rows (ldo > C), several frames               test_relu_avgpool2
+  chw_to_hwc (padding), hwc_to_chw (strided rows)                                            test_layouts
   conv3x3_s2_relu   odd / even H, W incl. 1x1 and 127x129, Ci 1 / 3, Co 1 / 16              test_conv3x3_s2_relu
   all               refused arguments                                                        test_refusals
 """
@@ -298,15 +299,18 @@ def test_residual_bn_relu(with_z):
         check("residual_bn_relu z", body(zbuf, M, C), F.relu(xn * sd + td), bound)
 
 
-@pytest.mark.parametrize("shape", [(16, 16, 64), (40, 72, 128), (2, 2, 512)])
+# (H, W, C, ldo, frames): one frame into dense rows; a strided output (the skip half of an Hourglass level); frames * H rows of
+# several frames, as the motion estimator pools a batch
+@pytest.mark.parametrize("shape", [(16, 16, 64, 64, 1), (40, 72, 128, 128, 1), (2, 2, 512, 512, 1), (8, 12, 64, 136, 1),
+                                   (8, 12, 128, 256, 3)])
 def test_relu_avgpool2(shape):
-    H, W, C = shape
-    x = gen((H * W, C), H * W + C)
-    obuf, optr = guarded(H * W // 4, C)
-    ok(run(_lib().LFG_RELU_AVGPOOL2, x=x, H=H, W=W, C=C, out=optr))
-    xd = x.double().cpu().reshape(1, H, W, C).permute(0, 3, 1, 2)
-    ref = F.avg_pool2d(F.relu(xd), 2)[0].permute(1, 2, 0).reshape(-1, C)
-    check(f"relu_avgpool2{shape}", body(obuf, H * W // 4, C), ref, 3 * R.U * ref + 1e-300)
+    H, W, C, ldo, n = shape
+    x = gen((n * H * W, C), n * H * W + C)
+    obuf, optr = guarded(n * H * W // 4, ldo)
+    ok(run(_lib().LFG_RELU_AVGPOOL2, x=x, H=n * H, W=W, C=C, out=optr, ldo=ldo))
+    xd = x.double().cpu().reshape(n, H, W, C).permute(0, 3, 1, 2)
+    ref = F.avg_pool2d(F.relu(xd), 2).permute(0, 2, 3, 1).reshape(-1, C)
+    check(f"relu_avgpool2{shape}", body(obuf, n * H * W // 4, C), ref, 3 * R.U * ref + 1e-300)
 
 
 def test_layouts():
@@ -350,7 +354,8 @@ def test_refusals():
         (L.LFG_FINAL_CONV, dict(x=t, ldx=60, C=60, F=1, H=4, W=4, h=4, w=4, weight=t, bias=t, out=t)),  # Cin % 8
         (L.LFG_FINAL_CONV, dict(x=t, ldx=64, C=64, F=1, H=4, W=4, h=4, w=4, weight=t, bias=t, out=t, blend=1)),  # no source
         (L.LFG_AFFINE_RELU, dict(x=t, ldx=64, C=64, M=4, out=t, ldo=64, scale=t)),                   # scale without shift
-        (L.LFG_RELU_AVGPOOL2, dict(x=t, H=1, W=4, C=64, out=t)),
+        (L.LFG_RELU_AVGPOOL2, dict(x=t, H=1, W=4, C=64, out=t, ldo=64)),
+        (L.LFG_RELU_AVGPOOL2, dict(x=t, H=4, W=4, C=64, out=t, ldo=60)),                             # ldo < C
         (L.LFG_CHW_TO_HWC, dict(x=t, C=8, H=4, W=4, Cpad=4, out=t)),
         (L.LFG_MOTION_PACK, dict(flow=t, layout=0, F=1, h=4, w=4, out=t)),                          # layout 0 without occ
         (L.LFG_MOTION_PACK, dict(flow=t, occ=t, layout=2, F=1, h=4, w=4, out=t)),
