@@ -5,3 +5,4 @@ from .diffusion import DynamicNfGaussianDiffusion, GaussianDiffusion  # noqa: F4
 from .lfg import Generator as LfgGenerator  # noqa: F401
 from .lfg import BGMotionPredictor, FlowAE, MotionGenerator, RegionPredictor  # noqa: F401
 from .flow_diffusion import Face_loc_Encoder, FlowDiffusion  # noqa: F401
+from .pbnet import get_model as get_pbnet_model  # noqa: F401

@@ -132,6 +132,19 @@ class DawnLfgMotionKernelCase(ctypes.Structure):
                 ("out", _p), ("out2", _p), ("out3", _p)]
 
 
+class DawnPbnetCfg(ctypes.Structure):
+    """include/dawn_pbnet.h: dawn_pbnet_cfg"""
+    _fields_ = [(n, ctypes.c_int) for n in ("band", "pose_dim", "audio_dim", "latent_dim", "audio_latent_dim", "pose_latent_dim",
+                                            "ff_size", "num_layers", "num_heads")]
+
+
+class DawnPbnetAttentionCase(ctypes.Structure):
+    """include/dawn_pbnet.h: dawn_pbnet_attention_case (pointers are device addresses)"""
+    _i, _p = ctypes.c_int, ctypes.c_void_p
+    _fields_ = [("bs", _i), ("F", _i), ("D", _i), ("H", _i), ("band", _i), ("npairs", _i), ("qscale", ctypes.c_float),
+                ("x_q", _p), ("x_kv", _p), ("wq", _p), ("wk", _p), ("wv", _p), ("freqs", _p), ("bias", _p), ("out", _p)]
+
+
 class DawnError(RuntimeError):
     pass
 
@@ -216,6 +229,19 @@ def _load():
     lib.dawn_lfg_motion_workspace_bytes.argtypes = [vp]
     lib.dawn_lfg_motion_workspace_bytes.restype = ctypes.c_int64
     lib.dawn_lfg_motion_test_kernel.argtypes = [ctypes.POINTER(DawnLfgMotionKernelCase), vp]
+    lib.dawn_pbnet_create.argtypes = [ctypes.POINTER(DawnPbnetCfg), ctypes.POINTER(vp)]
+    lib.dawn_pbnet_destroy.argtypes = [vp]
+    lib.dawn_pbnet_destroy.restype = None
+    lib.dawn_pbnet_set_param.argtypes = [vp, cp, fp, i64p, ctypes.c_int]
+    lib.dawn_pbnet_commit_params.argtypes = [vp]
+    lib.dawn_pbnet_generate.argtypes = [vp, fp, fp, fp, fp, ctypes.c_int, ctypes.c_int, fp, vp]
+    lib.dawn_pbnet_last_launch_count.argtypes = [vp]
+    lib.dawn_pbnet_last_launch_count.restype = ctypes.c_int64
+    lib.dawn_pbnet_workspace_bytes.argtypes = [vp]
+    lib.dawn_pbnet_workspace_bytes.restype = ctypes.c_int64
+    lib.dawn_pbnet_live_bytes.argtypes = []
+    lib.dawn_pbnet_live_bytes.restype = ctypes.c_int64
+    lib.dawn_pbnet_test_attention.argtypes = [ctypes.POINTER(DawnPbnetAttentionCase), vp]
     lib.dawn_last_error.restype = cp
     lib.dawn_build_info.restype = cp
     return lib
@@ -241,6 +267,9 @@ LFG_MOTION_EXPORTS = ["dawn_lfg_motion_create", "dawn_lfg_motion_destroy", "dawn
                       "dawn_lfg_motion_workspace_bytes", "dawn_lfg_motion_test_kernel"]
 LFG_EXPORTS += LFG_MOTION_EXPORTS                       # both handles are declared in include/dawn_lfg.h
 MISC_EXPORTS = ["dawn_conv3x3_s2_relu"]
+PBNET_EXPORTS = ["dawn_pbnet_create", "dawn_pbnet_destroy", "dawn_pbnet_set_param", "dawn_pbnet_commit_params",
+                 "dawn_pbnet_generate", "dawn_pbnet_last_launch_count", "dawn_pbnet_workspace_bytes", "dawn_pbnet_live_bytes",
+                 "dawn_pbnet_test_attention"]
 
 PROF_CATS = ["conv3x3", "conv_other", "qkv_proj", "out_proj", "ca_gate", "gn_hcond", "attn_core", "sla_context",
              "gn_apply", "rowstats", "ca_rstd", "misc", "prep", "temporal_fused_l0", "conv3x3_l0", "comm_allreduce", "comm_halo"]

@@ -421,16 +421,16 @@ int launch_film(const FilmDesc* descs_dev, int ndesc, int max_n, int clips, cons
   return 0;
 }
 
-__global__ void rotary_table_kernel(const float* __restrict__ freqs, int F, int pos0, float* __restrict__ out) {
+__global__ void rotary_table_kernel(const float* __restrict__ freqs, int npairs, int F, int pos0, float* __restrict__ out) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= F * 16) return;
-  const int f = idx >> 4, i = idx & 15;
+  if (idx >= F * npairs) return;
+  const int f = idx / npairs, i = idx - f * npairs;
   const float a = (float)(pos0 + f) * freqs[i];
   out[2 * idx] = cosf(a);
   out[2 * idx + 1] = sinf(a);
 }
-int launch_rotary_table(const float* freqs, int F, int pos0, float* out, cudaStream_t st) {
-  rotary_table_kernel<<<(F * 16 + 255) / 256, 256, 0, st>>>(freqs, F, pos0, out);
+int launch_rotary_table(const float* freqs, int npairs, int F, int pos0, float* out, cudaStream_t st) {
+  rotary_table_kernel<<<(F * npairs + 255) / 256, 256, 0, st>>>(freqs, npairs, F, pos0, out);
   DAWN_LAUNCH_OK();
   return 0;
 }

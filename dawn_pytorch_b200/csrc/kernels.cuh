@@ -51,8 +51,8 @@ int launch_time_mlp(const int64_t* t_dev, int t_stride, int clips, const float* 
 // max_n >= every descriptor's n: all outputs of every descriptor are written
 int launch_film(const FilmDesc* descs_dev, int ndesc, int max_n, int clips, const float* t_silu, int tdim, cudaStream_t st);
 
-// rotary cos/sin table [F][16][2] from freqs[16], position = pos0 + f
-int launch_rotary_table(const float* freqs, int F, int pos0, float* out, cudaStream_t st);
+// rotary cos/sin table [F][npairs][2] from freqs[npairs], position = pos0 + f (the UNet's 32-wide rotary: npairs = 16)
+int launch_rotary_table(const float* freqs, int npairs, int F, int pos0, float* out, cudaStream_t st);
 
 // ---------------------------------------------------------------- attention cores
 // banded / full softmax attention over strided sequences; qkv rows are [q(256) | k(256) | v(256)], head = 32 dims

@@ -141,7 +141,7 @@ int test_kernel(const dawn_kernel_case& c, Owned& own, cudaStream_t st) {
     case DAWN_KERNEL_ROTARY:
       if (!c.freqs || !c.out) return refuse("missing pointer");
       if (c.F < 1 || c.pos0 < 0 || c.F > (1 << 20)) return refuse("bad geometry");
-      return launch_rotary_table(c.freqs, c.F, c.pos0, c.out, st);
+      return launch_rotary_table(c.freqs, 16, c.F, c.pos0, c.out, st);
     case DAWN_KERNEL_SPLIT_ROWS:
       if (!c.x || !c.out_hi || !c.out_lo) return refuse("missing pointer");
       if (c.M < 1 || !row_ok(c.ld, c.C)) return refuse("bad geometry");

@@ -1183,7 +1183,7 @@ int dawn_unet_set_geometry(dawn_unet* h, int B, int F, int height, int width) {
   }
   h->sh_nranks = 1; h->sh_rank = 0; h->sh_Fglobal = F; h->sh_halo_l = 0; h->sh_halo_r = 0;   // a new geometry is unsharded until init_shard
   h->p2p_ready = false;
-  DAWN_TRY(launch_rotary_table(h->rot_freqs, F, 0, h->ROT, 0));
+  DAWN_TRY(launch_rotary_table(h->rot_freqs, 16, F, 0, h->ROT, 0));
   DAWN_CUDA_OK(cudaDeviceSynchronize());
   return 0;
 }
@@ -1345,7 +1345,7 @@ int dawn_unet_init_shard(dawn_unet* h, const char* id128, int nranks, int rank, 
   h->sh_halo_r = (rank < nranks - 1) ? h->cfg.win_width : 0;
   // rotary positions of the halo-extended local sequence are GLOBAL frame indices
   const int pos0 = rank * h->F - h->sh_halo_l;
-  DAWN_TRY(launch_rotary_table(h->rot_freqs, h->sh_halo_l + h->F + h->sh_halo_r, pos0, h->ROT, 0));
+  DAWN_TRY(launch_rotary_table(h->rot_freqs, 16, h->sh_halo_l + h->F + h->sh_halo_r, pos0, h->ROT, 0));
   DAWN_CUDA_OK(cudaDeviceSynchronize());
   return 0;
 }

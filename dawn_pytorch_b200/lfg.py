@@ -40,13 +40,15 @@ def _res_block(c):                                          # ResBlock2d (util.p
 
 
 class _Handle:
-    """One native handle of include/dawn_lfg.h (entry points `<api>_*`, api "dawn_lfg" or "dawn_lfg_motion") that holds a
-    module's parameters.  It is created on the device of the module's inputs and created again after a device change, and the
-    module's state_dict is uploaded and committed whenever `dirty`.  param_name(key) is the library's name of a state_dict
-    entry, or None for an entry the handle does not take.  `geom` is the geometry its user set last; create and commit void it."""
+    """One native handle of include/dawn_lfg.h or include/dawn_pbnet.h (entry points `<api>_*`, api "dawn_lfg",
+    "dawn_lfg_motion" or "dawn_pbnet") that holds a module's parameters.  It is created on the device of the module's inputs and
+    created again after a device change, and the module's state_dict is uploaded and committed whenever `dirty`.
+    param_name(key) is the library's name of a state_dict entry, or None for an entry the handle does not take; extra(module)
+    gives further {name: tensor} entries derived from the module.  `geom` is the geometry its user set last; create and commit
+    void it."""
 
-    def __init__(self, api, cfg, what, param_name=lambda key: key):
-        self.api, self.cfg, self.what, self.param_name = api, cfg, what, param_name
+    def __init__(self, api, cfg, what, param_name=lambda key: key, extra=lambda module: {}):
+        self.api, self.cfg, self.what, self.param_name, self.extra = api, cfg, what, param_name, extra
         self.handle, self.device_index, self.dirty, self.geom = None, None, True, None
 
     def _entry(self, name):
@@ -82,6 +84,8 @@ class _Handle:
                     name = None if key.endswith("num_batches_tracked") else self.param_name(key)
                     if name is not None:
                         _lib.put_param(self._entry("set_param"), self.handle, name, t)
+                for name, t in self.extra(module).items():
+                    _lib.put_param(self._entry("set_param"), self.handle, name, t)
                 check(self._entry("commit_params")(self.handle), f"{self.api}_commit_params")
                 self.dirty, self.geom = False, None
         return idx
@@ -91,8 +95,8 @@ class _Handle:
 
 
 class _LfgModule(nn.Module):
-    """Base of the LFG modules, whose parameters feed the native handles in `_handles`: load_state_dict and .to() / .cuda()
-    mark every handle dirty, and the handles die with the module.  Inference only: train(True) raises `TRAIN_REFUSAL`."""
+    """Base of the LFG modules and the PBnet decoder, whose parameters feed the native handles in `_handles`: load_state_dict and
+    .to() / .cuda() mark every handle dirty, and the handles die with the module.  Inference only: train(True) raises `TRAIN_REFUSAL`."""
     TRAIN_REFUSAL = ""
 
     def _hold(self, *handles):
