@@ -1,9 +1,11 @@
-"""ctypes binding of include/dawn_unet.h.  The product path has no fallback: if the CUDA library is
-missing or fails to load, importing this module raises."""
+"""ctypes binding of include/dawn_unet.h, include/dawn_lfg.h and include/dawn_pbnet.h, and the lifecycle every module shares
+with its native handles.  The product path has no fallback: if the CUDA library is missing or fails to load, importing this
+module raises."""
 import ctypes
 import os
 
 import torch
+from torch import nn
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libdawn_unet.so")
@@ -239,10 +241,10 @@ def _load():
     lib.dawn_pbnet_last_launch_count.restype = ctypes.c_int64
     lib.dawn_pbnet_workspace_bytes.argtypes = [vp]
     lib.dawn_pbnet_workspace_bytes.restype = ctypes.c_int64
-    lib.dawn_pbnet_live_bytes.argtypes = []
-    lib.dawn_pbnet_live_bytes.restype = ctypes.c_int64
     lib.dawn_pbnet_test_attention.argtypes = [ctypes.POINTER(DawnPbnetAttentionCase), vp]
     lib.dawn_last_error.restype = cp
+    lib.dawn_live_bytes.argtypes = []
+    lib.dawn_live_bytes.restype = ctypes.c_int64
     lib.dawn_build_info.restype = cp
     return lib
 
@@ -255,7 +257,7 @@ EXPORTS = ["dawn_unet_create", "dawn_unet_destroy", "dawn_unet_set_param", "dawn
            "dawn_unet_profile_enable", "dawn_unet_profile_read", "dawn_unet_last_launch_count", "dawn_unet_workspace_bytes", "dawn_ddim_step", "dawn_unet_ddim_step", "dawn_unet_sampler_capture", "dawn_unet_sampler_launch",
            "dawn_unet_ddim_step_guided", "dawn_unet_sampler_capture_guided", "dawn_unet_sampler_launch_guided",
            "dawn_ddpm_step", "dawn_unet_ddpm_step", "dawn_unet_ddpm_capture", "dawn_unet_ddpm_launch",
-           "dawn_test_contraction", "dawn_test_fused", "dawn_test_kernel", "dawn_last_error", "dawn_build_info"]
+           "dawn_test_contraction", "dawn_test_fused", "dawn_test_kernel", "dawn_last_error", "dawn_live_bytes", "dawn_build_info"]
 
 
 LFG_EXPORTS = ["dawn_lfg_create", "dawn_lfg_destroy", "dawn_lfg_set_param", "dawn_lfg_commit_params", "dawn_lfg_set_geometry",
@@ -268,8 +270,7 @@ LFG_MOTION_EXPORTS = ["dawn_lfg_motion_create", "dawn_lfg_motion_destroy", "dawn
 LFG_EXPORTS += LFG_MOTION_EXPORTS                       # both handles are declared in include/dawn_lfg.h
 MISC_EXPORTS = ["dawn_conv3x3_s2_relu"]
 PBNET_EXPORTS = ["dawn_pbnet_create", "dawn_pbnet_destroy", "dawn_pbnet_set_param", "dawn_pbnet_commit_params",
-                 "dawn_pbnet_generate", "dawn_pbnet_last_launch_count", "dawn_pbnet_workspace_bytes", "dawn_pbnet_live_bytes",
-                 "dawn_pbnet_test_attention"]
+                 "dawn_pbnet_generate", "dawn_pbnet_last_launch_count", "dawn_pbnet_workspace_bytes", "dawn_pbnet_test_attention"]
 
 PROF_CATS = ["conv3x3", "conv_other", "qkv_proj", "out_proj", "ca_gate", "gn_hcond", "attn_core", "sla_context",
              "gn_apply", "rowstats", "ca_rstd", "misc", "prep", "temporal_fused_l0", "conv3x3_l0", "comm_allreduce", "comm_halo"]
@@ -296,3 +297,114 @@ def put_param(set_param, handle, name, t):
     t = t.detach().to(device="cpu", dtype=torch.float32).contiguous()
     shape = (ctypes.c_int64 * max(t.dim(), 1))(*t.shape)
     check(set_param(handle, name.encode(), ctypes.c_void_p(t.data_ptr()), shape, t.dim()), f"{set_param.__name__}({name})")
+
+
+class _Holder(nn.Module):
+    """Container of parameters whose forward is never called."""
+
+    def forward(self, *a, **k):  # pragma: no cover
+        raise RuntimeError("parameter holder: the computation runs in the CUDA library")
+
+
+class _Handle:
+    """One native handle (entry points `<api>_*`, api "dawn_unet", "dawn_lfg", "dawn_lfg_motion" or "dawn_pbnet") that holds a
+    module's parameters.  It is created on the device of the module's inputs and created again after a device change, and the
+    module's state_dict is uploaded and committed whenever `dirty`; `commits` counts the commits.  param_name(key) is the library's
+    name of a state_dict entry, or None for an entry the handle does not take; extra(module) gives further {name: tensor} entries
+    derived from the module.  `geom` is the geometry its user set last: create voids it, and so does a commit unless keeps_geom
+    (the library re-applies its geometry on commit)."""
+
+    def __init__(self, api, cfg, what, param_name=lambda key: key, extra=lambda module: {}, keeps_geom=False):
+        self.api, self.cfg, self.what, self.param_name, self.extra, self.keeps_geom = api, cfg, what, param_name, extra, keeps_geom
+        self.handle, self.device_index, self.dirty, self.geom, self.commits = None, None, True, None, 0
+
+    def _entry(self, name):
+        return getattr(lib, f"{self.api}_{name}")
+
+    def _create(self):
+        hd = ctypes.c_void_p()
+        check(self._entry("create")(ctypes.byref(self.cfg), ctypes.byref(hd)), f"{self.api}_create")
+        return hd
+
+    def validate(self):
+        """Create refuses what the library cannot run; it needs no GPU."""
+        self._entry("destroy")(self._create())
+
+    def destroy(self):
+        if self.handle is not None:
+            self._entry("destroy")(self.handle)
+        self.handle, self.geom = None, None
+
+    def ensure(self, module, device):
+        """Readies the handle for a call on `device` with the parameters of `module`; returns the device index."""
+        if device.type != "cuda":
+            raise DawnError(f"{self.what} runs on CUDA (sm_90a) only; there is no CPU path")
+        idx = device.index if device.index is not None else torch.cuda.current_device()
+        if self.handle is not None and self.device_index != idx:
+            self.destroy()
+            self.dirty = True
+        with torch.cuda.device(idx):
+            if self.handle is None:
+                self.handle, self.device_index = self._create(), idx
+            if self.dirty:
+                for key, t in module.state_dict().items():
+                    name = None if key.endswith("num_batches_tracked") else self.param_name(key)
+                    if name is not None:
+                        put_param(self._entry("set_param"), self.handle, name, t)
+                for name, t in self.extra(module).items():
+                    put_param(self._entry("set_param"), self.handle, name, t)
+                check(self._entry("commit_params")(self.handle), f"{self.api}_commit_params")
+                self.dirty, self.commits = False, self.commits + 1
+                if not self.keeps_geom:
+                    self.geom = None
+        return idx
+
+    def last_launch_count(self):
+        return int(self._entry("last_launch_count")(self.handle)) if self.handle is not None else 0
+
+    def workspace_bytes(self):
+        return int(self._entry("workspace_bytes")(self.handle)) if self.handle is not None else 0
+
+
+class _NativeModule(nn.Module):
+    """Base of the modules whose parameters feed the native handles in `_handles`: load_state_dict and .to() / .cuda() mark every
+    handle dirty, and the handles die with the module.  A class with a TRAIN_REFUSAL is inference only: it starts in eval mode and
+    its train(True) raises with that message."""
+    TRAIN_REFUSAL = None
+
+    def _hold(self, *handles):
+        self._handles = list(handles)
+        self.register_load_state_dict_post_hook(lambda module, incompatible: module.mark_dirty())
+        if self.TRAIN_REFUSAL:
+            self.eval()
+
+    def mark_dirty(self):
+        """Call after mutating parameters in place; load_state_dict / .to() / .cuda() do it automatically."""
+        for h in self._handles:
+            h.dirty = True
+
+    def _apply(self, fn, *a, **k):
+        for h in self.__dict__.get("_handles", ()):
+            h.dirty = True
+        return super()._apply(fn, *a, **k)
+
+    def train(self, mode=True):
+        if mode and self.TRAIN_REFUSAL:
+            raise NotImplementedError(self.TRAIN_REFUSAL)
+        return super().train(mode)
+
+    def __del__(self):
+        # plain dict access: nn.Module.__getattr__ may already be torn down at interpreter shutdown
+        for h in self.__dict__.get("_handles", ()):
+            try:
+                h.destroy()
+            except Exception:
+                pass
+
+    def last_launch_count(self):
+        """Kernels the last call of the module's first handle enqueued."""
+        return self._handles[0].last_launch_count()
+
+    def workspace_bytes(self):
+        """Device bytes of the workspace of the module's first handle."""
+        return self._handles[0].workspace_bytes()

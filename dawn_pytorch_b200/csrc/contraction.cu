@@ -1,6 +1,7 @@
 // Host side of every contraction (contraction.cuh), and dawn_test_contraction (include/dawn_unet.h), which runs one
 // contraction through the same weight upload and path launcher as the networks.
 #include <algorithm>
+#include <atomic>
 #include <cmath>
 #include <cstring>
 
@@ -37,46 +38,44 @@ int HostParams::need(const std::string& name, const std::vector<int64_t>& shape,
   return 0;
 }
 
-int dev_alloc(std::vector<void*>& owner, size_t nfloats, float** out, int64_t* counter) {
-  void* p = nullptr;
-  const size_t bytes = std::max<size_t>(nfloats, 4) * sizeof(float);
-  DAWN_CUDA_OK(cudaMalloc(&p, bytes));
-  owner.push_back(p);
-  if (counter) *counter += (int64_t)bytes;
-  *out = (float*)p;
+namespace {
+std::atomic<int64_t> g_arena_bytes{0};     // blocks of every DeviceArena
+}  // namespace
+
+int DeviceArena::alloc_bytes(size_t bytes, void** out) {
+  *out = nullptr;
+  bytes = std::max<size_t>(bytes, 16);
+  DAWN_CUDA_OK(cudaMalloc(out, bytes));
+  blocks_.emplace_back(*out);
+  bytes_ += (int64_t)bytes;
+  g_arena_bytes += (int64_t)bytes;
   return 0;
 }
-int dev_upload(std::vector<void*>& owner, const std::vector<float>& v, float** out) {
-  DAWN_TRY(dev_alloc(owner, v.size(), out));
-  DAWN_CUDA_OK(cudaMemcpy(*out, v.data(), v.size() * sizeof(float), cudaMemcpyHostToDevice));
+int DeviceArena::copy_in(void* dst, const void* src, size_t bytes) {
+  DAWN_CUDA_OK(cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice));
   return 0;
 }
-int dev_upload(std::vector<void*>& owner, const std::vector<uint16_t>& v, uint16_t** out) {
-  float* d = nullptr;
-  DAWN_TRY(dev_alloc(owner, (v.size() + 1) / 2, &d));
-  DAWN_CUDA_OK(cudaMemcpy(d, v.data(), v.size() * sizeof(uint16_t), cudaMemcpyHostToDevice));
-  *out = reinterpret_cast<uint16_t*>(d);
-  return 0;
+void DeviceArena::release() {
+  blocks_.clear();
+  g_arena_bytes -= bytes_;
+  bytes_ = 0;
 }
-void free_all(std::vector<void*>& v) {
-  for (void* p : v) cudaFree(p);
-  v.clear();
-}
+int64_t DeviceArena::live_bytes() { return g_arena_bytes.load(); }
 
 // ------------------------------------------------------------------------------------------ packed weights
-int upload_weight(std::vector<void*>& owner, const std::vector<float>& m, int K, int N, int ldb, const std::vector<float>& bias,
+int upload_weight(DeviceArena& arena, const std::vector<float>& m, int K, int N, int ldb, const std::vector<float>& bias,
                   PackedWeight* out) {
   *out = PackedWeight{};
-  DAWN_TRY(dev_upload(owner, m, &out->w));
+  DAWN_TRY(arena.upload(m, &out->w));
   if (N % 64 == 0 && K % 64 == 0) {             // the shapes the wgmma kernels can take
     std::vector<float> img;
     tc_pack_weights(m.data(), K, N, ldb, img, &out->img_scale);
-    DAWN_TRY(dev_upload(owner, img, &out->img));
+    DAWN_TRY(arena.upload(img, &out->img));
   }
   if (!bias.empty()) {
     std::vector<float> b(ldb, 0.f);
     std::copy(bias.begin(), bias.end(), b.begin());
-    DAWN_TRY(dev_upload(owner, b, &out->b));
+    DAWN_TRY(arena.upload(b, &out->b));
   }
   out->K = K; out->N = N; out->ldb = ldb;
   return 0;
@@ -141,7 +140,7 @@ void pack_conv_taps(const float* w, int co, int ci, int taps, int ci_pad, int ld
   }
 }
 
-int pack_lfg_conv(const HostParams& raw, std::vector<void*>& owner, const std::vector<std::pair<std::string, int>>& convs,
+int pack_lfg_conv(const HostParams& raw, DeviceArena& arena, const std::vector<std::pair<std::string, int>>& convs,
                   const std::string& bn_after, int ci, int k, int ci_pad, PackedWeight* out) {
   int N = 0;
   for (auto& c : convs) N += c.second;
@@ -159,7 +158,7 @@ int pack_lfg_conv(const HostParams& raw, std::vector<void*>& owner, const std::v
     pack_conv_taps(w->data.data(), co, ci, k * k, ci_pad, ldb, n0, s.data(), m);
     n0 += co;
   }
-  return upload_weight(owner, m, K, N, ldb, bias, out);
+  return upload_weight(arena, m, K, N, ldb, bias, out);
 }
 
 // ------------------------------------------------------------------------------------------ GemmParams
@@ -226,7 +225,7 @@ int launch_path(const GemmParams& p, int epi, int path, void* scratch, cudaStrea
 }
 
 // ------------------------------------------------------------------------------------------ 2x upsampling conv
-int pack_up(std::vector<void*>& owner, int ci, int co, const int (&off)[2][2], const std::vector<float>& bias, const UpWeight& weight,
+int pack_up(DeviceArena& arena, int ci, int co, const int (&off)[2][2], const std::vector<float>& bias, const UpWeight& weight,
             UpConv* u) {
   memcpy(u->off, off, sizeof(u->off));
   const int ldb = round_up(co, 64);
@@ -237,7 +236,7 @@ int pack_up(std::vector<void*>& owner, int ci, int co, const int (&off)[2][2], c
         for (int tx = 0; tx < 2; ++tx)
           for (int c = 0; c < ci; ++c)
             for (int n = 0; n < co; ++n) m[((size_t)(ty * 2 + tx) * ci + c) * ldb + n] = weight(py, px, ty, tx, c, n);
-      DAWN_TRY(upload_weight(owner, m, 4 * ci, co, ldb, bias, &u->cls[py * 2 + px]));
+      DAWN_TRY(upload_weight(arena, m, 4 * ci, co, ldb, bias, &u->cls[py * 2 + px]));
     }
   if (co == 64 && ci % 64 == 0) {
     // one 3x3 conv over the input grid: weight rows (tap, cin), columns (class, cout); 2.25x the MACs of the four class convs,
@@ -255,14 +254,14 @@ int pack_up(std::vector<void*>& owner, int ci, int co, const int (&off)[2][2], c
               for (int n = 0; n < co; ++n) m[((size_t)tap * ci + c) * N4 + cls * co + n] = weight(py, px, ty, tx, c, n);
           }
       }
-    DAWN_TRY(upload_weight(owner, m, 9 * ci, N4, N4, b4, &u->all));
+    DAWN_TRY(upload_weight(arena, m, 9 * ci, N4, N4, b4, &u->all));
   }
   return 0;
 }
 
-int pack_up_nearest(std::vector<void*>& owner, const float* w, int ci, int co, const double* scale, const std::vector<float>& bias,
+int pack_up_nearest(DeviceArena& arena, const float* w, int ci, int co, const double* scale, const std::vector<float>& bias,
                     UpConv* u) {
-  return pack_up(owner, ci, co, kUpOff, bias, [&](int py, int px, int ty, int tx, int c, int n) {
+  return pack_up(arena, ci, co, kUpOff, bias, [&](int py, int px, int ty, int tx, int c, int n) {
     double acc = 0.0;
     for (int ky = 0; ky < 3; ++ky)
       for (int kx = 0; kx < 3; ++kx)
@@ -271,7 +270,7 @@ int pack_up_nearest(std::vector<void*>& owner, const float* w, int ci, int co, c
   }, u);
 }
 
-int pack_lfg_up(const HostParams& raw, std::vector<void*>& owner, const std::string& name, int co, int ci, UpConv* u) {
+int pack_lfg_up(const HostParams& raw, DeviceArena& arena, const std::string& name, int co, int ci, UpConv* u) {
   // on the low-resolution grid each output-parity class is a 2x2 conv: 2.25x fewer MACs, and the upsampled tensor never exists
   const HostParam *w, *b;
   DAWN_TRY(raw.need(name + ".conv.weight", {co, ci, 3, 3}, &w));
@@ -280,7 +279,7 @@ int pack_lfg_up(const HostParams& raw, std::vector<void*>& owner, const std::str
   DAWN_TRY(bn_affine(raw, name + ".norm", co, s, t));
   std::vector<float> bias(co);
   for (int n = 0; n < co; ++n) bias[n] = (float)((double)b->data[n] * s[n] + t[n]);
-  return pack_up_nearest(owner, w->data.data(), ci, co, s.data(), bias, u);
+  return pack_up_nearest(arena, w->data.data(), ci, co, s.data(), bias, u);
 }
 
 int run_up(const GemmParams& in, const UpConv& u, float* out, int ldo, const std::function<int(const GemmParams&)>& run, int border) {
@@ -313,11 +312,6 @@ int refuse(const char* why) {
   set_last_error(std::string("dawn_test_contraction: ") + why);
   return -1;
 }
-
-struct Owned {
-  std::vector<void*> v;
-  ~Owned() { free_all(v); }
-};
 
 int test_contraction(const dawn_contraction_case& c, cudaStream_t st) {
   if (c.path < DAWN_PATH_MMA_SYNC || c.path > DAWN_PATH_TC_CONV3_TMA) return refuse("unknown path");
@@ -353,21 +347,21 @@ int test_contraction(const dawn_contraction_case& c, cudaStream_t st) {
   if (ln && !p.wsum) return refuse("LayerNorm epilogue without wsum");
   if (c.epi == EPI_PLAIN && p.stats && (p.cpg <= 0 || p.N / p.cpg > 8)) return refuse("GroupNorm statistics need 8 groups");
 
-  Owned own;
+  DeviceArena arena;
   if (c.path != DAWN_PATH_MMA_SYNC) {
     // the wgmma paths read the weight image the network's upload builds from the same fp32 matrix
     std::vector<float> hB((size_t)p.K * p.ldb);
     DAWN_CUDA_OK(cudaMemcpy(hB.data(), p.B, hB.size() * sizeof(float), cudaMemcpyDeviceToHost));
     PackedWeight w;
-    DAWN_TRY(upload_weight(own.v, hB, p.K, p.N, p.ldb, {}, &w));
+    DAWN_TRY(upload_weight(arena, hB, p.K, p.N, p.ldb, {}, &w));
     set_weights(p, w);
     p.bias = c.bias;
   }
   const bool split = c.path == DAWN_PATH_TC_GEMM_PRESPLIT || c.path == DAWN_PATH_TC_CONV3_TMA;
   const size_t scratch_bytes = split ? (size_t)split_rows(p) * p.Cin * 4 : 0;
   if (!path_ok(p, c.epi, c.path, scratch_bytes)) return refuse("the path does not accept this geometry");
-  float* scratch = nullptr;
-  if (split) DAWN_TRY(dev_alloc(own.v, scratch_bytes / sizeof(float), &scratch));
+  unsigned short* scratch = nullptr;                     // the fp16 hi | lo planes of A
+  if (split) DAWN_TRY(arena.alloc(scratch_bytes / sizeof(unsigned short), &scratch));
   DAWN_TRY(launch_path(p, c.epi, c.path, scratch, st));
   DAWN_CUDA_OK(cudaStreamSynchronize(st));
   return 0;

@@ -5,6 +5,7 @@
 #pragma once
 #include <cstdint>
 #include <functional>
+#include <memory>
 #include <string>
 #include <unordered_map>
 #include <utility>
@@ -28,10 +29,39 @@ struct HostParams {
   int need(const std::string& name, const std::vector<int64_t>& shape, const HostParam** out) const;
 };
 
-int dev_alloc(std::vector<void*>& owner, size_t nfloats, float** out, int64_t* counter = nullptr);
-int dev_upload(std::vector<void*>& owner, const std::vector<float>& v, float** out);
-int dev_upload(std::vector<void*>& owner, const std::vector<uint16_t>& v, uint16_t** out);   // fp16 images of the fused kernels
-void free_all(std::vector<void*>& v);
+// Owner of device allocations: every block is its own cudaMalloc of at least 16 bytes, freed by release() or the destructor.
+// bytes() counts this arena's blocks; live_bytes() counts the blocks of every arena in the process.
+class DeviceArena {
+ public:
+  DeviceArena() = default;
+  DeviceArena(const DeviceArena&) = delete;
+  DeviceArena& operator=(const DeviceArena&) = delete;
+  ~DeviceArena() { release(); }
+
+  template <class T>
+  int alloc(size_t count, T** out) {
+    void* p = nullptr;
+    const int rc = alloc_bytes(count * sizeof(T), &p);
+    *out = static_cast<T*>(p);
+    return rc;
+  }
+  // a block holding v (fp32 weights, fp16 images of the fused kernels)
+  template <class T>
+  int upload(const std::vector<T>& v, T** out) {
+    const int rc = alloc(v.size(), out);
+    return rc != 0 ? rc : copy_in(*out, v.data(), v.size() * sizeof(T));
+  }
+  void release();
+  int64_t bytes() const { return bytes_; }
+  static int64_t live_bytes();
+
+ private:
+  struct Free { void operator()(void* p) const { cudaFree(p); } };
+  int alloc_bytes(size_t bytes, void** out);
+  static int copy_in(void* dst, const void* src, size_t bytes);
+  std::vector<std::unique_ptr<void, Free>> blocks_;
+  int64_t bytes_ = 0;
+};
 inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
 
 // ---------------------------------------------------------------- packed weights
@@ -41,7 +71,7 @@ struct PackedWeight {
   float* w = nullptr; float* b = nullptr; float* img = nullptr; float img_scale = 1.f;
   int K = 0, N = 0, ldb = 0;
 };
-int upload_weight(std::vector<void*>& owner, const std::vector<float>& m, int K, int N, int ldb, const std::vector<float>& bias,
+int upload_weight(DeviceArena& arena, const std::vector<float>& m, int K, int N, int ldb, const std::vector<float>& bias,
                   PackedWeight* out);
 
 // Folds shared by the network's weight upload and dawn_test_fused.  Linear weight w [N][K] (row-major) with a per-input gain
@@ -59,7 +89,7 @@ int bn_affine(const HostParams& raw, const std::string& prefix, int c, std::vect
 void pack_conv_taps(const float* w, int co, int ci, int taps, int ci_pad, int ldb, int n0, const double* scale, std::vector<float>& m);
 // The LFG networks' Conv2d weights (co_j, ci, k, k) and biases of `convs` (state_dict prefix, co_j), side by side in the output
 // columns, with the BatchNorm `bn_after` (none when empty) folded in: W' = W s, b' = b s + t.  Input channels ci..ci_pad stay zero.
-int pack_lfg_conv(const HostParams& raw, std::vector<void*>& owner, const std::vector<std::pair<std::string, int>>& convs,
+int pack_lfg_conv(const HostParams& raw, DeviceArena& arena, const std::vector<std::pair<std::string, int>>& convs,
                   const std::string& bn_after, int ci, int k, int ci_pad, PackedWeight* out);
 
 // ---------------------------------------------------------------- GemmParams
@@ -90,14 +120,14 @@ using UpWeight = std::function<float(int py, int px, int ty, int tx, int c, int 
 // +1 <- k2}.  Zero padding is the same on both grids (upsampled index -1 / 2H <-> low-resolution index -1 / H).
 constexpr int kUpOff[2][2] = {{-1, 0}, {0, 1}};
 inline bool up_in_set(int parity, int tap, int k) { return parity == 0 ? (tap == 0 ? k == 0 : k >= 1) : (tap == 0 ? k <= 1 : k == 2); }
-int pack_up(std::vector<void*>& owner, int ci, int co, const int (&off)[2][2], const std::vector<float>& bias, const UpWeight& weight,
+int pack_up(DeviceArena& arena, int ci, int co, const int (&off)[2][2], const std::vector<float>& bias, const UpWeight& weight,
             UpConv* u);
 // nearest x2 -> 3x3 conv with weight w (co, ci, 3, 3) [times scale[n]] as the parity classes above: each class tap is the sum of
 // the 3x3 taps it covers, summed in fp64 and rounded once (scale null: no scale)
-int pack_up_nearest(std::vector<void*>& owner, const float* w, int ci, int co, const double* scale, const std::vector<float>& bias,
+int pack_up_nearest(DeviceArena& arena, const float* w, int ci, int co, const double* scale, const std::vector<float>& bias,
                     UpConv* u);
 // the LFG networks' UpBlock2d `name` (util.py:106-111): nearest x2 -> conv3x3 (name.conv) -> BatchNorm (name.norm) folded
-int pack_lfg_up(const HostParams& raw, std::vector<void*>& owner, const std::string& name, int co, int ci, UpConv* u);
+int pack_lfg_up(const HostParams& raw, DeviceArena& arena, const std::string& name, int co, int ci, UpConv* u);
 // in: base_params of the low-resolution input; out: (frames, 2H, 2W) rows of stride ldo.  run launches one contraction: once with
 // the up2 halo conv when that path takes it, otherwise once per parity class.  border = 1: `in` reads a grid that carries a
 // one-pixel border (IH = OHs + 2, IW = OWs + 2); the classes then run as valid 2x2 convs over it, so no tap leaves the grid.

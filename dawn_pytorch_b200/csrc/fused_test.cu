@@ -19,11 +19,6 @@ int refuse(const char* why) {
   return -1;
 }
 
-struct Owned {
-  std::vector<void*> v;
-  ~Owned() { free_all(v); }
-};
-
 int to_host(const float* d, size_t n, std::vector<float>& h) {
   h.resize(n);
   DAWN_CUDA_OK(cudaMemcpy(h.data(), d, n * sizeof(float), cudaMemcpyDeviceToHost));
@@ -38,7 +33,7 @@ AttnArgs attn_args(const dawn_fused_case& c) {
   return a;
 }
 
-int test_fused(const dawn_fused_case& c, Owned& own, cudaStream_t st) {
+int test_fused(const dawn_fused_case& c, DeviceArena& arena, cudaStream_t st) {
   switch (c.kernel) {
     case DAWN_FUSED_TEMPORAL:
     case DAWN_FUSED_TEMPORAL_MMA_SYNC: {
@@ -53,8 +48,8 @@ int test_fused(const dawn_fused_case& c, Owned& own, cudaStream_t st) {
       temporal_fused_pack(wf.data(), wout.data(), Wq, Wo, &a.inv_wscale, &a.inv_oscale);
       uint16_t *dq, *dwo;
       float* wsum;
-      DAWN_TRY(dev_upload(own.v, Wq, &dq)); DAWN_TRY(dev_upload(own.v, Wo, &dwo));
-      DAWN_TRY(dev_upload(own.v, row_sums(wf, 768, 64), &wsum));
+      DAWN_TRY(arena.upload(Wq, &dq)); DAWN_TRY(arena.upload(Wo, &dwo));
+      DAWN_TRY(arena.upload(row_sums(wf, 768, 64), &wsum));
       a.x = c.x; a.ldx = c.ldx; a.res = c.res; a.ldr = c.ldr; a.out = c.out; a.ldo = c.ldo;
       a.F = c.F; a.P = c.P; a.q_lo = c.q_lo; a.q_hi = c.q_hi;
       a.Wqkv = dq; a.Wout = dwo; a.wsum = wsum; a.rot = c.rot; a.bias = c.bias; a.band = c.band;
@@ -91,8 +86,8 @@ int test_fused(const dawn_fused_case& c, Owned& own, cudaStream_t st) {
         sla_fused_pack(wf.data(), W, &a.inv_wscale);
         uint16_t* dw;
         float *dwt, *part;
-        DAWN_TRY(dev_upload(own.v, W, &dw)); DAWN_TRY(dev_upload(own.v, wt, &dwt));
-        DAWN_TRY(dev_alloc(own.v, sla_fused_part_floats(c.F, c.P), &part));
+        DAWN_TRY(arena.upload(W, &dw)); DAWN_TRY(arena.upload(wt, &dwt));
+        DAWN_TRY(arena.alloc(sla_fused_part_floats(c.F, c.P), &part));
         a.x = c.x; a.ldx = c.ldx; a.F = c.F; a.P = c.P; a.Wkv = dw; a.part = part;
         return launch_sla_ctx_fused(a, dwt, c.Bf, c.ldb, st);
       }
@@ -100,7 +95,7 @@ int test_fused(const dawn_fused_case& c, Owned& own, cudaStream_t st) {
       SlaOutArgs o{};
       sla_out_pack(wf.data(), W, &o.inv_wscale);
       uint16_t* dw;
-      DAWN_TRY(dev_upload(own.v, W, &dw));
+      DAWN_TRY(arena.upload(W, &dw));
       o.x = c.x; o.ldx = c.ldx; o.out = c.out; o.ldo = c.ldo; o.F = c.F; o.P = c.P; o.Wq = dw;
       o.Bf = c.Bf; o.ldb = c.ldb; o.bias = c.out_bias;
       return launch_sla_out_fused(o, st);
@@ -113,7 +108,7 @@ int test_fused(const dawn_fused_case& c, Owned& own, cudaStream_t st) {
       for (int ch = 0; ch < c.C; ++ch)
         for (int k = 0; k < 256; ++k) wt[(size_t)k * c.C + ch] = wout[(size_t)ch * 256 + k];
       float* dwt;
-      DAWN_TRY(dev_upload(own.v, wt, &dwt));
+      DAWN_TRY(arena.upload(wt, &dwt));
       return launch_sla_context(c.qkv, c.ld, c.F, c.P, dwt, c.C, c.Bf, c.ldb, st);
     }
     case DAWN_FUSED_CA_WT: {
@@ -130,7 +125,7 @@ int test_fused(const dawn_fused_case& c, Owned& own, cudaStream_t st) {
       std::vector<uint16_t> W;
       ca_fused_pack(wq.data(), c.C, W, &a.inv_wscale);
       uint16_t* dw;
-      DAWN_TRY(dev_upload(own.v, W, &dw));
+      DAWN_TRY(arena.upload(W, &dw));
       a.x = c.x; a.ldx = c.ldx; a.F = c.F; a.P = c.P; a.Wq = dw; a.kq = c.kq; a.nkq = c.nkq; a.G = c.G; a.Wt = c.Wt;
       return launch_ca_fused(a, c.C, st);
     }
@@ -162,8 +157,8 @@ int test_fused(const dawn_fused_case& c, Owned& own, cudaStream_t st) {
 extern "C" int dawn_test_fused(const dawn_fused_case* c, void* stream) {
   if (!c) return dawn::refuse("null case");
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  dawn::Owned own;
-  const int rc = dawn::test_fused(*c, own, st);
+  dawn::DeviceArena arena;
+  const int rc = dawn::test_fused(*c, arena, st);
   if (rc != 0) return rc;
   DAWN_CUDA_OK(cudaStreamSynchronize(st));
   return 0;

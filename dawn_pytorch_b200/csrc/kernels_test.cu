@@ -19,25 +19,11 @@ int refuse(const char* why) {
   return -1;
 }
 
-struct Owned {
-  std::vector<void*> v;
-  ~Owned() { free_all(v); }
-};
-
 // a row stride the float4 kernels can take
 bool row_ok(int ld, int C) { return C >= 4 && (C & 3) == 0 && ld >= C && (ld & 3) == 0; }
 bool clips_ok(int clips) { return clips >= 1 && clips <= kMaxClips; }
 
-template <class T>
-int upload_descs(Owned& own, const std::vector<T>& h, const T** out) {
-  float* d;
-  DAWN_TRY(dev_alloc(own.v, (h.size() * sizeof(T) + sizeof(float) - 1) / sizeof(float), &d));
-  DAWN_CUDA_OK(cudaMemcpy(d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice));
-  *out = reinterpret_cast<const T*>(d);
-  return 0;
-}
-
-int cond_tables(const dawn_kernel_case& c, Owned& own, cudaStream_t st) {
+int cond_tables(const dawn_kernel_case& c, DeviceArena& arena, cudaStream_t st) {
   if (!c.x) return refuse("missing pointer");
   if (c.ndesc < 1 || c.ndesc > DAWN_KERNEL_MAX_DESC || c.F < 1 || !clips_ok(c.clips) || c.F % c.clips) return refuse("bad geometry");
   std::vector<CondDesc> cd;
@@ -58,12 +44,12 @@ int cond_tables(const dawn_kernel_case& c, Owned& own, cudaStream_t st) {
   // every stage's dynamic shared memory must fit the opt-in limit of one block
   if ((size_t)8 * std::max(max_k, max_n1) * sizeof(float) > 227 * 1024 || (size_t)9 * max_co * sizeof(float) > 227 * 1024)
     return refuse("tables too wide for shared memory");
-  const CondDesc* dd;
-  DAWN_TRY(upload_descs(own, cd, &dd));
+  CondDesc* dd;
+  DAWN_TRY(arena.upload(cd, &dd));
   return launch_cond_batched(c.x, c.cond_ld, dd, c.ndesc, max_n1, max_k, max_co, c.F, c.clips, st);
 }
 
-int film(const dawn_kernel_case& c, Owned& own, cudaStream_t st) {
+int film(const dawn_kernel_case& c, DeviceArena& arena, cudaStream_t st) {
   if (!c.x) return refuse("missing pointer");
   if (c.ndesc < 1 || c.ndesc > DAWN_KERNEL_MAX_DESC || c.C < 1 || !clips_ok(c.clips)) return refuse("bad geometry");
   std::vector<FilmDesc> fd;
@@ -75,8 +61,8 @@ int film(const dawn_kernel_case& c, Owned& own, cudaStream_t st) {
     fd.push_back(FilmDesc{e.W, e.b, e.out, e.n});
     max_n = std::max(max_n, e.n);
   }
-  const FilmDesc* dd;
-  DAWN_TRY(upload_descs(own, fd, &dd));
+  FilmDesc* dd;
+  DAWN_TRY(arena.upload(fd, &dd));
   return launch_film(dd, c.ndesc, max_n, c.clips, c.x, c.C, st);
 }
 
@@ -114,7 +100,7 @@ int sampler_step(const dawn_kernel_case& c, cudaStream_t st) {
                         c.scratch, st, red);
 }
 
-int test_kernel(const dawn_kernel_case& c, Owned& own, cudaStream_t st) {
+int test_kernel(const dawn_kernel_case& c, DeviceArena& arena, cudaStream_t st) {
   switch (c.kernel) {
     case DAWN_KERNEL_ROWSTATS:
       if (!c.x || !c.out) return refuse("missing pointer");
@@ -129,7 +115,7 @@ int test_kernel(const dawn_kernel_case& c, Owned& own, cudaStream_t st) {
       return launch_gn_apply(c.y, c.ldy, c.C, c.M, c.stats, c.count, c.cpg, c.P, c.clips, c.w, c.b, nullptr, c.res, c.ldr, c.out,
                              c.ldo, st);
     case DAWN_KERNEL_COND_TABLES:
-      return cond_tables(c, own, st);
+      return cond_tables(c, arena, st);
     case DAWN_KERNEL_TIME_MLP:
       if (!c.t || !c.freqs || !c.w || !c.b || !c.w2 || !c.b2 || !c.out) return refuse("missing pointer");
       if (c.dim < 2 || (c.dim & 1) || (size_t)5 * c.dim * sizeof(float) > 48 * 1024 || !clips_ok(c.clips) ||
@@ -137,7 +123,7 @@ int test_kernel(const dawn_kernel_case& c, Owned& own, cudaStream_t st) {
         return refuse("bad geometry");
       return launch_time_mlp(c.t, c.t_stride, c.clips, c.freqs, c.dim, c.w, c.b, c.w2, c.b2, c.out, st);
     case DAWN_KERNEL_FILM:
-      return film(c, own, st);
+      return film(c, arena, st);
     case DAWN_KERNEL_ROTARY:
       if (!c.freqs || !c.out) return refuse("missing pointer");
       if (c.F < 1 || c.pos0 < 0 || c.F > (1 << 20)) return refuse("bad geometry");
@@ -192,8 +178,8 @@ int test_kernel(const dawn_kernel_case& c, Owned& own, cudaStream_t st) {
 extern "C" int dawn_test_kernel(const dawn_kernel_case* c, void* stream) {
   if (!c) return dawn::refuse("null case");
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  dawn::Owned own;
-  const int rc = dawn::test_kernel(*c, own, st);
+  dawn::DeviceArena arena;
+  const int rc = dawn::test_kernel(*c, arena, st);
   if (rc != 0) return rc;
   DAWN_CUDA_OK(cudaStreamSynchronize(st));
   return 0;

@@ -30,8 +30,8 @@ struct dawn_lfg {
   std::vector<int> C;                          // channels per level 0..n
   HostParams raw{{}, "lfg: "};
   bool committed = false;
-  std::vector<void*> owned, ws_owned;
-  int64_t ws_bytes = 0, launches = 0;
+  DeviceArena weights, workspace;
+  int64_t launches = 0;
   // packed weights
   PackedWeight first;
   std::vector<PackedWeight> down;
@@ -156,9 +156,6 @@ int dawn_lfg_create(const dawn_lfg_cfg* cfg, dawn_lfg** out) {
 }
 
 void dawn_lfg_destroy(dawn_lfg* h) {
-  if (!h) return;
-  free_all(h->owned);
-  free_all(h->ws_owned);
   delete h;
 }
 
@@ -175,34 +172,34 @@ int dawn_lfg_set_param(dawn_lfg* h, const char* name, const float* host, const i
 
 int dawn_lfg_commit_params(dawn_lfg* h) {
   DAWN_CHECK(h, "null handle");
-  free_all(h->owned);
+  h->weights.release();
   h->down.clear(); h->res.clear(); h->up.clear();
   const int n = h->n;
   const HostParams& raw = h->raw;
-  auto& own = h->owned;
-  DAWN_TRY(pack_lfg_conv(raw, own, {{"first.conv", h->C[0]}}, "first.norm", h->cfg.num_channels, 7, 32, &h->first));    // generator.py:36
+  auto& arena = h->weights;
+  DAWN_TRY(pack_lfg_conv(raw, arena, {{"first.conv", h->C[0]}}, "first.norm", h->cfg.num_channels, 7, 32, &h->first));    // generator.py:36
   for (int i = 0; i < n; ++i) {
     PackedWeight d;
     const std::string p = "down_blocks." + std::to_string(i);
-    DAWN_TRY(pack_lfg_conv(raw, own, {{p + ".conv", h->C[i + 1]}}, p + ".norm", h->C[i], 3, h->C[i], &d));                 // :38-44
+    DAWN_TRY(pack_lfg_conv(raw, arena, {{p + ".conv", h->C[i + 1]}}, p + ".norm", h->C[i], 3, h->C[i], &d));                 // :38-44
     h->down.push_back(d);
   }
   const int Cb = h->C[n];
   for (int r = 0; r < h->cfg.num_bottleneck_blocks; ++r) {
     ResPack rp;
     const std::string p = "bottleneck.r" + std::to_string(r);
-    DAWN_TRY(pack_lfg_conv(raw, own, {{p + ".conv1", Cb}}, p + ".norm2", Cb, 3, Cb, &rp.c1));   // util.py:88-89: conv1 -> norm2 folded
-    DAWN_TRY(pack_lfg_conv(raw, own, {{p + ".conv2", Cb}}, "", Cb, 3, Cb, &rp.c2));
+    DAWN_TRY(pack_lfg_conv(raw, arena, {{p + ".conv1", Cb}}, p + ".norm2", Cb, 3, Cb, &rp.c1));   // util.py:88-89: conv1 -> norm2 folded
+    DAWN_TRY(pack_lfg_conv(raw, arena, {{p + ".conv2", Cb}}, "", Cb, 3, Cb, &rp.c2));
     std::vector<double> s, t;
     DAWN_TRY(bn_affine(raw, p + ".norm1", Cb, s, t));
     std::vector<float> sf(s.begin(), s.end()), tf(t.begin(), t.end());
-    DAWN_TRY(dev_upload(own, sf, &rp.s1));
-    DAWN_TRY(dev_upload(own, tf, &rp.t1));
+    DAWN_TRY(arena.upload(sf, &rp.s1));
+    DAWN_TRY(arena.upload(tf, &rp.t1));
     h->res.push_back(rp);
   }
   for (int i = 0; i < n; ++i) {
     UpConv u;
-    DAWN_TRY(pack_lfg_up(raw, own, "up_blocks." + std::to_string(i), h->C[n - i - 1], h->C[n - i], &u));            // generator.py:46-52
+    DAWN_TRY(pack_lfg_up(raw, arena, "up_blocks." + std::to_string(i), h->C[n - i - 1], h->C[n - i], &u));            // generator.py:46-52
     h->up.push_back(u);
   }
   {
@@ -211,8 +208,8 @@ int dawn_lfg_commit_params(dawn_lfg* h) {
     DAWN_TRY(h->raw.need("final.bias", {3}, &b));
     std::vector<float> bp(4, 0.f);
     for (int o = 0; o < 3; ++o) bp[o] = b->data[o];
-    DAWN_TRY(dev_upload(h->owned, lfg_final_pack(w->data.data(), h->C[0]), &h->final_w));
-    DAWN_TRY(dev_upload(h->owned, bp, &h->final_b));
+    DAWN_TRY(h->weights.upload(lfg_final_pack(w->data.data(), h->C[0]), &h->final_w));
+    DAWN_TRY(h->weights.upload(bp, &h->final_b));
   }
   h->committed = true;
   h->have_source = false;
@@ -226,31 +223,29 @@ int dawn_lfg_set_geometry(dawn_lfg* h, int frames, int H, int W, int flow_h, int
   const int n = h->n, div = 1 << n;
   DAWN_CHECK(H >= div && W >= div && H % div == 0 && W % div == 0, "lfg: image height/width must be divisible by 2^num_down_blocks");
   DAWN_CHECK(flow_h >= 1 && flow_w >= 1, "lfg: bad flow size");
-  free_all(h->ws_owned);
-  h->ws_bytes = 0;
+  h->workspace.release();
   h->F = frames; h->H = H; h->W = W; h->fh = flow_h; h->fw = flow_w;
   h->lH.assign(n + 1, 0); h->lW.assign(n + 1, 0);
   for (int l = 0; l <= n; ++l) { h->lH[l] = H >> l; h->lW[l] = W >> l; }
-  auto& own = h->ws_owned;
-  int64_t* cnt = &h->ws_bytes;
+  auto& ws = h->workspace;
   const size_t P0 = (size_t)H * W;
-  DAWN_TRY(dev_alloc(own, 3 * P0, &h->SRC, cnt));
-  DAWN_TRY(dev_alloc(own, 32 * P0, &h->SRC_HWC, cnt));
+  DAWN_TRY(ws.alloc(3 * P0, &h->SRC));
+  DAWN_TRY(ws.alloc(32 * P0, &h->SRC_HWC));
   size_t tmp = 0;
   for (int l = 0; l < n; ++l) tmp = std::max(tmp, (size_t)h->lH[l] * h->lW[l] * h->C[l + 1]);
-  DAWN_TRY(dev_alloc(own, tmp, &h->TMP, cnt));
+  DAWN_TRY(ws.alloc(tmp, &h->TMP));
   h->SKIP.assign(n + 1, nullptr); h->UP.assign(n + 1, nullptr); h->BL.assign(n + 1, nullptr);
-  for (int l = 0; l <= n; ++l) DAWN_TRY(dev_alloc(own, (size_t)h->lH[l] * h->lW[l] * h->C[l], &h->SKIP[l], cnt));
+  for (int l = 0; l <= n; ++l) DAWN_TRY(ws.alloc((size_t)h->lH[l] * h->lW[l] * h->C[l], &h->SKIP[l]));
   for (int l = 0; l < n; ++l) {
     const size_t e = (size_t)frames * h->lH[l] * h->lW[l] * h->C[l];
-    DAWN_TRY(dev_alloc(own, e, &h->UP[l], cnt));
-    if (h->cfg.skips) DAWN_TRY(dev_alloc(own, e, &h->BL[l], cnt));
+    DAWN_TRY(ws.alloc(e, &h->UP[l]));
+    if (h->cfg.skips) DAWN_TRY(ws.alloc(e, &h->BL[l]));
   }
   const size_t eb = (size_t)frames * h->lH[n] * h->lW[n] * h->C[n];
-  DAWN_TRY(dev_alloc(own, eb, &h->X, cnt));
-  DAWN_TRY(dev_alloc(own, eb, &h->Y, cnt));
-  DAWN_TRY(dev_alloc(own, eb, &h->Z, cnt));
-  { float* m; DAWN_TRY(dev_alloc(own, (size_t)frames * flow_h * flow_w * 4, &m, cnt)); h->MOTION = (float4*)m; }
+  DAWN_TRY(ws.alloc(eb, &h->X));
+  DAWN_TRY(ws.alloc(eb, &h->Y));
+  DAWN_TRY(ws.alloc(eb, &h->Z));
+  DAWN_TRY(ws.alloc((size_t)frames * flow_h * flow_w, &h->MOTION));
   h->have_source = false; h->decoded = false;
   return 0;
 }
@@ -326,6 +321,6 @@ int dawn_conv3x3_s2_relu(const float* x, int Ci, int H, int W, const float* weig
 }
 
 int64_t dawn_lfg_last_launch_count(dawn_lfg* h) { return h ? h->launches : 0; }
-int64_t dawn_lfg_workspace_bytes(dawn_lfg* h) { return h ? h->ws_bytes : 0; }
+int64_t dawn_lfg_workspace_bytes(dawn_lfg* h) { return h ? h->workspace.bytes() : 0; }
 
 }  // extern "C"

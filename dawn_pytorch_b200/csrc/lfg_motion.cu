@@ -46,8 +46,8 @@ struct dawn_lfg_motion {
   dawn_lfg_motion_cfg cfg{};
   HostParams raw{{}, "lfg_motion: "};
   bool committed = false, have_rp = false, have_pw = false, have_bg = false;
-  std::vector<void*> owned, ws_owned;
-  int64_t ws_bytes = 0, launches = 0;
+  DeviceArena weights, workspace;
+  int64_t launches = 0;
   Net rp, bg, pw;
   PackedWeight regions, mask_occ;
   float *rp_aa = nullptr, *pw_aa = nullptr, *fc_w = nullptr, *fc_b = nullptr;
@@ -71,7 +71,7 @@ int pack_net(dawn_lfg_motion* h, Net& net) {
   for (int i = 0; i < net.nb; ++i) {
     const std::string p = net.prefix + ".encoder.down_blocks." + std::to_string(i);
     PackedWeight d;
-    DAWN_TRY(pack_lfg_conv(h->raw, h->owned, {{p + ".conv", net.Ce[i + 1]}}, p + ".norm", net.Ce[i], 3, i == 0 ? net.cpad : net.Ce[i],
+    DAWN_TRY(pack_lfg_conv(h->raw, h->weights, {{p + ".conv", net.Ce[i + 1]}}, p + ".norm", net.Ce[i], 3, i == 0 ? net.cpad : net.Ce[i],
                            &d));
     net.down.push_back(d);
   }
@@ -80,7 +80,7 @@ int pack_net(dawn_lfg_motion* h, Net& net) {
     const int i = net.nb - 1 - j;
     const int ci = (i == net.nb - 1 ? 1 : 2) * net.width(i + 1), co = net.width(i);
     UpConv u;
-    DAWN_TRY(pack_lfg_up(h->raw, h->owned, net.prefix + ".decoder.up_blocks." + std::to_string(j), co, ci, &u));
+    DAWN_TRY(pack_lfg_up(h->raw, h->weights, net.prefix + ".decoder.up_blocks." + std::to_string(j), co, ci, &u));
     net.up.push_back(u);
     net.upco.push_back(co);
   }
@@ -97,7 +97,7 @@ int alloc_net(dawn_lfg_motion* h, Net& net, int H0, int W0) {
     else if (i == 0) ld = round_up(net.width(0) + net.cpad, 64);                    // [up | input, zero padded | zeros]
     else ld = 2 * net.width(i);                                                     // [up | skip]
     net.ld[i] = ld;
-    DAWN_TRY(dev_alloc(h->ws_owned, (size_t)h->F * (H0 >> i) * (W0 >> i) * ld, &net.L[i], &h->ws_bytes));
+    DAWN_TRY(h->workspace.alloc((size_t)h->F * (H0 >> i) * (W0 >> i) * ld, &net.L[i]));
     if (i == 0) DAWN_CUDA_OK(cudaMemset(net.L[0], 0, (size_t)h->F * H0 * W0 * ld * sizeof(float)));
   }
   return 0;
@@ -189,9 +189,6 @@ int dawn_lfg_motion_create(const dawn_lfg_motion_cfg* cfg, dawn_lfg_motion** out
 }
 
 void dawn_lfg_motion_destroy(dawn_lfg_motion* h) {
-  if (!h) return;
-  free_all(h->owned);
-  free_all(h->ws_owned);
   delete h;
 }
 
@@ -209,7 +206,7 @@ int dawn_lfg_motion_set_param(dawn_lfg_motion* h, const char* name, const float*
 
 int dawn_lfg_motion_commit_params(dawn_lfg_motion* h) {
   DAWN_CHECK(h, "null handle");
-  free_all(h->owned);
+  h->weights.release();
   // each module may hold only its own part (RegionPredictor, BGMotionPredictor, the Generator's flow predictor): a part is
   // packed when any of its parameters was set, and its stage refuses to run otherwise
   auto has = [&](const char* prefix) {
@@ -223,19 +220,19 @@ int dawn_lfg_motion_commit_params(dawn_lfg_motion* h) {
   const int R = h->cfg.num_regions;
   if (h->have_rp) {
     DAWN_TRY(pack_net(h, h->rp));
-    DAWN_TRY(pack_lfg_conv(h->raw, h->owned, {{"region_predictor.regions", R}}, "", h->rp.be + h->rp.cin, 7,
+    DAWN_TRY(pack_lfg_conv(h->raw, h->weights, {{"region_predictor.regions", R}}, "", h->rp.be + h->rp.cin, 7,
                            round_up(h->rp.be + h->rp.cpad, 64), &h->regions));                 // region_predictor.py:39-40
     const HostParam* g;
     DAWN_TRY(h->raw.need("region_predictor.down.weight", {3, 1, kAAK, kAAK}, &g));
-    DAWN_TRY(dev_upload(h->owned, g->data, &h->rp_aa));
+    DAWN_TRY(h->weights.upload(g->data, &h->rp_aa));
   }
   if (h->have_pw) {
     DAWN_TRY(pack_net(h, h->pw));
-    DAWN_TRY(pack_lfg_conv(h->raw, h->owned, {{"pixelwise_flow_predictor.mask", R + 1}, {"pixelwise_flow_predictor.occlusion", 1}}, "",
+    DAWN_TRY(pack_lfg_conv(h->raw, h->weights, {{"pixelwise_flow_predictor.mask", R + 1}, {"pixelwise_flow_predictor.occlusion", 1}}, "",
                            h->pw.be + h->pw.cin, 7, round_up(h->pw.be + h->pw.cpad, 64), &h->mask_occ));   // pixelwise_flow_predictor.py:32-37
     const HostParam* g;
     DAWN_TRY(h->raw.need("pixelwise_flow_predictor.down.weight", {3, 1, kAAK, kAAK}, &g));
-    DAWN_TRY(dev_upload(h->owned, g->data, &h->pw_aa));
+    DAWN_TRY(h->weights.upload(g->data, &h->pw_aa));
   }
   h->fc_w = h->fc_b = nullptr;
   if (h->cfg.bg_type == DAWN_LFG_BG_AFFINE && h->have_bg) {
@@ -243,8 +240,8 @@ int dawn_lfg_motion_commit_params(dawn_lfg_motion* h) {
     const HostParam *w, *b;
     DAWN_TRY(h->raw.need("bg_predictor.fc.weight", {6, h->bg.Ce[h->bg.nb]}, &w));
     DAWN_TRY(h->raw.need("bg_predictor.fc.bias", {6}, &b));
-    DAWN_TRY(dev_upload(h->owned, w->data, &h->fc_w));
-    DAWN_TRY(dev_upload(h->owned, b->data, &h->fc_b));
+    DAWN_TRY(h->weights.upload(w->data, &h->fc_w));
+    DAWN_TRY(h->weights.upload(b->data, &h->fc_b));
   }
   h->committed = true;
   h->F = 0;
@@ -257,8 +254,7 @@ int dawn_lfg_motion_set_geometry(dawn_lfg_motion* h, int frames, int H, int W) {
   DAWN_CHECK(frames >= 1 && frames <= 1024, "lfg_motion: frames out of range [1, 1024]");
   DAWN_CHECK(H >= 128 && W >= 128 && H % 128 == 0 && W % 128 == 0, "lfg_motion: H and W must be multiples of 128");
   DAWN_CHECK((long long)frames * H * W * 64 < (1LL << 31), "lfg_motion: frames x H x W too large for one call; use fewer frames per call");
-  free_all(h->ws_owned);
-  h->ws_bytes = 0;
+  h->workspace.release();
   h->F = frames; h->H = H; h->W = W; h->h = H / 4; h->w = W / 4;
   const int hh = h->h, ww = h->w;
   const bool bg_net = h->have_bg && h->cfg.bg_type == DAWN_LFG_BG_AFFINE;
@@ -270,10 +266,10 @@ int dawn_lfg_motion_set_geometry(dawn_lfg_motion* h, int frames, int H, int W) {
     if (net->L.empty()) continue;
     for (int i = 0; i < net->nb; ++i) tmp = std::max(tmp, (size_t)(net->H0 >> i) * (net->W0 >> i) * net->Ce[i + 1]);
   }
-  DAWN_TRY(dev_alloc(h->ws_owned, tmp * frames, &h->TMP, &h->ws_bytes));
-  DAWN_TRY(dev_alloc(h->ws_owned, (size_t)frames * hh * ww * kLdLogits, &h->LOGITS, &h->ws_bytes));
-  DAWN_TRY(dev_alloc(h->ws_owned, (size_t)hh * ww * 4, &h->SRC4, &h->ws_bytes));
-  DAWN_TRY(dev_alloc(h->ws_owned, (size_t)frames * hh * ww * 2 * (h->cfg.num_regions + 1), &h->MOTION, &h->ws_bytes));
+  DAWN_TRY(h->workspace.alloc(tmp * frames, &h->TMP));
+  DAWN_TRY(h->workspace.alloc((size_t)frames * hh * ww * kLdLogits, &h->LOGITS));
+  DAWN_TRY(h->workspace.alloc((size_t)hh * ww * 4, &h->SRC4));
+  DAWN_TRY(h->workspace.alloc((size_t)frames * hh * ww * 2 * (h->cfg.num_regions + 1), &h->MOTION));
   return 0;
 }
 
@@ -343,6 +339,6 @@ int dawn_lfg_motion_read_tap(dawn_lfg_motion* h, const char* name, float* dst, i
 }
 
 int64_t dawn_lfg_motion_last_launch_count(dawn_lfg_motion* h) { return h ? h->launches : 0; }
-int64_t dawn_lfg_motion_workspace_bytes(dawn_lfg_motion* h) { return h ? h->ws_bytes : 0; }
+int64_t dawn_lfg_motion_workspace_bytes(dawn_lfg_motion* h) { return h ? h->workspace.bytes() : 0; }
 
 }  // extern "C"

@@ -21,15 +21,10 @@ int refuse(const char* entry, const char* why) {
   return -1;
 }
 
-struct Owned {
-  std::vector<void*> v;
-  ~Owned() { free_all(v); }
-};
-
 // a channels-last row stride the float4 kernels can take
 bool row_ok(int ld, int C) { return C >= 4 && (C & 3) == 0 && ld >= C && (ld & 3) == 0; }
 
-int test_kernel(const dawn_lfg_kernel_case& c, Owned& own, cudaStream_t st) {
+int test_kernel(const dawn_lfg_kernel_case& c, DeviceArena& arena, cudaStream_t st) {
   const float4* motion = reinterpret_cast<const float4*>(c.motion);
   switch (c.kernel) {
     case DAWN_LFG_MOTION_PACK:
@@ -69,7 +64,7 @@ int test_kernel(const dawn_lfg_kernel_case& c, Owned& own, cudaStream_t st) {
       std::vector<float> w((size_t)3 * c.C * 49);
       DAWN_CUDA_OK(cudaMemcpy(w.data(), c.weight, w.size() * sizeof(float), cudaMemcpyDeviceToHost));
       float* wp;
-      DAWN_TRY(dev_upload(own.v, lfg_final_pack(w.data(), c.C), &wp));
+      DAWN_TRY(arena.upload(lfg_final_pack(w.data(), c.C), &wp));
       return launch_lfg_final(c.x, c.ldx, c.C, c.F, c.H, c.W, wp, c.bias, c.source, motion, c.h, c.w, c.blend, c.out, c.out2, st);
     }
   }
@@ -119,8 +114,8 @@ int synchronize(int rc, cudaStream_t st) {
 extern "C" int dawn_lfg_test_kernel(const dawn_lfg_kernel_case* c, void* stream) {
   if (!c) return dawn::refuse(dawn::kLfg, "null case");
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  dawn::Owned own;
-  return dawn::synchronize(dawn::test_kernel(*c, own, st), st);
+  dawn::DeviceArena arena;
+  return dawn::synchronize(dawn::test_kernel(*c, arena, st), st);
 }
 
 extern "C" int dawn_lfg_motion_test_kernel(const dawn_lfg_motion_kernel_case* c, void* stream) {

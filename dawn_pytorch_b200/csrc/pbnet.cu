@@ -9,7 +9,6 @@
 // self-attention then average identical value rows with softmax weights that sum to 1, so their result is that same row: it is
 // evaluated once per commit on the host (fp64) and the first layer starts at its cross-attention.
 #include <algorithm>
-#include <atomic>
 #include <cmath>
 #include <initializer_list>
 #include <string>
@@ -26,8 +25,6 @@ using namespace dawn;
 
 namespace {
 
-std::atomic<int64_t> g_live_bytes{0};
-
 struct LayerPack {
   float *w_qkv = nullptr, *w_out_self = nullptr;          // self-attention (layers >= 1)
   float *w_q = nullptr, *w_out_cross = nullptr;           // cross-attention
@@ -42,8 +39,8 @@ struct dawn_pbnet {
   int D = 0, hid = 0, npairs = 0, nout = 0;
   HostParams raw{{}, "pbnet: "};
   bool committed = false;
-  std::vector<void*> owned, ws_owned;
-  int64_t param_bytes = 0, ws_bytes = 0, launches = 0;
+  DeviceArena weights, workspace;
+  int64_t launches = 0;
   // packed parameters
   PackedWeight aud;                                       // (audio_dim, D): audioEmbedding folded through ztimelinear
   float *wz = nullptr, *wp = nullptr;                     // ztimelinear's z slice (Lz, D); first-pose slice folded (pose_dim, D)
@@ -59,20 +56,6 @@ struct dawn_pbnet {
 
 namespace {
 
-void release(std::vector<void*>& v, int64_t& bytes) {
-  free_all(v);
-  g_live_bytes -= bytes;
-  bytes = 0;
-}
-
-int upload(dawn_pbnet* h, const std::vector<float>& v, float** out) {
-  DAWN_TRY(dev_upload(h->owned, v, out));
-  const int64_t b = (int64_t)std::max<size_t>(v.size(), 4) * sizeof(float);
-  h->param_bytes += b;
-  g_live_bytes += b;
-  return 0;
-}
-
 // nn.Linear weight (N, K) -> k-major (K, N), optionally into columns [n0, n0 + N) of a (K, ldn) matrix
 void transpose_into(const float* w, int N, int K, std::vector<float>& m, int ldn, int n0) {
   for (int n = 0; n < N; ++n)
@@ -84,13 +67,13 @@ int upload_linear_t(dawn_pbnet* h, const std::string& name, int N, int K, float*
   DAWN_TRY(h->raw.need(name, {N, K}, &w));
   std::vector<float> m((size_t)K * N);
   transpose_into(w->data.data(), N, K, m, N, 0);
-  return upload(h, m, out);
+  return h->weights.upload(m, out);
 }
 
 int upload_vec(dawn_pbnet* h, const std::string& name, const std::vector<int64_t>& shape, float** out) {
   const HostParam* p;
   DAWN_TRY(h->raw.need(name, shape, &p));
-  return upload(h, p->data, out);
+  return h->weights.upload(p->data, out);
 }
 
 // y = W x (+ b), W (N, K) row-major fp32, in fp64
@@ -156,25 +139,23 @@ int frame_invariant_row(const dawn_pbnet* h, std::vector<double>& row) {
 
 int ensure_workspace(dawn_pbnet* h, int T, int F) {
   if (T <= h->cap_T && F <= h->cap_F) return 0;
-  release(h->ws_owned, h->ws_bytes);
+  h->workspace.release();
   const int D = h->D, hid = h->hid, L = h->cfg.num_layers;
   const int cT = std::max(T, h->cap_T), cF = std::max(F, h->cap_F);
-  auto& own = h->ws_owned;
-  int64_t* cnt = &h->ws_bytes;
+  auto& ws = h->workspace;
   auto alloc = [&]() -> int {
-    DAWN_TRY(dev_alloc(own, (size_t)cT * D, &h->AUD, cnt));
-    DAWN_TRY(dev_alloc(own, (size_t)cT * D, &h->MEM, cnt));
-    DAWN_TRY(dev_alloc(own, (size_t)cT * D, &h->X, cnt));
-    DAWN_TRY(dev_alloc(own, (size_t)cT * 2 * hid * L, &h->KV, cnt));
-    DAWN_TRY(dev_alloc(own, (size_t)cT * 3 * hid, &h->QKV, cnt));
-    DAWN_TRY(dev_alloc(own, (size_t)cT * hid, &h->O, cnt));
-    DAWN_TRY(dev_alloc(own, (size_t)cF * h->npairs * 2, &h->ROT, cnt));
+    DAWN_TRY(ws.alloc((size_t)cT * D, &h->AUD));
+    DAWN_TRY(ws.alloc((size_t)cT * D, &h->MEM));
+    DAWN_TRY(ws.alloc((size_t)cT * D, &h->X));
+    DAWN_TRY(ws.alloc((size_t)cT * 2 * hid * L, &h->KV));
+    DAWN_TRY(ws.alloc((size_t)cT * 3 * hid, &h->QKV));
+    DAWN_TRY(ws.alloc((size_t)cT * hid, &h->O));
+    DAWN_TRY(ws.alloc((size_t)cF * h->npairs * 2, &h->ROT));
     return 0;
   };
   const int rc = alloc();
-  g_live_bytes += h->ws_bytes;
   if (rc != 0) {
-    release(h->ws_owned, h->ws_bytes);
+    h->workspace.release();
     h->cap_T = h->cap_F = 0;
     return rc;
   }
@@ -219,9 +200,6 @@ int dawn_pbnet_create(const dawn_pbnet_cfg* cfg, dawn_pbnet** out) {
 }
 
 void dawn_pbnet_destroy(dawn_pbnet* h) {
-  if (!h) return;
-  release(h->owned, h->param_bytes);
-  release(h->ws_owned, h->ws_bytes);
   delete h;
 }
 
@@ -234,7 +212,7 @@ int dawn_pbnet_set_param(dawn_pbnet* h, const char* name, const float* host, con
 
 int dawn_pbnet_commit_params(dawn_pbnet* h) {
   DAWN_CHECK(h, "null handle");
-  release(h->owned, h->param_bytes);
+  h->weights.release();
   h->layers.clear();
   h->committed = false;
   const dawn_pbnet_cfg& c = h->cfg;
@@ -268,9 +246,7 @@ int dawn_pbnet_commit_params(dawn_pbnet* h) {
       for (int j = 0; j < D; ++j) b += zt(n, j) * (double)bfp->data[j];
       bias[n] = (float)b;
     }
-    DAWN_TRY(upload_weight(h->owned, m, K, D, ldb, bias, &h->aud));
-    const int64_t b = (int64_t)(m.size() + (h->aud.img ? (size_t)K * D : 0) + ldb) * sizeof(float);   // w, fp16 hi | lo image, bias
-    h->param_bytes += b; g_live_bytes += b;
+    DAWN_TRY(upload_weight(h->weights, m, K, D, ldb, bias, &h->aud));
     std::vector<float> wz((size_t)A * D), wp((size_t)P * D);
     for (int k = 0; k < A; ++k)
       for (int n = 0; n < D; ++n) wz[(size_t)k * D + n] = wzt->data[(size_t)n * ldz + D + k];
@@ -280,14 +256,14 @@ int dawn_pbnet_commit_params(dawn_pbnet* h) {
         for (int j = 0; j < D; ++j) s += zt(n, j) * (double)wfp->data[(size_t)j * P + p];
         wp[(size_t)p * D + n] = (float)s;
       }
-    DAWN_TRY(upload(h, wz, &h->wz));
-    DAWN_TRY(upload(h, wp, &h->wp));
+    DAWN_TRY(h->weights.upload(wz, &h->wz));
+    DAWN_TRY(h->weights.upload(wp, &h->wp));
   }
   // ---- frame-invariant prefix
   {
     std::vector<double> row;
     DAWN_TRY(frame_invariant_row(h, row));
-    DAWN_TRY(upload(h, std::vector<float>(row.begin(), row.end()), &h->c0));
+    DAWN_TRY(h->weights.upload(std::vector<float>(row.begin(), row.end()), &h->c0));
   }
   // ---- layers
   std::vector<float> kv((size_t)D * 2 * hid * L);
@@ -316,7 +292,7 @@ int dawn_pbnet_commit_params(dawn_pbnet* h) {
     }
     h->layers.push_back(lp);
   }
-  DAWN_TRY(upload(h, kv, &h->w_kv));
+  DAWN_TRY(h->weights.upload(kv, &h->w_kv));
   DAWN_TRY(upload_linear_t(h, "finallayer.weight", P, D, &h->wf));
   DAWN_TRY(upload_vec(h, "finallayer.bias", {P}, &h->bf));
   DAWN_TRY(upload_vec(h, layer_prefix(L - 1) + "multihead_attn.rotary_emb.freqs", {h->npairs}, &h->freqs));
@@ -384,8 +360,7 @@ int dawn_pbnet_generate(dawn_pbnet* h, const float* audio, const float* z, const
 }
 
 int64_t dawn_pbnet_last_launch_count(dawn_pbnet* h) { return h ? h->launches : 0; }
-int64_t dawn_pbnet_workspace_bytes(dawn_pbnet* h) { return h ? h->ws_bytes : 0; }
-int64_t dawn_pbnet_live_bytes(void) { return g_live_bytes.load(); }
+int64_t dawn_pbnet_workspace_bytes(dawn_pbnet* h) { return h ? h->workspace.bytes() : 0; }
 
 int dawn_pbnet_test_attention(const dawn_pbnet_attention_case* c, void* stream) {
   DAWN_CHECK(c && c->x_q && c->x_kv && c->wq && c->wk && c->wv && c->freqs && c->bias && c->out, "pbnet test: missing pointer");
@@ -394,24 +369,19 @@ int dawn_pbnet_test_attention(const dawn_pbnet_attention_case* c, void* stream) 
              "pbnet test: bad geometry");
   cudaStream_t st = (cudaStream_t)stream;
   const int T = c->bs * c->F, hid = 32 * c->H;
-  std::vector<void*> own;
+  DeviceArena arena;
   float *rot, *q, *k, *v;
-  auto run = [&]() -> int {
-    DAWN_TRY(dev_alloc(own, (size_t)c->F * std::max(c->npairs, 1) * 2, &rot));
-    DAWN_TRY(dev_alloc(own, (size_t)T * hid, &q));
-    DAWN_TRY(dev_alloc(own, (size_t)T * hid, &k));
-    DAWN_TRY(dev_alloc(own, (size_t)T * hid, &v));
-    if (c->npairs > 0) DAWN_TRY(launch_rotary_table(c->freqs, c->npairs, c->F, 0, rot, st));
-    DAWN_TRY(launch_pb_proj(c->x_q, c->D, T, c->F, c->D, c->wq, hid, 1, groups_of({PB_SCALE | PB_ROTARY}), c->qscale, rot, c->npairs, q, st));
-    DAWN_TRY(launch_pb_proj(c->x_kv, c->D, T, c->F, c->D, c->wk, hid, 1, groups_of({PB_ROTARY}), 1.f, rot, c->npairs, k, st));
-    DAWN_TRY(launch_pb_proj(c->x_kv, c->D, T, c->F, c->D, c->wv, hid, 1, groups_of({0}), 1.f, rot, c->npairs, v, st));
-    DAWN_TRY(launch_pb_attention(q, hid, k, hid, v, hid, c->bias, c->band, c->bs, c->F, c->H, c->out, st));
-    DAWN_CUDA_OK(cudaStreamSynchronize(st));
-    return 0;
-  };
-  const int rc = run();
-  free_all(own);
-  return rc;
+  DAWN_TRY(arena.alloc((size_t)c->F * std::max(c->npairs, 1) * 2, &rot));
+  DAWN_TRY(arena.alloc((size_t)T * hid, &q));
+  DAWN_TRY(arena.alloc((size_t)T * hid, &k));
+  DAWN_TRY(arena.alloc((size_t)T * hid, &v));
+  if (c->npairs > 0) DAWN_TRY(launch_rotary_table(c->freqs, c->npairs, c->F, 0, rot, st));
+  DAWN_TRY(launch_pb_proj(c->x_q, c->D, T, c->F, c->D, c->wq, hid, 1, groups_of({PB_SCALE | PB_ROTARY}), c->qscale, rot, c->npairs, q, st));
+  DAWN_TRY(launch_pb_proj(c->x_kv, c->D, T, c->F, c->D, c->wk, hid, 1, groups_of({PB_ROTARY}), 1.f, rot, c->npairs, k, st));
+  DAWN_TRY(launch_pb_proj(c->x_kv, c->D, T, c->F, c->D, c->wv, hid, 1, groups_of({0}), 1.f, rot, c->npairs, v, st));
+  DAWN_TRY(launch_pb_attention(q, hid, k, hid, v, hid, c->bias, c->band, c->bs, c->F, c->H, c->out, st));
+  DAWN_CUDA_OK(cudaStreamSynchronize(st));
+  return 0;
 }
 
 }  // extern "C"

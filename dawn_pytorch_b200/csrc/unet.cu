@@ -170,9 +170,8 @@ struct dawn_unet {
   bool committed = false;
 
   // packed weights
-  std::vector<void*> owned;                    // weight allocations
-  std::vector<void*> ws_owned;                 // workspace allocations
-  int64_t ws_bytes = 0;
+  DeviceArena weights;                         // freed by commit_params
+  DeviceArena workspace;                       // freed by set_geometry
   PackedWeight init_full;                      // 7x7 over channels padded to cin_pad
   float* init_w3 = nullptr;                    // [k*k*3][dim] for the 3 noisy channels
   int cin_pad = 0;
@@ -211,6 +210,7 @@ struct dawn_unet {
   float* XE = nullptr;                         // (halo_l + F + halo_r) frames of a temporal layer's input, dense
   // GroupNorm all-reduce over NVLink peer memory (one kernel: every rank stores its 16 partial sums into every peer's mailbox, then
   // sums the mailboxes in rank order); set up by dawn_unet_shard_ipc_export / _import, otherwise ncclAllReduce is used
+  DeviceArena mailbox;                         // p2p_own and p2p_ctr: live as long as the handle, through commits and geometries
   P2pMail* p2p_own = nullptr;                  // this rank's mailbox (cudaMalloc, exported through cudaIpc)
   P2pMail* p2p_peer[kP2pMaxRanks] = {nullptr}; // every rank's mailbox as mapped into this process ([rank] == own)
   unsigned int* p2p_ctr = nullptr;             // device-side sequence number (graph replays keep counting)
@@ -249,7 +249,7 @@ int pack_conv(dawn_unet* h, const std::string& prefix, int co, int ci, int kh, i
   const int K = kh * kw * ci_pad;
   std::vector<float> m((size_t)K * ldb, 0.f);
   pack_conv_taps(w->data.data(), co, ci, kh * kw, ci_pad, ldb, 0, nullptr, m);
-  return upload_weight(h->owned, m, K, co, ldb, b ? b->data : std::vector<float>{}, out);
+  return upload_weight(h->weights, m, K, co, ldb, b ? b->data : std::vector<float>{}, out);
 }
 
 // Linear weight (N, K) [+ optional per-input gain, + per-output-row scale for the first `nscale` rows]
@@ -262,15 +262,15 @@ int pack_linear(dawn_unet* h, const HostParam* w, int N, int K, const float* gai
   for (int n = 0; n < N; ++n)
     for (int k = 0; k < K; ++k) m[(size_t)k * ldb + n] = f[(size_t)n * K + k];
   s.resize(ldb, 0.f);
-  DAWN_TRY(upload_weight(h->owned, m, K, N, ldb, {}, out));
-  if (wsum) DAWN_TRY(dev_upload(h->owned, s, wsum));
+  DAWN_TRY(upload_weight(h->weights, m, K, N, ldb, {}, out));
+  if (wsum) DAWN_TRY(h->weights.upload(s, wsum));
   return 0;
 }
 
 int upload_raw(dawn_unet* h, const std::string& name, std::vector<int64_t> shape, float** out) {
   const HostParam* p;
   DAWN_TRY(h->raw.need(name, shape, &p));
-  return dev_upload(h->owned, p->data, out);
+  return h->weights.upload(p->data, out);
 }
 
 int pack_resblock(dawn_unet* h, const std::string& name, int ci, int co, bool cond, int* stat_counter) {
@@ -312,12 +312,12 @@ int pack_resblock(dawn_unet* h, const std::string& name, int ci, int co, bool co
     }
     std::vector<float> wq, wsum;
     fold_ca_q(to_q, gain, ci, wq, wsum);
-    DAWN_TRY(upload_weight(h->owned, wq, ci, 192, 192, {}, &r.wq));
-    DAWN_TRY(dev_upload(h->owned, wsum, &r.wsumq));
+    DAWN_TRY(upload_weight(h->weights, wq, ci, 192, 192, {}, &r.wq));
+    DAWN_TRY(h->weights.upload(wsum, &r.wsumq));
     if (ci == 64 || ci == 128) {
       std::vector<uint16_t> W;
       ca_fused_pack(wq.data(), ci, W, &r.f_inv_wscale);
-      DAWN_TRY(dev_upload(h->owned, W, &r.fWq));
+      DAWN_TRY(h->weights.upload(W, &r.fWq));
     }
   }
   h->rb_index[name] = (int)h->rb.size();
@@ -338,8 +338,8 @@ int pack_attn(dawn_unet* h, const std::string& norm_name, const std::string& fn,
     const std::vector<float> wq = fold_linear(qkv->data.data(), 768, C, g->data.data(), scale, 256);
     std::vector<uint16_t> Wq, Wo;
     temporal_fused_pack(wq.data(), o->data.data(), Wq, Wo, &a->f_inv_wscale, &a->f_inv_oscale);
-    DAWN_TRY(dev_upload(h->owned, Wq, &a->fq));
-    DAWN_TRY(dev_upload(h->owned, Wo, &a->fo));
+    DAWN_TRY(h->weights.upload(Wq, &a->fq));
+    DAWN_TRY(h->weights.upload(Wo, &a->fo));
   }
   return 0;
 }
@@ -356,17 +356,17 @@ int pack_sla(dawn_unet* h, const std::string& p, int C, SlaW* s) {        // p =
     const std::vector<float> wf = fold_linear(qkv->data.data(), 768, C, g->data.data(), 1.f, 0);
     std::vector<uint16_t> W;
     sla_fused_pack(wf.data(), W, &s->f_inv_wscale);
-    DAWN_TRY(dev_upload(h->owned, W, &s->fkv));
+    DAWN_TRY(h->weights.upload(W, &s->fkv));
     sla_out_pack(wf.data(), W, &s->fq_inv_wscale);
-    DAWN_TRY(dev_upload(h->owned, W, &s->fq));
+    DAWN_TRY(h->weights.upload(W, &s->fq));
   }
   std::vector<float> wt((size_t)256 * C);
   for (int c = 0; c < C; ++c)
     for (int k = 0; k < 256; ++k) wt[(size_t)k * C + c] = o->data[(size_t)c * 256 + k];
-  DAWN_TRY(dev_upload(h->owned, wt, &s->WoutT));
+  DAWN_TRY(h->weights.upload(wt, &s->WoutT));
   std::vector<float> bb(round_up(C, 64), 0.f);
   std::copy(b->data.begin(), b->data.end(), bb.begin());
-  DAWN_TRY(dev_upload(h->owned, bb, &s->bout));
+  DAWN_TRY(h->weights.upload(bb, &s->bout));
   return 0;
 }
 
@@ -378,7 +378,7 @@ int pack_up(dawn_unet* h, const std::string& name, int C, UpConv* u) {
   const HostParam *w, *b;
   DAWN_TRY(h->raw.need(name + ".weight", {C, C, 1, 4, 4}, &w));
   DAWN_TRY(h->raw.need(name + ".bias", {C}, &b));
-  return dawn::pack_up(h->owned, C, C, kUpD, b->data, [&](int py, int px, int ty, int tx, int c, int n) {
+  return dawn::pack_up(h->weights, C, C, kUpD, b->data, [&](int py, int px, int ty, int tx, int c, int n) {
     return w->data[(((size_t)c * C + n) * 4 + kUpK[py][ty]) * 4 + kUpK[px][tx]];
   }, u);
 }
@@ -389,7 +389,7 @@ int pack_upconv(dawn_unet* h, const std::string& name, int C, UpConv* u) {
   const HostParam *w, *b;
   DAWN_TRY(h->raw.need(name + ".1.weight", {C, C, 1, 3, 3}, &w));
   DAWN_TRY(h->raw.need(name + ".1.bias", {C}, &b));
-  return pack_up_nearest(h->owned, w->data.data(), C, C, nullptr, b->data, u);
+  return pack_up_nearest(h->weights, w->data.data(), C, C, nullptr, b->data, u);
 }
 
 // ------------------------------------------------------------------------------------------ GEMM wrappers
@@ -917,6 +917,7 @@ int forward_core(dawn_unet* h, const int64_t* t_dev, int t_stride, float* out, c
 extern "C" {
 
 const char* dawn_last_error(void) { return g_last_error.c_str(); }
+int64_t dawn_live_bytes(void) { return dawn::DeviceArena::live_bytes(); }
 const char* dawn_build_info(void) { return "dawn_unet sm_90a; contractions: wgmma m64n64k16 FP16x3 (register accumulators, RN fp32 drains) + mma.sync m16n8k16 FP16x3 fused attention kernels; fallback mma.sync 3xTF32"; }
 
 // The kernel launchers cache per-function attributes (dynamic shared-memory opt-in, SM count) in process-wide statics: the
@@ -981,9 +982,7 @@ void dawn_unet_destroy(dawn_unet* h) {
   if (h->sh_comm && g_nccl.ok) g_nccl.CommDestroy(h->sh_comm);
   for (int r = 0; r < kP2pMaxRanks; ++r)
     if (h->p2p_peer[r] && h->p2p_peer[r] != h->p2p_own) cudaIpcCloseMemHandle(h->p2p_peer[r]);
-  free_all(h->owned);
-  free_all(h->ws_owned);
-  delete h;
+  delete h;                                    // the arenas free their memory last, after the IPC mappings of it are closed
 }
 
 int dawn_unet_set_param(dawn_unet* h, const char* name, const float* host, const int64_t* shape, int ndim) {
@@ -996,7 +995,7 @@ int dawn_unet_set_param(dawn_unet* h, const char* name, const float* host, const
 int dawn_unet_commit_params(dawn_unet* h) {
   DAWN_CHECK(h, "null handle");
   drop_graphs(h);
-  free_all(h->owned);
+  h->weights.release();
   h->rb.clear(); h->rb_index.clear();
   h->down_ta.clear(); h->up_ta.clear(); h->down_sla.clear(); h->up_sla.clear(); h->down_conv.clear(); h->up_conv.clear();
   const auto& cfg = h->cfg;
@@ -1010,7 +1009,7 @@ int dawn_unet_commit_params(dawn_unet* h) {
     for (int t = 0; t < k * k; ++t)
       for (int c = 0; c < 3; ++c)
         for (int n = 0; n < dim; ++n) w3[((size_t)t * 3 + c) * dim + n] = w->data[((size_t)n * cfg.channels + c) * k * k + t];
-    DAWN_TRY(dev_upload(h->owned, w3, &h->init_w3));
+    DAWN_TRY(h->weights.upload(w3, &h->init_w3));
   }
   DAWN_TRY(upload_raw(h, "aux.time_freqs", {dim / 2}, &h->time_freqs));
   DAWN_TRY(upload_raw(h, "aux.rel_bias", {8, 2 * cfg.win_width + 1}, &h->rel_bias));
@@ -1079,33 +1078,31 @@ int dawn_unet_set_geometry(dawn_unet* h, int B, int F, int height, int width) {
   const int div = 1 << (nlev - 1);
   DAWN_CHECK(height % div == 0 && width % div == 0 && height >= div && width >= div,
              "latent height/width must be divisible by 2^(levels-1)");
-  free_all(h->ws_owned);
-  h->ws_bytes = 0;
+  h->workspace.release();
   h->have_invariants = false;
   h->B = B; h->F = F; h->H = height; h->W = width;
   h->lH.assign(nlev, 0); h->lW.assign(nlev, 0);
   for (int l = 0; l < nlev; ++l) { h->lH[l] = height >> l; h->lW[l] = width >> l; }
-  auto& own = h->ws_owned;
+  auto& ws = h->workspace;
   const int NF = B * F;                                              // frames of all clips
   const size_t P0 = (size_t)height * width, M0 = (size_t)NF * P0;
-  int64_t* cnt = &h->ws_bytes;
-  DAWN_TRY(dev_alloc(own, M0 * h->cin_pad, &h->X288, cnt));
-  DAWN_TRY(dev_alloc(own, B * P0 * h->cin_pad * h->cfg.init_kernel_size, &h->FEA288, cnt));   // k row-shifted copies per clip
-  DAWN_TRY(dev_alloc(own, B * P0 * dim * h->cfg.init_kernel_size, &h->MAPPART, cnt));
-  { float* f; DAWN_TRY(dev_alloc(own, B + 4, &f, cnt)); h->VARY = (int*)f; }
-  DAWN_TRY(dev_alloc(own, B * P0 * dim, &h->MAP, cnt));
-  DAWN_TRY(dev_alloc(own, M0 * 2 * dim, &h->XR, cnt));
-  DAWN_TRY(dev_alloc(own, M0 * dim, &h->S0, cnt));
+  DAWN_TRY(ws.alloc(M0 * h->cin_pad, &h->X288));
+  DAWN_TRY(ws.alloc(B * P0 * h->cin_pad * h->cfg.init_kernel_size, &h->FEA288));   // k row-shifted copies per clip
+  DAWN_TRY(ws.alloc(B * P0 * dim * h->cfg.init_kernel_size, &h->MAPPART));
+  DAWN_TRY(ws.alloc(B + 4, &h->VARY));
+  DAWN_TRY(ws.alloc(B * P0 * dim, &h->MAP));
+  DAWN_TRY(ws.alloc(M0 * 2 * dim, &h->XR));
+  DAWN_TRY(ws.alloc(M0 * dim, &h->S0));
   h->bufA.assign(nlev, nullptr); h->bufB.assign(nlev, nullptr); h->CAT.assign(nlev, nullptr); h->DS.assign(nlev, nullptr);
   size_t max_mc = 0, max_bf = 0, max_pc = P0 * dim;                 // max_pc: pixels x channels of the widest temporal layer
   for (int l = 0; l < nlev; ++l) {
     const size_t Ml = (size_t)NF * h->lH[l] * h->lW[l];
     const int ci = h->in_out[l].first, co = h->in_out[l].second;
     const int cw = std::max(ci, co);                                   // down blocks run at co channels, up blocks at ci
-    DAWN_TRY(dev_alloc(own, Ml * cw, &h->bufA[l], cnt));
-    DAWN_TRY(dev_alloc(own, Ml * cw, &h->bufB[l], cnt));
-    DAWN_TRY(dev_alloc(own, Ml * 2 * co, &h->CAT[l], cnt));
-    if (l > 0) DAWN_TRY(dev_alloc(own, Ml * ci, &h->DS[l], cnt));
+    DAWN_TRY(ws.alloc(Ml * cw, &h->bufA[l]));
+    DAWN_TRY(ws.alloc(Ml * cw, &h->bufB[l]));
+    DAWN_TRY(ws.alloc(Ml * 2 * co, &h->CAT[l]));
+    if (l > 0) DAWN_TRY(ws.alloc(Ml * ci, &h->DS[l]));
     max_mc = std::max(max_mc, Ml * cw);
     max_bf = std::max(max_bf, (size_t)NF * 256 * round_up(cw, 64));
     max_pc = std::max(max_pc, (size_t)h->lH[l] * h->lW[l] * cw);
@@ -1113,48 +1110,45 @@ int dawn_unet_set_geometry(dawn_unet* h, int B, int F, int height, int width) {
   if (h->cfg.pad_mode != 0) {                                         // bordered inputs of the up path's upconvs (levels >= 1)
     size_t n = 0;
     for (int l = 1; l < nlev; ++l) n = std::max(n, (size_t)NF * (h->lH[l] + 2) * (h->lW[l] + 2) * h->in_out[l].first);
-    DAWN_TRY(dev_alloc(own, n, &h->UPPAD, cnt));
+    DAWN_TRY(ws.alloc(n, &h->UPPAD));
   }
   max_mc = std::max(max_mc, M0 * dim);
-  DAWN_TRY(dev_alloc(own, max_mc, &h->Y, cnt));
-  DAWN_TRY(dev_alloc(own, max_mc, &h->A1, cnt));
+  DAWN_TRY(ws.alloc(max_mc, &h->Y));
+  DAWN_TRY(ws.alloc(max_mc, &h->A1));
   const size_t Mext = (size_t)(NF + 2 * h->cfg.win_width) * P0;     // rows incl. temporal halos of a sharded clip
-  DAWN_TRY(dev_alloc(own, Mext * 768, &h->QKV, cnt));
-  DAWN_TRY(dev_alloc(own, Mext * 256, &h->O, cnt));
-  DAWN_TRY(dev_alloc(own, Mext * 2, &h->ROWSTATS, cnt));
-  DAWN_TRY(dev_alloc(own, (size_t)(NF + 2 * h->cfg.win_width) * max_pc, &h->XE, cnt));
-  DAWN_TRY(dev_alloc(own, M0 * 24, &h->GATES, cnt));
-  DAWN_TRY(dev_alloc(own, M0 * 32, &h->WT, cnt));
-  DAWN_TRY(dev_alloc(own, max_bf, &h->BF, cnt));
-  DAWN_TRY(dev_alloc(own, M0 * dim, &h->HF, cnt));
-  DAWN_TRY(dev_alloc(own, M0 * dim, &h->HO, cnt));
-  DAWN_TRY(dev_alloc(own, (size_t)(F + 2 * h->cfg.win_width) * 32, &h->ROT, cnt));
-  DAWN_TRY(dev_alloc(own, (size_t)B * h->tdim, &h->TSILU, cnt));
-  {
-    float* s; DAWN_TRY(dev_alloc(own, (size_t)h->n_stats * 32 * B, &s, cnt)); h->STATS = (double*)s;
-    float* t; DAWN_TRY(dev_alloc(own, 4, &t, cnt)); h->T_HOSTSIDE = (int64_t*)t;
-  }
-  DAWN_TRY(dev_alloc(own, 3 * M0, &h->H_XT, cnt));
-  DAWN_TRY(dev_alloc(own, (size_t)(h->cfg.channels - 3) * P0, &h->H_FEA, cnt));
-  DAWN_TRY(dev_alloc(own, (size_t)F * h->cond_dim, &h->H_COND, cnt));
-  DAWN_TRY(dev_alloc(own, (size_t)(h->cfg.out_grid_dim + h->cfg.out_conf_dim) * M0, &h->H_OUT, cnt));
+  DAWN_TRY(ws.alloc(Mext * 768, &h->QKV));
+  DAWN_TRY(ws.alloc(Mext * 256, &h->O));
+  DAWN_TRY(ws.alloc(Mext * 2, &h->ROWSTATS));
+  DAWN_TRY(ws.alloc((size_t)(NF + 2 * h->cfg.win_width) * max_pc, &h->XE));
+  DAWN_TRY(ws.alloc(M0 * 24, &h->GATES));
+  DAWN_TRY(ws.alloc(M0 * 32, &h->WT));
+  DAWN_TRY(ws.alloc(max_bf, &h->BF));
+  DAWN_TRY(ws.alloc(M0 * dim, &h->HF));
+  DAWN_TRY(ws.alloc(M0 * dim, &h->HO));
+  DAWN_TRY(ws.alloc((size_t)(F + 2 * h->cfg.win_width) * 32, &h->ROT));
+  DAWN_TRY(ws.alloc((size_t)B * h->tdim, &h->TSILU));
+  DAWN_TRY(ws.alloc((size_t)h->n_stats * 16 * B, &h->STATS));
+  DAWN_TRY(ws.alloc(2, &h->T_HOSTSIDE));
+  DAWN_TRY(ws.alloc(3 * M0, &h->H_XT));
+  DAWN_TRY(ws.alloc((size_t)(h->cfg.channels - 3) * P0, &h->H_FEA));
+  DAWN_TRY(ws.alloc((size_t)F * h->cond_dim, &h->H_COND));
+  DAWN_TRY(ws.alloc((size_t)(h->cfg.out_grid_dim + h->cfg.out_conf_dim) * M0, &h->H_OUT));
   // per-block per-clip tables
   std::vector<FilmDesc> descs;
   for (auto& r : h->rb) {
     if (!r.cond) continue;
     r.ldbT = round_up(r.co, 64);
-    DAWN_TRY(dev_alloc(own, (size_t)B * 2 * r.co, &r.film, cnt));
-    DAWN_TRY(dev_alloc(own, (size_t)NF * 3 * 64, &r.kq, cnt));
-    DAWN_TRY(dev_alloc(own, 24, &r.nkq, cnt));
-    DAWN_TRY(dev_alloc(own, (size_t)NF * 32 * r.ldbT, &r.T, cnt));
+    DAWN_TRY(ws.alloc((size_t)B * 2 * r.co, &r.film));
+    DAWN_TRY(ws.alloc((size_t)NF * 3 * 64, &r.kq));
+    DAWN_TRY(ws.alloc(24, &r.nkq));
+    DAWN_TRY(ws.alloc((size_t)NF * 32 * r.ldbT, &r.T));
     DAWN_CUDA_OK(cudaMemset(r.T, 0, (size_t)NF * 32 * r.ldbT * sizeof(float)));
-    DAWN_TRY(dev_alloc(own, (size_t)NF * 3 * 81, &r.G, cnt));
+    DAWN_TRY(ws.alloc((size_t)NF * 3 * 81, &r.G));
     descs.push_back(FilmDesc{r.tW, r.tB, r.film, 2 * r.co});
   }
   {
-    float* d; DAWN_TRY(dev_alloc(own, descs.size() * sizeof(FilmDesc) / sizeof(float) + 4, &d, cnt));
-    DAWN_CUDA_OK(cudaMemcpy(d, descs.data(), descs.size() * sizeof(FilmDesc), cudaMemcpyHostToDevice));
-    h->film_descs = (FilmDesc*)d; h->n_film = (int)descs.size();
+    DAWN_TRY(ws.upload(descs, &h->film_descs));
+    h->n_film = (int)descs.size();
     h->film_max_n = 0;
     for (const auto& fd : descs) h->film_max_n = std::max(h->film_max_n, fd.n);
   }
@@ -1169,17 +1163,16 @@ int dawn_unet_set_geometry(dawn_unet* h, int B, int F, int height, int width) {
       for (int a = 0; a < 3; ++a) {
         CondDesc d{};
         d.mW = r.mW[a]; d.mB = r.mB[a]; d.off = off[a]; d.K = kd[a]; d.n1 = 2 * r.co; d.Wkv = r.ca[a].Wkv;
-        DAWN_TRY(dev_alloc(own, (size_t)NF * d.n1, &d.ctx, cnt));
-        DAWN_TRY(dev_alloc(own, (size_t)NF * 128, &d.kv, cnt));
+        DAWN_TRY(ws.alloc((size_t)NF * d.n1, &d.ctx));
+        DAWN_TRY(ws.alloc((size_t)NF * 128, &d.kv));
         d.t.kv = d.kv; d.t.nkv = r.ca[a].nkv; d.t.qs = r.ca[a].qs; d.t.ks = r.ca[a].ks; d.t.Wout = r.ca[a].Wout; d.t.gout = r.ca[a].gout;
         d.t.co = r.co; d.t.ldbT = r.ldbT; d.t.ca = a; d.t.kq = r.kq; d.t.nkq = r.nkq; d.t.T = r.T; d.t.G = r.G;
         cd.push_back(d);
         h->cond_max_n1 = std::max(h->cond_max_n1, d.n1); h->cond_max_k = std::max(h->cond_max_k, d.K); h->cond_max_co = std::max(h->cond_max_co, r.co);
       }
     }
-    float* d; DAWN_TRY(dev_alloc(own, cd.size() * sizeof(CondDesc) / sizeof(float) + 4, &d, cnt));
-    DAWN_CUDA_OK(cudaMemcpy(d, cd.data(), cd.size() * sizeof(CondDesc), cudaMemcpyHostToDevice));
-    h->cond_descs = (CondDesc*)d; h->n_cond = (int)cd.size();
+    DAWN_TRY(ws.upload(cd, &h->cond_descs));
+    h->n_cond = (int)cd.size();
   }
   h->sh_nranks = 1; h->sh_rank = 0; h->sh_Fglobal = F; h->sh_halo_l = 0; h->sh_halo_r = 0;   // a new geometry is unsharded until init_shard
   h->p2p_ready = false;
@@ -1355,11 +1348,8 @@ int dawn_unet_shard_ipc_export(dawn_unet* h, char* out64) {
   DAWN_CHECK(h && out64, "null argument");
   DAWN_CHECK(h->sh_nranks > 1 && h->sh_nranks <= kP2pMaxRanks, "init_shard (2..8 ranks) must precede shard_ipc_export");
   if (!h->p2p_own) {
-    float* p = nullptr;
-    DAWN_TRY(dev_alloc(h->owned, (sizeof(P2pMail) + 3) / 4, &p));
-    h->p2p_own = reinterpret_cast<P2pMail*>(p);
-    DAWN_TRY(dev_alloc(h->owned, 4, &p));
-    h->p2p_ctr = reinterpret_cast<unsigned int*>(p);
+    DAWN_TRY(h->mailbox.alloc(1, &h->p2p_own));
+    DAWN_TRY(h->mailbox.alloc(4, &h->p2p_ctr));
   }
   DAWN_CUDA_OK(cudaMemset(h->p2p_own, 0, sizeof(P2pMail)));
   DAWN_CUDA_OK(cudaMemset(h->p2p_ctr, 0, 16));
@@ -1602,6 +1592,6 @@ int dawn_unet_profile_read(dawn_unet* h, double* ms, double* flops, double* byte
   for (int i = 0; i < DAWN_PROF_NCAT; ++i) { ms[i] = h->prof_ms[i]; flops[i] = h->prof_flops[i]; bytes[i] = h->prof_bytes[i]; count[i] = h->prof_cnt[i]; }
   return 0;
 }
-int64_t dawn_unet_workspace_bytes(dawn_unet* h) { return h ? h->ws_bytes : 0; }
+int64_t dawn_unet_workspace_bytes(dawn_unet* h) { return h ? h->workspace.bytes() : 0; }
 
 }  // extern "C"

@@ -15,12 +15,7 @@ import torch
 from torch import nn
 
 from . import _lib
-from ._lib import DawnLfgCfg, check, lib, ptr, stream
-
-
-class _Holder(nn.Module):
-    def forward(self, *a, **k):  # pragma: no cover
-        raise RuntimeError("parameter holder: the computation runs in the CUDA library")
+from ._lib import DawnLfgCfg, _Handle, _Holder, _NativeModule, check, lib, ptr, stream
 
 
 def _conv_bn(ci, co, k):                                   # SameBlock2d / DownBlock2d / UpBlock2d (util.py:95-150)
@@ -39,98 +34,7 @@ def _res_block(c):                                          # ResBlock2d (util.p
     return m
 
 
-class _Handle:
-    """One native handle of include/dawn_lfg.h or include/dawn_pbnet.h (entry points `<api>_*`, api "dawn_lfg",
-    "dawn_lfg_motion" or "dawn_pbnet") that holds a module's parameters.  It is created on the device of the module's inputs and
-    created again after a device change, and the module's state_dict is uploaded and committed whenever `dirty`.
-    param_name(key) is the library's name of a state_dict entry, or None for an entry the handle does not take; extra(module)
-    gives further {name: tensor} entries derived from the module.  `geom` is the geometry its user set last; create and commit
-    void it."""
-
-    def __init__(self, api, cfg, what, param_name=lambda key: key, extra=lambda module: {}):
-        self.api, self.cfg, self.what, self.param_name, self.extra = api, cfg, what, param_name, extra
-        self.handle, self.device_index, self.dirty, self.geom = None, None, True, None
-
-    def _entry(self, name):
-        return getattr(lib, f"{self.api}_{name}")
-
-    def _create(self):
-        hd = ctypes.c_void_p()
-        check(self._entry("create")(ctypes.byref(self.cfg), ctypes.byref(hd)), f"{self.api}_create")
-        return hd
-
-    def validate(self):
-        """Create refuses what the library cannot run; it needs no GPU."""
-        self._entry("destroy")(self._create())
-
-    def destroy(self):
-        if self.handle is not None:
-            self._entry("destroy")(self.handle)
-        self.handle, self.geom = None, None
-
-    def ensure(self, module, device):
-        """Readies the handle for a call on `device` with the parameters of `module`; returns the device index."""
-        if device.type != "cuda":
-            raise _lib.DawnError(f"{self.what} runs on CUDA (sm_90a) only; there is no CPU path")
-        idx = device.index if device.index is not None else torch.cuda.current_device()
-        if self.handle is not None and self.device_index != idx:
-            self.destroy()
-            self.dirty = True
-        with torch.cuda.device(idx):
-            if self.handle is None:
-                self.handle, self.device_index = self._create(), idx
-            if self.dirty:
-                for key, t in module.state_dict().items():
-                    name = None if key.endswith("num_batches_tracked") else self.param_name(key)
-                    if name is not None:
-                        _lib.put_param(self._entry("set_param"), self.handle, name, t)
-                for name, t in self.extra(module).items():
-                    _lib.put_param(self._entry("set_param"), self.handle, name, t)
-                check(self._entry("commit_params")(self.handle), f"{self.api}_commit_params")
-                self.dirty, self.geom = False, None
-        return idx
-
-    def last_launch_count(self):
-        return int(self._entry("last_launch_count")(self.handle)) if self.handle is not None else 0
-
-
-class _LfgModule(nn.Module):
-    """Base of the LFG modules and the PBnet decoder, whose parameters feed the native handles in `_handles`: load_state_dict and
-    .to() / .cuda() mark every handle dirty, and the handles die with the module.  Inference only: train(True) raises `TRAIN_REFUSAL`."""
-    TRAIN_REFUSAL = ""
-
-    def _hold(self, *handles):
-        self._handles = list(handles)
-        self.register_load_state_dict_post_hook(lambda module, incompatible: module.mark_dirty())
-        self.eval()
-
-    def mark_dirty(self):
-        for h in self._handles:
-            h.dirty = True
-
-    def _apply(self, fn, *a, **k):
-        for h in self.__dict__.get("_handles", ()):
-            h.dirty = True
-        return super()._apply(fn, *a, **k)
-
-    def train(self, mode=True):
-        if mode:
-            raise NotImplementedError(self.TRAIN_REFUSAL)
-        return super().train(False)
-
-    def __del__(self):
-        for h in self.__dict__.get("_handles", ()):
-            try:
-                h.destroy()
-            except Exception:
-                pass
-
-    def last_launch_count(self):
-        """Kernels the last call of the module's first handle enqueued."""
-        return self._handles[0].last_launch_count()
-
-
-class Generator(_LfgModule):
+class Generator(_NativeModule):
     IGNORED_PREFIX = "pixelwise_flow_predictor."
     TRAIN_REFUSAL = "this LFG decoder is inference-only (eval-mode BatchNorm, FD:121)"
 
@@ -253,8 +157,6 @@ class Generator(_LfgModule):
                   "dawn_lfg_read_tap")
         return t.permute(1, 0, 2, 3).contiguous()
 
-    def workspace_bytes(self):
-        return int(lib.dawn_lfg_workspace_bytes(self._lfg.handle)) if self._lfg.handle is not None else 0
 
 
 # ====================================================================================================================================
@@ -338,7 +240,7 @@ def _motion_read_tap(h, name):
 _MOTION_TRAIN_REFUSAL = "the LFG motion estimator is inference-only (eval-mode BatchNorm)"
 
 
-class RegionPredictor(_LfgModule):
+class RegionPredictor(_NativeModule):
     """region_predictor.py:28-117 with DAWN's region_predictor_params (pca_based, host SVD)."""
     TRAIN_REFUSAL = _MOTION_TRAIN_REFUSAL
 
@@ -386,7 +288,7 @@ class RegionPredictor(_LfgModule):
         return _motion_read_tap(self._motion, name)
 
 
-class BGMotionPredictor(_LfgModule):
+class BGMotionPredictor(_NativeModule):
     """bg_motion_predictor.py:15-57 with bg_type 'affine' (DAWN's) or 'zero'."""
     TRAIN_REFUSAL = _MOTION_TRAIN_REFUSAL
 

@@ -13,28 +13,13 @@ import torch
 from torch import nn
 
 from . import _lib
-from ._lib import DawnPbnetCfg, check, lib, ptr, stream
-from .lfg import _Handle, _LfgModule
-from .unet import _rel_bias_table
+from ._lib import DawnPbnetCfg, _Handle, _Holder, _NativeModule, check, lib, ptr, stream
+from .unet import _Rotary, _rel_bias_table
 
 MODELTYPES = ("cvae",)
 ARCHINAMES = ("transformerreemb5", "transformerreemb6")
 BANDS = {"transformerreemb5": 200, "transformerreemb6": 100}   # eval-mode masks of RelativePositionBias (reemb5:119-123, reemb6)
 DIM_HEAD = 32                                                  # Attention / Attention_2 of transformerdecoder4.py:190-191
-
-
-class _Holder(nn.Module):
-    def forward(self, *a, **k):  # pragma: no cover
-        raise RuntimeError("parameter holder: the computation runs in the CUDA library")
-
-
-class _Rotary(_Holder):
-    """rotary-embedding-torch's RotaryEmbedding(dim): a non-trainable `freqs` Parameter"""
-
-    def __init__(self, dim, theta=10000):
-        super().__init__()
-        freqs = 1. / (theta ** (torch.arange(0, dim, 2)[:(dim // 2)].float() / dim))
-        self.freqs = nn.Parameter(freqs, requires_grad=False)
 
 
 class _PositionalEncoding(_Holder):
@@ -109,7 +94,7 @@ class Encoder(_Holder):
         raise NotImplementedError("the PBnet encoder runs in training only, which is out of scope: use CVAE.generate")
 
 
-class Decoder(_LfgModule):
+class Decoder(_NativeModule):
     """Decoder_TRANSFORMERREEMB5 / 6 (reemb5:234-378): same keywords and state_dict; forward(batch) runs on the device."""
     TRAIN_REFUSAL = "the PBnet decoder here is inference-only: training (dropout, the training-mode bias) is out of scope"
 
@@ -176,9 +161,6 @@ class Decoder(_LfgModule):
                   "dawn_pbnet_generate")
         batch["output"] = out
         return batch
-
-    def workspace_bytes(self):
-        return int(lib.dawn_pbnet_workspace_bytes(self._pbnet.handle)) if self._pbnet.handle is not None else 0
 
 
 class CVAE(nn.Module):

@@ -15,7 +15,7 @@ import torch
 from torch import nn
 
 from . import _lib
-from ._lib import DawnUnetCfg, check, lib, ptr, stream
+from ._lib import DawnUnetCfg, _Handle, _Holder, _NativeModule, check, lib, ptr, stream
 
 PADDING_MODES = ("zeros", "reflect", "replicate", "circular")   # nn.Conv3d's, in the order of dawn_unet_cfg.pad_mode
 MAX_CLIPS = 16                  # clips per native pass the library accepts (kMaxClips, csrc/common.cuh)
@@ -25,13 +25,6 @@ BATCH_PIXEL_FRAMES = 1 << 21
 
 
 # ----------------------------------------------------------------------------- parameter holders
-class _Holder(nn.Module):
-    """Container whose forward is never called."""
-
-    def forward(self, *a, **k):  # pragma: no cover
-        raise RuntimeError("parameter holder: the computation runs in the CUDA library")
-
-
 class _Gain(_Holder):
     def __init__(self, name, shape):
         super().__init__()
@@ -143,7 +136,7 @@ def _time_freqs(dim):
 
 
 # ----------------------------------------------------------------------------- the module
-class Unet3D(nn.Module):
+class Unet3D(_NativeModule):
     def __init__(self, dim, cond_aud=1024, cond_pose=7, cond_eye=2, cond_dim=None, out_grid_dim=2, out_conf_dim=1,
                  num_frames=40, dim_mults=(1, 2, 4, 8), channels=3, attn_heads=8, attn_dim_head=32,
                  use_hubert_audio_cond=False, init_dim=None, init_kernel_size=7, use_sparse_linear_attn=True,
@@ -240,30 +233,24 @@ class Unet3D(nn.Module):
         cfg.pad_mode = 0 if use_deconv else PADDING_MODES.index(padding_mode)
         cfg.no_sla = 0 if use_sparse_linear_attn else 1
         self._cfg = cfg
-        self._handle = None
-        self._dirty = True
-        self._geom = None
-        self._device_index = None
-        self.register_load_state_dict_post_hook(lambda module, incompatible: module.mark_dirty())
+        # the library re-applies the geometry on commit (dawn_unet_commit_params), so a commit leaves `geom` standing
+        self._unet = _Handle("dawn_unet", cfg, "the DAWN denoising UNet", extra=Unet3D._aux, keeps_geom=True)
+        self._hold(self._unet)
 
     # ------------------------------------------------------------------ native handle management
-    def mark_dirty(self):
-        """Call after mutating parameters in place; load_state_dict / .to() / .cuda() do it automatically."""
-        self._dirty = True
+    @property
+    def _handle(self):
+        """the dawn_unet handle, for the C-ABI entries that take one; a test may set it to stand in for the library's"""
+        return self._unet.handle
 
-    def _apply(self, fn, *a, **k):
-        self._dirty = True
-        return super()._apply(fn, *a, **k)
+    @_handle.setter
+    def _handle(self, h):
+        self._unet.handle = h
 
-    def __del__(self):
-        # plain dict access: nn.Module.__setattr__/__getattr__ may already be torn down at interpreter shutdown
-        h = self.__dict__.get("_handle")
-        self.__dict__["_handle"] = None
-        if h is not None:
-            try:
-                lib.dawn_unet_destroy(h)
-            except Exception:
-                pass
+    def _aux(self):
+        """tables derived from the parameters: sinusoidal time frequencies and the temporal attention's relative-position bias"""
+        return {"aux.time_freqs": _time_freqs(self.dim),
+                "aux.rel_bias": _rel_bias_table(self.time_rel_pos_bias.relative_attention_bias.weight, self.win_width)}
 
     def clips_per_pass(self, b, F, h, w):
         """How many of b clips of F frames x h x w one native pass runs: all of them up to MAX_CLIPS and BATCH_PIXEL_FRAMES,
@@ -279,46 +266,24 @@ class Unet3D(nn.Module):
         return getattr(self, "_clips", 1)
 
     def _ensure(self, device, F, h, w, B=1):
-        if device.type != "cuda":
-            raise _lib.DawnError("the DAWN denoising UNet runs on CUDA (sm_90a) only; there is no CPU path")
-        idx = device.index if device.index is not None else torch.cuda.current_device()
-        if self._handle is not None and self._device_index != idx:
-            lib.dawn_unet_destroy(self._handle)
-            self._handle, self._dirty, self._geom = None, True, None
-        with torch.cuda.device(idx):
-            if self._handle is None:
-                hd = ctypes.c_void_p()
-                check(lib.dawn_unet_create(ctypes.byref(self._cfg), ctypes.byref(hd)), "dawn_unet_create")
-                self._handle, self._device_index = hd, idx
-            if self._dirty:
-                self.sync_parameters()
-            if self._geom != (F, h, w) or self.clip_count() != B:
+        commits = self._unet.commits
+        idx = self._unet.ensure(self, device)
+        if self._unet.commits != commits:
+            self._gen = getattr(self, "_gen", 0) + 1
+            # commit re-runs set_geometry in the library, which leaves the handle unsharded: running on would silently drop the
+            # temporal halos, the clip-wide GroupNorm statistics and the clip-wide quantile, so the next use raises instead
+            if getattr(self, "_shard", None) is not None:
+                self._shard_lost = self._shard
+            self._shard = None
+        if self._unet.geom != (F, h, w) or self.clip_count() != B:
+            with torch.cuda.device(idx):
                 check(lib.dawn_unet_set_geometry(self._handle, B, F, h, w), "dawn_unet_set_geometry")
-                self._geom, self._clips = (F, h, w), B
-                self._gen = getattr(self, "_gen", 0) + 1
-            lost = getattr(self, "_shard_lost", None)
-            if lost is not None and not getattr(self, "_in_init_shard", False):
-                raise _lib.DawnError(f"frame sharding (rank {lost[0]} of {lost[1]}) was dropped by a parameter re-commit "
-                                "(.to()/.cuda()/load_state_dict after init_shard): call init_shard again on every rank")
-
-    def sync_parameters(self):
-        """Repack the module's parameters into kernel layouts (once per parameter change)."""
-        def put(name, t):
-            _lib.put_param(lib.dawn_unet_set_param, self._handle, name, t)
-        for name, t in self.state_dict().items():
-            put(name, t)
-        put("aux.time_freqs", _time_freqs(self.dim))
-        put("aux.rel_bias", _rel_bias_table(self.time_rel_pos_bias.relative_attention_bias.weight, self.win_width))
-        check(lib.dawn_unet_commit_params(self._handle), "dawn_unet_commit_params")
-        self._dirty = False
-        self._gen = getattr(self, "_gen", 0) + 1
-        # commit re-runs set_num_frames in the library, which leaves the handle unsharded: running on would silently drop the
-        # temporal halos, the clip-wide GroupNorm statistics and the clip-wide quantile, so the next use raises instead
-        if getattr(self, "_shard", None) is not None:
-            self._shard_lost = self._shard
-        self._shard = None
-        if self._geom is not None:
-            self._geom = self._geom  # commit re-sized the per-clip tables for the current geometry
+            self._unet.geom, self._clips = (F, h, w), B
+            self._gen = getattr(self, "_gen", 0) + 1
+        lost = getattr(self, "_shard_lost", None)
+        if lost is not None and not getattr(self, "_in_init_shard", False):
+            raise _lib.DawnError(f"frame sharding (rank {lost[0]} of {lost[1]}) was dropped by a parameter re-commit "
+                                 "(.to()/.cuda()/load_state_dict after init_shard): call init_shard again on every rank")
 
     # ------------------------------------------------------------------ reference API
     def forward_with_cond_scale(self, *args, cond_scale=2., **kwargs):      # reference :879-890
@@ -435,7 +400,7 @@ class Unet3D(nn.Module):
     def shard_info(self):
         """(rank, world) of the frame sharding in force for the current geometry; (0, 1) when unsharded."""
         sh = getattr(self, "_shard", None)
-        if sh is None or sh[2] != self._geom:
+        if sh is None or sh[2] != self._unet.geom:
             return 0, 1
         return sh[0], sh[1]
 
@@ -446,11 +411,12 @@ class Unet3D(nn.Module):
     def forward_x3(self, x_t, time, out=None):
         """x_t (3, F, h, w) of the clip whose invariants were set and time int64 (1,) on the device; after batched
         invariants x_t (B, 3, F, h, w) and time (B,), one timestep per clip."""
-        if self._geom is None or getattr(self, "_fea", None) is None:
+        geom = self._unet.geom
+        if geom is None or getattr(self, "_fea", None) is None:
             raise _lib.DawnError("forward_x3: call set_clip_invariants first")
         lead = (self.clip_count(),) if getattr(self, "_inv_batched", False) else ()
-        if tuple(x_t.shape) != lead + (3,) + tuple(self._geom) or x_t.dtype != torch.float32 or x_t.device != self._fea.device:
-            raise ValueError(f"forward_x3: x_t must be float32 {lead + (3,) + tuple(self._geom)} on "
+        if tuple(x_t.shape) != lead + (3,) + tuple(geom) or x_t.dtype != torch.float32 or x_t.device != self._fea.device:
+            raise ValueError(f"forward_x3: x_t must be float32 {lead + (3,) + tuple(geom)} on "
                              f"{self._fea.device}; got {x_t.dtype} {tuple(x_t.shape)} on {x_t.device}")
         if time.numel() != self.clip_count():
             raise ValueError(f"forward_x3: one timestep per clip ({self.clip_count()}), got {time.numel()}")
@@ -504,12 +470,6 @@ class Unet3D(nn.Module):
         cnt = (ctypes.c_int64 * n)()
         check(lib.dawn_unet_profile_read(self._handle, ms, fl, by, cnt), "dawn_unet_profile_read")
         return {c: dict(ms=ms[i], flops=fl[i], bytes=by[i], count=int(cnt[i])) for i, c in enumerate(_lib.PROF_CATS)}
-
-    def last_launch_count(self):
-        return int(lib.dawn_unet_last_launch_count(self._handle)) if self._handle is not None else 0
-
-    def workspace_bytes(self):
-        return int(lib.dawn_unet_workspace_bytes(self._handle)) if self._handle is not None else 0
 
 
 class DynamicNfUnet3D(Unet3D):

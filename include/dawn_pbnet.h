@@ -56,8 +56,6 @@ int dawn_pbnet_generate(dawn_pbnet* h, const float* audio, const float* z, const
 int64_t dawn_pbnet_last_launch_count(dawn_pbnet* h);
 /* device bytes of the handle's activation workspace (grows to the largest bs x F generated) */
 int64_t dawn_pbnet_workspace_bytes(dawn_pbnet* h);
-/* device bytes held by every live dawn_pbnet handle of the process: packed parameters and workspaces */
-int64_t dawn_pbnet_live_bytes(void);
 
 /* Kernel test: the banded attention of one site on caller-owned device buffers, then a stream synchronise.
  *   q = (x_q @ wq) * qscale, k = x_kv @ wk, v = x_kv @ wv, rotary (freqs, npairs) on q and k by frame, then

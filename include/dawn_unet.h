@@ -350,6 +350,9 @@ typedef struct {
 int dawn_test_kernel(const dawn_kernel_case* c, void* stream);
 
 const char* dawn_last_error(void);
+/* device bytes the library holds in the process: the packed parameters and workspaces of every live handle of include/dawn_unet.h,
+   include/dawn_lfg.h and include/dawn_pbnet.h */
+int64_t dawn_live_bytes(void);
 const char* dawn_build_info(void);
 
 #ifdef __cplusplus

@@ -86,6 +86,16 @@ def main():
             net.forward_x3(x_t[0, :, lo:lo + Fl].contiguous().to(dev), tt)
         e1.record(); torch.cuda.synchronize()
         ms = e0.elapsed_time(e1) / 3
+        # a parameter re-commit drops the sharding; init_shard on every rank restores it, on the GroupNorm mailboxes the first
+        # init_shard allocated, and the sharded forward then returns the same eps (to the last bits the GroupNorm statistics'
+        # atomics leave to chance)
+        net.load_state_dict(G.synth_sd(), strict=True)
+        net.init_shard(Fl, h, w, dev)
+        net.set_clip_invariants(fea[0].to(dev), cond[0, lo:lo + Fl].contiguous().to(dev))
+        again = net.forward_x3(x_t[0, :, lo:lo + Fl].contiguous().to(dev), tt)
+        print(f"[{name}] rank {rank}: sharded forward after a re-commit and init_shard: max|d| {(again - out).abs().max():.2e}",
+              flush=True)
+        assert (again - out).abs().max().item() <= 1e-5, "the sharded forward changed after a re-commit and init_shard"
         parts = [torch.empty_like(out) for _ in range(world)]
         dist.all_gather(parts, out)
         full = torch.cat(parts, dim=1).cpu()[None]
