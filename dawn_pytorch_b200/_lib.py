@@ -1,4 +1,4 @@
-"""ctypes binding of include/dawn_unet.h, include/dawn_lfg.h and include/dawn_pbnet.h, and the lifecycle every module shares
+"""ctypes binding of include/dawn_unet.h, include/dawn_lfg.h, include/dawn_pbnet.h and include/dawn_hubert.h, and the lifecycle every module shares
 with its native handles.  The product path has no fallback: if the CUDA library is missing or fails to load, importing this
 module raises."""
 import ctypes
@@ -147,6 +147,25 @@ class DawnPbnetAttentionCase(ctypes.Structure):
                 ("x_q", _p), ("x_kv", _p), ("wq", _p), ("wk", _p), ("wv", _p), ("freqs", _p), ("bias", _p), ("out", _p)]
 
 
+class DawnHubertCfg(ctypes.Structure):
+    """include/dawn_hubert.h: dawn_hubert_cfg"""
+    _i = ctypes.c_int
+    _fields_ = [("hidden_size", _i), ("num_layers", _i), ("num_heads", _i), ("intermediate_size", _i), ("num_conv", _i),
+                ("conv_dim", _i * 8), ("conv_kernel", _i * 8), ("conv_stride", _i * 8), ("conv_bias", _i), ("pos_kernel", _i),
+                ("pos_groups", _i), ("layer_norm_eps", ctypes.c_float)]
+
+
+HUBERT_ATTENTION, HUBERT_CONV0, HUBERT_POS_CONV = range(3)
+
+
+class DawnHubertKernelCase(ctypes.Structure):
+    """include/dawn_hubert.h: dawn_hubert_kernel_case (pointers are device addresses)"""
+    _i, _p = ctypes.c_int, ctypes.c_void_p
+    _fields_ = [("kernel", _i), ("B", _i), ("T", _i), ("L", _i), ("H", _i), ("ld", _i), ("C", _i), ("k", _i), ("s", _i), ("G", _i),
+                ("eps", ctypes.c_float), ("q", _p), ("kk", _p), ("v", _p), ("x", _p), ("w", _p), ("bias", _p), ("gamma", _p),
+                ("beta", _p), ("g", _p), ("out", _p)]
+
+
 class DawnError(RuntimeError):
     pass
 
@@ -242,6 +261,19 @@ def _load():
     lib.dawn_pbnet_workspace_bytes.argtypes = [vp]
     lib.dawn_pbnet_workspace_bytes.restype = ctypes.c_int64
     lib.dawn_pbnet_test_attention.argtypes = [ctypes.POINTER(DawnPbnetAttentionCase), vp]
+    lib.dawn_hubert_create.argtypes = [ctypes.POINTER(DawnHubertCfg), ctypes.POINTER(vp)]
+    lib.dawn_hubert_destroy.argtypes = [vp]
+    lib.dawn_hubert_destroy.restype = None
+    lib.dawn_hubert_set_param.argtypes = [vp, cp, fp, i64p, ctypes.c_int]
+    lib.dawn_hubert_commit_params.argtypes = [vp]
+    lib.dawn_hubert_forward.argtypes = [vp, fp, ctypes.c_int, ctypes.c_int, fp, vp]
+    lib.dawn_hubert_output_length.argtypes = [vp, ctypes.c_int]
+    lib.dawn_hubert_hidden.argtypes = [vp, fp, ctypes.c_int, ctypes.c_int, ctypes.c_int, fp, vp]
+    lib.dawn_hubert_last_launch_count.argtypes = [vp]
+    lib.dawn_hubert_last_launch_count.restype = ctypes.c_int64
+    lib.dawn_hubert_workspace_bytes.argtypes = [vp]
+    lib.dawn_hubert_workspace_bytes.restype = ctypes.c_int64
+    lib.dawn_hubert_test_kernel.argtypes = [ctypes.POINTER(DawnHubertKernelCase), vp]
     lib.dawn_last_error.restype = cp
     lib.dawn_live_bytes.argtypes = []
     lib.dawn_live_bytes.restype = ctypes.c_int64
@@ -271,6 +303,9 @@ LFG_EXPORTS += LFG_MOTION_EXPORTS                       # both handles are decla
 MISC_EXPORTS = ["dawn_conv3x3_s2_relu"]
 PBNET_EXPORTS = ["dawn_pbnet_create", "dawn_pbnet_destroy", "dawn_pbnet_set_param", "dawn_pbnet_commit_params",
                  "dawn_pbnet_generate", "dawn_pbnet_last_launch_count", "dawn_pbnet_workspace_bytes", "dawn_pbnet_test_attention"]
+HUBERT_EXPORTS = ["dawn_hubert_create", "dawn_hubert_destroy", "dawn_hubert_set_param", "dawn_hubert_commit_params",
+                  "dawn_hubert_forward", "dawn_hubert_output_length", "dawn_hubert_hidden", "dawn_hubert_last_launch_count", "dawn_hubert_workspace_bytes",
+                  "dawn_hubert_test_kernel"]
 
 PROF_CATS = ["conv3x3", "conv_other", "qkv_proj", "out_proj", "ca_gate", "gn_hcond", "attn_core", "sla_context",
              "gn_apply", "rowstats", "ca_rstd", "misc", "prep", "temporal_fused_l0", "conv3x3_l0", "comm_allreduce", "comm_halo"]
@@ -307,7 +342,8 @@ class _Holder(nn.Module):
 
 
 class _Handle:
-    """One native handle (entry points `<api>_*`, api "dawn_unet", "dawn_lfg", "dawn_lfg_motion" or "dawn_pbnet") that holds a
+    """One native handle (entry points `<api>_*`, api "dawn_unet", "dawn_lfg", "dawn_lfg_motion", "dawn_pbnet" or
+    "dawn_hubert") that holds a
     module's parameters.  It is created on the device of the module's inputs and created again after a device change, and the
     module's state_dict is uploaded and committed whenever `dirty`; `commits` counts the commits.  param_name(key) is the library's
     name of a state_dict entry, or None for an entry the handle does not take; extra(module) gives further {name: tensor} entries

@@ -21,7 +21,7 @@ def sources():
 def _digest():
     h = hashlib.sha256()
     for f in sorted(os.listdir(CSRC)) + ["../../include/dawn_unet.h", "../../include/dawn_lfg.h",
-                                          "../../include/dawn_pbnet.h"]:
+                                          "../../include/dawn_pbnet.h", "../../include/dawn_hubert.h"]:
         with open(os.path.join(CSRC, f), "rb") as fh:
             h.update(f.encode()); h.update(fh.read())
     h.update(" ".join(FLAGS).encode())

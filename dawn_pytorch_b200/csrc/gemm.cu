@@ -184,7 +184,7 @@ __global__ void __launch_bounds__(THREADS, 2) gemm_kernel(const GemmParams p) {
         v[nt][1] = acc[mt][nt][2 * h + 1];
       }
 
-      if (EPI == EPI_PLAIN) {
+      if (EPI == EPI_PLAIN || EPI == EPI_GELU) {
         float rs_[4] = {0.f, 0.f, 0.f, 0.f}, rss_[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
         for (int nt = 0; nt < 4; ++nt) {
@@ -193,6 +193,7 @@ __global__ void __launch_bounds__(THREADS, 2) gemm_kernel(const GemmParams p) {
             float b0 = 0.f, b1 = 0.f;
             if (p.bias) { b0 = p.bias[n]; b1 = p.bias[n + 1]; }
             float x0 = v[nt][0] + b0, x1 = v[nt][1] + b1;
+            if (EPI == EPI_GELU) { x0 = gelu_erf(x0); x1 = gelu_erf(x1); }
             if (rv) {
               if (p.Res) {
                 const float2 r = *reinterpret_cast<const float2*>(p.Res + opix * p.ldr + n);
@@ -248,6 +249,10 @@ __global__ void __launch_bounds__(THREADS, 2) gemm_kernel(const GemmParams p) {
           const int n = ncol0 + nt * 8;
           v[nt][0] = rs * (v[nt][0] - mu * p.wsum[n]);
           v[nt][1] = rs * (v[nt][1] - mu * p.wsum[n + 1]);
+          if (EPI == EPI_LN_BIAS || EPI == EPI_LN_BIAS_GELU) {      // the folded LayerNorm beta and the Linear bias
+            v[nt][0] += p.bias[n]; v[nt][1] += p.bias[n + 1];
+          }
+          if (EPI == EPI_LN_BIAS_GELU) { v[nt][0] = gelu_erf(v[nt][0]); v[nt][1] = gelu_erf(v[nt][1]); }
         }
         if (EPI == EPI_QKV_TEMPORAL) {
           const int fr = srow / p.P;
@@ -365,6 +370,9 @@ int launch_gemm(const GemmParams& p, int epi, cudaStream_t st) {
     case EPI_QKV_MID: return launch_t<EPI_QKV_MID>(p, st);
     case EPI_CA_GATE: return launch_t<EPI_CA_GATE>(p, st);
     case EPI_GN_APPLY: return launch_t<EPI_GN_APPLY>(p, st);
+    case EPI_GELU: return launch_t<EPI_GELU>(p, st);
+    case EPI_LN_BIAS: return launch_t<EPI_LN_BIAS>(p, st);
+    case EPI_LN_BIAS_GELU: return launch_t<EPI_LN_BIAS_GELU>(p, st);
   }
   set_last_error("launch_gemm: bad epilogue id");
   return -1;

@@ -15,7 +15,12 @@ enum Epi : int {
   EPI_QKV_MID = 3,       // LayerNorm fold only                        (U:841-843)
   EPI_CA_GATE = 4,       // LayerNorm_img fold + cosine-sim 2-key softmax -> gate  (U:519-555)
   EPI_GN_APPLY = 5,      // Out = SiLU(FiLM(GroupNorm(Y))) + acc       (U:235-248, 473-476)
+  EPI_GELU = 6,          // gelu(acc + bias) (+ residual), erf GELU     (HuBERT positional conv)
+  EPI_LN_BIAS = 7,       // LayerNorm fold + bias                       (HuBERT q|k|v, feature projection)
+  EPI_LN_BIAS_GELU = 8,  // LayerNorm fold + bias, then erf GELU        (HuBERT fc1)
 };
+
+__device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
 
 struct GemmParams {
   // A operand (gathered)

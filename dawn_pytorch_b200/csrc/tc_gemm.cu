@@ -381,7 +381,7 @@ __global__ void __launch_bounds__(Cfg<BN>::NTHREADS, 1) tc_gemm_kernel(const Gem
                                      : (size_t)(f * p.OH + oi * p.out_stride + p.oy0) * p.OW + oj * p.out_stride + p.ox0;
       const int srow = p.perm_in ? seq_blocked_pixel(mc, p.perm_pb, p.perm_F, p.P) : mc;     // pixel behind this row
 
-      if (EPI == EPI_PLAIN) {
+      if (EPI == EPI_PLAIN || EPI == EPI_GELU) {
         const float sc = p.tc_scale;                          // undoes the exact power-of-two weight pre-scale
         if (bias_s) {
           const float4* bp = reinterpret_cast<const float4*>(s_biasv + n0);
@@ -402,6 +402,10 @@ __global__ void __launch_bounds__(Cfg<BN>::NTHREADS, 1) tc_gemm_kernel(const Gem
         } else {
 #pragma unroll
           for (int i = 0; i < EN; ++i) acc[i] *= sc;
+        }
+        if (EPI == EPI_GELU) {
+#pragma unroll
+          for (int i = 0; i < EN; ++i) acc[i] = gelu_erf(acc[i]);
         }
         if (rv && p.Res) {
           const float4* rp = reinterpret_cast<const float4*>(p.Res + opix * p.ldr + n0);
@@ -477,6 +481,18 @@ __global__ void __launch_bounds__(Cfg<BN>::NTHREADS, 1) tc_gemm_kernel(const Gem
             acc[4 * i] = fmaf(fb, w.x, fa * acc[4 * i]); acc[4 * i + 1] = fmaf(fb, w.y, fa * acc[4 * i + 1]);
             acc[4 * i + 2] = fmaf(fb, w.z, fa * acc[4 * i + 2]); acc[4 * i + 3] = fmaf(fb, w.w, fa * acc[4 * i + 3]);
           }
+        }
+        if (EPI == EPI_LN_BIAS || EPI == EPI_LN_BIAS_GELU) {   // the folded LayerNorm beta and the Linear bias
+          const float4* bp = reinterpret_cast<const float4*>(p.bias + n0);
+#pragma unroll
+          for (int i = 0; i < EN / 4; ++i) {
+            const float4 b = __ldg(bp + i);
+            acc[4 * i] += b.x; acc[4 * i + 1] += b.y; acc[4 * i + 2] += b.z; acc[4 * i + 3] += b.w;
+          }
+        }
+        if (EPI == EPI_LN_BIAS_GELU) {
+#pragma unroll
+          for (int i = 0; i < EN; ++i) acc[i] = gelu_erf(acc[i]);
         }
         if (EPI == EPI_QKV_TEMPORAL) {
           if (n0 < 512) {
@@ -613,6 +629,9 @@ int launch_tc_gemm(const GemmParams& p, const float* Bimg, int epi, cudaStream_t
     case EPI_QKV_SLA: return launch_bn<EPI_QKV_SLA>(p, Bimg, st);
     case EPI_QKV_MID: return launch_bn<EPI_QKV_MID>(p, Bimg, st);
     case EPI_CA_GATE: return launch_bn<EPI_CA_GATE>(p, Bimg, st);
+    case EPI_GELU: return launch_bn<EPI_GELU>(p, Bimg, st);
+    case EPI_LN_BIAS: return launch_bn<EPI_LN_BIAS>(p, Bimg, st);
+    case EPI_LN_BIAS_GELU: return launch_bn<EPI_LN_BIAS_GELU>(p, Bimg, st);
   }
   set_last_error("launch_tc_gemm: bad epilogue id");
   return -1;
