@@ -1,5 +1,5 @@
-// Shared device helpers of the wgmma kernels (tc_gemm.cu, tc_conv3.cu, temporal_fused.cu): mbarrier / bulk-copy / wgmma PTX wrappers,
-// shared-memory matrix descriptors and the coalesced row store.
+// Shared device helpers of the wgmma kernels (tc_gemm.cu, tc_conv3.cu, temporal_fused.cu, sla_fused.cu): mbarrier / bulk-copy /
+// wgmma PTX wrappers, shared-memory matrix descriptors and the coalesced row store.
 #pragma once
 #include <type_traits>
 #include "common.cuh"
