@@ -27,7 +27,7 @@ class DawnLfgCfg(ctypes.Structure):
 
 
 PATH_MMA_SYNC, PATH_TC_GEMM, PATH_TC_GEMM_PRESPLIT, PATH_TC_CONV3, PATH_TC_CONV3_TMA = range(5)
-EPI_PLAIN, EPI_QKV_TEMPORAL, EPI_QKV_SLA, EPI_QKV_MID, EPI_CA_GATE, EPI_GN_APPLY = range(6)
+EPI_PLAIN, EPI_QKV_TEMPORAL, EPI_QKV_SLA, EPI_QKV_MID, EPI_CA_GATE, EPI_GN_APPLY, EPI_GELU, EPI_LN_BIAS, EPI_LN_BIAS_GELU = range(9)
 
 
 class DawnContractionCase(ctypes.Structure):
@@ -155,7 +155,7 @@ class DawnHubertCfg(ctypes.Structure):
                 ("pos_groups", _i), ("layer_norm_eps", ctypes.c_float)]
 
 
-HUBERT_ATTENTION, HUBERT_CONV0, HUBERT_POS_CONV = range(3)
+HUBERT_ATTENTION, HUBERT_CONV0, HUBERT_POS_CONV, HUBERT_ROW_LN, HUBERT_FE_CONV, HUBERT_LN_LINEAR = range(6)
 
 
 class DawnHubertKernelCase(ctypes.Structure):
@@ -163,7 +163,8 @@ class DawnHubertKernelCase(ctypes.Structure):
     _i, _p = ctypes.c_int, ctypes.c_void_p
     _fields_ = [("kernel", _i), ("B", _i), ("T", _i), ("L", _i), ("H", _i), ("ld", _i), ("C", _i), ("k", _i), ("s", _i), ("G", _i),
                 ("eps", ctypes.c_float), ("q", _p), ("kk", _p), ("v", _p), ("x", _p), ("w", _p), ("bias", _p), ("gamma", _p),
-                ("beta", _p), ("g", _p), ("out", _p)]
+                ("beta", _p), ("g", _p), ("out", _p),
+                ("M", _i), ("N", _i), ("ldo", _i), ("gelu", _i), ("parts", _i), ("qscale", ctypes.c_float)]
 
 
 class DawnError(RuntimeError):

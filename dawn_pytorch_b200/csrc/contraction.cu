@@ -315,8 +315,10 @@ int refuse(const char* why) {
 
 int test_contraction(const dawn_contraction_case& c, cudaStream_t st) {
   if (c.path < DAWN_PATH_MMA_SYNC || c.path > DAWN_PATH_TC_CONV3_TMA) return refuse("unknown path");
-  if (c.epi < EPI_PLAIN || c.epi > EPI_GN_APPLY) return refuse("unknown epilogue");
-  if (c.ntaps < 1 || c.ntaps > 52 || c.F < 1 || c.N < 1 || c.ldb < c.N || c.lda < c.Cin) return refuse("bad geometry");
+  if (c.epi < EPI_PLAIN || c.epi > EPI_LN_BIAS_GELU) return refuse("unknown epilogue");
+  // one tap may read overlapping rows (lda < Cin): the positional conv's 64 x k windows over a 64-channel plane
+  if (c.ntaps < 1 || c.ntaps > 52 || c.F < 1 || c.N < 1 || c.ldb < c.N || c.lda < 1 || (c.ntaps > 1 && c.lda < c.Cin))
+    return refuse("bad geometry");
   if (!c.A || !c.B) return refuse("A and B are required");
   if (c.epi == EPI_CA_GATE ? !c.gates : !c.Out) return refuse("no output buffer");
 
@@ -341,10 +343,15 @@ int test_contraction(const dawn_contraction_case& c, cudaStream_t st) {
   p.Y = c.Y; p.ldy = c.ldy; p.gn_stats = c.gn_stats; p.gn_w = c.gn_w; p.gn_b = c.gn_b; p.film = c.film; p.gn_count = c.gn_count;
   p.drain = c.drain;
 
-  const bool ln = c.epi >= EPI_QKV_TEMPORAL && c.epi <= EPI_CA_GATE;
+  const bool ln_bias = c.epi == EPI_LN_BIAS || c.epi == EPI_LN_BIAS_GELU;
+  const bool ln = (c.epi >= EPI_QKV_TEMPORAL && c.epi <= EPI_CA_GATE) || ln_bias;
   if (p.ln_inline && (c.path != DAWN_PATH_TC_GEMM || p.ntaps != 1)) return refuse("inline LayerNorm statistics need the gather-producer wgmma GEMM and one tap");
   if (ln && !p.ln_inline && !p.rowstats) return refuse("LayerNorm epilogue without row statistics");
   if (ln && !p.wsum) return refuse("LayerNorm epilogue without wsum");
+  if (ln_bias && !p.bias) return refuse("LayerNorm + bias epilogue without a bias");          // both kernels read bias[n] unguarded
+  // the plain epilogue is the only one whose partial sums both kernels accumulate (the wgmma GEMM would also sum GELU outputs,
+  // the mma.sync kernel would not)
+  if (p.stats && c.epi != EPI_PLAIN) return refuse("GroupNorm statistics with an epilogue other than the plain one");
   if (c.epi == EPI_PLAIN && p.stats && (p.cpg <= 0 || p.N / p.cpg > 8)) return refuse("GroupNorm statistics need 8 groups");
 
   DeviceArena arena;

@@ -69,37 +69,60 @@ int upload_vec(dawn_hubert* h, const std::string& name, int n, float** out) {
   return h->weights.upload(p->data, out);
 }
 
+struct LinearPart {                     // one nn.Linear of a LayerNorm-folded projection: W (Nj, K), b (Nj), output scale
+  const float* w;
+  const float* b;
+  float scale;
+};
+
 // nn.Linear weights (N_j, K) of `parts` side by side in the output columns, k-major (K, sum N_j), each scaled by its factor
-// (an exact power of two), with the LayerNorm `ln` (gamma, beta over K) folded in, in fp64:
+// (an exact power of two), with the LayerNorm (gamma, beta over K) folded in, in fp64:
 //   W'[k][n] = W[n][k] gamma[k] sc,  b'[n] = (b[n] + sum_k W[n][k] beta[k]) sc,  wsum[n] = sum_k W'[k][n]
-int pack_ln_linear(dawn_hubert* h, const std::vector<std::pair<std::string, float>>& parts, int Nj, int K, const std::string& ln,
+int pack_ln_linear(DeviceArena& arena, const std::vector<LinearPart>& parts, int Nj, int K, const float* gamma, const float* beta,
                    LnLinear* out) {
-  const HostParam *g, *be;
-  DAWN_TRY(h->raw.need(ln + ".weight", {K}, &g));
-  DAWN_TRY(h->raw.need(ln + ".bias", {K}, &be));
   const int N = Nj * (int)parts.size(), ldb = round_up(N, 64);
   std::vector<float> m((size_t)K * ldb, 0.f), bias(N), wsum(ldb, 0.f);
   for (size_t j = 0; j < parts.size(); ++j) {
-    const HostParam *w, *b;
-    DAWN_TRY(h->raw.need(parts[j].first + ".weight", {Nj, K}, &w));
-    DAWN_TRY(h->raw.need(parts[j].first + ".bias", {Nj}, &b));
-    const double sc = parts[j].second;
+    const double sc = parts[j].scale;
     for (int n = 0; n < Nj; ++n) {
-      const float* wr = w->data.data() + (size_t)n * K;
+      const float* wr = parts[j].w + (size_t)n * K;
       const int col = (int)j * Nj + n;
-      double bb = b->data[n], ws = 0.0;
+      double bb = parts[j].b[n], ws = 0.0;
       for (int k = 0; k < K; ++k) {
-        const float v = (float)((double)wr[k] * (double)g->data[k] * sc);
+        const float v = (float)((double)wr[k] * (double)gamma[k] * sc);
         m[(size_t)k * ldb + col] = v;
         ws += v;
-        bb += (double)wr[k] * (double)be->data[k];
+        bb += (double)wr[k] * (double)beta[k];
       }
       bias[col] = (float)(bb * sc);
       wsum[col] = (float)ws;
     }
   }
-  DAWN_TRY(upload_weight(h->weights, m, K, N, ldb, bias, &out->w));
-  return h->weights.upload(wsum, &out->wsum);
+  DAWN_TRY(upload_weight(arena, m, K, N, ldb, bias, &out->w));
+  return arena.upload(wsum, &out->wsum);
+}
+
+// the same from the handle's parameters: (Linear name, scale) per part, the LayerNorm's name
+int pack_ln_linear(dawn_hubert* h, const std::vector<std::pair<std::string, float>>& names, int Nj, int K, const std::string& ln,
+                   LnLinear* out) {
+  const HostParam *g, *be;
+  DAWN_TRY(h->raw.need(ln + ".weight", {K}, &g));
+  DAWN_TRY(h->raw.need(ln + ".bias", {K}, &be));
+  std::vector<LinearPart> parts;
+  for (const auto& nm : names) {
+    const HostParam *w, *b;
+    DAWN_TRY(h->raw.need(nm.first + ".weight", {Nj, K}, &w));
+    DAWN_TRY(h->raw.need(nm.first + ".bias", {Nj}, &b));
+    parts.push_back({w->data.data(), b->data.data(), nm.second});
+  }
+  return pack_ln_linear(h->weights, parts, Nj, K, g->data.data(), be->data.data(), out);
+}
+
+// feature-extractor conv >= 1: Conv1d weight (co, ci, k) -> tap-major (k ci, co) rows, bias (co) or null (conv_bias false)
+int pack_fe_conv(DeviceArena& arena, const float* w, const float* bias, int co, int ci, int k, PackedWeight* out) {
+  std::vector<float> m((size_t)k * ci * co);
+  pack_conv_taps(w, co, ci, k, ci, co, 0, nullptr, m);
+  return upload_weight(arena, m, k * ci, co, co, bias ? std::vector<float>(bias, bias + co) : std::vector<float>(co, 0.f), out);
 }
 
 // nn.Linear (N, K) + bias -> k-major packed weight
@@ -156,6 +179,36 @@ int run_pos_conv(const std::vector<PackedWeight>& pos, const float* h, int B, in
     DAWN_TRY(run(p, EPI_GELU, st, launches));
   }
   return 0;
+}
+
+// feature-extractor conv >= 1 of B sequences, Tin -> Tout rows: dst (B Tout, co) = GELU(LayerNorm(conv(in))), gamma / beta = ln[0 / 1]
+int run_fe_conv(const PackedWeight& w, const float* const ln[2], const float* in, int B, int Tin, int Tout, int ci, int co, int k, int s,
+                float* dst, cudaStream_t st, int64_t* launches) {
+  GemmParams p;
+  base_params(p, in, ci, ci, B, 1, Tin);
+  p.OWs = p.OW = Tout; p.M = p.rows_per_batch = B * Tout; p.P = Tout;
+  p.in_stride = s;
+  p.ntaps = k;
+  for (int t = 0; t < p.ntaps; ++t) { p.dy[t] = 0; p.dx[t] = (signed char)t; }
+  set_weights(p, w);
+  p.Out = dst; p.ldo = co;
+  DAWN_TRY(run(p, EPI_PLAIN, st, launches));
+  DAWN_TRY(launch_hb_row_ln(dst, co, B * Tout, co, ln[0], ln[1], kConvLnEps, 1, dst, co, st));
+  ++*launches;
+  return 0;
+}
+
+// a pre-LN projection of `rows` dense rows of K: the rows' (mu, rstd) into rs, then the contraction through the fold
+int run_ln_linear(const LnLinear& w, const float* A, int K, int rows, float eps, int epi, float* rs, float* dst, cudaStream_t st,
+                  int64_t* launches) {
+  DAWN_TRY(launch_rowstats(A, K, K, rows, eps, rs, st));
+  ++*launches;
+  GemmParams p;
+  base_params(p, A, K, K, 1, 1, rows);
+  set_weights(p, w.w);
+  p.rowstats = rs; p.wsum = w.wsum;
+  p.Out = dst; p.ldo = w.w.N;
+  return run(p, epi, st, launches);
 }
 
 int ensure_workspace(dawn_hubert* h, long long fe0, long long fe1, long long BT, long long xg) {
@@ -257,9 +310,7 @@ int dawn_hubert_commit_params(dawn_hubert* h) {
       DAWN_TRY(h->weights.upload(m, &h->w0));
       if (b) DAWN_TRY(h->weights.upload(b->data, &h->b0));
     } else {
-      std::vector<float> m((size_t)k * ci * co);
-      pack_conv_taps(w->data.data(), co, ci, k, ci, co, 0, nullptr, m);
-      DAWN_TRY(upload_weight(h->weights, m, k * ci, co, co, b ? b->data : std::vector<float>(co, 0.f), &h->conv[i]));
+      DAWN_TRY(pack_fe_conv(h->weights, w->data.data(), b ? b->data.data() : nullptr, co, ci, k, &h->conv[i]));
     }
     DAWN_TRY(upload_vec(h, p + "layer_norm.weight", co, &h->conv_ln[i][0]));
     DAWN_TRY(upload_vec(h, p + "layer_norm.bias", co, &h->conv_ln[i][1]));
@@ -327,33 +378,14 @@ int run_forward(dawn_hubert* h, const float* input, int B, int L, int layers, bo
   DAWN_TRY(launch_hb_conv0(input, B, L, h->w0, h->b0, c.conv_kernel[0], c.conv_stride[0], c.conv_dim[0], h->conv_ln[0][0],
                            h->conv_ln[0][1], kConvLnEps, h->FE[0], st));
   h->launches++;
-  for (int i = 1; i < c.num_conv; ++i) {
-    const int ci = c.conv_dim[i - 1], co = c.conv_dim[i];
-    float* dst = h->FE[i & 1];
-    GemmParams p;
-    base_params(p, h->FE[(i - 1) & 1], ci, ci, B, 1, Ts[i - 1]);
-    p.OWs = p.OW = Ts[i]; p.M = p.rows_per_batch = B * Ts[i]; p.P = Ts[i];
-    p.in_stride = c.conv_stride[i];
-    p.ntaps = c.conv_kernel[i];
-    for (int t = 0; t < p.ntaps; ++t) { p.dy[t] = 0; p.dx[t] = (signed char)t; }
-    set_weights(p, h->conv[i]);
-    p.Out = dst; p.ldo = co;
-    DAWN_TRY(run(p, EPI_PLAIN, st, &h->launches));
-    DAWN_TRY(launch_hb_row_ln(dst, co, B * Ts[i], co, h->conv_ln[i][0], h->conv_ln[i][1], kConvLnEps, 1, dst, co, st));
-    h->launches++;
-  }
+  for (int i = 1; i < c.num_conv; ++i)
+    DAWN_TRY(run_fe_conv(h->conv[i], h->conv_ln[i], h->FE[(i - 1) & 1], B, Ts[i - 1], Ts[i], c.conv_dim[i - 1], c.conv_dim[i],
+                         c.conv_kernel[i], c.conv_stride[i], h->FE[i & 1], st, &h->launches));
   const float* feat = h->FE[(c.num_conv - 1) & 1];
   const int Cl = c.conv_dim[c.num_conv - 1];
-  // ---- feature projection: LayerNorm folded into the Linear
-  DAWN_TRY(launch_rowstats(feat, Cl, Cl, (int)BT, c.layer_norm_eps, h->RS, st));
-  h->launches++;
+  // pre-LN projections: row statistics, then the LayerNorm folded into the Linear
   auto ln_gemm = [&](const float* A, int K, const LnLinear& w, int epi, float* dst) -> int {
-    GemmParams p;
-    base_params(p, A, K, K, 1, 1, (int)BT);
-    set_weights(p, w.w);
-    p.rowstats = h->RS; p.wsum = w.wsum;
-    p.Out = dst; p.ldo = w.w.N;
-    return run(p, epi, st, &h->launches);
+    return run_ln_linear(w, A, K, (int)BT, c.layer_norm_eps, epi, h->RS, dst, st, &h->launches);
   };
   auto res_gemm = [&](const float* A, int K, const PackedWeight& w, float* hid) -> int {
     GemmParams p;
@@ -368,14 +400,12 @@ int run_forward(dawn_hubert* h, const float* input, int B, int L, int layers, bo
   // ---- encoder layers
   for (int l = 0; l < layers; ++l) {
     const LayerPack& lp = h->layers[l];
-    DAWN_TRY(launch_rowstats(h->H, D, D, (int)BT, c.layer_norm_eps, h->RS, st));
     DAWN_TRY(ln_gemm(h->H, D, lp.qkv, EPI_LN_BIAS, h->QKV));
     DAWN_TRY(launch_hb_attention(h->QKV, h->QKV + D, h->QKV + 2 * D, 3 * D, B, T, c.num_heads, h->O, D, st));
+    h->launches++;
     DAWN_TRY(res_gemm(h->O, D, lp.out, h->H));
-    DAWN_TRY(launch_rowstats(h->H, D, D, (int)BT, c.layer_norm_eps, h->RS, st));
     DAWN_TRY(ln_gemm(h->H, D, lp.fc1, EPI_LN_BIAS_GELU, h->F1));
     DAWN_TRY(res_gemm(h->F1, c.intermediate_size, lp.fc2, h->H));
-    h->launches += 3;
   }
   if (final_ln) {
     DAWN_TRY(launch_hb_row_ln(h->H, D, (int)BT, D, h->enc_ln[0], h->enc_ln[1], c.layer_norm_eps, 0, out, D, st));
@@ -410,8 +440,57 @@ int dawn_hubert_test_kernel(const dawn_hubert_kernel_case* c, void* stream) {
   switch (c->kernel) {
     case DAWN_HUBERT_ATTENTION:
       if (!c->q || !c->kk || !c->v) return refuse_case("attention needs q, k and v");
-      DAWN_TRY(launch_hb_attention(c->q, c->kk, c->v, c->ld, c->B, c->T, c->H, c->out, kHbHeadDim * c->H, st));
+      if (c->ldo != 0 && c->ldo < kHbHeadDim * c->H) return refuse_case("attention ldo must be 0 or at least 64 H");
+      DAWN_TRY(launch_hb_attention(c->q, c->kk, c->v, c->ld, c->B, c->T, c->H, c->out, c->ldo ? c->ldo : kHbHeadDim * c->H, st));
       break;
+    case DAWN_HUBERT_ROW_LN:
+      if (!c->x || !c->gamma || !c->beta) return refuse_case("row LayerNorm needs x, gamma and beta");
+      if (c->ld < c->C || c->ldo < c->C) return refuse_case("row LayerNorm strides must be at least C");
+      DAWN_TRY(launch_hb_row_ln(c->x, c->ld, c->M, c->C, c->gamma, c->beta, c->eps, c->gelu, c->out, c->ldo, st));
+      break;
+    case DAWN_HUBERT_FE_CONV: {
+      if (!c->x || !c->w || !c->gamma || !c->beta) return refuse_case("feature-extractor conv needs x, w, gamma and beta");
+      if (c->B < 1 || c->k < 1 || c->k > 52 || c->s < 1 || c->L < c->k || c->C < 64 || c->C % 64 || c->N < 64 || c->N % 64 ||
+          c->N > kHbMaxC)
+        return refuse_case("bad feature-extractor conv geometry");
+      std::vector<float> hw((size_t)c->N * c->C * c->k), hb;
+      DAWN_CUDA_OK(cudaMemcpy(hw.data(), c->w, hw.size() * sizeof(float), cudaMemcpyDeviceToHost));
+      if (c->bias) {
+        hb.resize(c->N);
+        DAWN_CUDA_OK(cudaMemcpy(hb.data(), c->bias, hb.size() * sizeof(float), cudaMemcpyDeviceToHost));
+      }
+      DeviceArena arena;
+      PackedWeight w;
+      DAWN_TRY(pack_fe_conv(arena, hw.data(), c->bias ? hb.data() : nullptr, c->N, c->C, c->k, &w));
+      const float* ln[2] = {c->gamma, c->beta};
+      int64_t launches = 0;
+      DAWN_TRY(run_fe_conv(w, ln, c->x, c->B, c->L, out_len(c->L, c->k, c->s), c->C, c->N, c->k, c->s, c->out, st, &launches));
+      DAWN_CUDA_OK(cudaStreamSynchronize(st));
+      break;
+    }
+    case DAWN_HUBERT_LN_LINEAR: {
+      if (!c->x || !c->w || !c->bias || !c->gamma || !c->beta) return refuse_case("LayerNorm + Linear needs x, w, bias, gamma and beta");
+      if (c->M < 1 || c->C < 64 || c->C % 64 || c->C > kHbMaxC || c->N < 1 || c->parts < 1 || c->parts > 3)
+        return refuse_case("bad LayerNorm + Linear geometry");
+      const int N = c->parts * c->N;
+      std::vector<float> hw((size_t)N * c->C), hb(N), hg(c->C), hbe(c->C);
+      DAWN_CUDA_OK(cudaMemcpy(hw.data(), c->w, hw.size() * sizeof(float), cudaMemcpyDeviceToHost));
+      DAWN_CUDA_OK(cudaMemcpy(hb.data(), c->bias, hb.size() * sizeof(float), cudaMemcpyDeviceToHost));
+      DAWN_CUDA_OK(cudaMemcpy(hg.data(), c->gamma, hg.size() * sizeof(float), cudaMemcpyDeviceToHost));
+      DAWN_CUDA_OK(cudaMemcpy(hbe.data(), c->beta, hbe.size() * sizeof(float), cudaMemcpyDeviceToHost));
+      std::vector<LinearPart> parts;
+      for (int j = 0; j < c->parts; ++j)
+        parts.push_back({hw.data() + (size_t)j * c->N * c->C, hb.data() + (size_t)j * c->N, j == 0 ? c->qscale : 1.f});
+      DeviceArena arena;
+      LnLinear lin;
+      DAWN_TRY(pack_ln_linear(arena, parts, c->N, c->C, hg.data(), hbe.data(), &lin));
+      float* rs;
+      DAWN_TRY(arena.alloc((size_t)c->M * 2, &rs));
+      int64_t launches = 0;
+      DAWN_TRY(run_ln_linear(lin, c->x, c->C, c->M, c->eps, c->gelu ? EPI_LN_BIAS_GELU : EPI_LN_BIAS, rs, c->out, st, &launches));
+      DAWN_CUDA_OK(cudaStreamSynchronize(st));
+      break;
+    }
     case DAWN_HUBERT_CONV0:
       if (!c->x || !c->w || !c->gamma || !c->beta) return refuse_case("conv0 needs x, w, gamma and beta");
       if (c->k < 1 || c->k > 64) return refuse_case("conv0 kernel must be 1 to 64");

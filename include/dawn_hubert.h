@@ -62,17 +62,31 @@ int64_t dawn_hubert_last_launch_count(dawn_hubert* h);
 int64_t dawn_hubert_workspace_bytes(dawn_hubert* h);
 
 /* Kernel test: one kernel on caller-owned device buffers, then a stream synchronise.
- *   DAWN_HUBERT_ATTENTION: out (B * T, 64 H) = softmax(q k^T) v per 64-wide head; q, k, v (B * T, ld) rows, q pre-scaled.
+ *   DAWN_HUBERT_ATTENTION: out (B * T, 64 H) rows of stride ldo (0: 64 H) = softmax(q k^T) v per 64-wide head; q, k, v
+ *                          (B * T, ld) rows, q pre-scaled.
  *   DAWN_HUBERT_CONV0:     out (B * T0, C) = GELU(LayerNorm(Conv1d(x (B, L); w (C, 1, k), bias, stride s); gamma, beta, eps)).
  *   DAWN_HUBERT_POS_CONV:  out (B, T, 64 G) = x + GELU(SamePad(Conv1d(x; weight_norm(g (1, 1, k), w (64 G, 64, k)), bias,
- *                          padding k / 2, G groups))), through the same fold and contractions as the network (w is weight_v). */
-enum { DAWN_HUBERT_ATTENTION = 0, DAWN_HUBERT_CONV0 = 1, DAWN_HUBERT_POS_CONV = 2 };
+ *                          padding k / 2, G groups))), through the same fold and contractions as the network (w is weight_v).
+ *   DAWN_HUBERT_ROW_LN:    out (M, C) rows of stride ldo = LayerNorm(x (M, C) rows of stride ld; gamma, beta, eps), then erf
+ *                          GELU when gelu; in place when out == x.
+ *   DAWN_HUBERT_FE_CONV:   feature-extractor layer >= 1: out (B * T, N) = GELU(LayerNorm(Conv1d(x (B, L, C) channels-last;
+ *                          w (N, C, k), bias or null, stride s); gamma, beta, eps 1e-5)), T = (L - k) / s + 1, packed and run as
+ *                          the network does.
+ *   DAWN_HUBERT_LN_LINEAR: out (M, parts N) = Linear(LayerNorm(x (M, C); gamma, beta, eps); w (parts N, C), bias (parts N)), the
+ *                          first N columns times qscale, then erf GELU when gelu: `parts` Linears of N outputs side by side
+ *                          (q|k|v: 3, fc1: 1), through the network's fold, row statistics and contraction dispatch. */
+enum {
+  DAWN_HUBERT_ATTENTION = 0, DAWN_HUBERT_CONV0 = 1, DAWN_HUBERT_POS_CONV = 2, DAWN_HUBERT_ROW_LN = 3, DAWN_HUBERT_FE_CONV = 4,
+  DAWN_HUBERT_LN_LINEAR = 5
+};
 typedef struct {
   int kernel;
   int B, T, L, H, ld, C, k, s, G;
   float eps;
   const float *q, *kk, *v, *x, *w, *bias, *gamma, *beta, *g;
   float* out;
+  int M, N, ldo, gelu, parts;
+  float qscale;
 } dawn_hubert_kernel_case;
 int dawn_hubert_test_kernel(const dawn_hubert_kernel_case* c, void* stream);
 

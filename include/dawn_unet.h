@@ -209,7 +209,8 @@ int dawn_unet_ddpm_launch(dawn_unet* h, void* stream);
 /* One contraction through exactly one kernel path, for per-kernel tests against a high-precision reference.
  * Out[m, n] = epilogue( sum_{tap, c} A[pixel(m, tap), c] * B[tap*Cin + c, n] ) with the product's GemmParams semantics
  * (dawn_pytorch_b200/csrc/gemm.cuh): rows m = (f, i, j) over an F x OHs x OWs output sub-grid (M = F*OHs*OWs), input pixel
- * (i*in_stride + dy[t], j*in_stride + dx[t]) of an F x IH x IW image with row stride lda, output pixel
+ * (i*in_stride + dy[t], j*in_stride + dx[t]) of an F x IH x IW image with row stride lda (one tap: lda < Cin reads
+ * overlapping rows), output pixel
  * (f*OH + i*out_stride + oy0) * OW + j*out_stride + ox0 with row stride ldo.  B is fp32 [K][ldb], K = ntaps*Cin.
  * The wgmma paths build their weight image and accumulator scale from B the way the network's weight upload does.
  * Returns -1 and launches nothing when the chosen path does not accept the geometry (it never falls back to
@@ -222,7 +223,9 @@ enum {
   DAWN_PATH_TC_CONV3_TMA = 4       /* wgmma 3x3 halo-tile conv, A pre-split, halo tiles fetched by TMA */
 };
 typedef struct {
-  int path, epi;                   /* DAWN_PATH_*; epilogue: 0 plain, 1 qkv+rotary, 2 qkv+SLA softmax, 3 qkv, 4 cross-attn gate, 5 GN apply */
+  int path, epi;                   /* DAWN_PATH_*; epilogue: 0 plain, 1 qkv+rotary, 2 qkv+SLA softmax, 3 qkv, 4 cross-attn gate, 5 GN apply,
+                                      6 bias + erf GELU (+ residual), 7 LayerNorm fold + bias, 8 LayerNorm fold + bias + erf GELU;
+                                      7 and 8 need a bias, GroupNorm stats only the plain epilogue */
   int F, IH, IW, Cin, lda;
   int ntaps; int dy[52]; int dx[52]; int in_stride;
   int OHs, OWs, OH, OW, out_stride, oy0, ox0;

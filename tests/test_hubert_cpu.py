@@ -9,7 +9,8 @@
 * frame counts equal transformers' _get_feat_extract_output_lengths for 400 to 10^6 samples;
 * the segment plan is the generator's loop, and full segments share a forward at most SEGMENTS_PER_CALL at a time;
 * the normalisation equals Wav2Vec2FeatureExtractor's and the interpolation scipy's interp1d, bit for bit;
-* include/dawn_hubert.h and the library's exports agree.
+* include/dawn_hubert.h and the library's exports agree, and so do the header's kernel-test case struct and its ctypes mirror,
+  field by field in order.
 """
 import json
 import os
@@ -259,3 +260,35 @@ def test_header_declares_the_bound_exports():
     assert declared == set(_lib.HUBERT_EXPORTS)
     for name in _lib.HUBERT_EXPORTS:
         assert hasattr(_lib.lib, name)
+
+
+def _c_struct_fields(header, name):
+    """(field, ctype) of `typedef struct { ... } name;` in declaration order; arrays as (field, type[n])"""
+    with open(os.path.join(ROOT, "include", header)) as f:
+        text = re.sub(r"/\*.*?\*/", "", f.read(), flags=re.S)
+    body = re.search(r"typedef struct \{([^{}]*)\}\s*" + name + r"\s*;", text).group(1)
+    fields = []
+    for decl in body.split(";"):
+        decl = decl.strip()
+        if not decl:
+            continue
+        m = re.match(r"((?:const\s+)?\w+)\s*(\*?)\s*(.*)", decl)
+        base, ptr = m.group(1).replace("const ", ""), m.group(2)
+        for item in m.group(3).split(","):
+            item = item.strip()
+            star = ptr or ("*" if item.startswith("*") else "")
+            item = item.lstrip("*").strip()
+            arr = re.match(r"(\w+)\[(\w+)\]", item)
+            fields.append((arr.group(1), f"{base}{star}[{arr.group(2)}]") if arr else (item, base + star))
+    return fields
+
+
+def test_kernel_case_struct_matches_the_header():
+    import ctypes
+    from dawn_pytorch_b200 import _lib
+    ctype = {ctypes.c_int: "int", ctypes.c_float: "float", ctypes.c_void_p: "float*"}
+    got = [(n, ctype[t]) for n, t in _lib.DawnHubertKernelCase._fields_]
+    assert got == _c_struct_fields("dawn_hubert.h", "dawn_hubert_kernel_case")
+    with open(os.path.join(ROOT, "include", "dawn_hubert.h")) as f:
+        kinds = re.findall(r"DAWN_HUBERT_(\w+) = (\d+)", f.read())
+    assert [(k, int(v)) for k, v in kinds] == [(k, getattr(_lib, "HUBERT_" + k)) for k, _ in kinds]
