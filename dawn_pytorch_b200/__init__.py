@@ -7,3 +7,4 @@ from .lfg import BGMotionPredictor, FlowAE, MotionGenerator, RegionPredictor  # 
 from .flow_diffusion import Face_loc_Encoder, FlowDiffusion  # noqa: F401
 from .pbnet import get_model as get_pbnet_model  # noqa: F401
 from .hubert import HubertModel, hubert_features  # noqa: F401
+from .generate import TalkingHeadGenerator  # noqa: F401

@@ -1,4 +1,5 @@
-"""ctypes binding of include/dawn_unet.h, include/dawn_lfg.h, include/dawn_pbnet.h and include/dawn_hubert.h, and the lifecycle every module shares
+"""ctypes binding of include/dawn_unet.h, include/dawn_lfg.h, include/dawn_pbnet.h, include/dawn_hubert.h and include/dawn_video.h,
+and the lifecycle every module shares
 with its native handles.  The product path has no fallback: if the CUDA library is missing or fails to load, importing this
 module raises."""
 import ctypes
@@ -229,6 +230,7 @@ def _load():
     lib.dawn_lfg_get_fea.argtypes = [vp, fp, vp]
     lib.dawn_lfg_decode.argtypes = [vp, fp, fp, fp, fp, vp]
     lib.dawn_lfg_decode_sample.argtypes = [vp, fp, fp, fp, vp]
+    lib.dawn_lfg_decode_sample_rgb8.argtypes = [vp, fp, ctypes.POINTER(ctypes.c_double), fp, vp]
     lib.dawn_lfg_read_tap.argtypes = [vp, cp, fp, ip, ip, ip, vp]
     lib.dawn_conv3x3_s2_relu.argtypes = [fp, ctypes.c_int, ctypes.c_int, ctypes.c_int, fp, fp, ctypes.c_int, fp, vp]
     lib.dawn_lfg_last_launch_count.argtypes = [vp]
@@ -275,6 +277,7 @@ def _load():
     lib.dawn_hubert_workspace_bytes.argtypes = [vp]
     lib.dawn_hubert_workspace_bytes.restype = ctypes.c_int64
     lib.dawn_hubert_test_kernel.argtypes = [ctypes.POINTER(DawnHubertKernelCase), vp]
+    lib.dawn_portrait_resize.argtypes = [fp, ctypes.c_int, ctypes.c_int, ctypes.c_int, fp, fp, vp]
     lib.dawn_last_error.restype = cp
     lib.dawn_live_bytes.argtypes = []
     lib.dawn_live_bytes.restype = ctypes.c_int64
@@ -294,7 +297,8 @@ EXPORTS = ["dawn_unet_create", "dawn_unet_destroy", "dawn_unet_set_param", "dawn
 
 
 LFG_EXPORTS = ["dawn_lfg_create", "dawn_lfg_destroy", "dawn_lfg_set_param", "dawn_lfg_commit_params", "dawn_lfg_set_geometry",
-               "dawn_lfg_set_source", "dawn_lfg_get_fea", "dawn_lfg_decode", "dawn_lfg_decode_sample", "dawn_lfg_read_tap",
+               "dawn_lfg_set_source", "dawn_lfg_get_fea", "dawn_lfg_decode", "dawn_lfg_decode_sample",
+               "dawn_lfg_decode_sample_rgb8", "dawn_lfg_read_tap",
                "dawn_lfg_last_launch_count", "dawn_lfg_workspace_bytes", "dawn_lfg_test_kernel"]
 LFG_MOTION_EXPORTS = ["dawn_lfg_motion_create", "dawn_lfg_motion_destroy", "dawn_lfg_motion_set_param",
                       "dawn_lfg_motion_commit_params", "dawn_lfg_motion_set_geometry", "dawn_lfg_motion_regions", "dawn_lfg_motion_bg",
@@ -307,6 +311,7 @@ PBNET_EXPORTS = ["dawn_pbnet_create", "dawn_pbnet_destroy", "dawn_pbnet_set_para
 HUBERT_EXPORTS = ["dawn_hubert_create", "dawn_hubert_destroy", "dawn_hubert_set_param", "dawn_hubert_commit_params",
                   "dawn_hubert_forward", "dawn_hubert_output_length", "dawn_hubert_hidden", "dawn_hubert_last_launch_count", "dawn_hubert_workspace_bytes",
                   "dawn_hubert_test_kernel"]
+VIDEO_EXPORTS = ["dawn_portrait_resize"]
 
 PROF_CATS = ["conv3x3", "conv_other", "qkv_proj", "out_proj", "ca_gate", "gn_hcond", "attn_core", "sla_context",
              "gn_apply", "rowstats", "ca_rstd", "misc", "prep", "temporal_fused_l0", "conv3x3_l0", "comm_allreduce", "comm_halo"]

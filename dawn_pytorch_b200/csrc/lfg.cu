@@ -75,7 +75,8 @@ int conv_up(dawn_lfg* h, const UpConv& u, const float* in, int Cin, int frames, 
   return run_up(p, u, out, co, [&](const GemmParams& q) { return run_conv(h, q, st); });
 }
 
-int decode_core(dawn_lfg* h, float* prediction, float* deformed, cudaStream_t st) {
+// prediction (F, 3, H, W) fp32 [+ deformed], or with rgb8 != null 8-bit RGB frames (F, H, W, 3) offset by mean (launch_lfg_final_rgb8)
+int decode_core(dawn_lfg* h, float* prediction, float* deformed, uint8_t* rgb8, const double* mean, cudaStream_t st) {
   const int n = h->n, F = h->F;
   const int Cb = h->C[n], Hn = h->lH[n], Wn = h->lW[n];
   const long long Mn = (long long)F * Hn * Wn;
@@ -122,8 +123,12 @@ int decode_core(dawn_lfg* h, float* prediction, float* deformed, cudaStream_t st
     fin = h->BL[0];
   }
   h->launches++;
-  DAWN_TRY(launch_lfg_final(fin, h->C[0], h->C[0], F, h->H, h->W, h->final_w, h->final_b, h->SRC, h->MOTION, h->fh, h->fw,
-                           h->cfg.skips ? 1 : 0, prediction, deformed, st));
+  if (rgb8)
+    DAWN_TRY(launch_lfg_final_rgb8(fin, h->C[0], h->C[0], F, h->H, h->W, h->final_w, h->final_b, h->SRC, h->MOTION, h->fh, h->fw,
+                                   h->cfg.skips ? 1 : 0, mean, rgb8, st));
+  else
+    DAWN_TRY(launch_lfg_final(fin, h->C[0], h->C[0], F, h->H, h->W, h->final_w, h->final_b, h->SRC, h->MOTION, h->fh, h->fw,
+                              h->cfg.skips ? 1 : 0, prediction, deformed, st));
   h->decoded = true;
   return 0;
 }
@@ -286,7 +291,7 @@ int dawn_lfg_decode(dawn_lfg* h, const float* flow, const float* occ, float* pre
   cudaStream_t st = (cudaStream_t)stream;
   h->launches = 1;
   DAWN_TRY(launch_lfg_motion_pack(flow, occ, 0, h->F, h->fh, h->fw, h->MOTION, st));
-  return decode_core(h, prediction, deformed, st);
+  return decode_core(h, prediction, deformed, nullptr, nullptr, st);
 }
 
 int dawn_lfg_decode_sample(dawn_lfg* h, const float* sample, float* prediction, float* deformed, void* stream) {
@@ -295,7 +300,16 @@ int dawn_lfg_decode_sample(dawn_lfg* h, const float* sample, float* prediction, 
   cudaStream_t st = (cudaStream_t)stream;
   h->launches = 1;
   DAWN_TRY(launch_lfg_motion_pack(sample, nullptr, 1, h->F, h->fh, h->fw, h->MOTION, st));
-  return decode_core(h, prediction, deformed, st);
+  return decode_core(h, prediction, deformed, nullptr, nullptr, st);
+}
+
+int dawn_lfg_decode_sample_rgb8(dawn_lfg* h, const float* sample, const double mean[3], uint8_t* frames, void* stream) {
+  DAWN_CHECK(h && sample && mean && frames, "null argument");
+  DAWN_CHECK(h->have_source, "lfg: set_source must precede decode");
+  cudaStream_t st = (cudaStream_t)stream;
+  h->launches = 1;
+  DAWN_TRY(launch_lfg_motion_pack(sample, nullptr, 1, h->F, h->fh, h->fw, h->MOTION, st));
+  return decode_core(h, nullptr, nullptr, frames, mean, st);
 }
 
 int dawn_lfg_read_tap(dawn_lfg* h, const char* name, float* dst, int* C, int* Hl, int* Wl, void* stream) {

@@ -152,14 +152,42 @@ __global__ void hwc_to_chw_kernel(const float* __restrict__ x, int ld, int C, lo
   out[idx] = x[(size_t)m * ld + c];
 }
 
+// The final conv's two ways of storing a pixel's three values o[c]:
+//   fp32 prediction (F, 3, H, W);
+//   8-bit RGB frames (F, H, W, 3) as unified_video_generator.py:544-548 makes them from that prediction: `frame += mean / 255.0`
+//   adds a float64 array to the float32 frame in place (rounded once to fp32), np.clip to [0, 1], `* 255` in fp32, astype(uint8)
+//   truncates.
+struct StoreF32 {
+  static constexpr int kMinBlocks = 0;             // no occupancy request: 64 registers
+  float* out;
+  __device__ __forceinline__ void operator()(const float o[3], int f, int y, int x, int H, int W) const {
+    const size_t HWs = (size_t)H * W, obase = (size_t)f * 3 * HWs + (size_t)y * W + x;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) out[obase + c * HWs] = o[c];
+  }
+};
+struct StoreRgb8 {
+  static constexpr int kMinBlocks = 2;             // without it ptxas caps this variant at 40 registers and spills
+  uint8_t* out;
+  double m0, m1, m2;                                   // mean[c] / 255.0
+  static __device__ __forceinline__ uint8_t level(float o, double m) {
+    const float v = fminf(fmaxf(__double2float_rn((double)o + m), 0.f), 1.f);
+    return (uint8_t)(int)__fmul_rn(v, 255.f);
+  }
+  __device__ __forceinline__ void operator()(const float o[3], int f, int y, int x, int H, int W) const {
+    uint8_t* px = out + (((size_t)f * H + y) * W + x) * 3;
+    px[0] = level(o[0], m0); px[1] = level(o[1], m1); px[2] = level(o[2], m2);
+  }
+};
+
 // final 7x7 conv (Cin -> 3) + sigmoid + source blend.  Block = 16 x 16 output pixels of one frame, thread = one pixel.
 // Input channels go through shared memory 8 at a time: halo tile [22][22][8] floats (15.5 KB) + weight slice [49][8][4] (6.3 KB).
 constexpr int FT = 16, FK = 7, FP = 3, FH = FT + FK - 1, FC = 8;
-__global__ void __launch_bounds__(FT * FT) final_conv_kernel(const float* __restrict__ x, int ldx, int Cin, int F, int H, int W,
+template <typename Store>
+__global__ void __launch_bounds__(FT * FT, Store::kMinBlocks) final_conv_kernel(const float* __restrict__ x, int ldx, int Cin, int F, int H, int W,
                                                              const float* __restrict__ wpack, const float* __restrict__ bias3,
                                                              const float* __restrict__ source, const float4* __restrict__ motion,
-                                                             int h, int w, int blend, float* __restrict__ prediction,
-                                                             float* __restrict__ deformed) {
+                                                             int h, int w, int blend, Store store, float* __restrict__ deformed) {
   __shared__ __align__(16) float s_in[FH * FH * FC];
   __shared__ __align__(16) float s_w[FK * FK * FC * 4];
   const int tx = threadIdx.x % FT, ty = threadIdx.x / FT;
@@ -218,8 +246,7 @@ __global__ void __launch_bounds__(FT * FT) final_conv_kernel(const float* __rest
       if (blend) o[c] = s * m.z + o[c] * (1.f - m.z);                                       // generator.py:166-167
     }
   }
-#pragma unroll
-  for (int c = 0; c < 3; ++c) prediction[obase + c * HWs] = o[c];
+  store(o, f, oy, ox, H, W);
 }
 
 // Face_loc_Encoder layer (FD:39-50): out = relu(conv3x3 stride 2, pad 1 (x) + b), planar (C, H, W) tensors, a handful of channels.
@@ -316,7 +343,18 @@ int launch_lfg_final(const float* x, int ldx, int Cin, int F, int H, int W, cons
                      cudaStream_t st) {
   if (Cin % FC != 0 || (ldx & 3)) { set_last_error("lfg final conv: Cin must be a multiple of 8"); return -1; }
   dim3 grid((W + FT - 1) / FT, (H + FT - 1) / FT, F);
-  final_conv_kernel<<<grid, FT * FT, 0, st>>>(x, ldx, Cin, F, H, W, wpack, bias3, source, motion, h, w, blend, prediction, deformed);
+  final_conv_kernel<<<grid, FT * FT, 0, st>>>(x, ldx, Cin, F, H, W, wpack, bias3, source, motion, h, w, blend, StoreF32{prediction},
+                                              deformed);
+  DAWN_LAUNCH_OK();
+  return 0;
+}
+int launch_lfg_final_rgb8(const float* x, int ldx, int Cin, int F, int H, int W, const float* wpack, const float* bias3,
+                          const float* source, const float4* motion, int h, int w, int blend, const double mean[3], uint8_t* frames,
+                          cudaStream_t st) {
+  if (Cin % FC != 0 || (ldx & 3)) { set_last_error("lfg final conv: Cin must be a multiple of 8"); return -1; }
+  StoreRgb8 store{frames, mean[0] / 255.0, mean[1] / 255.0, mean[2] / 255.0};
+  dim3 grid((W + FT - 1) / FT, (H + FT - 1) / FT, F);
+  final_conv_kernel<<<grid, FT * FT, 0, st>>>(x, ldx, Cin, F, H, W, wpack, bias3, source, motion, h, w, blend, store, nullptr);
   DAWN_LAUNCH_OK();
   return 0;
 }

@@ -2,6 +2,7 @@
 // All activations are channels-last fp32 (frames, H, W, C); the per-clip source features are one frame (H, W, C).
 #pragma once
 #include <cuda_runtime.h>
+#include <cstdint>
 #include <vector>
 
 namespace dawn {
@@ -62,5 +63,10 @@ std::vector<float> lfg_final_pack(const float* weight, int Cin);
 int launch_lfg_final(const float* x, int ldx, int Cin, int F, int H, int W, const float* wpack, const float* bias3,
                      const float* source, const float4* motion, int h, int w, int blend, float* prediction, float* deformed,
                      cudaStream_t st);
+// the same, storing 8-bit RGB frames (F, H, W, 3): frames = (uint8) trunc(fl32(clamp(fl32((double) prediction + mean_c / 255), 0, 1)
+// * 255)), the conversion of unified_video_generator.py:544-548 (in RGB order; the BGR flip there is for cv2's writer)
+int launch_lfg_final_rgb8(const float* x, int ldx, int Cin, int F, int H, int W, const float* wpack, const float* bias3,
+                          const float* source, const float4* motion, int h, int w, int blend, const double mean[3], uint8_t* frames,
+                          cudaStream_t st);
 
 }  // namespace dawn

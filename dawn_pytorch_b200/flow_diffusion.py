@@ -120,7 +120,24 @@ class FlowDiffusion(nn.Module):
         sample_eye (b, 2, F); sample_bbox (b, >= 6, F).  Returns the reference's dictionary: sample_vid_grid (b, 2, F, h, w),
         sample_vid_conf (b, 1, F, h, w), sample_out_vid (b, 3, F, H, W), sample_warped_vid (b, 3, F, H, W).
         noise_fn / use_graph are passed to the sampler (tests inject the noise the reference draws with torch.randn)."""
+        pred = self._sample_latent(sample_img, sample_audio_hubert, sample_pose, sample_eye, sample_bbox, cond_scale, init_pose,
+                                   init_eye, noise_fn, use_graph)
         out = {}
+        out["sample_vid_grid"] = pred[:, :2]                                            # FD:366
+        out["sample_vid_conf"] = (pred[:, 2].unsqueeze(1) + 1) * 0.5                    # FD:369
+        vids, warped = [], []
+        for i in range(pred.shape[0]):                                                  # FD:375-383, all frames of a clip at once
+            p, d = self.generator.decode_sample(sample_img[i:i + 1], pred[i], need_deformed=True)
+            vids.append(p.permute(1, 0, 2, 3))
+            warped.append(d.permute(1, 0, 2, 3))
+        out["sample_out_vid"] = torch.stack(vids)
+        out["sample_warped_vid"] = torch.stack(warped)
+        return out
+
+    def _sample_latent(self, sample_img, sample_audio_hubert, sample_pose, sample_eye, sample_bbox, cond_scale, init_pose, init_eye,
+                       noise_fn, use_graph):
+        """FD:327-365: source features, face-box embedding, conditioning and the sampling loop -> pred (b, 3, F, h, w) = [grid_x,
+        grid_y, conf], the sampled latent both sample_one_video and the talking-head generator decode."""
         fea = self.generator.compute_fea(sample_img)                                    # FD:327
         bbox_mask = self.generate_bbox_mask(sample_bbox, size=sample_img.shape[-1])     # FD:328
         bbox_mask = self.face_loc_emb(bbox_mask)                                        # FD:330
@@ -142,16 +159,7 @@ class FlowDiffusion(nn.Module):
                          use_graph=use_graph)
         if self.use_residual_flow:
             raise NotImplementedError("use_residual_flow=True is not used by the shipped configs (FD:362-364)")
-        out["sample_vid_grid"] = pred[:, :2]                                            # FD:366
-        out["sample_vid_conf"] = (pred[:, 2].unsqueeze(1) + 1) * 0.5                    # FD:369
-        vids, warped = [], []
-        for i in range(b):                                                              # FD:375-383, all frames of a clip at once
-            p, d = self.generator.decode_sample(sample_img[i:i + 1], pred[i], need_deformed=True)
-            vids.append(p.permute(1, 0, 2, 3))
-            warped.append(d.permute(1, 0, 2, 3))
-        out["sample_out_vid"] = torch.stack(vids)
-        out["sample_warped_vid"] = torch.stack(warped)
-        return out
+        return pred
 
     def forward(self, *a, **k):
         raise NotImplementedError("FlowDiffusion.forward is the training step (FD:203-323): out of scope of this inference path")

@@ -140,6 +140,22 @@ class Generator(_NativeModule):
             check(lib.dawn_lfg_decode_sample(self._lfg.handle, ptr(s), ptr(pred), ptr(deformed), stream()), "dawn_lfg_decode_sample")
         return (pred, deformed) if need_deformed else pred
 
+    @torch.no_grad()
+    def decode_sample_rgb8(self, source_image, sample, mean=(0.0, 0.0, 0.0)):
+        """decode_sample straight to 8-bit RGB frames (F, H, W, 3) uint8 on the device: each fp32 prediction offset by mean / 255,
+        clipped to [0, 1], times 255 and truncated, as unified_video_generator.py:544-548 converts a frame (RGB order)."""
+        _, F_, fh, fw = sample.shape
+        H, W = source_image.shape[-2:]
+        dev = source_image.device
+        self._ensure(dev, F_, H, W, fh, fw)
+        self._set_source(source_image)
+        s = sample.contiguous().float()
+        m = (ctypes.c_double * 3)(*[float(v) for v in mean])
+        frames = torch.empty((F_, H, W, 3), device=dev, dtype=torch.uint8)
+        with torch.cuda.device(dev):
+            check(lib.dawn_lfg_decode_sample_rgb8(self._lfg.handle, ptr(s), m, ptr(frames), stream()), "dawn_lfg_decode_sample_rgb8")
+        return frames
+
     def forward(self, *a, **k):
         raise NotImplementedError("Generator.forward (region-driven training path, generator.py:92-130) is out of scope; "
                                   "use forward_with_flow / compute_fea")

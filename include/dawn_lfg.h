@@ -54,6 +54,10 @@ int dawn_lfg_get_fea(dawn_lfg* h, float* fea, void* stream);
 int dawn_lfg_decode(dawn_lfg* h, const float* flow, const float* occ, float* prediction, float* deformed, void* stream);
 /* same from the sampler's output: sample (3, frames, h, w) = [grid_x, grid_y, conf], occlusion = (conf + 1) / 2 (FD:366-369) */
 int dawn_lfg_decode_sample(dawn_lfg* h, const float* sample, float* prediction, float* deformed, void* stream);
+/* dawn_lfg_decode_sample with deformed == NULL, storing the frames as 8-bit RGB instead of fp32: frames (frames, H, W, 3) uint8 on
+ * the device, frames[f, y, x, c] = (uint8) trunc(fl32(clamp(fl32((double) prediction[f, c, y, x] + mean[c] / 255.0), 0, 1) * 255f)),
+ * the conversion unified_video_generator.py:544-548 applies to each frame (channels in RGB order) */
+int dawn_lfg_decode_sample_rgb8(dawn_lfg* h, const float* sample, const double mean[3], uint8_t* frames, void* stream);
 
 /* debugging / sub-module parity: copy of an internal activation of the last decode as (C, frames, Hl, Wl):
  * "bottleneck", "up0", "up1" (names as in oracle/lfg_oracle.py taps).  Writes C, Hl, Wl; dst may be NULL to query the shape. */
