@@ -148,6 +148,18 @@ class DawnPbnetAttentionCase(ctypes.Structure):
                 ("x_q", _p), ("x_kv", _p), ("wq", _p), ("wk", _p), ("wv", _p), ("freqs", _p), ("bias", _p), ("out", _p)]
 
 
+PBNET_MEMORY, PBNET_PROJ, PBNET_OUT_LN, PBNET_FFN_LN = range(4)
+
+
+class DawnPbnetKernelCase(ctypes.Structure):
+    """include/dawn_pbnet.h: dawn_pbnet_kernel_case (pointers are device addresses)"""
+    _fields_ = [(n, ctypes.c_int) for n in ("kernel", "T", "bs", "F", "D", "Lz", "PE", "ldx", "hid", "ngroups", "npairs", "ldr", "ff",
+                                            "nout")] + \
+               [("flags", ctypes.c_int * 8), ("qscale", ctypes.c_float)] + \
+               [(n, ctypes.c_void_p) for n in ("x", "z", "xref", "w", "w2", "b1", "b2", "gamma", "beta", "wf", "bf", "rot", "res",
+                                               "mask", "out")]
+
+
 class DawnHubertCfg(ctypes.Structure):
     """include/dawn_hubert.h: dawn_hubert_cfg"""
     _i = ctypes.c_int
@@ -264,6 +276,7 @@ def _load():
     lib.dawn_pbnet_workspace_bytes.argtypes = [vp]
     lib.dawn_pbnet_workspace_bytes.restype = ctypes.c_int64
     lib.dawn_pbnet_test_attention.argtypes = [ctypes.POINTER(DawnPbnetAttentionCase), vp]
+    lib.dawn_pbnet_test_kernel.argtypes = [ctypes.POINTER(DawnPbnetKernelCase), vp]
     lib.dawn_hubert_create.argtypes = [ctypes.POINTER(DawnHubertCfg), ctypes.POINTER(vp)]
     lib.dawn_hubert_destroy.argtypes = [vp]
     lib.dawn_hubert_destroy.restype = None
@@ -307,7 +320,8 @@ LFG_MOTION_EXPORTS = ["dawn_lfg_motion_create", "dawn_lfg_motion_destroy", "dawn
 LFG_EXPORTS += LFG_MOTION_EXPORTS                       # both handles are declared in include/dawn_lfg.h
 MISC_EXPORTS = ["dawn_conv3x3_s2_relu"]
 PBNET_EXPORTS = ["dawn_pbnet_create", "dawn_pbnet_destroy", "dawn_pbnet_set_param", "dawn_pbnet_commit_params",
-                 "dawn_pbnet_generate", "dawn_pbnet_last_launch_count", "dawn_pbnet_workspace_bytes", "dawn_pbnet_test_attention"]
+                 "dawn_pbnet_generate", "dawn_pbnet_last_launch_count", "dawn_pbnet_workspace_bytes", "dawn_pbnet_test_attention",
+                 "dawn_pbnet_test_kernel"]
 HUBERT_EXPORTS = ["dawn_hubert_create", "dawn_hubert_destroy", "dawn_hubert_set_param", "dawn_hubert_commit_params",
                   "dawn_hubert_forward", "dawn_hubert_output_length", "dawn_hubert_hidden", "dawn_hubert_last_launch_count", "dawn_hubert_workspace_bytes",
                   "dawn_hubert_test_kernel"]

@@ -332,6 +332,7 @@ int dawn_pbnet_generate(dawn_pbnet* h, const float* audio, const float* z, const
     DAWN_TRY(launch_pb_proj(h->MEM, D, T, F, D, h->w_kv, hid, 2 * L, g, 1.f, h->ROT, h->npairs, h->KV, st));
     h->launches++;
   }
+  int attn = 0;                                                    // attention launches: one per 65 535 clips per site
   for (int l = 0; l < L; ++l) {
     const LayerPack& lp = h->layers[l];
     const float* xin = h->c0;
@@ -340,22 +341,23 @@ int dawn_pbnet_generate(dawn_pbnet* h, const float* audio, const float* z, const
       DAWN_TRY(launch_pb_proj(h->X, D, T, F, D, lp.w_qkv, hid, 3, groups_of({PB_SCALE | PB_ROTARY, PB_ROTARY, 0}), qscale, h->ROT,
                               h->npairs, h->QKV, st));
       DAWN_TRY(launch_pb_attention(h->QKV, 3 * hid, h->QKV + hid, 3 * hid, h->QKV + 2 * hid, 3 * hid, h->bias_tgt, band, bs, F, H,
-                                   h->O, st));
+                                   h->O, st, &attn));
       DAWN_TRY(launch_pb_out_ln(h->O, hid, lp.w_out_self, h->X, D, lp.ln[0][0], lp.ln[0][1], T, D, h->X, st));
-      h->launches += 3;
+      h->launches += 2;
       xin = h->X; ldx = D;
     }
     // cross-attention over the memory + layer_norm2 (:203)
     DAWN_TRY(launch_pb_proj(xin, ldx, T, F, D, lp.w_q, hid, 1, groups_of({PB_SCALE | PB_ROTARY}), qscale, h->ROT, h->npairs, h->QKV, st));
     DAWN_TRY(launch_pb_attention(h->QKV, hid, h->KV + 2 * hid * l, ldkv, h->KV + 2 * hid * l + hid, ldkv, h->bias_mem, band, bs, F, H,
-                                 h->O, st));
+                                 h->O, st, &attn));
     DAWN_TRY(launch_pb_out_ln(h->O, hid, lp.w_out_cross, xin, ldx, lp.ln[1][0], lp.ln[1][1], T, D, h->X, st));
     // FFN + layer_norm3 (:204); after the last layer finallayer + the length mask (reemb5:370-374)
     const bool last = l + 1 == L;
     DAWN_TRY(launch_pb_ffn_ln(h->X, T, D, lp.w1, lp.b1, c.ff_size, lp.w2, lp.b2, lp.ln[2][0], lp.ln[2][1], last ? h->wf : nullptr,
                               last ? h->bf : nullptr, h->nout, mask, out, st));
-    h->launches += 4;
+    h->launches += 3;
   }
+  h->launches += attn;
   return 0;
 }
 

@@ -1,6 +1,7 @@
 // Kernels of PBnet's transformer decoder (pbnet_kernels.cuh).  The decoder is small (d_model 64, 4 heads, ff 128 in DAWN) and
 // runs over every frame of the audio, so the kernels are plain fp32 SIMT: one warp per row for the row kernels, one thread per
 // query for the banded attention, which only visits the keys within +-band of its query.
+#include <algorithm>
 #include <cmath>
 
 #include "common.cuh"
@@ -275,10 +276,16 @@ int launch_pb_proj(const float* x, int ldx, int T, int F, int D, const float* w,
 }
 
 int launch_pb_attention(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv, const float* bias, int band,
-                        int bs, int F, int H, float* out, cudaStream_t st) {
-  dim3 grid((F + kAttnQ - 1) / kAttnQ, H, bs);
-  pb_attention_kernel<<<grid, kAttnQ, 0, st>>>(q, ldq, k, ldk, v, ldv, bias, band, F, H, out);
-  DAWN_LAUNCH_OK();
+                        int bs, int F, int H, float* out, cudaStream_t st, int* launches) {
+  constexpr int kMaxGridZ = 65535;                                 // clips per launch: gridDim.z's limit
+  for (int b0 = 0; b0 < bs; b0 += kMaxGridZ) {
+    const size_t r0 = (size_t)b0 * F;
+    dim3 grid((F + kAttnQ - 1) / kAttnQ, H, std::min(kMaxGridZ, bs - b0));
+    pb_attention_kernel<<<grid, kAttnQ, 0, st>>>(q + r0 * ldq, ldq, k + r0 * ldk, ldk, v + r0 * ldv, ldv, bias, band, F, H,
+                                                 out + r0 * 32 * H);
+    DAWN_LAUNCH_OK();
+    if (launches) ++*launches;
+  }
   return 0;
 }
 

@@ -28,9 +28,9 @@ int launch_pb_proj(const float* x, int ldx, int T, int F, int D, const float* w,
 
 // banded multi-head attention of (bs clips) x (F frames): out[b, i, h] = softmax_j(q_i . k_j + bias[h][j - i + band]) v_j over
 // |j - i| <= band, online softmax.  q, k, v: (bs * F, ld*) rows, head h at columns [32 h, 32 h + 32); bias (H, 2 band + 1);
-// out (bs * F, 32 H).
+// out (bs * F, 32 H).  One launch per 65 535 clips (gridDim.z); each launch adds 1 to *launches when it is not null.
 int launch_pb_attention(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv, const float* bias, int band,
-                        int bs, int F, int H, float* out, cudaStream_t st);
+                        int bs, int F, int H, float* out, cudaStream_t st, int* launches = nullptr);
 
 // x_out[m] = LayerNorm(res[m] + o[m] @ wo) with weight / bias (nn.LayerNorm, eps 1e-5); o (T, hid); ldr = 0: one residual row
 int launch_pb_out_ln(const float* o, int hid, const float* wo, const float* res, int ldr, const float* gamma, const float* beta,

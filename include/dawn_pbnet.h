@@ -29,7 +29,7 @@ typedef struct {
   int audio_latent_dim;      /* 256 */
   int pose_latent_dim;       /* 64: d_model, a multiple of 32, at most 256 */
   int ff_size;               /* 128: at most 2048 */
-  int num_layers;            /* 2: 1 to 8 */
+  int num_layers;            /* 2: 1 to 4 (k | v of every layer's cross-attention are projected together, 2 num_layers <= 8) */
   int num_heads;             /* 4: even, at most 32; heads are 32 wide and the rotary covers min(32, num_heads) features */
 } dawn_pbnet_cfg;
 
@@ -68,6 +68,32 @@ typedef struct {
   float* out;
 } dawn_pbnet_attention_case;
 int dawn_pbnet_test_attention(const dawn_pbnet_attention_case* c, void* stream);
+
+/* Kernel test: one of the decoder's row kernels on caller-owned device buffers, with the launch code generate uses, then a
+ * stream synchronise.  Rows are m = b F + f; D (d_model) is a multiple of 32 from 32 to 256; weights are k-major (K, N).
+ *   DAWN_PBNET_MEMORY:  out (bs F, D) = x (bs F, D) + z[f][b] @ w + xref[b] @ w2; z (F, bs, Lz), w (Lz, D), xref (bs, PE),
+ *                       w2 (PE, D); PE may be 0.
+ *   DAWN_PBNET_PROJ:    out (T, ngroups hid) = x @ w, x (T, D) rows of stride ldx (0: one row for every m), w (D, ngroups hid);
+ *                       group g's columns times qscale when flags[g] & 1, then, when flags[g] & 2, the pairs (2i, 2i + 1),
+ *                       i < npairs, of every 32-wide head rotated by rot[m % F][i] = (cos, sin); rot (F, npairs, 2).
+ *   DAWN_PBNET_OUT_LN:  out (T, D) = LayerNorm(res + x @ w; gamma, beta, eps 1e-5), x (T, hid), w (hid, D), res (T, D) rows of
+ *                       stride ldr (0: one row for every m); res may be out (in place).
+ *   DAWN_PBNET_FFN_LN:  y = LayerNorm(x + gelu(x @ w + b1) @ w2 + b2; gamma, beta), x (T, D), w (D, ff), w2 (ff, D) (erf GELU).
+ *                       wf null: x = y in place.  Otherwise x is left as it was and out (T, nout) = mask[m] ? y @ wf + bf : 0,
+ *                       wf (D, nout), mask (T) bytes.
+ * Returns -1 without touching the device for a bad kernel, geometry or missing pointer. */
+enum { DAWN_PBNET_MEMORY = 0, DAWN_PBNET_PROJ = 1, DAWN_PBNET_OUT_LN = 2, DAWN_PBNET_FFN_LN = 3 };
+typedef struct {
+  int kernel;
+  int T, bs, F, D, Lz, PE, ldx, hid, ngroups, npairs, ldr, ff, nout;
+  int flags[8];
+  float qscale;
+  float* x;
+  const float *z, *xref, *w, *w2, *b1, *b2, *gamma, *beta, *wf, *bf, *rot, *res;
+  const uint8_t* mask;
+  float* out;
+} dawn_pbnet_kernel_case;
+int dawn_pbnet_test_kernel(const dawn_pbnet_kernel_case* c, void* stream);
 
 #ifdef __cplusplus
 }

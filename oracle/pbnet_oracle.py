@@ -57,6 +57,22 @@ CASES = {
     "reemb5_pose_1": (PbCfg(), [1]),
 }
 
+# name -> (cfg, lengths): the golden cases of other configurations the library accepts (tests/golden/pbnet_configs.npz).  Widths
+# that are not multiples of 64 (d_model 32 and 96) run with bs x F rows on both sides of the contraction dispatcher's 128-row
+# line; the reference's encoder needs (audio_latent_dim + 2 d_model) % num_heads == 0.
+CONFIG_CASES = {
+    "d96_h6_l3_reemb5": (PbCfg(pose_latent_dim=96, num_heads=6, num_layers=3, ff_size=100, audio_dim=128, latent_dim=42,
+                               audio_latent_dim=42), [70, 33]),
+    "d256_h32_l1_reemb6": (PbCfg(archiname="transformerreemb6", pos_dim=1, pose_latent_dim=256, num_heads=32, num_layers=1,
+                                 ff_size=2048, audio_dim=64, latent_dim=96, audio_latent_dim=96), [230]),
+    "d32_h2_l4_reemb5": (PbCfg(pos_dim=20, eye_dim=12, pose_latent_dim=32, num_heads=2, num_layers=4, ff_size=1, latent_dim=18,
+                               audio_latent_dim=18), [9]),
+    "d32_h4_l2_rows150": (PbCfg(pos_dim=3, eye_dim=2, pose_latent_dim=32, num_heads=4, num_layers=2, ff_size=64, audio_dim=192,
+                                latent_dim=28, audio_latent_dim=28), [150]),
+    "d96_h2_l1_rows80": (PbCfg(archiname="transformerreemb6", pose_latent_dim=96, num_heads=2, num_layers=1, ff_size=256,
+                               audio_dim=256, latent_dim=8, audio_latent_dim=8), [40, 17]),
+}
+
 
 # ----------------------------------------------------------------------------- synthetic weights and inputs
 def positional_encoding(d_model, max_len=20000):
@@ -119,10 +135,16 @@ def rel_bias(table, F, band, num_buckets, max_distance, dtype):
     return b.masked_fill((rel.abs() > band)[None], float("-inf"))
 
 
+def rotary_angles(F, freqs):
+    """(F, len(freqs)) float64 angles f * freq, each rounded to fp32 as the reference's fp32 einsum (and the device's rotary
+    table) form it: at 15 000 frames an exact product differs from that by up to half an fp32 ulp of 15 000, 4.9e-4 rad"""
+    return (torch.arange(F, device=freqs.device, dtype=torch.float32)[:, None] * freqs.float()[None, :]).double()
+
+
 def rotate(t, freqs):
-    """rotary over the first 2 len(freqs) features of each head, interleaved pairs, position = frame index"""
-    F = t.shape[-2]
-    ang = torch.arange(F, device=t.device, dtype=freqs.dtype)[:, None] * freqs[None, :]
+    """rotary over the first 2 len(freqs) features of each head, interleaved pairs, position = frame index; the fp32 angle,
+    then cos / sin in float64"""
+    ang = rotary_angles(t.shape[-2], freqs)
     cos, sin = ang.cos().to(t.dtype), ang.sin().to(t.dtype)
     r = 2 * freqs.shape[0]
     a, b = t[..., 0:r:2], t[..., 1:r:2]
