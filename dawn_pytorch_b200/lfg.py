@@ -181,8 +181,8 @@ class Generator(_NativeModule):
 # dawn_lfg_motion handle of include/dawn_lfg.h.  Same constructor keywords and state_dict keys as the reference modules; the
 # sub-modules only hold parameters.  The 2x2 SVD of the region covariances runs on the host, as in the reference
 # (region_predictor.py:16-25): one device-to-host copy per RegionPredictor call.
-MOTION_CHUNK = 50                    # frames per stage call: bounds the workspace (the full-resolution background encoder) and
-                                     # keeps every activation index below 2^31
+MOTION_CHUNK = 50                    # frames per stage call: bounds the workspace (the full-resolution background encoder)
+MOTION_MAX_ELEMENTS = 2 ** 31 - 1    # dawn_lfg_motion_set_geometry refuses frames x H x W x 64 above this (int32 indexing)
 
 
 def _encoder(be, cin, mx, nb):                               # Encoder (util.py:153-169)
@@ -230,11 +230,18 @@ def _motion_handle(cfg, param_name):
     return h
 
 
+def motion_frames_per_call(n, H, W):
+    """Frames per stage call for n frames of (H, W) images: at most MOTION_CHUNK, and few enough that the largest activation
+    (the background encoder's first conv, 64 channels at full resolution) stays within the library's int32 bound.  At least
+    one: a single frame too large for the bound is refused by the library with its own message."""
+    return max(1, min(n, MOTION_CHUNK, MOTION_MAX_ELEMENTS // (H * W * 64)))
+
+
 def _motion_geometry(h, module, device, n, H, W):
     """Readies the motion handle h of `module` for n frames of (H, W) images; returns the frames per stage call.  The
     workspace only grows: fewer frames of the same size reuse it."""
     idx = h.ensure(module, device)
-    frames = min(n, MOTION_CHUNK)
+    frames = motion_frames_per_call(n, H, W)
     if h.geom is None or h.geom[1:] != (H, W) or h.geom[0] < frames:
         with torch.cuda.device(idx):
             check(lib.dawn_lfg_motion_set_geometry(h.handle, frames, H, W), "dawn_lfg_motion_set_geometry")
