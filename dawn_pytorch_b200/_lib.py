@@ -68,7 +68,7 @@ class DawnFusedCase(ctypes.Structure):
 
 KERNEL_ROWSTATS, KERNEL_GN_APPLY, KERNEL_COND_TABLES, KERNEL_TIME_MLP, KERNEL_FILM, KERNEL_ROTARY, KERNEL_SPLIT_ROWS, \
     KERNEL_NCF_TO_NHWC, KERNEL_FRAME_INVARIANCE, KERNEL_FEA_SHIFT, KERNEL_MAP_REDUCE, KERNEL_INIT_CONV_X3, KERNEL_HEADS_OUT, \
-    KERNEL_DDIM_STEP, KERNEL_DDPM_STEP = range(15)
+    KERNEL_DDIM_STEP, KERNEL_DDPM_STEP, KERNEL_Q_SAMPLE, KERNEL_MOTION_TO_LATENT = range(17)
 KERNEL_MAX_DESC = 16
 
 
@@ -231,6 +231,8 @@ def _load():
     lib.dawn_unet_ddpm_step.argtypes = [vp, fp, fp, fp, ctypes.c_int64] + [ctypes.c_float] * 6 + [vp, vp]
     lib.dawn_unet_ddpm_capture.argtypes = [vp, fp, fp, fp, vp, fp, ctypes.c_int, ctypes.c_float, vp]
     lib.dawn_unet_ddpm_launch.argtypes = [vp, vp]
+    lib.dawn_q_sample.argtypes = [fp, fp, vp, fp, fp, ctypes.c_int, ctypes.c_int64, ctypes.c_int64, fp, vp]
+    lib.dawn_motion_to_latent.argtypes = [fp, fp, ctypes.c_int64] + [ctypes.c_int] * 3 + [vp, fp, fp, fp, ctypes.c_int, fp, vp]
     ip = ctypes.POINTER(ctypes.c_int)
     lib.dawn_lfg_create.argtypes = [ctypes.POINTER(DawnLfgCfg), ctypes.POINTER(vp)]
     lib.dawn_lfg_destroy.argtypes = [vp]
@@ -306,6 +308,7 @@ EXPORTS = ["dawn_unet_create", "dawn_unet_destroy", "dawn_unet_set_param", "dawn
            "dawn_unet_profile_enable", "dawn_unet_profile_read", "dawn_unet_last_launch_count", "dawn_unet_workspace_bytes", "dawn_ddim_step", "dawn_unet_ddim_step", "dawn_unet_sampler_capture", "dawn_unet_sampler_launch",
            "dawn_unet_ddim_step_guided", "dawn_unet_sampler_capture_guided", "dawn_unet_sampler_launch_guided",
            "dawn_ddpm_step", "dawn_unet_ddpm_step", "dawn_unet_ddpm_capture", "dawn_unet_ddpm_launch",
+           "dawn_q_sample", "dawn_motion_to_latent",
            "dawn_test_contraction", "dawn_test_fused", "dawn_test_kernel", "dawn_last_error", "dawn_live_bytes", "dawn_build_info"]
 
 

@@ -168,6 +168,14 @@ int test_kernel(const dawn_kernel_case& c, DeviceArena& arena, cudaStream_t st) 
     case DAWN_KERNEL_DDIM_STEP:
     case DAWN_KERNEL_DDPM_STEP:
       return sampler_step(c, st);
+    case DAWN_KERNEL_Q_SAMPLE:
+      if (!c.x || !c.noise || !c.t || !c.w || !c.b || !c.out) return refuse("missing pointer");
+      if (c.n < 1 || c.num_t < 1 || c.clips < 1 || c.clips > 65535) return refuse("bad geometry");
+      return q_sample_impl(c.x, c.noise, c.t, c.w, c.b, c.num_t, c.clips, c.n, c.out, st);
+    case DAWN_KERNEL_MOTION_TO_LATENT:
+      if (!c.x || !c.y || !c.out || (c.t && (!c.noise || !c.w || !c.b))) return refuse("missing pointer");
+      if (c.F < 1 || c.H < 1 || c.W < 1 || c.clips < 1 || c.clips > 65535 || (c.t && c.num_t < 1)) return refuse("bad geometry");
+      return motion_to_latent_impl(c.x, c.y, c.clips, c.F, c.H, c.W, c.t, c.noise, c.w, c.b, c.num_t, c.out, st);
   }
   return refuse("unknown kernel");
 }

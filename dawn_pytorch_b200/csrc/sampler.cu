@@ -1,6 +1,7 @@
 // DDIM update around the denoising UNet (reference U:1169-1205): x0 prediction, dynamic thresholding with the exact
 // 0.9-quantile of |x0| over the whole clip (torch.quantile semantics, linear interpolation), and the eta-noise update.
-// The ancestral (DDPM) update of p_sample (U:1087-1121) shares the same threshold.
+// The ancestral (DDPM) update of p_sample (U:1087-1121) shares the same threshold.  q_sample (U:1226-1232) and the motion
+// estimator's output -> latent pass (FD:248-262, 280-282) start a sampler from a real clip.
 // Everything stays on the device: no host synchronisation inside a sampling step.
 #include "common.cuh"
 #include "sampler.cuh"
@@ -287,6 +288,88 @@ int ddpm_advance_slot(int64_t* t_slot, cudaStream_t st) {
   return 0;
 }
 
+namespace {
+
+// the schedule row of clip b's timestep, clamped into the table (the host wrappers check the range where t is on the host)
+__device__ __forceinline__ int q_row(const int64_t* __restrict__ t, long long b, int num_t) {
+  const long long v = t[b];
+  return (int)(v < 0 ? 0 : (v >= num_t ? num_t - 1 : v));
+}
+
+// a[t] * x0 + b[t] * noise rounded as the reference's two fp32 products and one sum (U:1226-1232; no fused multiply-add)
+__device__ __forceinline__ float q_mix(float ca, float x0, float cb, float z) { return __fadd_rn(__fmul_rn(ca, x0), __fmul_rn(cb, z)); }
+
+// x_t = a[t_c] x0 + b[t_c] noise over B clips of n values: blockIdx.y is the clip
+__global__ void q_sample_kernel(const float* __restrict__ x0, const float* __restrict__ noise, const int64_t* __restrict__ t,
+                                const float* __restrict__ a, const float* __restrict__ b, int num_t, long long n,
+                                float* __restrict__ out) {
+  const long long c = blockIdx.y;
+  const int r = q_row(t, c, num_t);
+  const float ca = a[r], cb = b[r];
+  const long long base = c * n;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    out[base + i] = q_mix(ca, x0[base + i], cb, noise[base + i]);
+}
+
+// the motion estimator's flow (F, h, w, 2) and occlusion (F, 1, h, w) of clip blockIdx.y -> its latent (3, F, h, w) =
+// [grid_x, grid_y, occ * 2 - 1] (FD:259-260, 281-282); with t != nullptr the latent is noised to x_t on the way out
+__global__ void motion_to_latent_kernel(const float* __restrict__ flow, const float* __restrict__ occ, int F, int hw,
+                                        const int64_t* __restrict__ t, const float* __restrict__ noise, const float* __restrict__ a,
+                                        const float* __restrict__ b, int num_t, float* __restrict__ out) {
+  const long long c = blockIdx.y;
+  const long long m = (long long)F * hw;                 // pixels of one clip
+  float ca = 0.f, cb = 0.f;
+  if (t) {
+    const int r = q_row(t, c, num_t);
+    ca = a[r]; cb = b[r];
+  }
+  const float2* fl = reinterpret_cast<const float2*>(flow) + c * m;
+  const float* oc = occ + c * m;
+  float* o = out + c * 3 * m;
+  const float* z = t ? noise + c * 3 * m : nullptr;
+  for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < m; p += (long long)gridDim.x * blockDim.x) {
+    const float2 g = fl[p];
+    float v[3] = {g.x, g.y, __fsub_rn(__fmul_rn(oc[p], 2.0f), 1.0f)};
+#pragma unroll
+    for (int j = 0; j < 3; ++j) o[j * m + p] = z ? q_mix(ca, v[j], cb, z[j * m + p]) : v[j];
+  }
+}
+
+// grid of a per-clip elementwise pass over n values of each of B clips
+dim3 clip_grid(long long n, int64_t B) {
+  return dim3((unsigned)std::min<long long>((n + kThreads - 1) / kThreads, 148LL * 8 / std::max<int64_t>(1, std::min<int64_t>(B, 8))),
+              (unsigned)B);
+}
+
+}  // namespace
+
+int q_sample_impl(const float* x0, const float* noise, const int64_t* t, const float* a, const float* b, int num_t, int64_t B,
+                  int64_t n, float* out, cudaStream_t st) {
+  if (!x0 || !noise || !t || !a || !b || !out || num_t < 1 || B < 1 || B > 65535 || n < 1) {
+    set_last_error("dawn_q_sample: bad argument");
+    return -1;
+  }
+  q_sample_kernel<<<clip_grid(n, B), kThreads, 0, st>>>(x0, noise, t, a, b, num_t, n, out);
+  DAWN_LAUNCH_OK();
+  return 0;
+}
+
+int motion_to_latent_impl(const float* flow, const float* occ, int64_t B, int F, int h, int w, const int64_t* t, const float* noise,
+                          const float* a, const float* b, int num_t, float* out, cudaStream_t st) {
+  if (!flow || !occ || !out || B < 1 || B > 65535 || F < 1 || h < 1 || w < 1 || (t && (!noise || !a || !b || num_t < 1))) {
+    set_last_error("dawn_motion_to_latent: bad argument");
+    return -1;
+  }
+  if (reinterpret_cast<uintptr_t>(flow) % sizeof(float2)) {
+    set_last_error("dawn_motion_to_latent: flow must be 8-byte aligned");
+    return -1;
+  }
+  const int hw = h * w;
+  motion_to_latent_kernel<<<clip_grid((long long)F * hw, B), kThreads, 0, st>>>(flow, occ, F, hw, t, noise, a, b, num_t, out);
+  DAWN_LAUNCH_OK();
+  return 0;
+}
+
 }  // namespace dawn
 
 using namespace dawn;
@@ -304,6 +387,16 @@ int dawn_ddpm_step(float* x, const float* eps, const float* noise, int64_t n, fl
                    float q, void* scratch, void* stream) {
   return ddpm_step_impl(x, eps, noise, n, n, DdpmCoef{ca, cb, c1, c2, sigma}, nullptr, nullptr, 0, q, scratch,
                         (cudaStream_t)stream, nullptr);
+}
+
+int dawn_q_sample(const float* x0, const float* noise, const int64_t* t, const float* sqrt_acp, const float* sqrt_1m_acp, int num_t,
+                  int64_t B, int64_t n, float* out, void* stream) {
+  return q_sample_impl(x0, noise, t, sqrt_acp, sqrt_1m_acp, num_t, B, n, out, (cudaStream_t)stream);
+}
+
+int dawn_motion_to_latent(const float* flow, const float* occlusion, int64_t B, int F, int h, int w, const int64_t* t,
+                          const float* noise, const float* sqrt_acp, const float* sqrt_1m_acp, int num_t, float* out, void* stream) {
+  return motion_to_latent_impl(flow, occlusion, B, F, h, w, t, noise, sqrt_acp, sqrt_1m_acp, num_t, out, (cudaStream_t)stream);
 }
 
 }  // extern "C"

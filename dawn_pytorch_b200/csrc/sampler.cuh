@@ -38,4 +38,11 @@ int ddpm_step_impl(float* x, const float* eps, const float* noise, int64_t n_loc
 // *t_slot -= 1 on the stream (one thread; the last node of the ancestral step graph)
 int ddpm_advance_slot(int64_t* t_slot, cudaStream_t st);
 
+// x_t = a[t[c]] x0 + b[t[c]] noise for B clips of n values (dawn_q_sample)
+int q_sample_impl(const float* x0, const float* noise, const int64_t* t, const float* a, const float* b, int num_t, int64_t B,
+                  int64_t n, float* out, cudaStream_t st);
+// flow (B*F, h, w, 2) and occlusion (B*F, 1, h, w) -> (B, 3, F, h, w) latent, noised when t != nullptr (dawn_motion_to_latent)
+int motion_to_latent_impl(const float* flow, const float* occ, int64_t B, int F, int h, int w, const int64_t* t, const float* noise,
+                          const float* a, const float* b, int num_t, float* out, cudaStream_t st);
+
 }  // namespace dawn

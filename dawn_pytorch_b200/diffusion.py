@@ -2,8 +2,8 @@
 (DM_3/modules/video_flow_diffusion_multiGPU_v0_crema_plus_faceemb_ca_multi_test.py:988-1313) around the CUDA UNet:
 same constructor keywords, the same 12 schedule buffers (so `diffusion.load_state_dict(checkpoint['diffusion'])`,
 unified_video_generator.py:527-528, fills `denoise_fn.*` and the buffers), `sample(fea, bbox_mask, cond, cond_scale)`,
-`ddim_sample` and the ancestral `p_sample_loop` / `p_sample`.  Training entry points (`forward`, `p_losses`) are out of
-scope and raise.
+`ddim_sample` and the ancestral `p_sample_loop` / `p_sample`, and for sampling from a real clip `q_sample`, `interpolate`,
+`ddim_sample_from` and `p_sample_loop_from`.  Training entry points (`forward`, `p_losses`) are out of scope and raise.
 
 The sampling loops keep the clip on the device: the 272 feature channels and the conditioning are handed to the UNet
 once per clip (`set_clip_invariants`), each step is `forward_x3` + one fused update (`dawn_ddim_step`, or
@@ -142,8 +142,14 @@ class GaussianDiffusion(nn.Module):
         pairs = self.ddim_schedule() if pairs is None else pairs
         draw = noise_fn if noise_fn is not None else self._default_noise(unet, device, seed)
         img = draw(-1, shape).to(device).contiguous()
-        q = self._clip_q(clip_denoised)
         self._check_sample_shape("ddim_sample", fea, shape, cond)
+        return self._ddim_run(fea, cond, img, pairs, draw, cond_scale, self._clip_q(clip_denoised), use_graph)
+
+    def _ddim_run(self, fea, cond, img, pairs, draw, cond_scale, q, use_graph):
+        """The DDIM loop over `pairs` in place on img, on the eager path, the plain graph or the guided graph; draw(k, shape) is
+        the noise of pairs[k]."""
+        device = self.betas.device
+        unet = self.denoise_fn
         st = stream()
         guided = cond_scale != 1 and getattr(unet, "has_cond", True)
         if use_graph:
@@ -153,6 +159,114 @@ class GaussianDiffusion(nn.Module):
         steps = [(t, self.ddim_coefficients(t, t_next)) for t, t_next in pairs]
         return self._sample_eager("dawn_unet_ddim_step", fea, cond, img, steps, cond_scale, q,
                                   lambda k, sel, one: draw(k, one).to(device).contiguous() if pairs[k][1] > 0 else None)
+
+    @torch.no_grad()
+    def ddim_sample_from(self, x_t, start, fea, cond=None, cond_scale=1., clip_denoised=True, noise_fn=None, use_graph=False,
+                         seed=None):
+        """ddim_sample from a given image instead of noise: x_t (b, 3, F, h, w) is taken to be at timestep
+        ddim_schedule()[start][0] (e.g. `q_sample` of a real clip's latent there) and the steps ddim_schedule()[start:] are run on
+        it, on the eager loop, the plain graph or the guided graph as ddim_sample runs them.  noise_fn(k, shape) is the draw of
+        step k of the whole schedule (k >= start; ddim_sample's numbering, so start = 0 from a randn x_t is ddim_sample with the
+        same draws).  A suffix schedule is its own graph key: its capture replaces the cached whole-schedule graph.  x_t is not
+        modified; returns the sample."""
+        pairs = self.ddim_schedule()
+        start = int(start)
+        if not 0 <= start < len(pairs):
+            raise ValueError(f"ddim_sample_from: start = {start} is outside [0, {len(pairs)}), the {len(pairs)}-step DDIM schedule")
+        img = self._start_image("ddim_sample_from", x_t, fea, cond)
+        full = noise_fn if noise_fn is not None else self._default_noise(self.denoise_fn, self.betas.device, seed)
+        return self._ddim_run(fea, cond, img, pairs[start:], lambda k, shp: full(start + k, shp), cond_scale,
+                              self._clip_q(clip_denoised), use_graph)
+
+    def _start_image(self, what, x_t, fea, cond):
+        """A fp32 device copy of the caller's start image, after the sample-shape checks."""
+        if not torch.is_tensor(x_t) or x_t.dim() != 5:
+            raise ValueError(f"{what}: x_t must be a (b, {self.channels}, F, h, w) tensor")
+        self._check_sample_shape(what, fea, tuple(x_t.shape), cond)
+        return x_t.to(device=self.betas.device, dtype=torch.float32).contiguous().clone()
+
+    # ------------------------------------------------------------------ noising a clean latent (reference :1211-1232)
+    def _q_tables(self, device):
+        """sqrt_alphas_cumprod and sqrt_one_minus_alphas_cumprod as contiguous fp32 tensors on `device`: the registered buffers
+        when they live there, else one copy per schedule, kept until the buffers change."""
+        bufs = (self.sqrt_alphas_cumprod, self.sqrt_one_minus_alphas_cumprod)
+        if all(b.device == device and b.dtype == torch.float32 and b.is_contiguous() for b in bufs):
+            return bufs
+        key = tuple((b.data_ptr(), b._version, b.device) for b in bufs) + (device,)
+        cached = getattr(self, "_q_tabs", None)
+        if cached is None or cached[0] != key:
+            cached = (key, tuple(b.detach().to(device=device, dtype=torch.float32).contiguous() for b in bufs))
+            self._q_tabs = cached
+        return cached[1]
+
+    def _q_timesteps(self, what, t, b, device):
+        """(b,) int64 device tensor of the per-clip timesteps t (an int or a (b,) tensor).  The range is checked unless t is a
+        device tensor read during a CUDA-graph capture, where a host read would break the capture (the kernel then clamps)."""
+        if not torch.is_tensor(t):
+            t = torch.full((b,), int(t), dtype=torch.long)
+        if t.dim() == 0:
+            t = t.expand(b)
+        if tuple(t.shape) != (b,) or t.dtype.is_floating_point or t.dtype.is_complex:
+            raise ValueError(f"{what}: t must be an integer timestep or a (b,) = ({b},) integer tensor, got {tuple(t.shape)} {t.dtype}")
+        if not (t.is_cuda and torch.cuda.is_current_stream_capturing()):
+            lo, hi = int(t.min()), int(t.max())
+            if lo < 0 or hi >= self.num_timesteps:
+                raise ValueError(f"{what}: t in [{lo}, {hi}] is outside [0, {self.num_timesteps})")
+        return t.to(device=device, dtype=torch.long).contiguous()
+
+    @torch.no_grad()
+    def q_sample(self, x_start, t, noise=None):
+        """reference q_sample (U:1226-1232): sqrt_alphas_cumprod[t] * x_start + sqrt_one_minus_alphas_cumprod[t] * noise per clip,
+        bit-identical to the reference's fp32 torch ops (`dawn_q_sample`).  x_start (b, ...); t (b,) integer tensor (or an int
+        for every clip); noise like x_start, by default the draw of `_default_noise` (on a frame-sharded UNet this rank's slice of
+        one clip-wide stream).  Returns x_t on the sampler's device."""
+        device = self.betas.device
+        if not torch.is_tensor(x_start) or x_start.dim() < 2:
+            raise ValueError("q_sample: x_start must be a (b, ...) tensor")
+        b = x_start.shape[0]
+        tt = self._q_timesteps("q_sample", t, b, device)
+        if noise is None:
+            noise = self._default_noise(self.denoise_fn, device, None)(0, tuple(x_start.shape))
+        if tuple(noise.shape) != tuple(x_start.shape):
+            raise ValueError(f"q_sample: noise {tuple(noise.shape)} does not match x_start {tuple(x_start.shape)}")
+        x0 = x_start.to(device=device, dtype=torch.float32).contiguous()
+        z = noise.to(device=device, dtype=torch.float32).contiguous()
+        out = torch.empty_like(x0)
+        if x0.numel() == 0:
+            return out
+        a, s = self._q_tables(device)
+        with torch.cuda.device(device):
+            check(lib.dawn_q_sample(ptr(x0), ptr(z), ptr(tt), ptr(a), ptr(s), self.num_timesteps, b, x0[0].numel(), ptr(out),
+                                    stream()), "dawn_q_sample")
+        return out
+
+    def motion_to_latent(self, flow, occlusion, num_frames, t=None, noise=None):
+        """The LFG motion estimator's output for b clips of num_frames frames, flow (b*F, h, w, 2) and occlusion (b*F, 1, h, w),
+        as the sampler's latent x0 (b, 3, F, h, w) = [grid, occlusion * 2 - 1] (FD:259-260, 281-282; `dawn_motion_to_latent`).
+        With t (as q_sample's) it returns q_sample(x0, t, noise) instead, computed in the same pass."""
+        device = self.betas.device
+        n, h, w, two = flow.shape
+        Fr = int(num_frames)
+        if two != 2 or tuple(occlusion.shape) != (n, 1, h, w) or Fr < 1 or n % Fr:
+            raise ValueError(f"motion_to_latent: flow {tuple(flow.shape)} / occlusion {tuple(occlusion.shape)} are not b clips of "
+                             f"{Fr} frames of (h, w, 2) / (1, h, w)")
+        b = n // Fr
+        fl = flow.to(device=device, dtype=torch.float32).contiguous()
+        oc = occlusion.to(device=device, dtype=torch.float32).contiguous()
+        out = torch.empty((b, 3, Fr, h, w), device=device)
+        tt = z = a = s = None
+        if t is not None:
+            tt = self._q_timesteps("motion_to_latent", t, b, device)
+            if noise is None:
+                noise = self._default_noise(self.denoise_fn, device, None)(0, tuple(out.shape))
+            if tuple(noise.shape) != tuple(out.shape):
+                raise ValueError(f"motion_to_latent: noise {tuple(noise.shape)} does not match the latent {tuple(out.shape)}")
+            z = noise.to(device=device, dtype=torch.float32).contiguous()
+            a, s = self._q_tables(device)
+        with torch.cuda.device(device):
+            check(lib.dawn_motion_to_latent(ptr(fl), ptr(oc), b, Fr, h, w, ptr(tt), ptr(z), ptr(a), ptr(s), self.num_timesteps,
+                                            ptr(out), stream()), "dawn_motion_to_latent")
+        return out
 
     def _sample_eager(self, entry, fea, cond, img, steps, cond_scale, q, noise):
         """Runs `steps`, a list of (t, coefficients of the native update `entry`), in place on img (b, 3, F, h, w): all b clips
@@ -387,9 +501,59 @@ class GaussianDiffusion(nn.Module):
         return self._sample_eager("dawn_unet_ddpm_step", fea, cond, img, steps, cond_scale, q,
                                   lambda k, sel, one: draw(k, one).to(device).contiguous())
 
-    def _p_sample_loop_graph(self, unet, fea, cond, img, draw, q, st):
+    @torch.no_grad()
+    def p_sample_loop_from(self, x_t, t, fea, cond=None, cond_scale=1., clip_denoised=True, noise_fn=None, use_graph=False,
+                           seed=None):
+        """The ancestral loop from a given image, as the reference's interpolate runs it (U:1220-1221): x_t (b, 3, F, h, w) at
+        timestep t (e.g. `q_sample` of a real clip's latent at t), then p_sample at t - 1, t - 2, ..., 0; t = 0 runs no step.
+        noise_fn(k, shape) is the draw of step k, timestep t - 1 - k.  Eager as p_sample_loop (guidance included); use_graph
+        replays the cached step graph of p_sample_loop t times from a slot set to t - 1 (no capture of its own), and like it
+        refuses cond_scale != 1.  x_t is not modified; returns the sample."""
+        T = self.num_timesteps
+        if torch.is_tensor(t):
+            if t.numel() == 0 or bool((t != t.flatten()[0]).any()):
+                raise ValueError("p_sample_loop_from: t must hold one timestep for the whole batch")
+            t = t.flatten()[0]
+        t = int(t)
+        if not 0 <= t <= T:
+            raise ValueError(f"p_sample_loop_from: t = {t} is outside [0, {T}]")
+        unet = self.denoise_fn
+        img = self._start_image("p_sample_loop_from", x_t, fea, cond)
+        draw = noise_fn if noise_fn is not None else self._default_noise(unet, self.betas.device, seed)
+        q = self._clip_q(clip_denoised)
+        if use_graph and cond_scale != 1 and getattr(unet, "has_cond", True):
+            raise NotImplementedError("use_graph captures the cond_scale = 1 step (DAWN's shipped setting); "
+                                      "classifier-free guidance runs eagerly")
+        if t == 0:
+            return img
+        if use_graph:
+            return self._p_sample_loop_graph(unet, fea, cond, img, draw, q, stream(), t)
+        steps = [(i, self.ddpm_coefficients(i)) for i in reversed(range(t))]
+        return self._sample_eager("dawn_unet_ddpm_step", fea, cond, img, steps, cond_scale, q,
+                                  lambda k, sel, one: draw(k, one).to(self.betas.device).contiguous())
+
+    @torch.no_grad()
+    def interpolate(self, x1, x2, fea, cond=None, t=None, lam=0.5, cond_scale=1., noise_fn=None, use_graph=False):
+        """reference interpolate (U:1211-1224): q_sample x1 and x2 (b, 3, F, h, w) at timestep t (default num_timesteps - 1),
+        mix them as (1 - lam) * xt1 + lam * xt2 in the reference's three fp32 ops, and run the ancestral loop down from t
+        (`p_sample_loop_from`).  The reference's loop calls p_sample(img, t) without the features and conditioning p_sample
+        needs, so it raises TypeError there; this method takes them: fea (b, 272, h, w), cond (b, F, cond_dim), cond_scale.
+        noise_fn(k, shape): k = -2 and -1 are the q_sample noises of x1 and x2, k >= 0 step k of the loop (timestep t - 1 - k)."""
+        if tuple(x1.shape) != tuple(x2.shape):
+            raise ValueError(f"interpolate: x1 {tuple(x1.shape)} and x2 {tuple(x2.shape)} differ in shape")
+        t = self.num_timesteps - 1 if t is None else int(t)
+        b = x1.shape[0]
+        tt = torch.full((b,), t, dtype=torch.long)
+        z1, z2 = (noise_fn(k, tuple(x1.shape)) if noise_fn is not None else None for k in (-2, -1))
+        xt1, xt2 = self.q_sample(x1, tt, noise=z1), self.q_sample(x2, tt, noise=z2)
+        img = (1 - lam) * xt1 + lam * xt2
+        return self.p_sample_loop_from(img, t, fea, cond=cond, cond_scale=cond_scale, noise_fn=noise_fn, use_graph=use_graph)
+
+    def _p_sample_loop_graph(self, unet, fea, cond, img, draw, q, st, steps=None):
+        """The cached step graph replayed `steps` times per clip (default num_timesteps) from timestep steps - 1."""
         b, ch, Fr, h, w = img.shape
         device, T = img.device, self.num_timesteps
+        steps = T if steps is None else steps
         batched = self._batched(unet, b, Fr, h, w)
         one = (b, ch, Fr, h, w) if batched else (ch, Fr, h, w)
         g, _ = self._captured_graph(
@@ -401,8 +565,8 @@ class GaussianDiffusion(nn.Module):
             sel = slice(None) if batched else i
             unet.set_clip_invariants(fea[sel], cond[sel])
             g["x"].copy_(img[sel])
-            g["t"].fill_(T - 1)
-            for k in range(T):
+            g["t"].fill_(steps - 1)
+            for k in range(steps):
                 g["noise"].copy_(draw(k, one))
                 check(lib.dawn_unet_ddpm_launch(unet._handle, st), "dawn_unet_ddpm_launch")
             img[sel].copy_(g["x"])

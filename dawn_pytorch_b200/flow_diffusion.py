@@ -6,7 +6,9 @@ Same attribute names (`generator`, `unet`, `diffusion`, `face_loc_emb`), so `mod
 (UVG:527-528) and `generator.load_state_dict(checkpoint['generator'])` (FD:120) work unchanged; `sample_one_video` keeps its
 signature and output dictionary.  Underneath: the source encoder, the sampling loop (DDIM, or the ancestral loop when
 `sampling_timesteps` >= 1000 or None) and the frame decoder are the CUDA paths of this package (LfgGenerator, DynamicNfGaussianDiffusion over DynamicNfUnet3D) — one batched decode instead of a Python loop over
-frames (FD:375-383).  Training-only members (region / background predictors, VGG loss, `forward`) are out of scope and absent.
+frames (FD:375-383).  Training-only members (region / background predictors, VGG loss, `forward`) are out of scope and absent;
+`real_video_latent` takes the motion estimator as an argument, and `resample_video` re-samples a real clip's latent from a
+mid-schedule step.
 """
 import ctypes
 
@@ -122,22 +124,26 @@ class FlowDiffusion(nn.Module):
         noise_fn / use_graph are passed to the sampler (tests inject the noise the reference draws with torch.randn)."""
         pred = self._sample_latent(sample_img, sample_audio_hubert, sample_pose, sample_eye, sample_bbox, cond_scale, init_pose,
                                    init_eye, noise_fn, use_graph)
-        out = {}
-        out["sample_vid_grid"] = pred[:, :2]                                            # FD:366
-        out["sample_vid_conf"] = (pred[:, 2].unsqueeze(1) + 1) * 0.5                    # FD:369
-        vids, warped = [], []
-        for i in range(pred.shape[0]):                                                  # FD:375-383, all frames of a clip at once
-            p, d = self.generator.decode_sample(sample_img[i:i + 1], pred[i], need_deformed=True)
-            vids.append(p.permute(1, 0, 2, 3))
-            warped.append(d.permute(1, 0, 2, 3))
-        out["sample_out_vid"] = torch.stack(vids)
-        out["sample_warped_vid"] = torch.stack(warped)
-        return out
+        return self._decode(sample_img, pred)
 
     def _sample_latent(self, sample_img, sample_audio_hubert, sample_pose, sample_eye, sample_bbox, cond_scale, init_pose, init_eye,
                        noise_fn, use_graph):
         """FD:327-365: source features, face-box embedding, conditioning and the sampling loop -> pred (b, 3, F, h, w) = [grid_x,
         grid_y, conf], the sampled latent both sample_one_video and the talking-head generator decode."""
+        fea272, ref_text = self._conditioning(sample_img, sample_audio_hubert, sample_pose, sample_eye, sample_bbox, init_pose, init_eye)
+        b = fea272.shape[0]
+        h, w = fea272.shape[-2:]
+        D = self.diffusion
+        sample_fn = D.p_sample_loop if not D.is_ddim_sampling else D.ddim_sample       # GaussianDiffusion.sample, U:1150
+        pred = sample_fn(fea272, (b, D.channels, D.num_frames, h, w), cond=ref_text, cond_scale=cond_scale, noise_fn=noise_fn,
+                         use_graph=use_graph)
+        if self.use_residual_flow:
+            raise NotImplementedError("use_residual_flow=True is not used by the shipped configs (FD:362-364)")
+        return pred
+
+    def _conditioning(self, sample_img, sample_audio_hubert, sample_pose, sample_eye, sample_bbox, init_pose, init_eye):
+        """FD:327-350 + U:1151: the UNet's 272 feature channels [fea; face-box embedding] (b, 272, h, w) and the per-frame
+        conditioning ref_text (b, F, 1024 + pose_dim + 2) of one sampling run."""
         fea = self.generator.compute_fea(sample_img)                                    # FD:327
         bbox_mask = self.generate_bbox_mask(sample_bbox, size=sample_img.shape[-1])     # FD:328
         bbox_mask = self.face_loc_emb(bbox_mask)                                        # FD:330
@@ -150,16 +156,93 @@ class FlowDiffusion(nn.Module):
         if ref_pose.shape[-1] != init_pose.shape[-1]:
             ref_pose = torch.cat([ref_pose, init_pose[:, :, -1].unsqueeze(-1)], dim=-1)
         ref_text = torch.cat([sample_audio_hubert, ref_pose - init_pose, ref_eye - init_eye], dim=-1)          # FD:350
-        b = fea.shape[0]
         fea272 = torch.cat([fea, bbox_mask], dim=1)                                     # GaussianDiffusion.sample, U:1151
-        h, w = fea272.shape[-2:]
+        return fea272, ref_text
+
+    def _decode(self, sample_img, pred):
+        """FD:366-383: the output dictionary of a sampled latent pred (b, 3, F, h, w)."""
+        out = {}
+        out["sample_vid_grid"] = pred[:, :2]                                            # FD:366
+        out["sample_vid_conf"] = (pred[:, 2].unsqueeze(1) + 1) * 0.5                    # FD:369
+        vids, warped = [], []
+        for i in range(pred.shape[0]):                                                  # FD:375-383, all frames of a clip at once
+            p, d = self.generator.decode_sample(sample_img[i:i + 1], pred[i], need_deformed=True)
+            vids.append(p.permute(1, 0, 2, 3))
+            warped.append(d.permute(1, 0, 2, 3))
+        out["sample_out_vid"] = torch.stack(vids)
+        out["sample_warped_vid"] = torch.stack(warped)
+        return out
+
+    @staticmethod
+    def _motion_parts(motion):
+        """(region_predictor, bg_predictor, generator) of a FlowAE, or the triple itself."""
+        if isinstance(motion, (tuple, list)) and len(motion) == 3:
+            return tuple(motion)
+        if all(hasattr(motion, k) for k in ("region_predictor", "bg_predictor", "generator")):
+            return motion.region_predictor, motion.bg_predictor, motion.generator
+        raise TypeError("motion must be a FlowAE or its (region_predictor, bg_predictor, generator) of one LFG checkpoint")
+
+    @torch.no_grad()
+    def real_video_latent(self, real_vid, ref_img, motion):
+        """FD:248-262 + FD:281-282: a real clip as the diffusion's clean latent x0 (b, 3, F, h, w) = [grid, occlusion * 2 - 1].
+        real_vid (b, 3, F, H, W) in [0, 1]; ref_img (b, 3, H, W), the source image each clip's motion is estimated against;
+        motion: this package's FlowAE, or the (RegionPredictor, BGMotionPredictor, MotionGenerator) it holds, loaded from the same
+        LFG checkpoint as `generator`.  It is an argument, not a submodule, so this module's state_dict is unchanged.  The
+        reference's training-time ColorJitter (FD:207-219) is an augmentation and is not applied: the frames are used as given.
+        Runs the motion estimator on the device, clip by clip, then `dawn_motion_to_latent`."""
+        rp, bgp, gen = self._motion_parts(motion)
+        if real_vid.dim() != 5 or real_vid.shape[1] != 3 or ref_img.dim() != 4 or ref_img.shape[0] != real_vid.shape[0] or \
+                tuple(ref_img.shape[1:]) != (3,) + tuple(real_vid.shape[-2:]):
+            raise ValueError(f"real_video_latent: real_vid {tuple(real_vid.shape)} must be (b, 3, F, H, W) and ref_img "
+                             f"{tuple(ref_img.shape)} (b, 3, H, W)")
+        b, _, nf, H, W = real_vid.shape
+        flows, occs = [], []
+        for i in range(b):
+            frames = real_vid[i].permute(1, 0, 2, 3).contiguous().float()             # '(b f) c h w' of one clip, FD:252
+            src = ref_img[i:i + 1].contiguous().float()                                 # FD:253: the source of every frame
+            source_region_params = rp(src)                                              # FD:254
+            driving_region_params = rp(frames)                                          # FD:256
+            bg_params = bgp(src, frames)                                                # FD:257
+            m = gen.flow(src, driving_region_params, source_region_params, bg_params)   # FD:258-260
+            flows.append(m["optical_flow"])
+            occs.append(m["occlusion_map"])
+        return self.diffusion.motion_to_latent(torch.cat(flows), torch.cat(occs), nf)
+
+    @torch.no_grad()
+    def resample_video(self, sample_img, x0, sample_audio_hubert, sample_pose, sample_eye, sample_bbox, cond_scale, start,
+                       init_pose=None, init_eye=None, noise_fn=None, use_graph=False):
+        """Re-generates a real clip's motion under new conditioning: x0 (b, 3, F, h, w), e.g. `real_video_latent`, is noised to the
+        timestep of step `start` of the sampler's schedule and denoised from there with the conditioning of sample_one_video
+        (same arguments, same face-box embedding and ref_text).  The later `start`, the more of the clip's own motion survives.
+        DDIM schedule: x_t = q_sample(x0, ddim_schedule()[start][0]), then `ddim_sample_from(x_t, start)`.  Ancestral schedule
+        (sampling_timesteps >= num_timesteps): t = num_timesteps - 1 - start, x_t = q_sample(x0, t), then `p_sample_loop_from(x_t, t)`.
+        noise_fn(k, shape): k = -1 the q_sample noise, k >= 0 the sampler's draws as ddim_sample_from / p_sample_loop_from number
+        them.  Returns sample_one_video's dictionary."""
         D = self.diffusion
-        sample_fn = D.p_sample_loop if not D.is_ddim_sampling else D.ddim_sample       # GaussianDiffusion.sample, U:1150
-        pred = sample_fn(fea272, (b, D.channels, D.num_frames, h, w), cond=ref_text, cond_scale=cond_scale, noise_fn=noise_fn,
-                         use_graph=use_graph)
+        fea272, ref_text = self._conditioning(sample_img, sample_audio_hubert, sample_pose, sample_eye, sample_bbox, init_pose, init_eye)
+        b = fea272.shape[0]
+        h, w = fea272.shape[-2:]
+        shape = (b, D.channels, D.num_frames, h, w)
+        if tuple(x0.shape) != shape:
+            raise ValueError(f"resample_video: x0 {tuple(x0.shape)} does not match the sample shape {shape}")
+        start = int(start)
+        if D.is_ddim_sampling:
+            n = len(D.ddim_schedule())
+            if not 0 <= start < n:
+                raise ValueError(f"resample_video: start = {start} is outside [0, {n}), the {n}-step DDIM schedule")
+            t = D.ddim_schedule()[start][0]
+        else:
+            if not 0 <= start < D.num_timesteps:
+                raise ValueError(f"resample_video: start = {start} is outside [0, {D.num_timesteps})")
+            t = D.num_timesteps - 1 - start
+        x_t = D.q_sample(x0, torch.full((b,), t, dtype=torch.long), noise=noise_fn(-1, shape) if noise_fn is not None else None)
+        if D.is_ddim_sampling:
+            pred = D.ddim_sample_from(x_t, start, fea272, cond=ref_text, cond_scale=cond_scale, noise_fn=noise_fn, use_graph=use_graph)
+        else:
+            pred = D.p_sample_loop_from(x_t, t, fea272, cond=ref_text, cond_scale=cond_scale, noise_fn=noise_fn, use_graph=use_graph)
         if self.use_residual_flow:
             raise NotImplementedError("use_residual_flow=True is not used by the shipped configs (FD:362-364)")
-        return pred
+        return self._decode(sample_img, pred)
 
     def forward(self, *a, **k):
         raise NotImplementedError("FlowDiffusion.forward is the training step (FD:203-323): out of scope of this inference path")

@@ -206,6 +206,24 @@ int dawn_unet_ddpm_capture(dawn_unet* h, float* x, float* eps, const float* nois
                            int num_timesteps, float q, void* scratch);
 int dawn_unet_ddpm_launch(dawn_unet* h, void* stream);
 
+/* Forward noising of a clean latent (reference GaussianDiffusion.q_sample U:1226-1232) for B clips of n floats each:
+ *   out[c] = sqrt_acp[t[c]] * x0[c] + sqrt_1m_acp[t[c]] * noise[c]
+ * rounded as the reference's two fp32 products and one sum (no fused multiply-add), so the result is bit-identical to torch.
+ * x0, noise, out: device (B, n); t: device int64[B], one timestep per clip; sqrt_acp / sqrt_1m_acp: device fp32 tables of
+ * num_t entries (the schedule's sqrt_alphas_cumprod and sqrt_one_minus_alphas_cumprod).  A timestep outside [0, num_t) reads
+ * the nearest table row: range checks belong to the caller, where t is known on the host.  out must not overlap x0 or noise.
+ * 1 <= B <= 65535.  No host synchronisation: it may be captured into a CUDA graph. */
+int dawn_q_sample(const float* x0, const float* noise, const int64_t* t, const float* sqrt_acp, const float* sqrt_1m_acp, int num_t,
+                  int64_t B, int64_t n, float* out, void* stream);
+
+/* The LFG motion estimator's output as the sampler's latent (FD:248-262, 280-282): for each of B clips of F frames, flow
+ * (F, h, w, 2) and occlusion (F, 1, h, w), as dawn_lfg_motion_flow writes them (clips back to back), become
+ *   out (B, 3, F, h, w) = [flow_x, flow_y, occlusion * 2 - 1]      (the product and difference rounded as fp32 torch ops)
+ * t == NULL: out is that x0.  t != NULL: out is dawn_q_sample of it with noise (B, 3, F, h, w) and the tables, in the same
+ * pass; bit-identical to the two calls.  flow 8-byte aligned; out must not overlap the inputs.  No host synchronisation. */
+int dawn_motion_to_latent(const float* flow, const float* occlusion, int64_t B, int F, int h, int w, const int64_t* t,
+                          const float* noise, const float* sqrt_acp, const float* sqrt_1m_acp, int num_t, float* out, void* stream);
+
 /* One contraction through exactly one kernel path, for per-kernel tests against a high-precision reference.
  * Out[m, n] = epilogue( sum_{tap, c} A[pixel(m, tap), c] * B[tap*Cin + c, n] ) with the product's GemmParams semantics
  * (dawn_pytorch_b200/csrc/gemm.cuh): rows m = (f, i, j) over an F x OHs x OWs output sub-grid (M = F*OHs*OWs), input pixel
@@ -315,8 +333,11 @@ enum {
   DAWN_KERNEL_HEADS_OUT = 12,      /* out[b][j][f][p] = 1x1 heads of x (j < ng: w, b) and y (j >= ng: w2, b2), C channels, P = H*W */
   DAWN_KERNEL_DDIM_STEP = 13,      /* the DDIM update of dawn_ddim_step on xs (n values, in place) with eps e, noise (may be NULL),
                                       coef {ca, cb, sqrt_alpha_next, c, sigma}, q and scratch (n + 512 words); see `replicas` */
-  DAWN_KERNEL_DDPM_STEP = 14       /* the ancestral update of dawn_ddpm_step, coef {ca, cb, c1, c2, sigma}; with tab (num_t rows of
+  DAWN_KERNEL_DDPM_STEP = 14,      /* the ancestral update of dawn_ddpm_step, coef {ca, cb, c1, c2, sigma}; with tab (num_t rows of
                                       those five) the coefficients are row clamp(*t_slot, 0, num_t - 1), read on the device */
+  DAWN_KERNEL_Q_SAMPLE = 15,       /* dawn_q_sample: out (clips, n) from x = x0, noise, t [clips], w / b = the two num_t-entry tables */
+  DAWN_KERNEL_MOTION_TO_LATENT = 16 /* dawn_motion_to_latent: x = flow (clips*F, H, W, 2), y = occlusion (clips*F, 1, H, W) ->
+                                      out (clips, 3, F, H, W); with t the fused noising (noise, w, b, num_t as Q_SAMPLE) */
 };
 #define DAWN_KERNEL_MAX_DESC 16
 typedef struct {
